@@ -1,8 +1,7 @@
 """Import the unmodified reference (zgcr/SimpleAICV_pytorch_training_examples).
 
-Search order: ``baseline/_ref`` (the offline pip install made by ``baseline/install_ref.sh``; it is
-git-ignored but travels to the GPU box with the gpurun snapshot), then ``/root/reference`` (build
-container only).  ``tools.utils`` / ``tools.scripts`` import ``calflops`` and ``pycocotools`` at module
+Search order: ``oracle/_ref`` (the copy ``__graft_entry__.build()`` makes with oracle/build_ref.py), then
+``baseline/_ref`` (the offline pip install made by ``baseline/install_ref.sh``); both are git-ignored.  ``tools.utils`` / ``tools.scripts`` import ``calflops`` and ``pycocotools`` at module
 level (tools/utils.py:19, tools/scripts.py:14-15) which are not installed here; the hot path never
 calls them, so empty stub modules are registered for those two names only.
 
@@ -14,7 +13,7 @@ import sys
 import types
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-CANDIDATES = [os.path.join(_HERE, '_ref'), '/root/reference']
+CANDIDATES = [os.path.join(os.path.dirname(_HERE), 'oracle', '_ref'), os.path.join(_HERE, '_ref')]
 
 
 def root():
@@ -31,7 +30,7 @@ def available():
 def _ensure_path():
     r = root()
     if r is None:
-        raise ImportError('reference not installed: run baseline/install_ref.sh in the build container')
+        raise ImportError('reference not installed: build() copies it into oracle/_ref (oracle/build_ref.py)')
     if r not in sys.path:
         sys.path.insert(0, r)
     for name in ('calflops', 'pycocotools', 'pycocotools.coco', 'pycocotools.cocoeval', 'pycocotools.mask'):

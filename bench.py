@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — images/sec of the SimpleAICV classification training step on B200.
+"""bench.py — images/sec of the SimpleAICV classification training step on H100.
 
 Headline workload (BASELINE.json configs[1]): ResNet-50, 224x224, batch 256 per GPU, synthetic images,
 CELoss, SGD(lr 0.1, momentum 0.9, wd 1e-4, 1-D params undecayed) — one "step" is forward + loss +
@@ -7,7 +7,7 @@ backward (+ bucketed gradient all-reduce when N > 1) + optimizer step, exactly t
 tools/scripts.py:141-270 in the reference.  The same JSON line carries a ``vit_base_patch16`` sub-record
 (BASELINE configs[2]: ViT-B/16, soft labels, AdamW with layer-wise lr decay) measured the same way.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]     our arm (sm_100a kernels)
+  python bench.py [--gpus N] [--steps K] [--warmup W]     our arm (sm_90a kernels)
   python bench.py --impl reference ...                    reference arm: the reference's CPU path (its own
                                                           modules from baseline/_ref, else the oracle port)
 Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for what every key means.
@@ -35,7 +35,7 @@ METRICS = {'resnet50': 'images/sec (ResNet-50 224x224 training step, whole job)'
            'vit_base_mae': 'images/sec (MAE ViT-B/16 224x224 pre-training step, whole job)'}
 WORKLOADS = {'resnet50': 'ResNet-50 224x224 bs256/GPU training step (fwd+CELoss+bwd+grad all-reduce+SGD)',
              'vit_base_patch16': 'ViT-B/16 224x224 bs256/GPU training step (fwd+OneHotLabelCELoss+bwd+grad all-reduce+AdamW)',
-             'sam_h_encoder': ('SAM ViT-H image encoder 1024x1024 bs8/GPU training step (encoder fwd + feature MSE against a synthetic '
+             'sam_h_encoder': ('SAM ViT-H image encoder 1024x1024 bs4/GPU training step (encoder fwd + feature MSE against a synthetic '
                                'teacher map, the train_distill_sam_encoder step body + bwd + grad all-reduce + AdamW); prompt encoder / '
                                'mask decoder are outside the built path'),
              'resnet50_detr': ('DETR-R50 1024x1024 bs4/GPU training step (the shipped res50_detr_yoloresize1024 shape; fwd + DETRLoss with the '
@@ -54,14 +54,7 @@ def _peaks():
         d = json.load(open(p))
         return {'hbm_gbs': d['hbm_gbs'], 'tf_burst': d['bf16_tflops'], 'tf_sustained': d.get('bf16_tflops_sustained', d['bf16_tflops']),
                 'source': 'measured'}
-    return {'hbm_gbs': 6650.0, 'tf_burst': 1590.0, 'tf_sustained': 1400.0, 'source': 'fallback'}
-
-
-def _traffic():
-    """DRAM traffic per launch of the dominant kernel from the committed ncu --set full capture
-    (profiles/r02_traffic.json, written by tests/summarize_profiles.py from the .ncu-rep)."""
-    p = os.path.join(ROOT, 'profiles', 'r02_traffic.json')
-    return json.load(open(p)) if os.path.exists(p) else None
+    return {'hbm_gbs': 3350.0, 'tf_burst': 989.0, 'tf_sustained': 989.0, 'source': 'H100 SXM data sheet (dense BF16, 700 W)'}
 
 
 class ClockSampler:
@@ -343,7 +336,7 @@ def describe(name, a):
 
 
 def roofline_from_table(table, peaks, model_name, B, ms_step, dump_path=None):
-    """All-launch roofline of the tensor-core engine kernels of one step (gemm_sm100_kernel + the attention
+    """All-launch roofline of the tensor-core engine kernels of one step (gemm_sm90_kernel + the attention
     kernels): every launch is bounded by max(FLOPs / tensor peak, algorithmic bytes / HBM peak); frac =
     sum of those roofline times / sum of the measured CUDA-event times.  The two classes are kept beside it."""
     gemm = {k: v for k, v in table.items() if v['flops'] > 0}
@@ -374,13 +367,10 @@ def roofline_from_table(table, peaks, model_name, B, ms_step, dump_path=None):
     d = cls_rec(dom)
     worst = min(gemm, key=lambda k: gemm[k]['roof_frac']) if gemm else None
     top = max(gemm, key=lambda k: gemm[k]['ms']) if gemm else None
-    tr = _traffic()
     roof = {'bound': dom, 'achieved': d['achieved'] * frac_all / d['frac'] if d and d['frac'] else None, 'peak': d['peak'] if d else None,
             'unit': d['unit'] if d else None, 'frac': frac_all,
-            'traffic': (tr or {}).get(model_name, {}).get('dram_bytes_per_launch'),
             'algorithmic_bytes_per_launch': (sum(v['bytes'] for v in gemm.values()) / max(1, sum(v['calls'] for v in gemm.values()))) if gemm else None,
-            'traffic_note': (tr or {}).get(model_name, {}).get('note'),
-            'kernel': 'gemm_sm100_kernel (+ attention kernels for ViT)',
+            'kernel': 'gemm_sm90_kernel (+ attention kernels for ViT)',
             'frac_definition': ('ALL launches of the tensor-core engine in one step: each launch is bounded by max(algorithmic '
                                 'FLOPs / sustained bf16 peak, algorithmic bytes / HBM peak) from MEASURED_PEAKS; frac = sum(bound '
                                 'times) / sum(CUDA-event times).  achieved/peak/unit restate frac in the units of the class that '
@@ -406,14 +396,27 @@ def roofline_from_table(table, peaks, model_name, B, ms_step, dump_path=None):
     return roof
 
 
-def measure_model(model_name, args, rank, world, local_rank, dump_path=None, with_ddp_check=False):
+def dump_outputs(out_dir, loss, model):
+    """--dump-outputs: what the timed training step hands its caller after its last step - the loss and the updated
+    parameters (a fixed, seeded sample of at most 4 Mi values) - as .npy files (float64 / float32, < 64 MB in all).  The
+    inputs and the initial parameters are seeded, so two builds run with the same arguments can be compared file by file."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, 'loss.npy'), loss.detach().double().reshape(-1).cpu().numpy())
+    flat = torch.cat([q.detach().float().reshape(-1) for q in model.parameters()]).cpu()
+    idx = torch.randint(0, flat.numel(), (min(flat.numel(), 4 << 20),), generator=torch.Generator().manual_seed(0)).sort().values
+    np.save(os.path.join(out_dir, 'params_sample.npy'), flat[idx].numpy())
+
+
+def measure_model(model_name, args, rank, world, local_rank, dump_path=None, with_ddp_check=False, outputs_dir=None):
     """Device-timed and end-to-end throughput + the roofline pass for one model.  Returns a dict (rank 0) or None."""
     from simpleaicv_pytorch_training_examples_b200 import _lib
     from simpleaicv_pytorch_training_examples_b200.classification import backbones, losses
     from simpleaicv_pytorch_training_examples_b200.distributed import B200DataParallel, overlap_self_check
     from simpleaicv_pytorch_training_examples_b200.tools import utils as tutils
     dev = torch.device('cuda', local_rank)
-    B = {'sam_h_encoder': 8, 'resnet50_detr': 4}.get(model_name, args.batch)
+    # SAM ViT-H without gradient checkpointing: batch 8 needs more than the 80 GB of an H100, batch 4 fits
+    B = {'sam_h_encoder': 4, 'resnet50_detr': 4}.get(model_name, args.batch)
     torch.manual_seed(0)
     x_host, y_host = synthetic_batch(model_name, B, rank, True)
     detr_masks = None
@@ -518,11 +521,12 @@ def measure_model(model_name, args, rank, world, local_rank, dump_path=None, wit
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    steps = args.steps if model_name != 'sam_h_encoder' else max(3, args.steps // 3)
+    steps = args.steps
     capturable_step = detr_masks is None     # DETRLoss matches on the host (a sync per step) and DETR trains with dropout
     l0 = _lib.launch_count()
-    ms_total = timed(lambda: step(x_dev, y_dev), steps)
-    launches = (_lib.launch_count() - l0) * args.steps // steps
+    last_loss = [None]
+    ms_total = timed(lambda: last_loss.__setitem__(0, step(x_dev, y_dev)), steps)
+    launches = _lib.launch_count() - l0
     eager_ms_step = ms_total / steps
 
     # end to end through the public API: every step's batch comes from pinned host memory through
@@ -555,12 +559,15 @@ def measure_model(model_name, args, rank, world, local_rank, dump_path=None, wit
     # device-resident throughput: the same graph replayed on resident inputs when there is one, else the eager loop above
     if split is not None:
         split([x_dev], y_dev)
-        ms_step = timed(lambda: split([x_dev], y_dev), steps) / steps
+        ms_step = timed(lambda: last_loss.__setitem__(0, split([x_dev], y_dev)), steps) / steps
     elif graphed is not None:
         graphed.replay()
         ms_step = timed(graphed.replay, steps) / steps
+        last_loss[0] = graphed.static_loss
     else:
         ms_step = eager_ms_step
+    if outputs_dir and rank == 0:
+        dump_outputs(outputs_dir, last_loss[0], model)
     value = B * world / (ms_step / 1e3)
 
     def e2e_loop(k):
@@ -641,7 +648,7 @@ def run_b200(args, rank, world, local_rank):
     dev = torch.device('cuda', local_rank)
     torch.cuda.set_device(dev)
     B = args.batch
-    main = measure_model(args.model, args, rank, world, local_rank, args.dump_ops, with_ddp_check=True)
+    main = measure_model(args.model, args, rank, world, local_rank, args.dump_ops, with_ddp_check=True, outputs_dir=args.dump_outputs)
     other = None
     if not args.no_second_model:
         second = 'vit_base_patch16' if args.model == 'resnet50' else 'resnet50'
@@ -669,7 +676,7 @@ def run_b200(args, rank, world, local_rank):
         'warmup': max(3, args.warmup), 'ms_per_step': main['ms_per_step'], 'higher_is_better': True, 'scaling': 'weak',
         'vs_baseline': None, 'dtype': 'bf16', 'data': 'synthetic',
         'config': {'workload': main['workload'], 'per_gpu_batch': B, 'global_batch': B * world, 'parallelism': f'dp{world}',
-                   'l2_policy': 'inputs+activations (>10 GB/step) far exceed the 126 MB L2; no explicit flush',
+                   'l2_policy': 'inputs+activations (>10 GB/step) far exceed the 50 MB L2; no explicit flush',
                    'images_per_sec_per_gpu': main['value'] / world},
         'clocks': main['clocks'], 'e2e': main['e2e'], 'gpu_launches': main['gpu_launches'], 'roofline': main['roofline'],
         'cpu_baseline': cpu_base,
@@ -695,10 +702,6 @@ def run_b200(args, rank, world, local_rank):
     if detr_rec is not None:
         line['resnet50_detr'] = {k: detr_rec[k] for k in SUB}
         line['resnet50_detr']['images_per_sec_per_gpu'] = detr_rec['value'] / world
-    torch_base = os.path.join(ROOT, 'profiles', 'r02_torch_gpu_baseline.json')
-    if os.path.exists(torch_base):
-        line['torch_ddp_target'] = {'source': 'profiles/r02_torch_gpu_baseline.json (unmodified reference under torch DDP, same pool)',
-                                    'records': json.load(open(torch_base)).get('summary')}
     print(json.dumps(line), flush=True)
 
 
@@ -712,11 +715,14 @@ def main():
     ap.add_argument('--model', default='resnet50', choices=['resnet50', 'vit_base_patch16'],
                     help='resnet50 = BASELINE configs[1] (default, the headline); vit_base_patch16 = configs[2]')
     ap.add_argument('--dump-ops', default=None, help='write the per-op timing table (csv) here')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help="after the timed steps, write the main model's last-step loss and a seeded sample of its updated parameters "
+                         'to DIR/<name>.npy')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-second-model', action='store_true', help='skip the sub-record of the other BASELINE model')
     ap.add_argument('--detr', action='store_true', help='add the DETR-R50 sub-record (BASELINE configs[4]; shipped 1024x1024 shape, bs4)')
     ap.add_argument('--mae', action='store_true', help='add the MAE ViT-B/16 pre-training sub-record (SURVEY.md 8 f4)')
-    ap.add_argument('--sam', action='store_true', help='add the SAM ViT-H image-encoder sub-record (BASELINE configs[3]: bs8, 1024x1024)')
+    ap.add_argument('--sam', action='store_true', help='add the SAM ViT-H image-encoder sub-record (BASELINE configs[3] shape at bs4, 1024x1024: bs8 does not fit in 80 GB)')
     ap.add_argument('--no-graph-ddp', action='store_true',
                     help='N > 1: launch the step eagerly instead of capturing it (NCCL bucket all-reduces included) in one CUDA graph')
     ap.add_argument('--prefetch-streams', type=int, default=4, help='copy streams of the end-to-end host prefetcher (tools.utils.CudaPrefetcher)')
@@ -729,7 +735,7 @@ def main():
         run_reference(args, rank)
         return
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference for the CPU path)')
+        raise SystemExit('bench.py: no CUDA device; the GPU arm has no CPU fallback (use --impl reference for the CPU path)')
     if world > 1:
         os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
         torch.cuda.set_device(local_rank)

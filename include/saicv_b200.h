@@ -1,4 +1,4 @@
-/* saicv_b200.h — C ABI of libsaicv_b200.so: the sm_100a kernels behind the SimpleAICV
+/* saicv_b200.h — C ABI of libsaicv_b200.so: the sm_90a kernels behind the SimpleAICV
  * data-parallel training hot path (conv / ViT backbones forward + backward).
  *
  * The reference (zgcr/SimpleAICV_pytorch_training_examples) ships no native code; every entry
@@ -29,7 +29,7 @@ extern "C" {
 
 int saicv_version(void);
 const char* saicv_last_error(void);
-/* Number of SMs the persistent kernels size their grids for (148 on B200). */
+/* Number of SMs the persistent kernels size their grids for (132 on H100 SXM). */
 int saicv_sm_count(void);
 /* Kernels launched by this library in this process so far (bench.py reports the delta). */
 long long saicv_launch_count(void);
@@ -114,7 +114,7 @@ int saicv_add_strided2(void* dx, const void* dd, int n, int p, int q, int h, int
 /* Column reductions are deterministic (no atomics): every block writes one row of partial sums
  * into a caller-provided workspace `partials` of SAICV_BN_PARTIAL_ROWS * 2 * c floats, folded in a
  * fixed order by the next call. */
-#define SAICV_BN_PARTIAL_ROWS 296
+#define SAICV_BN_PARTIAL_ROWS 264
 /* per-channel partial sum / sum of squares of y[rows][c] (bf16) -> partials. */
 int saicv_bn_stats(const void* y, float* partials, long long rows, int c, void* stream);
 /* folds `partial_rows` rows of `partials` (0: the row count saicv_bn_stats used for this rows, c;
@@ -268,7 +268,7 @@ int saicv_relpos_shift(const void* dqe, void* ef, int bw, int heads, int hd, int
 int saicv_relpos_dq_combine(const void* dqe, const float* dqx, void* dqkv, int bw, int heads, int hd, int l, int dqk,
                             float scale, void* stream);
 
-/* ---- fused multi-head attention on tcgen05 / TMEM (csrc/attn_sm100.cuh) ------------------------------
+/* ---- fused multi-head attention on wgmma (csrc/attn_sm90.cuh) ------------------------------
  * Replaces the materialised attention of the reference: vit.py:62-80 (q k^T * scale, softmax, @ v),
  * segment_anything/image_encoder.py:167-184 (+ decomposed rel-pos bias, folded into extra score columns by
  * the caller: dqk = head_dim + bias columns), detection/models/detr.py:54-56,103-109 (nn.MultiheadAttention
@@ -310,8 +310,6 @@ typedef struct {
   int dk_cols;
 } saicv_attn_bwd_args;
 int saicv_attn_bwd(const saicv_attn_bwd_args* a, void* stream);
-/* 1 if an attention kernel found its shared-memory window misaligned (synchronises; for tests). */
-int saicv_attn_error(void);
 /* ViT convenience entries (vit.py:66-76): qkv bf16 [b][l][3][h][d] -> out bf16 [b][l][h*d]; lse [b][h][l];
  * backward writes dqkv in the layout of qkv; delta: fp32 workspace [b][h][l]. */
 int saicv_attention_fwd(const void* qkv, void* out, float* lse, int b, int l, int h, int d,

@@ -78,7 +78,7 @@ def param_names(sd):
     return [k for k in sd if not (k.endswith('running_mean') or k.endswith('running_var') or k.endswith('num_batches_tracked'))]
 
 
-# ---- optional emulation of the B200 path's storage precision -----------------------------------
+# ---- optional emulation of the kernels' storage precision -----------------------------------
 # The kernels keep activations and activation gradients in bf16 and feed bf16 operands to the
 # tensor cores (fp32 accumulation; BN statistics, parameters and parameter gradients in fp32).
 # With emulate_bf16=True the SAME reference algorithm is evaluated with a round-to-bf16 at exactly

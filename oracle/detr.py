@@ -159,7 +159,7 @@ def _mha(sd, name, q_in, k_in, v_in, key_bias, fns):
 
 def forward(sd, x, masks, arch, training=True, emulate_bf16=False, trace=None, enc_layers=ENC_LAYERS, dec_layers=DEC_LAYERS):
     """(cls_outputs [dec_layers, B, Q, classes + 1], reg_outputs [dec_layers, B, Q, 4]) for the NCHW fp32 batch x and the
-    bool padding masks [B, H, W].  emulate_bf16 inserts round-to-bf16 at the B200 path's storage points: GEMM operand
+    bool padding masks [B, H, W].  emulate_bf16 inserts round-to-bf16 at the kernels' storage points: GEMM operand
     copies (weights, bf16 copies of the fp32 token stream, attention probabilities), GEMM outputs that are stored in
     bf16 (q, k, v, attention outputs, FFN hidden) and the gradients that travel in bf16; the token stream, LayerNorm
     and softmax stay fp32."""

@@ -122,7 +122,7 @@ def _blocks(sd, prefix, x, dim, depth, heads, rb, rw, rg):
 
 
 def forward(sd, x, noise, arch, mask_ratio=0.75, emulate_bf16=False, enc_depth=None, dec_depth=None):
-    """Returns (pred [B, L, p*p*3], mask [B, L]).  emulate_bf16 rounds to bf16 at the B200 path's storage points (as
+    """Returns (pred [B, L, p*p*3], mask [B, L]).  emulate_bf16 rounds to bf16 at the kernels' storage points (as
     oracle/vit.py); the residual streams stay fp32."""
     patch, dim, depth, heads, ddim, ddepth, dheads, ratio = ARCHS[arch]
     depth, ddepth = enc_depth or depth, dec_depth or ddepth

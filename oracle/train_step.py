@@ -23,7 +23,7 @@ def ce_loss(logits, labels):
 
 def loss_and_grads(sd, x, labels, arch, emulate_bf16=False, trace=None):
     """Returns (logits, loss, {param name: grad}); BN running stats in sd are updated.
-    emulate_bf16: evaluate with the B200 path's bf16 storage points (convnets.forward)."""
+    emulate_bf16: evaluate with the kernels' bf16 storage points (convnets.forward)."""
     names = convnets.param_names(sd)
     for n in names:
         sd[n].requires_grad_(True)

@@ -101,7 +101,7 @@ def _bn(sd, name, x, training):
 
 
 def forward(sd, x, arch, training=True, emulate_bf16=False, trace=None):
-    """Logits for the NCHW fp32 batch x.  emulate_bf16 inserts round-to-bf16 at the B200 path's storage points
+    """Logits for the NCHW fp32 batch x.  emulate_bf16 inserts round-to-bf16 at the kernels' storage points
     (every GEMM / depthwise operand and output, BN outputs; the residual stream and all statistics stay fp32)."""
     planes, ratios, nums = ARCHS[arch]
     emu = emulate_bf16

@@ -81,7 +81,7 @@ def param_names(sd):
 
 
 def forward(sd, x, arch, global_pool=False, emulate_bf16=False, trace=None, depth=None):
-    """Logits for the NCHW fp32 batch x.  emulate_bf16 inserts round-to-bf16 at the B200 path's
+    """Logits for the NCHW fp32 batch x.  emulate_bf16 inserts round-to-bf16 at the kernels'
     storage points (LayerNorm outputs, qkv, attention probabilities/outputs, MLP hidden, GEMM
     operand copies of weights and of output gradients); the residual stream stays fp32."""
     emu = emulate_bf16

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libsaicv_b200.so')
-BN_PARTIAL_ROWS = 296  # SAICV_BN_PARTIAL_ROWS
+BN_PARTIAL_ROWS = 264  # SAICV_BN_PARTIAL_ROWS
 
 c_void_p = ctypes.c_void_p
 c_int = ctypes.c_int
@@ -87,7 +87,6 @@ SIGNATURES = {
     'saicv_attention_bwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p],
     'saicv_attn_fwd': [ctypes.POINTER(AttnArgs), c_void_p],
     'saicv_attn_bwd': [ctypes.POINTER(AttnBwdArgs), c_void_p],
-    'saicv_attn_error': [],
     'saicv_window_partition': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_window_unpartition': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_add_pos_embed': [c_void_p, c_void_p, c_int, c_ll, c_void_p],

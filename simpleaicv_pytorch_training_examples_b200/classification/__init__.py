@@ -1,3 +1,3 @@
-"""Drop-in counterpart of ``SimpleAICV.classification`` for the B200 hot path: ``backbones``
+"""Drop-in counterpart of ``SimpleAICV.classification`` for the H100 hot path: ``backbones``
 (model constructors with the reference's names and state_dict layout) and ``losses``."""
 from . import backbones, losses  # noqa: F401

@@ -1,7 +1,7 @@
 """DarknetTiny / Darknet19 / Darknet53 with the reference's constructor surface and state_dict layout
 (SimpleAICV/classification/backbones/darknet.py:16-31 ActivationBlock, :34-65 ConvBnActBlock,
 :68-113 Darknet19Block, :116-144 Darknet53Block, :147-244 DarknetTiny, :247-320 Darknet19,
-:323-432 Darknet53, :435-450 constructors), executed by engine.convnet on sm_100a kernels.
+:323-432 Darknet53, :435-450 constructors), executed by engine.convnet on sm_90a kernels.
 
 Layers whose channel counts are not multiples of 64 (16/32-channel stacks) run on channel-padded
 activations inside the runtime; parameters keep the reference's shapes.  The 2x2 max-pools, the
@@ -92,7 +92,7 @@ class _DarknetBase(nn.Module):
 
     def forward(self, x):
         if not x.is_cuda:
-            raise RuntimeError('this model runs on B200 kernels only; move the batch to the GPU '
+            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU '
                                '(no CPU fallback exists)')
         return run_network(self._runtime(), x.float(), self.training)
 

@@ -1,7 +1,7 @@
 """ResNet 18/34/50/101/152 with the reference's constructor surface and state_dict layout
 (SimpleAICV/classification/backbones/resnet.py:19-48 ConvBnActBlock, :51-97 BasicBlock,
 :100-155 Bottleneck, :158-245 ResNet, :254-271 constructors), executed by
-engine.convnet.ResNetRT on hand-written sm_100a kernels.
+engine.convnet.ResNetRT on hand-written sm_90a kernels.
 
 The nn.Modules below are parameter containers: they create the same torch submodules in the same
 order as the reference (so seeded initialisation and ``state_dict()`` keys/shapes are identical)
@@ -21,7 +21,7 @@ class ConvBnActBlock(nn.Module):
 
     def __init__(self, inplanes, planes, kernel_size, stride, padding, groups=1, has_bn=True, has_act=True):
         super().__init__()
-        assert groups == 1 and has_bn, 'the B200 runtime implements the conv+BN blocks the ResNets use'
+        assert groups == 1 and has_bn, 'the H100 runtime implements the conv+BN blocks the ResNets use'
         conv = nn.Conv2d(inplanes, planes, kernel_size, stride=stride, padding=padding, groups=groups, bias=False)
         self.layer = nn.Sequential(conv, nn.BatchNorm2d(planes),
                                    nn.ReLU(inplace=True) if has_act else nn.Sequential())
@@ -103,7 +103,7 @@ class _ResNetBase(nn.Module):
 
     def forward(self, x):
         if not x.is_cuda:
-            raise RuntimeError('this model runs on B200 kernels only; move the batch to the GPU '
+            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU '
                                '(no CPU fallback exists)')
         return run_network(self._runtime(), x.float(), self.training)
 

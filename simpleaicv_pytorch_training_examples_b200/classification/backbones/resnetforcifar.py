@@ -1,5 +1,5 @@
 """CIFAR ResNets (3x3 stride-1 stem, no max-pool) with the reference's constructor surface
-(SimpleAICV/classification/backbones/resnetforcifar.py:27-125), on the B200 runtime."""
+(SimpleAICV/classification/backbones/resnetforcifar.py:27-125), on the H100 runtime."""
 from .resnet import BasicBlock, Bottleneck, ConvBnActBlock, _init_like_reference, _ResNetBase
 
 __all__ = ['resnet18cifar', 'resnet34cifar', 'resnet50cifar', 'resnet101cifar', 'resnet152cifar']

@@ -1,7 +1,7 @@
 """VAN b0..b6 with the reference's constructor surface and state_dict layout
 (SimpleAICV/classification/backbones/van.py:20-35 DWConv, :38-56 Mlp, :59-93 LKA, :96-115 Attention,
 :118-151 DropPathBlock, :154-186 Block, :189-208 OverlapPatchEmbed, :211-310 VAN, :322-368 constructors),
-executed by engine.van.VANRT on sm_100a kernels.  The nn.Modules are parameter containers created in the
+executed by engine.van.VANRT on sm_90a kernels.  The nn.Modules are parameter containers created in the
 reference's order (identical seeded init and state_dict keys); ``forward`` hands the batch to the runtime.
 """
 import math
@@ -137,7 +137,7 @@ class VAN(nn.Module):
 
     def forward(self, x):
         if not x.is_cuda:
-            raise RuntimeError('this model runs on B200 kernels only; move the batch to the GPU (no CPU fallback exists)')
+            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
         return run_network(self._runtime(), x.float(), self.training)
 
 

@@ -1,7 +1,7 @@
 """ViT-B/L/H with the reference's constructor surface and state_dict layout
 (SimpleAICV/classification/backbones/vit.py:18-47 PatchEmbeddingBlock, :50-80 MultiHeadAttention,
 :83-99 FeedForward, :138-163 TransformerEncoderLayer, :166-262 ViT, :273-282 constructors),
-executed by engine.vit.ViTRT on hand-written sm_100a kernels.
+executed by engine.vit.ViTRT on hand-written sm_90a kernels.
 
 The nn.Modules are parameter containers built in the reference's order (identical seeded init and
 state_dict keys); ``forward`` hands the batch to the runtime.  CPU tensors raise.
@@ -117,7 +117,7 @@ class ViT(nn.Module):
 
     def forward(self, x):
         if not x.is_cuda:
-            raise RuntimeError('this model runs on B200 kernels only; move the batch to the GPU '
+            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU '
                                '(no CPU fallback exists)')
         return run_network(self._runtime(), x.float(), self.training)
 

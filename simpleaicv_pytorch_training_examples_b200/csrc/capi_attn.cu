@@ -1,10 +1,10 @@
-// Host side of the tcgen05 attention family (attn_sm100.cuh): tensor maps, template dispatch, launches.
+// Host side of the wgmma attention family (attn_sm90.cuh): tensor maps, template dispatch, launches.
 #include <cudaTypedefs.h>
 
 #include <mutex>
 
 #include "../../include/saicv_b200.h"
-#include "attn_sm100.cuh"
+#include "attn_sm90.cuh"
 #include "host_util.h"
 
 using namespace saicv;
@@ -15,7 +15,6 @@ PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
 int g_sms = 0;
 std::once_flag g_once;
 bool g_ok = false;
-__device__ int g_attn_error = 0;
 
 void init() {
   cudaDriverEntryPointQueryResult qres;
@@ -32,8 +31,8 @@ void init() {
     set_error("cudaGetDeviceProperties failed");
     return;
   }
-  if (prop.major != 10) {
-    set_error("libsaicv_b200 requires an sm_100 (B200) device, found sm_%d%d", prop.major, prop.minor);
+  if (prop.major != 9) {
+    set_error("libsaicv_b200 requires an sm_90 (H100) device, found sm_%d%d", prop.major, prop.minor);
     return;
   }
   g_sms = prop.multiProcessorCount;
@@ -67,18 +66,8 @@ bool encode_4d(CUtensorMap* m, const void* ptr, int D, int L, int H, int B, cons
   return true;
 }
 
-// persistent grid: MINB (1 or 2) CTAs per SM; the kernels are compiled with __launch_bounds__(192, MINB) and
-// their shared-memory / TMEM footprints were sized for exactly that residency (320 threads: 2 x 102 registers)
-int* error_flag_ptr() {   // resolved once (not during a later CUDA-graph capture)
-  static int* ptr = nullptr;
-  if (!ptr) {
-    void* f = nullptr;
-    cudaGetSymbolAddress(&f, g_attn_error);
-    ptr = reinterpret_cast<int*>(f);
-  }
-  return ptr;
-}
-
+// persistent grid: MINB (1 or 2) CTAs per SM; the kernels are compiled with __launch_bounds__(160, MINB) and
+// their shared-memory footprints are sized for exactly that residency
 template <typename K>
 int persistent_grid(K kernel, int minb, long long total) {
   static bool carve = false;
@@ -104,8 +93,8 @@ AttnDrop make_drop(const saicv_attn_args* a) {
 
 template <int DQK, int DV, int MINB, bool DROP>
 int launch_fwd(const saicv_attn_args* a, cudaStream_t st) {
-  using Cfg = AttnFwdCfg<DQK, DV, MINB>;
-  auto kernel = attn_fwd_sm100_kernel<DQK, DV, MINB, DROP>;
+  using Cfg = AttnFwdCfg<DQK, DV>;
+  auto kernel = attn_fwd_sm90_kernel<DQK, DV, MINB, DROP>;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
@@ -116,12 +105,12 @@ int launch_fwd(const saicv_attn_args* a, cudaStream_t st) {
     attr = true;
   }
   CUtensorMap tq, tk, tv;
-  if (!encode_4d(&tq, a->q, DQK, a->lq, a->h, a->b, a->q_strides, 128)) return 2;
-  if (!encode_4d(&tk, a->k, DQK, a->lk, a->h, a->b, a->k_strides, 128)) return 2;
-  if (!encode_4d(&tv, a->v, DV, a->lk, a->h, a->b, a->v_strides, 128)) return 2;
+  if (!encode_4d(&tq, a->q, DQK, a->lq, a->h, a->b, a->q_strides, kAttnRows)) return 2;
+  if (!encode_4d(&tk, a->k, DQK, a->lk, a->h, a->b, a->k_strides, kAttnCols)) return 2;
+  if (!encode_4d(&tv, a->v, DV, a->lk, a->h, a->b, a->v_strides, kAttnCols)) return 2;
   AttnParams p{};
   p.B = a->b; p.H = a->h; p.Lq = a->lq; p.Lk = a->lk;
-  p.num_q_tiles = (a->lq + 127) / 128;
+  p.num_q_tiles = (a->lq + kAttnRows - 1) / kAttnRows;
   p.scale = a->scale;
   p.scale_log2 = a->scale * 1.4426950408889634f;
   p.out = reinterpret_cast<__nv_bfloat16*>(a->out);
@@ -129,17 +118,16 @@ int launch_fwd(const saicv_attn_args* a, cudaStream_t st) {
   p.lse = a->lse;
   p.mask_bits = a->key_mask_bits; p.mask_words = a->mask_words;
   p.drop = make_drop(a);
-  p.error_flag = error_flag_ptr();
   const long long total = (long long)a->b * a->h * p.num_q_tiles;
   const int grid = persistent_grid(kernel, MINB, total);
   kernel<<<grid, kAttnThreads, Cfg::kSmemBytes, st>>>(tq, tk, tv, p);
-  return check_launch("attn_fwd_sm100_kernel");
+  return check_launch("attn_fwd_sm90_kernel");
 }
 
-template <int DQK, int DV, bool KEYS, int TCOLS, int MINB, bool DROP>
+template <int DQK, int DV, bool KEYS, int MINB, bool DROP>
 int launch_bwd_phase(const saicv_attn_bwd_args* a, cudaStream_t st) {
-  using Cfg = AttnBwdCfg<DQK, DV, KEYS, TCOLS, MINB>;
-  auto kernel = attn_bwd_sm100_kernel<DQK, DV, KEYS, TCOLS, MINB, DROP>;
+  using Cfg = AttnBwdCfg<DQK, DV, KEYS>;
+  auto kernel = attn_bwd_sm90_kernel<DQK, DV, KEYS, MINB, DROP>;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
@@ -152,19 +140,19 @@ int launch_bwd_phase(const saicv_attn_bwd_args* a, cudaStream_t st) {
   const saicv_attn_args* f = &a->fwd;
   CUtensorMap r0, r1, c0, c1;
   if (!KEYS) {
-    if (!encode_4d(&r0, f->q, DQK, f->lq, f->h, f->b, f->q_strides, 128)) return 2;
-    if (!encode_4d(&r1, a->dout, DV, f->lq, f->h, f->b, f->o_strides, 128)) return 2;
-    if (!encode_4d(&c0, f->k, DQK, f->lk, f->h, f->b, f->k_strides, 64)) return 2;
-    if (!encode_4d(&c1, f->v, DV, f->lk, f->h, f->b, f->v_strides, 64)) return 2;
+    if (!encode_4d(&r0, f->q, DQK, f->lq, f->h, f->b, f->q_strides, kAttnRows)) return 2;
+    if (!encode_4d(&r1, a->dout, DV, f->lq, f->h, f->b, f->o_strides, kAttnRows)) return 2;
+    if (!encode_4d(&c0, f->k, DQK, f->lk, f->h, f->b, f->k_strides, kAttnCols)) return 2;
+    if (!encode_4d(&c1, f->v, DV, f->lk, f->h, f->b, f->v_strides, kAttnCols)) return 2;
   } else {
-    if (!encode_4d(&r0, f->k, DQK, f->lk, f->h, f->b, f->k_strides, 128)) return 2;
-    if (!encode_4d(&r1, f->v, DV, f->lk, f->h, f->b, f->v_strides, 128)) return 2;
-    if (!encode_4d(&c0, f->q, DQK, f->lq, f->h, f->b, f->q_strides, 64)) return 2;
-    if (!encode_4d(&c1, a->dout, DV, f->lq, f->h, f->b, f->o_strides, 64)) return 2;
+    if (!encode_4d(&r0, f->k, DQK, f->lk, f->h, f->b, f->k_strides, kAttnRows)) return 2;
+    if (!encode_4d(&r1, f->v, DV, f->lk, f->h, f->b, f->v_strides, kAttnRows)) return 2;
+    if (!encode_4d(&c0, f->q, DQK, f->lq, f->h, f->b, f->q_strides, kAttnCols)) return 2;
+    if (!encode_4d(&c1, a->dout, DV, f->lq, f->h, f->b, f->o_strides, kAttnCols)) return 2;
   }
   AttnBwdParams p{};
   p.B = f->b; p.H = f->h; p.Lq = f->lq; p.Lk = f->lk;
-  p.num_tiles = ((KEYS ? f->lk : f->lq) + 127) / 128;
+  p.num_tiles = ((KEYS ? f->lk : f->lq) + kAttnRows - 1) / kAttnRows;
   p.scale = f->scale;
   p.scale_log2 = f->scale * 1.4426950408889634f;
   p.lse = f->lse; p.delta = a->delta;
@@ -180,16 +168,14 @@ int launch_bwd_phase(const saicv_attn_bwd_args* a, cudaStream_t st) {
     p.s1b = a->dv_strides[0]; p.s1h = a->dv_strides[1]; p.s1l = a->dv_strides[2];
   }
   p.dk_cols = a->dk_cols > 0 ? a->dk_cols : DQK;
-  p.error_flag = error_flag_ptr();
   const long long total = (long long)f->b * f->h * p.num_tiles;
   const int grid = persistent_grid(kernel, MINB, total);
   kernel<<<grid, kAttnThreads, Cfg::kSmemBytes, st>>>(r0, r1, c0, c1, p);
-  return check_launch("attn_bwd_sm100_kernel");
+  return check_launch("attn_bwd_sm90_kernel");
 }
 
 // delta[b][h][q] = sum_d dO * O.  Each thread reads 16-byte pieces (8 bf16) of both rows; a row of DV values is shared
 // by DV / 8 adjacent lanes (8 for hd 64, 10 for hd 80, 4 for hd 32) and folded with shuffles inside groups of 16 lanes.
-// (One warp per row with 4-byte loads took 108 us per ViT-B layer for 154 MB: 1.4 TB/s.)
 __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ d_o, float* __restrict__ delta,
                                   int B, int H, int L, int DV, long long sb, long long sh, long long sl) {
   const long long rows = (long long)B * H * L;
@@ -223,8 +209,8 @@ constexpr bool kDropoutShape = (DQK == 32 && DV == 32) || (DQK == 48 && DV == 32
 
 template <int DQK, int DV>
 int fwd_for(const saicv_attn_args* a, cudaStream_t st) {
-  // two CTAs per SM whenever the tiles of both fit (hd <= 64 without bias columns)
-  constexpr bool two = AttnFwdCfg<DQK, DV, 2>::kSmemBytes <= 115712;
+  // two CTAs per SM whenever the tiles of both fit
+  constexpr bool two = AttnFwdCfg<DQK, DV>::kSmemBytes <= 115712;
   if (a->dropout_p > 0.f) {
     // attention-probability dropout is compiled for the head sizes that train with it (DETR hd 32 with / without the
     // key-bias column, ViT hd 64); the other shapes keep the mask-free instruction stream only
@@ -235,20 +221,19 @@ int fwd_for(const saicv_attn_args* a, cudaStream_t st) {
 }
 template <int DQK, int DV>
 int bwd_for(const saicv_attn_bwd_args* a, cudaStream_t st) {
-  constexpr int colsA = 128 + ((DQK + 31) & ~31), colsB = 128 + ((DV + 31) & ~31) + ((DQK + 31) & ~31);
-  constexpr int tA = colsA <= 256 ? 256 : 512, tB = colsB <= 256 ? 256 : 512;
-  constexpr bool twoA = tA == 256 && AttnBwdCfg<DQK, DV, false, tA, 2>::kSmemBytes <= 115712;
-  constexpr bool twoB = tB == 256 && AttnBwdCfg<DQK, DV, true, tB, 2>::kSmemBytes <= 115712;
+  // two CTAs per SM (<= 204 registers a thread) while the accumulators stay small: S, dP (32 + 32) + dQ or dV + dK
+  constexpr bool twoA = 64 + DQK / 2 <= 128 && AttnBwdCfg<DQK, DV, false>::kSmemBytes <= 115712;
+  constexpr bool twoB = 64 + DV / 2 + DQK / 2 <= 128 && AttnBwdCfg<DQK, DV, true>::kSmemBytes <= 115712;
   if (a->fwd.dropout_p > 0.f) {
     if constexpr (kDropoutShape<DQK, DV>) {
-      if (int e = launch_bwd_phase<DQK, DV, false, tA, twoA ? 2 : 1, true>(a, st)) return e;
-      return launch_bwd_phase<DQK, DV, true, tB, twoB ? 2 : 1, true>(a, st);
+      if (int e = launch_bwd_phase<DQK, DV, false, twoA ? 2 : 1, true>(a, st)) return e;
+      return launch_bwd_phase<DQK, DV, true, twoB ? 2 : 1, true>(a, st);
     } else {
       return set_error("attention dropout is not compiled for (score width, value width) = (%d, %d)", DQK, DV);
     }
   }
-  if (int e = launch_bwd_phase<DQK, DV, false, tA, twoA ? 2 : 1, false>(a, st)) return e;
-  return launch_bwd_phase<DQK, DV, true, tB, twoB ? 2 : 1, false>(a, st);
+  if (int e = launch_bwd_phase<DQK, DV, false, twoA ? 2 : 1, false>(a, st)) return e;
+  return launch_bwd_phase<DQK, DV, true, twoB ? 2 : 1, false>(a, st);
 }
 
 #define SAICV_ATTN_SHAPES(X) X(32, 32) X(48, 32) X(64, 64) X(80, 80) X(96, 64) X(112, 64) X(112, 80) X(128, 80) X(192, 64) X(208, 80)
@@ -256,12 +241,6 @@ int bwd_for(const saicv_attn_bwd_args* a, cudaStream_t st) {
 }  // namespace
 
 extern "C" {
-
-int saicv_attn_error(void) {
-  int v = 0;
-  cudaMemcpyFromSymbol(&v, g_attn_error, sizeof(int));
-  return v;
-}
 
 int saicv_attn_fwd(const saicv_attn_args* a, void* stream) {
   if (!ensure()) return 1;
@@ -284,7 +263,7 @@ int saicv_attn_bwd(const saicv_attn_bwd_args* a, void* stream) {
     const long long rows = (long long)f->b * f->h * f->lq;
     if (f->dv % 8 || f->dv > 128) return set_error("saicv_attn_bwd: the value width must be a multiple of 8, <= 128 (got %d)", f->dv);
     long long blocks = (rows + 15) / 16;               // 16 rows per 256-thread block
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > (long long)g_sms * 16) blocks = (long long)g_sms * 16;
     attn_delta_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
         reinterpret_cast<const __nv_bfloat16*>(f->out), reinterpret_cast<const __nv_bfloat16*>(a->dout), a->delta, f->b, f->h,
         f->lq, f->dv, f->o_strides[0], f->o_strides[1], f->o_strides[2]);

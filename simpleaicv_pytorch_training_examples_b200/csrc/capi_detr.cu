@@ -273,7 +273,7 @@ __global__ void heads_unpack_kernel(const __nv_bfloat16* __restrict__ src, __nv_
   }
 }
 
-int grid_1d(long long items, int per_block = 256, int cap = 148 * 16) {
+int grid_1d(long long items, int per_block = 256, int cap = 132 * 16) {
   long long b = (items + per_block - 1) / per_block;
   if (b < 1) b = 1;
   if (b > cap) b = cap;
@@ -291,7 +291,7 @@ extern "C" {
 int saicv_postln_fwd(const float* z, const float* gamma, const float* beta, float eps, float* y, void* yb, const float* pos,
                      long long pos_rows, void* ypb, float* stats, long long rows, int c, void* stream) {
   if (ypb && (!pos || pos_rows <= 0)) return set_error("saicv_postln_fwd: ypb needs pos and pos_rows > 0");
-  const int grid = grid_1d(rows, 8, 148 * 8);
+  const int grid = grid_1d(rows, 8, 132 * 8);
   __nv_bfloat16* b0 = reinterpret_cast<__nv_bfloat16*>(yb);
   __nv_bfloat16* b1 = reinterpret_cast<__nv_bfloat16*>(ypb);
   switch (c) {
@@ -308,7 +308,7 @@ int saicv_postln_bwd(const float* dy, const float* z, const float* gamma, const 
                      void* dzb, float* partials, float* dgamma, float* dbeta, long long rows, int c, int accumulate,
                      void* stream) {
   if (!partials) return set_error("saicv_postln_bwd: needs a [SAICV_BN_PARTIAL_ROWS][2*c] fp32 workspace");
-  const int grid = grid_1d(rows, 8 * 8, 148 * 2);
+  const int grid = grid_1d(rows, 8 * 8, 132 * 2);
   __nv_bfloat16* b0 = reinterpret_cast<__nv_bfloat16*>(dzb);
   switch (c) {
     case 128: postln_bwd_kernel<1><<<grid, 256, 0, ST>>>(dy, z, gamma, stats, dres, dz, b0, partials, rows); break;

@@ -55,7 +55,7 @@ __device__ __forceinline__ float act_grad(float out, int act) {
   return act == 1 ? (out > 0.f ? 1.f : 0.f) : (act == 2 ? (out > 0.f ? 1.f : 0.1f) : 1.f);
 }
 
-int grid_for(long long work_items, int per_block = kThreads, int max_blocks = 148 * 16) {
+int grid_for(long long work_items, int per_block = kThreads, int max_blocks = 132 * 16) {
   long long b = (work_items + per_block - 1) / per_block;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
@@ -191,7 +191,7 @@ colreduce_kernel(const void* __restrict__ a, const void* __restrict__ b, const v
   }
 }
 
-// out[j] (+)= sum_b partial[b][j]: 8 columns x 32 row groups per block (the <= 296 partial rows are
+// out[j] (+)= sum_b partial[b][j]: 8 columns x 32 row groups per block (the <= 264 partial rows are
 // spread over 32 threads per column so the fold is a handful of loads deep)
 __global__ void fold_partials_kernel(const float* __restrict__ partial, float* __restrict__ out, int nblk, int ncols,
                                      int accumulate) {
@@ -213,7 +213,7 @@ __global__ void fold_partials_kernel(const float* __restrict__ partial, float* _
 
 constexpr int kMaxPartials = SAICV_BN_PARTIAL_ROWS;  // 2 blocks per SM
 
-bool slab_geom(long long rows, int C, int unroll, SlabGeom* g, int* blocks, int max_blocks = 148 * 8) {
+bool slab_geom(long long rows, int C, int unroll, SlabGeom* g, int* blocks, int max_blocks = 132 * 8) {
   const int min_rows_per_thread = unroll;
   if (C % 8 || C > 2048) {
     set_error("BatchNorm / column kernels need C %% 8 == 0 and C <= 2048 (C=%d)", C);
@@ -644,7 +644,7 @@ __global__ void add_strided2_kernel(void* __restrict__ dx, const void* __restric
 // with oob_zero, take part with the value 0 (nn.ZeroPad2d followed by an unpadded pool,
 // darknet.py:212-213): their code is 255 and they receive no gradient.  argmax byte = r*K + s.
 // KT > 0: the window size is a compile-time constant, so the K*K window loads are unrolled and all in flight at once
-// (the runtime-K loop issues them one by one: 3.5 TB/s of L1 traffic, 3x off the HBM time of the 3x3/2 stem pool)
+// (the runtime-K loop issues them one by one)
 template <int KT>
 __global__ void maxpool_fwd_kernel(const void* __restrict__ x, void* __restrict__ y, uint8_t* __restrict__ amax,
                                    int N, int H, int W, int C, int P, int Q, int Krt, int stride, int pad, int oob_zero) {

@@ -1,4 +1,4 @@
-// Host side of the tcgen05 GEMM / implicit-GEMM engine: tensor-map encoding and launches
+// Host side of the wgmma GEMM / implicit-GEMM engine: tensor-map encoding and launches
 // behind the C ABI declared in include/saicv_b200.h.
 #include <cudaTypedefs.h>
 
@@ -9,7 +9,7 @@
 #include <mutex>
 
 #include "../../include/saicv_b200.h"
-#include "gemm_sm100.cuh"
+#include "gemm_sm90.cuh"
 #include "host_util.h"
 
 using namespace saicv;
@@ -43,8 +43,8 @@ void init_driver() {
   if (cudaGetDevice(&dev) != cudaSuccess) { set_error("cudaGetDevice failed"); return; }
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) { set_error("cudaGetDeviceProperties failed"); return; }
-  if (prop.major != 10) {
-    set_error("libsaicv_b200 requires an sm_100 (B200) device, found sm_%d%d", prop.major, prop.minor);
+  if (prop.major != 9) {
+    set_error("libsaicv_b200 requires an sm_90 (H100) device, found sm_%d%d", prop.major, prop.minor);
     return;
   }
   g_sm_count = prop.multiProcessorCount;
@@ -129,19 +129,18 @@ void tune_override(int* bn, int* stages, int* nb) {
   if (!e || !*e) return;
   int a = 0, b = 0, c = 0;
   sscanf(e, "%d:%d:%d", &a, &b, &c);
-  if (bn && (a == 64 || a == 128 || a == 192 || a == 256)) *bn = a;
+  if (bn && (a == 64 || a == 128)) *bn = a;
   if (stages && b > 0) *stages = b;
   if (nb && c > 0) *nb = c;
 }
 
-// Split of the 227 KB between the operand ring (stages) and the epilogue staging slices (nb per half), from the sweep
-// of tests/profile_gemm_tune.py on a B200 (profiles/r02_gemm_epilogue_ncu.md):
+// Split of the 227 KB between the operand ring (stages) and the epilogue staging slices (nb per half)
+// (tests/profile_gemm_tune.py sweeps it):
 //  * no aux operand: two slices per half whenever >= 3 stages remain (>= 4 for reductions of 4+ k-blocks) - a TMA store
-//    is then never waited for right after it was issued (conv 1x1 c64->k256 56x56: 118 -> 96 us);
+//    is then not waited for right after it was issued;
 //  * aux operand by TMA: the slices are also the landing buffers of the next aux tiles, so depth matters more than ring
-//    stages while the reduction is short: <= 4 k-blocks -> 3 slices / 2+ stages (c256->k64 dgrad + shortcut: 257 -> 203 us),
-//    fp32 tiles (8 slices per 128 x 256 tile) of <= 16 k-blocks -> 2 slices / 3 stages (ViT proj + fp32 residual: 96 -> 92 us);
-//    everything longer keeps 4 stages first (ViT fc2 data gradient with dGELU: 328 us at 4 / 1, 346 us at 3 / 2).
+//    stages while the reduction is short: <= 4 k-blocks -> 3 slices / 2+ stages, fp32 tiles of <= 16 k-blocks -> 2 slices /
+//    3 stages; everything longer keeps 4 stages first.
 template <int BN>
 void pick_smem_split(const GemmParams& p, int stat_bytes, int* stages_out, int* nb_out) {
   using Cfg = GemmCfg<BN>;
@@ -167,7 +166,7 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, con
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_sm100_kernel<BN, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_sm90_kernel<BN, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
     if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(smem=%d): %s", Cfg::kSmemBytes, cudaGetErrorString(e));
     attr_set = true;
@@ -178,22 +177,23 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, con
   const int stat_bytes = (p.epi_flags & EPI_STATS) ? ((8 * p.N + 15) & ~15) : 0;
   int stages = 0, nb = 1;
   pick_smem_split<BN>(p, stat_bytes, &stages, &nb);
-  if (stages < 2) return set_error("gemm_sm100_kernel<%d>: %d bytes of statistics do not fit in shared memory", BN, stat_bytes);
+  if (stages < 2) return set_error("gemm_sm90_kernel<%d>: %d bytes of statistics do not fit in shared memory", BN, stat_bytes);
   const_cast<GemmParams&>(p).num_stages = stages;
   const_cast<GemmParams&>(p).store_bufs = nb;
-  gemm_sm100_kernel<BN, VAR><<<grid, GemmVariant<VAR>::kThreads, Cfg::kSmemBytes, st>>>(a, b, d, r, p);
+  gemm_sm90_kernel<BN, VAR><<<grid, GemmVariant<VAR>::kThreads, Cfg::kSmemBytes, st>>>(a, b, d, r, p);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("gemm_sm100_kernel<%d> launch: %s", BN, cudaGetErrorString(e));
+  if (e != cudaSuccess) return set_error("gemm_sm90_kernel<%d> launch: %s", BN, cudaGetErrorString(e));
   count_launch(1);
   return 0;
 }
 
-// Tile width with the least padded columns (ties -> wider tile).
+// Tile width with the least padded columns (ties -> wider tile).  128 is the widest: each of the two consumer
+// warpgroups keeps a 128 x 64 fp32 accumulator in registers next to its epilogue.
 int pick_bn(int N) {
-  const int cand[4] = {256, 192, 128, 64};
-  int best = 256;
+  const int cand[2] = {128, 64};
+  int best = 128;
   long long best_cost = -1;
-  for (int i = 0; i < 4; ++i) {
+  for (int i = 0; i < 2; ++i) {
     const long long cost = (long long)((N + cand[i] - 1) / cand[i]) * cand[i];
     if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = cand[i]; }
   }
@@ -205,7 +205,6 @@ int pick_bn(int N) {
 // pre-activation).  When its element width equals the output's it travels by TMA (GemmParams::aux_tma).
 int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, GemmParams& p,
              cudaStream_t st, const void* aux = nullptr, bool aux_f32 = false) {
-  p.idesc = make_idesc_bf16(128, bn, p.a_mode == A_MN2D ? 1 : 0, p.b_mode != B_K2D ? 1 : 0);
   CUtensorMap r = d;
   p.aux_tma = 0;
   const bool both = (p.epi_flags & EPI_RESID) && (p.epi_flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU));
@@ -214,7 +213,7 @@ int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorM
     if (!encode_out(&r, aux, aux_f32, p.N, p.M, p.ldd, 1, 0)) return 2;
     p.aux_tma = 1;
   }
-  // compile-time epilogue variant (gemm_sm100.cuh GemmVariant); SAICV_GEMM_FULL_VARIANT=1 forces the run-time one
+  // compile-time epilogue variant (gemm_sm90.cuh GemmVariant); SAICV_GEMM_FULL_VARIANT=1 forces the run-time one
   int var = VAR_FULL;
   if (!getenv("SAICV_GEMM_FULL_VARIANT")) {
     if (p.aux_tma && !(p.epi_flags & ~GemmVariant<VAR_AUX>::kMask)) var = VAR_AUX;
@@ -232,9 +231,7 @@ int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorM
   }
   switch (bn) {
     case 64: SAICV_LAUNCH_BN(64)
-    case 128: SAICV_LAUNCH_BN(128)
-    case 192: SAICV_LAUNCH_BN(192)
-    default: SAICV_LAUNCH_BN(256)
+    default: SAICV_LAUNCH_BN(128)
   }
 #undef SAICV_LAUNCH_BN
 }
@@ -249,7 +246,7 @@ int saicv_gemm_stats_rows(long long out_rows, int out_cols) {
   // number of partial rows a stats-fused forward GEMM writes = its grid size
   const int bn = pick_bn(out_cols);
   const long long tiles = ((out_rows + BM - 1) / BM) * ((out_cols + bn - 1) / bn);
-  const int sms = ensure_init() ? g_sm_count : 148;
+  const int sms = ensure_init() ? g_sm_count : 132;
   return (int)(tiles < sms ? tiles : sms);
 }
 
@@ -257,7 +254,7 @@ int saicv_wgrad_splits(int out_rows, int out_cols, long long reduce_len) {
   const int bn = pick_bn(out_cols);
   const long long tiles = (long long)((out_rows + BM - 1) / BM) * ((out_cols + bn - 1) / bn);
   const long long num_kb = (reduce_len + BK - 1) / BK;
-  const int sms = g_sm_count > 0 ? g_sm_count : 148;
+  const int sms = g_sm_count > 0 ? g_sm_count : 132;
   long long want = (2LL * sms + tiles - 1) / tiles;      // ~2 work items per SM
   long long max_by_k = num_kb / 8 > 0 ? num_kb / 8 : 1;  // at least 8 k-blocks per split
   long long s = want < max_by_k ? want : max_by_k;

@@ -74,11 +74,11 @@ extern "C" int saicv_u8_nhwc_to_nchw_norm(const void* in, float* out, int n, int
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (hw % 4 == 0 && ((uintptr_t)in & 3) == 0 && ((uintptr_t)out & 15) == 0) {
     const long long groups = pixels / 4;
-    const int blocks = (int)((groups + kInThreads - 1) / kInThreads < 148 * 16 ? (groups + kInThreads - 1) / kInThreads : 148 * 16);
+    const int blocks = (int)((groups + kInThreads - 1) / kInThreads < 132 * 16 ? (groups + kInThreads - 1) / kInThreads : 132 * 16);
     u8_nhwc_to_nchw_norm_vec_kernel<<<blocks, kInThreads, 0, st>>>(reinterpret_cast<const uint32_t*>(in), out, groups, (int)(hw / 4), nm);
     return check_launch("u8_nhwc_to_nchw_norm_vec_kernel");
   }
-  const int blocks = (int)((pixels + kInThreads - 1) / kInThreads < 148 * 16 ? (pixels + kInThreads - 1) / kInThreads : 148 * 16);
+  const int blocks = (int)((pixels + kInThreads - 1) / kInThreads < 132 * 16 ? (pixels + kInThreads - 1) / kInThreads : 132 * 16);
   u8_nhwc_to_nchw_norm_kernel<<<blocks, kInThreads, 0, st>>>(reinterpret_cast<const uint8_t*>(in), out, pixels, hw, nm);
   return check_launch("u8_nhwc_to_nchw_norm_kernel");
 }

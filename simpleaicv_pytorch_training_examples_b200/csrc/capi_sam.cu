@@ -1,7 +1,7 @@
 // SAM image-encoder specific kernels (SimpleAICV/interactive_segmentation/models/segment_anything/image_encoder.py):
 //   window partition / unpartition with zero padding (:32-79),
 //   decomposed relative-position bias (:82-144): the bias rel_h[q, kh] + rel_w[q, kw] is turned into extra score
-//   columns so that the tcgen05 attention kernel adds it on the tensor cores:
+//   columns so that the wgmma attention kernel adds it on the tensor cores:
 //       Qe[l] = [ q[l] * scale | rel_h[l, 0..Sh) | rel_w[l, 0..Sw) | 0 ]      rel_h[l, kh] = q[l] . Rh[qh(l) - kh + Sh - 1]
 //       Ke[l] = [ k[l]         | onehot(kh(l))   | onehot(kw(l))   | 0 ]
 //       Qe . Ke^T = scale * q.k + rel_h[q, kh(k)] + rel_w[q, kw(k)]            (= image_encoder.py:171-174)
@@ -18,7 +18,7 @@ namespace saicv {
 namespace {
 
 
-int grid1d(long long items, int per_block = 256, int cap = 148 * 16) {
+int grid1d(long long items, int per_block = 256, int cap = 132 * 16) {
   long long b = (items + per_block - 1) / per_block;
   if (b < 1) b = 1;
   if (b > cap) b = cap;

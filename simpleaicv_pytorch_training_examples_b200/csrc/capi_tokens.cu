@@ -89,7 +89,7 @@ token_fill_grad_kernel(const float* __restrict__ dout, const int* __restrict__ i
 
 int blocks_for(long long items) {
   long long b = (items + kTokThreads - 1) / kTokThreads;
-  return (int)(b < 1 ? 1 : b > 148 * 16 ? 148 * 16 : b);
+  return (int)(b < 1 ? 1 : b > 132 * 16 ? 132 * 16 : b);
 }
 
 }  // namespace

@@ -427,7 +427,7 @@ __global__ void col2im_nhwc_kernel(const __nv_bfloat16* __restrict__ dcols, __nv
   }
 }
 
-int grid1d(long long items, int per_block = 256, int cap = 148 * 16) {
+int grid1d(long long items, int per_block = 256, int cap = 132 * 16) {
   long long b = (items + per_block - 1) / per_block;
   if (b < 1) b = 1;
   if (b > cap) b = cap;
@@ -438,7 +438,7 @@ int pow2_ge(int v) {
   while (p < v) p <<= 1;
   return p;
 }
-// slab geometry of the column reductions: tx_count threads across 8-column vectors, rows split over <= 296 blocks
+// slab geometry of the column reductions: tx_count threads across 8-column vectors, rows split over <= 264 blocks
 void slab(long long rows, int C, int* tx_count, long long* rows_per_block, int* nblk) {
   const int vpr = C / 8;
   int tx = pow2_ge(vpr);
@@ -466,7 +466,7 @@ int saicv_dwconv_fwd(const void* x, const float* w, const float* bias, void* y, 
                      int relu, int flip, void* stream) {
   if (c % 8) return set_error("saicv_dwconv_fwd: C %% 8 != 0");
   const long long npix = (long long)n * h * wd;
-  dim3 grid((unsigned)grid1d(npix, 32, 148 * 8), (unsigned)((c + 63) / 64));
+  dim3 grid((unsigned)grid1d(npix, 32, 132 * 8), (unsigned)((c + 63) / 64));
   const __nv_bfloat16* xx = reinterpret_cast<const __nv_bfloat16*>(x);
   __nv_bfloat16* yy = reinterpret_cast<__nv_bfloat16*>(y);
   switch (k) {
@@ -480,7 +480,7 @@ int saicv_dwconv_fwd(const void* x, const float* w, const float* bias, void* y, 
 
 int saicv_dwconv_wgrad_blocks(long long npix) {
   long long b = (npix + 255) / 256;
-  if (b > 148) b = 148;
+  if (b > 132) b = 132;
   return (int)(b < 1 ? 1 : b);
 }
 

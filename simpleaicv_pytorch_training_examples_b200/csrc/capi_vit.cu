@@ -1,6 +1,6 @@
 // ViT-specific kernels of the hot path (SimpleAICV/classification/backbones/vit.py): LayerNorm
 // forward/backward with the residual-stream add fused, exact-erf GELU, token assembly
-// (cls + positional embedding) and token pooling.  The fused attention lives in attn_sm100.cuh / capi_attn.cu.
+// (cls + positional embedding) and token pooling.  The fused attention lives in attn_sm90.cuh / capi_attn.cu.
 //
 // Numerics follow the reference under autocast (SURVEY.md Appendix C): the residual stream, LayerNorm
 // statistics and softmax are fp32; GEMM / attention operands are bf16 with fp32 accumulation.
@@ -141,8 +141,8 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restrict__ x,
   }
 }
 
-// dgamma / dbeta (+)= sum over the per-block partial rows, fixed order: 8 columns x 32 row groups per block (the <= 296
-// partial rows are spread over 32 threads per column so the fold is a handful of loads deep instead of a 296-long chain)
+// dgamma / dbeta (+)= sum over the per-block partial rows, fixed order: 8 columns x 32 row groups per block (the <= 264
+// partial rows are spread over 32 threads per column so the fold is a handful of loads deep instead of a 264-long chain)
 __global__ void ln_fold_kernel(const float* __restrict__ partials, float* __restrict__ dgamma, float* __restrict__ dbeta,
                                int nblk, int C, int accumulate) {
   __shared__ float sm[32][9];
@@ -260,7 +260,7 @@ __global__ void token_pool_bwd_kernel(const float* __restrict__ dpooled, float* 
   }
 }
 
-int grid_1d(long long items, int per_block = 256, int cap = 148 * 16) {
+int grid_1d(long long items, int per_block = 256, int cap = 132 * 16) {
   long long b = (items + per_block - 1) / per_block;
   if (b < 1) b = 1;
   if (b > cap) b = cap;
@@ -277,7 +277,7 @@ extern "C" {
 
 int saicv_layernorm_fwd(const float* x, const float* gamma, const float* beta, void* y, float* stats,
                         long long rows, int c, float eps, void* stream) {
-  const int grid = grid_1d(rows, 8, 148 * 8);
+  const int grid = grid_1d(rows, 8, 132 * 8);
   __nv_bfloat16* yy = reinterpret_cast<__nv_bfloat16*>(y);
   switch (c) {
     case 768: ln_fwd_kernel<6><<<grid, 256, 0, ST>>>(x, gamma, beta, yy, stats, rows, eps); break;
@@ -297,7 +297,7 @@ int saicv_layernorm_bwd(const void* dy, const float* x, const float* gamma, cons
                         float* dgamma, float* dbeta, long long rows, int c, int accumulate, void* stream) {
   if (bf16_row_scale && rows_per_scale <= 0) return set_error("saicv_layernorm_bwd: rows_per_scale must be > 0");
   if (!partials) return set_error("saicv_layernorm_bwd: needs a [SAICV_BN_PARTIAL_ROWS][2*c] fp32 workspace");
-  const int grid = grid_1d(rows, 8 * 8, 148 * 2);
+  const int grid = grid_1d(rows, 8 * 8, 132 * 2);
   const __nv_bfloat16* d = reinterpret_cast<const __nv_bfloat16*>(dy);
   __nv_bfloat16* xb = reinterpret_cast<__nv_bfloat16*>(dx_bf16);
   switch (c) {

@@ -1,5 +1,5 @@
 // Counter-hash dropout shared by the elementwise dropout kernel (capi_detr.cu) and the attention kernels
-// (attn_sm100.cuh): the keep decision of element (a, b) under a 64-bit seed is a pure function, so the backward
+// (attn_sm90.cuh): the keep decision of element (a, b) under a 64-bit seed is a pure function, so the backward
 // pass recomputes the forward's mask instead of storing it.  keep <=> hash >= round(p * 2^32).
 // tests/test_detr_gpu.py restates the same integer arithmetic in torch to inject identical masks into the oracle.
 #pragma once

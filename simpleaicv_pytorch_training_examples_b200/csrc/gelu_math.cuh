@@ -1,4 +1,4 @@
-// Exact-erf GELU terms shared by the GEMM epilogues (gemm_sm100.cuh) and the streaming kernels (capi_vit.cu).
+// Exact-erf GELU terms shared by the GEMM epilogues (gemm_sm90.cuh) and the streaming kernels (capi_vit.cu).
 //
 //   Phi(x) = 0.5 (1 + erf(x / sqrt 2)),  phi(x) = exp(-x^2 / 2) / sqrt(2 pi);  gelu = x Phi,  gelu' = Phi + x phi
 //

@@ -1,7 +1,6 @@
 // Eight bf16 values as ONE 16-byte vector.  The storage is a uint4 so that every global access is a single
 // LDG.128 / STG.128: a struct of four __nv_bfloat162 members is split by the compiler into four 32-bit accesses,
-// which quadruples the L1 wavefronts of the streaming kernels (measured on the BatchNorm slab kernels: 3.7 TB/s
-// with the split accesses against > 6 TB/s of HBM traffic with the vector ones).
+// which quadruples the L1 wavefronts of the streaming kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cstdint>

@@ -1,7 +1,7 @@
 """DETR with the reference's constructor surface and state_dict layout (SimpleAICV/detection/models/detr.py:44-90
 TransformerEncoderLayer, :93-180 TransformerDecoderLayer, :183-270 DETRTransformer, :273-364 DETR, :367-399
-constructors), executed by engine.detr.DetrRT on sm_100a kernels: ResNet body on the conv/BN engine, every Linear on
-the tcgen05 GEMM engine, attention (head size 32, additive key bias in an extra score column) on the tcgen05 attention
+constructors), executed by engine.detr.DetrRT on sm_90a kernels: ResNet body on the conv/BN engine, every Linear on
+the wgmma GEMM engine, attention (head size 32, additive key bias in an extra score column) on the wgmma attention
 kernels, post-LayerNorm / dropout / head packing in csrc/capi_detr.cu.
 
 The nn.Modules are parameter containers created in the reference's order (identical seeded initialisation and
@@ -25,7 +25,7 @@ class ActivationBlock(nn.Module):
 
     def __init__(self, act_type='relu'):
         super().__init__()
-        assert act_type == 'relu', 'the B200 runtime implements the ReLU feed-forward DETR builds'
+        assert act_type == 'relu', 'the H100 runtime implements the ReLU feed-forward DETR builds'
         self.act = nn.ReLU(inplace=True)
 
 
@@ -109,7 +109,7 @@ class DETR(nn.Module):
         reg_outputs [6, B, Q, 4]] like the reference (detr.py:309-364)."""
         assert masks is not None
         if not inputs.is_cuda:
-            raise RuntimeError('this model runs on B200 kernels only; move the batch to the GPU (no CPU fallback exists)')
+            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
         fh, fw = _feature_size(inputs.shape[2]), _feature_size(inputs.shape[3])
         fm = F.interpolate(masks.float().unsqueeze(1), size=[fh, fw]).to(torch.bool).squeeze(1)
         pos = self.position_embedding(fm).flatten(2).transpose(1, 2).reshape(-1, self.hidden_inplanes).contiguous()

@@ -7,7 +7,7 @@ class DETRClsRegHead(nn.Module):
 
     def __init__(self, hidden_inplanes, num_classes, num_layers=3):
         super().__init__()
-        assert num_layers == 3, 'the B200 runtime implements the 3-layer box head DETR builds'
+        assert num_layers == 3, 'the H100 runtime implements the 3-layer box head DETR builds'
         self.cls_head = nn.Linear(hidden_inplanes, num_classes)
         reg_layers = []
         for _ in range(num_layers - 1):

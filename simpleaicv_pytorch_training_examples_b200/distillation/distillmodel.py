@@ -1,6 +1,6 @@
 """Knowledge-distillation wrapper (SURVEY.md 8 f4) with the reference's constructor surface
 (SimpleAICV/distillation/distillmodel.py:19-60): teacher and student are backbones of THIS package (so both forwards,
-and the student's backward, run on the B200 runtime), the teacher is frozen and evaluated without a tape.
+and the student's backward, run on the H100 runtime), the teacher is frozen and evaluated without a tape.
 ``forward(x)`` returns ``(tea_out, stu_out)``."""
 import torch
 import torch.nn as nn

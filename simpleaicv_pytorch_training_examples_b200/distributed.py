@@ -1,4 +1,4 @@
-"""Data-parallel wrapper replacing torch DDP for models executed by the B200 runtime
+"""Data-parallel wrapper replacing torch DDP for models executed by the H100 runtime
 (reference: tools/utils.py:175-202 build_training_mode wraps the model in
 nn.parallel.DistributedDataParallel; tools/scripts.py:168-181 uses ``model.no_sync()``).
 

@@ -1,9 +1,9 @@
 """Forward/backward runtime of the ConvBnAct residual networks (ResNet, ResNetCifar).
 
 The nn.Module shells in ``classification/backbones`` keep the reference's parameters, names and
-constructors; this runtime executes their math on the B200 kernels of libsaicv_b200.so:
+constructors; this runtime executes their math on the H100 kernels of libsaicv_b200.so:
 
-  conv     tcgen05 implicit GEMM (TMA im2col -> smem -> UMMA -> TMEM)      csrc/gemm_sm100.cuh
+  conv     wgmma implicit GEMM (TMA im2col -> smem -> wgmma -> registers)      csrc/gemm_sm90.cuh
   BN       batch statistics / finalize / apply(+residual)(+ReLU), backward csrc/capi_elementwise.cu
   pooling  max 3x3/2, global average                                       csrc/capi_elementwise.cu
 
@@ -317,7 +317,7 @@ class ResidualBlockRT:
             if isinstance(shortcut, tuple):
                 strided, shortcut = shortcut[1], None
         # The shortcut gradient joins the main path inside the data-gradient GEMM of the block's FIRST conv: its tile is
-        # the aux operand of that launch's epilogue (TMA-loaded into the staging slice, gemm_sm100.cuh aux_tma), which
+        # the aux operand of that launch's epilogue (TMA-loaded into the staging slice, gemm_sm90.cuh aux_tma), which
         # replaces a separate read-read-write pass over the block input (add_bf16: 13 launches, 1.06 ms per ResNet-50 step).
         first_unit = self.units[0]
         fuse = shortcut is not None and not (first_unit.stride == 2 and first_unit.r == 1)   # that case returns a compact gradient

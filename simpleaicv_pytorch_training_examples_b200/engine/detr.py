@@ -9,7 +9,7 @@ Data flow (tokens batch-major, M = B*L image tokens, Mq = B*Q query tokens, C = 
   * every layer is post-LN: z = stream + branch is produced by the branch's last GEMM (fp32 residual fused in the
     epilogue), then ONE saicv_postln_fwd pass writes the new fp32 stream and the bf16 operand copies the next GEMMs need
     (y and y + positional embedding);
-  * attention runs on the tcgen05 attention kernels with head size 32.  The reference passes a FLOAT key_padding_mask
+  * attention runs on the wgmma attention kernels with head size 32.  The reference passes a FLOAT key_padding_mask
     (detr.py:333-346), which nn.MultiheadAttention adds to the logits; that bias rides in one extra column of the score
     operands (q operand: constant 1, k operand: the bias), so the kernel is the same one SAM's rel-pos bias uses;
   * gradients of a stream tensor that feeds several GEMMs are summed by chaining the fp32 `resid` operand of the

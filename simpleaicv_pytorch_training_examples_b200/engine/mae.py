@@ -1,7 +1,7 @@
 """Forward/backward runtime of the MAE pre-training model (SURVEY.md 8 f4;
 SimpleAICV/masked_image_modeling/models/vit_mae.py) on libsaicv_b200.so.
 
-    patches  = patch_embed(images) + pos[1:]                                  (stem im2col + tcgen05 GEMM)
+    patches  = patch_embed(images) + pos[1:]                                  (stem im2col + wgmma GEMM)
     keep     = argsort(noise)[:, :L (1 - mask_ratio)]                         (index work: torch.argsort on the device)
     x        = [cls + pos[0] ; patches[keep] + pos[1 + keep]]                 (saicv_token_gather_fwd)
     x        = encoder blocks (engine.vit._Block, L = 1 + kept tokens), LayerNorm, encoder_to_decoder Linear

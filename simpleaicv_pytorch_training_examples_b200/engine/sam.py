@@ -5,8 +5,8 @@ Tokens are an fp32 residual stream [B*H*W, C] (patch embedding bf16 + fp32 pos_e
 reference under autocast).  Per Block (image_encoder.py:201-239):
     y   = LN1(x)                                   bf16
     [window partition with zero padding]           csrc/capi_sam.cu            (:32-55)
-    qkv = Linear(y)                                tcgen05 GEMM
-    att = softmax(q k^T scale + rel_h + rel_w) v   tcgen05 attention; the decomposed rel-pos bias (:82-144) rides in
+    qkv = Linear(y)                                wgmma GEMM
+    att = softmax(q k^T scale + rel_h + rel_w) v   wgmma attention; the decomposed rel-pos bias (:82-144) rides in
                                                    extra score columns built by ops.relpos_build (one GEMM + gather)
     [window unpartition]                                                       (:58-79)
     x   = x + proj(att);  x = x + lin2(gelu(lin1(LN2(x))))                     GEMM epilogues fuse bias/residual/dGELU

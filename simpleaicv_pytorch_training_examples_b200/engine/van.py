@@ -3,7 +3,7 @@ libsaicv_b200.so.
 
 Per Block (van.py:154-186), residual stream x fp32 [rows, C] (rows = N*H*W, NHWC):
     a  = BN1(x)                         bf16     csrc/capi_van.cu  (BatchNorm over the fp32 stream)
-    p1 = relu(proj_1(a))                         tcgen05 GEMM, bias + ReLU in the epilogue   (van.py:101,106-108)
+    p1 = relu(proj_1(a))                         wgmma GEMM, bias + ReLU in the epilogue   (van.py:101,106-108)
     c1 = conv1(dw7x7d3(dw5x5(p1)))               depthwise kernels + GEMM                    (van.py:63-90)
     y  = proj_2(p1 * c1) + a                     gate multiply, GEMM                         (van.py:91,109-110)
     x  = x + drop_path(ls1 * y)                  layer-scale residual kernel                 (van.py:183)
@@ -88,7 +88,7 @@ class _Block:
         self.fc1, self.fc2, self.dw = _Linear(mlp.fc1), _Linear(mlp.fc2), _DW(mlp.dwconv.dwconv)
         self.drop_path = getattr(blk.drop_path, 'drop_path_prob', 0.)
         if getattr(mlp.drop, 'p', 0.) > 0.:
-            raise NotImplementedError('VAN dropout_prob > 0 is not implemented by the B200 runtime (0 in every shipped config)')
+            raise NotImplementedError('VAN dropout_prob > 0 is not implemented by the H100 runtime (0 in every shipped config)')
 
     def linears(self):
         return [self.proj1, self.proj2, self.conv1, self.fc1, self.fc2]

@@ -3,7 +3,7 @@
 Per block (SimpleAICV/classification/backbones/vit.py:159-161, pre-LN):
     x = x + drop_path(proj(attention(qkv(LN1(x)))))        x: fp32 residual stream [B*L, C]
     x = x + drop_path(fc2(gelu(fc1(LN2(x)))))
-Every Linear is one launch of the tcgen05 GEMM engine (csrc/gemm_sm100.cuh): forward with the
+Every Linear is one launch of the wgmma GEMM engine (csrc/gemm_sm90.cuh): forward with the
 bias (+ fp32 residual) fused in the epilogue, data gradient with W consumed MN-major, weight
 gradient with both operands MN-major and split-K.  LayerNorm, GELU, token assembly / pooling and
 the fused attention are in csrc/capi_vit.cu.  dtype flow = the reference under autocast

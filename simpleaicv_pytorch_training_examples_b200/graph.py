@@ -1,6 +1,6 @@
 """One CUDA graph per training step.
 
-A step of the B200 runtime is several hundred small-to-medium kernel launches issued from Python through the C ABI
+A step of the H100 runtime is several hundred small-to-medium kernel launches issued from Python through the C ABI
 (ResNet-50: ~600, ViT-B: ~450).  When the host has to wait for every step's loss (tools/scripts.py reads it each
 iteration, like the reference does), the launch work of step i+1 cannot be hidden behind step i and the GPU idles
 for several milliseconds per step.  ``GraphedTrainStep`` captures forward + criterion + backward + optimizer step

@@ -21,7 +21,7 @@ class _MaskTerms(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, targets, alpha, gamma, thr):
         if not logits.is_cuda:
-            raise RuntimeError('SAMLoss runs on B200 kernels only; move the predictions to the GPU (no CPU fallback exists)')
+            raise RuntimeError('SAMLoss runs on H100 kernels only; move the predictions to the GPU (no CPU fallback exists)')
         logits = logits.contiguous()
         if logits.dtype not in (torch.float32, torch.bfloat16):
             logits = logits.float()

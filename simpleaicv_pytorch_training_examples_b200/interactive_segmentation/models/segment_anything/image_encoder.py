@@ -1,7 +1,7 @@
 """SAM ViT image encoder with the reference's constructor surface and state_dict layout
 (SimpleAICV/interactive_segmentation/models/segment_anything/image_encoder.py:8-29 PatchEmbed, :147-184 Attention,
 :187-198 MLPBlock, :201-239 Block, :242-256 LayerNorm2d, :259-331 ViTImageEncoder), executed by
-engine.sam.SamEncoderRT on sm_100a kernels (tcgen05 GEMMs and attention with the decomposed rel-pos bias in the
+engine.sam.SamEncoderRT on sm_90a kernels (wgmma GEMMs and attention with the decomposed rel-pos bias in the
 score GEMM).  The nn.Modules are parameter containers created in the reference's order."""
 import torch
 import torch.nn as nn
@@ -93,5 +93,5 @@ class ViTImageEncoder(nn.Module):
     def forward(self, x):
         """x: fp32 [B, 3, S, S] -> fp32 [B, out_planes, S/patch, S/patch]"""
         if not x.is_cuda:
-            raise RuntimeError('this model runs on B200 kernels only; move the batch to the GPU (no CPU fallback exists)')
+            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
         return run_network(self._runtime(), x.float(), self.training)

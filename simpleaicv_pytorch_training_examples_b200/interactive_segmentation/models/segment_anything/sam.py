@@ -1,6 +1,6 @@
 """``sam_b / sam_l / sam_h`` with the reference's signatures (segment_anything/sam.py:180-210).
 
-The image encoder (BASELINE.json config #4, SURVEY.md 8 a5) runs on the B200 runtime and keeps the reference's
+The image encoder (BASELINE.json config #4, SURVEY.md 8 a5) runs on the H100 runtime and keeps the reference's
 ``image_encoder.*`` state_dict keys.  The prompt encoder and the mask decoder are SURVEY.md 8(f1) ("next") rows:
 they are not built yet, so ``forward`` / ``forward_prompt_encoder_mask_decoder`` raise NotImplementedError instead
 of silently falling back to anything; ``forward_image_encoder`` is the hot path of the encoder-distillation and
@@ -37,7 +37,7 @@ class SAM(nn.Module):
 
     def forward_prompt_encoder_mask_decoder(self, *args, **kwargs):
         raise NotImplementedError('SAM prompt encoder / mask decoder are not built yet (SURVEY.md 8 f1); only the image encoder '
-                                  'runs on the B200 runtime')
+                                  'runs on the H100 runtime')
 
     def forward(self, *args, **kwargs):
         raise NotImplementedError('SAM.forward needs the prompt encoder / mask decoder (SURVEY.md 8 f1); use forward_image_encoder')

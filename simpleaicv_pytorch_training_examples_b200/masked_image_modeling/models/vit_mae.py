@@ -106,7 +106,7 @@ class VITMAEPretrainModel(nn.Module):
         self.encoder_to_decoder = nn.Linear(encoder_embedding_planes, decoder_embedding_planes)
         _xavier_linears(self.encoder_to_decoder)
         if encoder_dropout_prob > 0. or decoder_dropout_prob > 0.:
-            raise NotImplementedError('MAE on the B200 runtime: dropout_prob > 0 is not wired (the shipped MAE configs use 0)')
+            raise NotImplementedError('MAE on the H100 runtime: dropout_prob > 0 is not wired (the shipped MAE configs use 0)')
 
     def _runtime(self):
         rt = self.__dict__.get('_rt')
@@ -123,7 +123,7 @@ class VITMAEPretrainModel(nn.Module):
         """x: fp32 [B, 3, H, W] on the GPU.  noise: optional [B, L] uniform draws that decide the masking (the reference
         draws them with torch.rand inside random_masking, vit_mae.py:203-225; tests pass them in to pin the masks)."""
         if not x.is_cuda:
-            raise RuntimeError('this model runs on B200 kernels only; move the batch to the GPU (no CPU fallback exists)')
+            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
         from ...engine.mae import run_mae
         return run_mae(self._runtime(), x.float(), self.training, noise)
 

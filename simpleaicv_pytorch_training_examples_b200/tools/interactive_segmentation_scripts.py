@@ -1,6 +1,6 @@
 """Step bodies of the interactive-segmentation training loops that only need the SAM image encoder
 (tools/interactive_segmentation_scripts.py:21-199 train_distill_sam_encoder).  train_sam_segmentation (:274-564) needs
-the prompt encoder / mask decoder and SAMLoss, which are not on the B200 path yet (SURVEY.md 8 f1)."""
+the prompt encoder / mask decoder and SAMLoss, which are not on the H100 path yet (SURVEY.md 8 f1)."""
 from ..classification.common import AverageMeter  # noqa: F401  (re-exported like the reference module)
 from .scripts import train_epoch_with_loss_terms
 from .utils import unwrap
@@ -24,4 +24,4 @@ def train_distill_sam_encoder(train_loader, model, criterion, optimizer, schedul
 
 def train_sam_segmentation(*args, **kwargs):
     raise NotImplementedError('train_sam_segmentation needs the SAM prompt encoder / mask decoder and SAMLoss, which are not '
-                              'built on the B200 path yet (SURVEY.md 8 f1)')
+                              'built on the H100 path yet (SURVEY.md 8 f1)')

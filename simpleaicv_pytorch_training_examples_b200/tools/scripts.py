@@ -2,8 +2,8 @@
 tools/scripts.py:36-113 (test_classification), :116-275 (train_classification) and :1774-1934 (train_mae_self_supervised_learning).
 
 Arithmetic per step is the reference's: forward, criterion, backward (gradient average across
-ranks), optional clipping, optimizer step, per-iteration LR.  Control flow is tightened for a
-B200: the NaN/Inf guards are evaluated on the device and travel, together with the loss, in ONE
+ranks), optional clipping, optimizer step, per-iteration LR.  Control flow is tightened for the
+GPU: the NaN/Inf guards are evaluated on the device and travel, together with the loss, in ONE
 small all-reduce and ONE device->host read per step; there is no per-step barrier.
 """
 import torch

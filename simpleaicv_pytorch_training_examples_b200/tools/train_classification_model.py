@@ -21,13 +21,13 @@ from .utils import (Scheduler, build_optimizer, build_training_mode, checkpoint_
 
 
 def parse_args():
-    parser = argparse.ArgumentParser(description='B200 classification training')
+    parser = argparse.ArgumentParser(description='H100 classification training')
     parser.add_argument('--work-dir', type=str, required=True, help='directory holding train_config.py')
     return parser.parse_args()
 
 
 def main():
-    assert torch.cuda.is_available(), 'need at least one B200 to train'
+    assert torch.cuda.is_available(), 'need at least one H100 to train'
     args = parse_args()
     sys.path.append(args.work_dir)
     from train_config import config

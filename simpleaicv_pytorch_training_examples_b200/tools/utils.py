@@ -1,4 +1,4 @@
-"""Host-side helpers with the semantics of the reference's tools/utils.py, for the B200 path.
+"""Host-side helpers with the semantics of the reference's tools/utils.py, for the H100 path.
 
   get_logger            tools/utils.py:66-92   (rank-0 file + stderr logging)
   set_seed              tools/utils.py:95-107
@@ -38,7 +38,7 @@ def get_logger(name, log_dir):
 
 def set_seed(seed):
     """Seeds python / numpy / torch (CPU + CUDA) like the reference.  The reference also forces
-    deterministic cuDNN; the B200 path does not use cuDNN, so there is nothing to pin there."""
+    deterministic cuDNN; the H100 path does not use cuDNN, so there is nothing to pin there."""
     random.seed(seed)
     np.random.seed(seed)
     os.environ['PYTHONHASHSEED'] = str(seed)
@@ -208,10 +208,8 @@ class CudaPrefetcher:
         """normalize=(mean, std): batches whose 'image' is a uint8 [B, H, W, 3] tensor (classification.common.
         Uint8ClassificationCollater) are copied as uint8 - a quarter of the bytes - and turned into the fp32 NCHW
         normalised batch on the device, on the copy stream (SURVEY.md 8 f3; csrc/capi_input.cu).
-        copy_streams > 1: tensors of 32 MB and more are copied in that many chunks on separate streams.  Measured on the
-        B200 boxes of this pool (tests/profile_h2d.py, profiles/r02_h2d_prefetch.md): a single copy stream moves the 154 MB
-        ResNet-50 batch at 34 GB/s on an idle GPU but at ~6 GB/s while kernels are running (25 ms, longer than the 27 ms
-        step hides), two or more streams keep 45 - 55 GB/s under load; end to end 7.3 k -> 9.4 k img/s with four."""
+        copy_streams > 1: tensors of 32 MB and more are copied in that many chunks on separate streams, so that the copy of
+        the next batch keeps its bandwidth while the current step's kernels run (tests/profile_h2d.py measures it)."""
         self.loader = loader
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else device
         self.stream = torch.cuda.Stream(self.device)
@@ -310,7 +308,7 @@ def build_training_mode(config, model):
     accumulation / statistics, which needs no loss scaling."""
     from ..distributed import B200DataParallel
     if getattr(config, 'sync_bn', False):
-        raise NotImplementedError('sync_bn is not implemented by the B200 runtime (off in every hot-path config)')
+        raise NotImplementedError('sync_bn is not implemented by the H100 runtime (off in every hot-path config)')
     ema_model = None
     if getattr(config, 'use_ema_model', False):
         ema_model = EmaModel(model, decay=config.ema_model_decay)

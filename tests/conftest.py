@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a B200 (run through gpurun)')
+    config.addinivalue_line('markers', 'gpu: needs an H100')
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,8 +1,8 @@
 """Context number (NOT a bench.py arm): the reference's GPU path on this box, i.e. its model code
 (restated by oracle/convnets.py, the same torch ops) executed by stock PyTorch CUDA kernels under
 autocast(bf16) + autograd + torch.optim.SGD, with the per-step host syncs of
-tools/scripts.py:141-270 (isinf/isnan checks, loss == 0 test, .item()).  This is the
-"torch-DDP on the same box" number BASELINE.md 2b asks for at N = 1.
+tools/scripts.py:141-270 (isinf/isnan checks, loss == 0 test, .item()): the reference's
+own single-GPU throughput on the same box.
 
     python tests/perf_torch_gpu_baseline.py [--batch 256] [--steps 10] [--channels-last] [--benchmark]
 """

@@ -40,4 +40,4 @@ for (h, c, k, r) in ((56, 64, 256, 1), (56, 256, 64, 1), (56, 64, 64, 3), (28, 1
         'wgrad': timeit(lambda: ops.conv_wgrad(dy, x, cs)),
     }
     for name, us in res.items():
-        print(f'conv {r}x{r} c{c} k{k} {h}x{h}: {name:24s} {us:8.1f} us   (x+y once = {bytes_io / 1e6:.0f} MB -> {bytes_io / 6.57e6:.0f} us at the HBM peak)')
+        print(f'conv {r}x{r} c{c} k{k} {h}x{h}: {name:24s} {us:8.1f} us   (x+y once = {bytes_io / 1e6:.0f} MB -> {bytes_io / 3.35e6:.0f} us at the H100 SXM HBM3 peak)')

@@ -9,7 +9,7 @@ import torch
 sys.path.insert(0, '.')
 from simpleaicv_pytorch_training_examples_b200 import ops  # noqa: E402
 
-HBM, TF = 6.57e12, 1429.5e12
+HBM, TF = 3.35e12, 989e12   # H100 SXM data sheet: HBM3 bandwidth, dense BF16 (700 W)
 
 
 def timeit(fn, n=10):

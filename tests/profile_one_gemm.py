@@ -1,5 +1,5 @@
-"""Launches the epilogue-bound GEMM shapes of ResNet-50 layer 1 a few times each, for an ncu --set full capture with source
-correlation (tests/run_gpu_r2_u.sh): conv 1x1 c64->k256 56x56 forward without / with the BatchNorm-statistics epilogue and
+"""Launches the epilogue-bound GEMM shapes of ResNet-50 layer 1 a few times each, for a profiler capture
+(torch.profiler): conv 1x1 c64->k256 56x56 forward without / with the BatchNorm-statistics epilogue and
 the c256->k64 data gradient with the shortcut addend (aux operand by TMA)."""
 import sys
 

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 attention family (csrc/attn_sm100.cuh) through the general C-ABI entry
+"""GPU parity of the wgmma attention family (csrc/attn_sm90.cuh) through the general C-ABI entry
 (saicv_attn_fwd / saicv_attn_bwd) against plain fp32 torch attention on the same bf16-representable inputs:
 every supported (score width, value width), long sequences (several key blocks / row tiles), cross attention
 (Lq != Lk), key-padding masks and strided (packed / head-major) layouts.  Tolerances: outputs 2e-2 abs,
@@ -67,8 +67,6 @@ def test_attn_fwd_bwd_matches_torch(B, H, Lq, Lk, dqk, dv, masked):
     dq, dk, dvv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
     ops.attn_bwd(q, k, v, out, lse, dout, scale, dq, dk, dvv, mask_bits=bits)
     torch.cuda.synchronize()
-    from simpleaicv_pytorch_training_examples_b200 import _lib
-    assert _lib.load().saicv_attn_error() == 0
     for name, got, want in (('dq', dq, qf.grad), ('dk', dk, kf.grad), ('dv', dvv, vf.grad)):
         r = _rel(got, want)
         assert r <= 2e-2, f'{name} rel L2 {r}'

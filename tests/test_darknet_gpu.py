@@ -1,4 +1,4 @@
-"""DarknetTiny / Darknet19 / Darknet53 on the B200 runtime vs the CPU oracle (oracle/darknet.py): end to end and stage by
+"""DarknetTiny / Darknet19 / Darknet53 on the H100 runtime vs the CPU oracle (oracle/darknet.py): end to end and stage by
 stage with the oracle's boundary tensors (same method and tolerances as tests/test_resnet_gpu.py).
 The 32-channel layers run channel-padded to 64 inside the runtime; only real channels are compared
 and the padded ones must be exactly zero."""

@@ -1,4 +1,4 @@
-"""Bit-reproducibility of the B200 runtime (the reference runs with cudnn.deterministic=True,
+"""Bit-reproducibility of the H100 runtime (the reference runs with cudnn.deterministic=True,
 tools/utils.py:95-107): two consecutive forward+backward passes on the same batch and weights give
 bit-identical logits and parameter gradients (no float atomics anywhere in the kernels), and a second
 forward run between a training forward and its backward does not disturb that backward (the tape of

@@ -1,4 +1,4 @@
-"""DETR on the B200 runtime vs the CPU oracle (oracle/detr.py, pinned to the reference by
+"""DETR on the H100 runtime vs the CPU oracle (oracle/detr.py, pinned to the reference by
 tests/golden/resnet18_detr_*.pt and live in tests/test_oracle_vs_reference.py).
 
 Kernel level: post-LayerNorm forward / backward, dropout, head packing, attention with the additive key-bias column and

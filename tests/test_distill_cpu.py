@@ -7,7 +7,7 @@ import torch
 def _ref_losses():
     from baseline import ref_import
     if not ref_import.available():
-        pytest.skip('reference not present (GPU box)')
+        pytest.skip('reference not installed (oracle/build_ref.py)')
     ref_import._ensure_path()
     from SimpleAICV.distillation import losses
     return losses

@@ -1,4 +1,4 @@
-"""Knowledge distillation on the B200 runtime (SURVEY.md 8 f4): KDModel's frozen teacher runs without a tape, the student's
+"""Knowledge distillation on the H100 runtime (SURVEY.md 8 f4): KDModel's frozen teacher runs without a tape, the student's
 gradients equal those of the same student trained stand-alone with the same combined loss, and the teacher receives none."""
 import pytest
 import torch

@@ -1,6 +1,6 @@
 """MAE pre-training (SURVEY.md 8 f4): the oracle (oracle/mae.py) replays outputs of the REFERENCE's VITMAEPretrainModel +
 MSELoss (tests/golden/mae_b2_64px.ptm, made by tests/golden/make_mae_golden.py), matches the live reference when it is
-present, and the B200 module shell has the reference's state_dict and seeded initialisation.  CPU only."""
+present, and the H100 module shell has the reference's state_dict and seeded initialisation.  CPU only."""
 import importlib.util
 import os
 
@@ -39,7 +39,7 @@ def test_oracle_reproduces_reference_mae_outputs():
 def test_oracle_matches_live_reference_mae():
     from baseline import ref_import
     if not ref_import.available():
-        pytest.skip('reference not present (GPU box)')
+        pytest.skip('reference not installed (oracle/build_ref.py)')
     from oracle import mae
     torch.set_num_threads(1)
     x, noise = gen.make_inputs()

@@ -1,4 +1,4 @@
-"""MAE pre-training on the B200 runtime (SURVEY.md 8 f4): the token gather / scatter kernels against torch.gather, and the
+"""MAE pre-training on the H100 runtime (SURVEY.md 8 f4): the token gather / scatter kernels against torch.gather, and the
 whole training step (masking, encoder, un-shuffle, decoder, MSELoss on removed patches, backward) against the CPU oracle
 (oracle/mae.py, pinned to the reference by tests/test_mae_cpu.py) with the masks pinned through the noise input.
 Tolerances as tests/test_vit_gpu.py: outputs vs the bf16-storage oracle, gradients bounded by the bf16 storage noise."""

@@ -78,7 +78,7 @@ def test_linear_epilogue_rowscale_and_dgelu():
 @pytest.mark.parametrize('M,N,K', [(300, 200, 64), (5000, 768, 256), (1111, 1000, 1024)])
 def test_epilogue_aux_operand_by_tma(M, N, K, tune, monkeypatch):
     """The aux operand of the epilogue (fp32 residual / bf16 addend, ReLU mask, GELU pre-activation) is TMA-loaded into the
-    staging slices (gemm_sm100.cuh, aux_tma) with 1-3 slices per half and any tile width: ragged M and N, several tiles per
+    staging slices (gemm_sm90.cuh, aux_tma) with 1-3 slices per half and any tile width: ragged M and N, several tiles per
     CTA so the slices wrap, compared with torch and with the per-thread-load path ('legacy')."""
     ops = _ops()
     if tune == 'legacy':

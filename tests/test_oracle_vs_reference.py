@@ -1,11 +1,11 @@
-"""Live comparison oracle <-> unmodified reference (baseline/_ref install, or /root/reference in the
-build container); skipped only where neither exists."""
+"""Live comparison oracle <-> unmodified reference (the copy build() installs into oracle/_ref); skipped only where
+no reference was available to build()."""
 import pytest
 import torch
 
 from baseline import ref_import
 
-pytestmark = pytest.mark.skipif(not ref_import.available(), reason='reference not installed (baseline/install_ref.sh)')
+pytestmark = pytest.mark.skipif(not ref_import.available(), reason='reference not installed (oracle/build_ref.py)')
 
 
 def _ref_backbones():
@@ -77,7 +77,7 @@ def test_vit_oracle_matches_reference(global_pool):
 
 @pytest.mark.parametrize('arch', ['darknettiny', 'darknet19', 'darknet53'])
 def test_darknet_oracle_and_constructors_match_reference(arch):
-    """oracle/darknet.py and the B200 constructor shells vs darknet.py:147-432."""
+    """oracle/darknet.py and the H100 constructor shells vs darknet.py:147-432."""
     from oracle import darknet
     from simpleaicv_pytorch_training_examples_b200.classification import backbones as mine
     torch.manual_seed(2)
@@ -118,7 +118,7 @@ def test_b200_vit_constructors_match_reference_state_dict(arch, kw):
 
 @pytest.mark.parametrize('arch', ['van_b0'])
 def test_van_oracle_and_constructor_match_reference(arch):
-    """oracle/van.py and the B200 constructor shell vs van.py:211-310 (seeded init, logits, every gradient)."""
+    """oracle/van.py and the H100 constructor shell vs van.py:211-310 (seeded init, logits, every gradient)."""
     from oracle import van
     from simpleaicv_pytorch_training_examples_b200.classification import backbones as mine
     torch.manual_seed(6)
@@ -144,7 +144,7 @@ def test_van_oracle_and_constructor_match_reference(arch):
 
 
 def test_sam_encoder_oracle_and_constructor_match_reference():
-    """oracle/sam_encoder.py and the B200 ViTImageEncoder shell vs segment_anything/image_encoder.py:259-331
+    """oracle/sam_encoder.py and the H100 ViTImageEncoder shell vs segment_anything/image_encoder.py:259-331
     (windowed blocks with padding + a global block; pos_embed / rel-pos tables randomised)."""
     from oracle import sam_encoder as se
     from simpleaicv_pytorch_training_examples_b200.interactive_segmentation.models.segment_anything import image_encoder as mine
@@ -179,7 +179,7 @@ def test_sam_encoder_oracle_and_constructor_match_reference():
 
 
 def test_detr_oracle_and_constructor_match_reference():
-    """oracle/detr.py and the B200 DETR shell vs detection/models/detr.py:273-364 (ResNet-18 body, 6 + 6 layers, padded
+    """oracle/detr.py and the H100 DETR shell vs detection/models/detr.py:273-364 (ResNet-18 body, 6 + 6 layers, padded
     images so that the float key_padding_mask bias matters; dropout zeroed on the reference)."""
     from oracle import detr as od
     from simpleaicv_pytorch_training_examples_b200.detection import models as mine

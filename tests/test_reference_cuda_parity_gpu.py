@@ -1,23 +1,52 @@
-"""Parity at the BENCHMARKED shape against the reference's own CUDA path (VERDICT r1 item 10).
+"""Parity at the BENCHMARKED shape against the reference's own CUDA path.
 
-The unmodified reference modules (baseline/_ref) run on the same GPU under ``torch.autocast(bf16)`` — what
-tools/scripts.py:153-170 does — on the same seeded weights and the same batch (256 x 3 x 224 x 224) as the
-B200 runtime.  Compared: logits, loss, BN running statistics and every parameter gradient.
+The unmodified reference modules, run on a GPU under ``torch.autocast(bf16)`` — what tools/scripts.py:153-170 does — and in
+fp32 on the same seeded weights and the same batch (256 x 3 x 224 x 224), are stored in tests/golden/ref_cuda_bs256_*.pt
+(written by tests/golden/make_ref_cuda_parity_golden.py).  Compared with this project's runtime: initial weights (bit
+for bit), logits of a seeded sample of rows, loss, a seeded sample of every BN running statistic and of every parameter
+gradient.
 
 Tolerances (SURVEY.md 8c): logits / loss 2e-2; gradients relative L2 <= 2e-2 and cosine >= 0.999 on
-well-conditioned tensors.  Which tensors are well conditioned is MEASURED, not assumed: the reference is also
-run in fp32, and ``noise = relL2(ref_bf16, ref_fp32)`` is the error the reference's own bf16 path makes on that
-tensor.  A tensor with noise <= 1e-2 is well conditioned and must meet the tight bound against the reference's
-bf16 result; the others (early layers of a randomly initialised network, listed in the output) must satisfy
-relL2(ours, ref_fp32) <= 2 * noise + 2e-2, i.e. be no further from the exact gradient than the reference itself.
+well-conditioned tensors.  Which tensors are well conditioned is MEASURED, not assumed: the reference was also
+run in fp32, and ``noise = relL2(ref_bf16, ref_fp32)`` (over the whole tensor) is the error the reference's own bf16 path
+makes on that tensor.  A tensor with noise <= 1e-2 is well conditioned and must meet the tight bound against the
+reference's bf16 result (and its norm must be within 2e-2); the others (early layers of a randomly initialised network,
+listed in the output) must satisfy relL2(ours, ref_fp32) <= 2 * noise + 2e-2, i.e. be no further from the exact gradient
+than the reference itself.  Gradient bounds are evaluated on the stored sample of each tensor.
 """
+import hashlib
+import os
+
 import pytest
 import torch
 
-from baseline import ref_import
+pytestmark = [pytest.mark.gpu]
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not ref_import.available(), reason='reference not installed (baseline/install_ref.sh)')]
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ref_cuda_bs256_{}.ptc')
+N_GRAD_SAMPLES = 128
+N_STAT_SAMPLES = 64
+N_LOGIT_ROWS = 4
+
+
+def sample_index(numel, k, seed):
+    """Seeded sample of k element indices (all of them when the tensor is that small)."""
+    if numel <= k:
+        return torch.arange(numel)
+    return torch.randint(0, numel, (k,), generator=torch.Generator().manual_seed(1000 + seed))
+
+
+def logit_rows(batch):
+    return sample_index(batch, N_LOGIT_ROWS, 0).sort().values
+
+
+def batch_for(loss_name, batch):
+    g = torch.Generator().manual_seed(2024)
+    x = torch.randn(batch, 3, 224, 224, generator=g)
+    lab = torch.randint(0, 1000, (batch,), generator=g)
+    if loss_name == 'CELoss':
+        return x, lab
+    oh = torch.nn.functional.one_hot(lab, 1000).float() * 0.9 + 0.1 / 1000
+    return x, 0.5 * oh + 0.5 * oh.roll(1, 0)
 
 
 def _rel(a, b):
@@ -29,85 +58,64 @@ def _cos(a, b):
     return (a @ b / (a.norm() * b.norm()).clamp_min(1e-30)).item()
 
 
-def _ref_run(model, crit, x, y, autocast):
-    model.zero_grad(set_to_none=True)
-    with torch.autocast('cuda', dtype=torch.bfloat16, enabled=autocast):
-        out = model(x)
-        loss = crit(out, y)
-    loss.backward()
-    torch.cuda.synchronize()
-    return out.detach().float(), loss.detach().float(), {n: p.grad.detach().float().clone() for n, p in model.named_parameters() if p.grad is not None}
-
-
 CASES = [('resnet50', {}, 'CELoss', 256), ('vit_base_patch16', {'image_size': 224, 'global_pool': True}, 'OneHotLabelCELoss', 256)]
 
 
 @pytest.mark.parametrize('arch,kw,loss_name,batch', CASES, ids=[c[0] for c in CASES])
 def test_bs256_matches_reference_cuda_autocast(arch, kw, loss_name, batch):
     from simpleaicv_pytorch_training_examples_b200.classification import backbones as mine_b, losses as mine_l
-    ref_b = ref_import.backbones()
-    ref_l = ref_import.module('SimpleAICV.classification.losses')
-    g = torch.Generator().manual_seed(2024)
-    x = torch.randn(batch, 3, 224, 224, generator=g).cuda()
-    lab = torch.randint(0, 1000, (batch,), generator=g)
-    if loss_name == 'CELoss':
-        y = lab.cuda()
-    else:
-        oh = torch.nn.functional.one_hot(lab, 1000).float() * 0.9 + 0.1 / 1000
-        y = (0.5 * oh + 0.5 * oh.roll(1, 0)).cuda()
-    torch.manual_seed(0)
-    ref = ref_b.__dict__[arch](num_classes=1000, **kw).cuda().train()
+    gold = torch.load(GOLDEN.format(arch), weights_only=False)
+    x, y = batch_for(loss_name, batch)
+    x, y = x.cuda(), y.cuda()
     torch.manual_seed(0)
     mine = mine_b.__dict__[arch](num_classes=1000, **kw).cuda().train()
-    assert all(torch.equal(a, b) for a, b in zip(ref.state_dict().values(), mine.state_dict().values()))
-    sd0 = {k: v.clone() for k, v in ref.state_dict().items()}
-    rcrit, mcrit = ref_l.__dict__[loss_name]().cuda(), mine_l.__dict__[loss_name]().cuda()
-
-    lo32, ls32, g32 = _ref_run(ref, rcrit, x, y, autocast=False)
-    ref.load_state_dict(sd0)                                   # undo the BN running-stat update
-    lo16, ls16, g16 = _ref_run(ref, rcrit, x, y, autocast=True)
-    ref_stats = {k: v.clone() for k, v in ref.state_dict().items() if 'running_' in k}
+    ms0 = mine.state_dict()
+    assert list(ms0) == list(gold['init_sha'])
+    assert all(hashlib.sha256(v.detach().cpu().contiguous().numpy().tobytes()).hexdigest() == gold['init_sha'][k]
+               for k, v in ms0.items())
+    mcrit = mine_l.__dict__[loss_name]().cuda()
 
     out = mine(x)
     loss = mcrit(out, y)
     loss.backward()
     torch.cuda.synchronize()
-    lom, lsm = out.detach().float(), loss.detach().float()
-    gm = {n: p.grad.detach().float() for n, p in mine.named_parameters() if p.grad is not None}
+    lom, lsm = out.detach().float().cpu(), loss.detach().float()
+    gm = {n: p.grad.detach().float().cpu() for n, p in mine.named_parameters() if p.grad is not None}
 
     # ---- logits / loss: 2e-2 (SURVEY 8c), measured against the reference's bf16-autocast CUDA output
-    scale = lo16.abs().max().item()
-    err = (lom - lo16).abs().max().item()
-    noise_logits = (lo16 - lo32).abs().max().item()
-    print(f'{arch}: logits max|ours-ref_bf16| {err:.4g} (ref_bf16 vs ref_fp32 {noise_logits:.4g}, max|logit| {scale:.3g}); '
-          f'loss ours {lsm.item():.6f} ref_bf16 {ls16.item():.6f} ref_fp32 {ls32.item():.6f}')
+    rows = gold['logit_rows']
+    assert torch.equal(rows, logit_rows(batch))
+    scale, noise_logits = gold['logit_absmax16'], gold['logit_noise']
+    err = (lom[rows] - gold['logits16']).abs().max().item()
+    print(f'{arch}: logits max|ours-ref_bf16| {err:.4g} on {len(rows)} rows (ref_bf16 vs ref_fp32 {noise_logits:.4g}, '
+          f'max|logit| {scale:.3g}); loss ours {lsm.item():.6f} ref_bf16 {gold["loss16"]:.6f} ref_fp32 {gold["loss32"]:.6f}')
     assert err <= 2e-2 + 2e-2 * scale + 2 * noise_logits
-    assert abs(lsm.item() - ls16.item()) <= 2e-2 * abs(ls16.item()) + 2e-2
-    # ---- BN running statistics: rtol 1e-3 against the fp32 run's statistics is too tight for bf16 inputs of
-    #      either implementation; both bf16 paths are held to 1e-2 of the tensor scale
+    assert abs(lsm.item() - gold['loss16']) <= 2e-2 * abs(gold['loss16']) + 2e-2
+    # ---- BN running statistics: both bf16 paths are held to 1e-2 of the tensor scale
     ms = mine.state_dict()
-    for k, v in ref_stats.items():
-        assert (ms[k] - v).abs().max().item() <= 1e-2 * v.abs().max().item() + 1e-3, k
+    for i, (k, st) in enumerate(gold['bn_stats'].items()):
+        idx = sample_index(ms[k].numel(), N_STAT_SAMPLES, i)
+        assert (ms[k].reshape(-1).float().cpu()[idx] - st['values']).abs().max().item() <= 1e-2 * st['absmax'] + 1e-3, k
     # ---- gradients
-    assert set(g16) <= set(gm)
-    assert all(gm[n].abs().max().item() == 0 for n in set(gm) - set(g16))   # params the reference gives no gradient
+    ref_g = gold['grads']
+    assert set(ref_g) <= set(gm)
+    assert all(gm[n].abs().max().item() == 0 for n in set(gm) - set(ref_g))   # params the reference gives no gradient
     well, ill, failures = 0, [], []
-    for n in g16:
-        noise = _rel(g16[n], g32[n])
-        if noise <= 1e-2:
+    for i, (n, g) in enumerate(ref_g.items()):
+        m = gm[n].reshape(-1)[sample_index(gm[n].numel(), N_GRAD_SAMPLES, i)] / max(g['norm16'], 1e-30)
+        g16, g32 = g['g16'].float(), g['g32'].float()
+        if g['noise'] <= 1e-2:
             well += 1
-            r, c = _rel(gm[n], g16[n]), _cos(gm[n], g16[n])
-            if not (r <= 2e-2 and c >= 0.999):
-                failures.append(f'{n}: relL2 {r:.3g} cos {c:.5f} vs ref_bf16 (well conditioned, noise {noise:.2g})')
+            r, c = _rel(m, g16), _cos(m, g16)
+            rn = abs(gm[n].double().norm().item() - g['norm16']) / max(g['norm16'], 1e-30)
+            if not (r <= 2e-2 and c >= 0.999 and rn <= 2e-2):
+                failures.append(f'{n}: relL2 {r:.3g} cos {c:.5f} norm {rn:.3g} vs ref_bf16 (well conditioned, noise {g["noise"]:.2g})')
         else:
-            r = _rel(gm[n], g32[n])
-            ill.append((n, noise, r))
-            if not r <= 2 * noise + 2e-2:
-                failures.append(f'{n}: relL2 to fp32 {r:.3g} > 2 x reference noise {noise:.3g} + 2e-2')
-    cat = lambda d: torch.cat([d[n].flatten() for n in g16])
-    whole = _rel(cat(gm), cat(g16))
+            r = _rel(m, g32)
+            ill.append((n, g['noise'], r))
+            if not r <= 2 * g['noise'] + 2e-2:
+                failures.append(f'{n}: relL2 to fp32 {r:.3g} > 2 x reference noise {g["noise"]:.3g} + 2e-2')
     print(f'{arch}: {well} well-conditioned gradient tensors within 2e-2 / cos 0.999 of the reference bf16 run; '
           f'{len(ill)} ill-conditioned (reference bf16-vs-fp32 noise > 1e-2), worst 5: '
-          + ', '.join(f'{n} noise {a:.2g} ours {b:.2g}' for n, a, b in sorted(ill, key=lambda t: -t[1])[:5])
-          + f'; whole-gradient relL2 vs ref_bf16 {whole:.4g} (ref noise {_rel(cat(g16), cat(g32)):.4g})')
+          + ', '.join(f'{n} noise {a:.2g} ours {b:.2g}' for n, a, b in sorted(ill, key=lambda t: -t[1])[:5]))
     assert not failures, f'{len(failures)} gradient tensors out of tolerance: ' + '; '.join(failures[:10])

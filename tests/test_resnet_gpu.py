@@ -1,4 +1,4 @@
-"""Whole-network parity on the GPU: the B200 runtime (through the C ABI) against the CPU oracle
+"""Whole-network parity on the GPU: the H100 runtime (through the C ABI) against the CPU oracle
 on the same seeded weights and inputs, and against the committed reference outputs.
 
 What is compared, and why two oracles.  The kernels store activations / activation gradients in

@@ -1,4 +1,4 @@
-"""SAM ViT image encoder on the B200 runtime vs the CPU oracle (oracle/sam_encoder.py, pinned to the reference by
+"""SAM ViT image encoder on the H100 runtime vs the CPU oracle (oracle/sam_encoder.py, pinned to the reference by
 tests/golden/sam_enc_*.pt and live in tests/test_oracle_vs_reference.py): kernel-level parity of the window
 partition / rel-pos kernels against plain torch, block-by-block parity driven with the oracle's boundary tensors
 (windowed blocks with padding and a global block), and an end-to-end forward / backward.  pos_embed and the rel-pos

@@ -1,4 +1,4 @@
-"""SAMLoss on the B200 kernels (csrc/capi_loss.cu) against the reference's formulas restated in plain fp32 torch
+"""SAMLoss on the H100 kernels (csrc/capi_loss.cu) against the reference's formulas restated in plain fp32 torch
 (interactive_segmentation/losses.py:11-198; tests/golden/make_sam_loss_golden.py runs the reference itself and commits
 its outputs for the same seeded inputs): the three loss terms, the best-mask selection (integer indices) and the
 gradients w.r.t. the mask logits and the IoU predictions."""

@@ -13,7 +13,6 @@ import torch
 from simpleaicv_pytorch_training_examples_b200.classification import backbones
 from simpleaicv_pytorch_training_examples_b200.tools import utils as my_utils
 
-REF = '/root/reference'
 
 
 class _Cfg:
@@ -59,7 +58,7 @@ def test_scheduler_closed_forms(name, params):
 def _ref_utils():
     from baseline import ref_import
     if not ref_import.available():
-        pytest.skip('reference not installed (baseline/install_ref.sh)')
+        pytest.skip('reference not installed (oracle/build_ref.py)')
     return ref_import.module('tools.utils')
 
 

@@ -1,4 +1,4 @@
-"""VAN on the B200 runtime vs the CPU oracle (oracle/van.py, pinned to the reference by tests/golden/van_*.pt and
+"""VAN on the H100 runtime vs the CPU oracle (oracle/van.py, pinned to the reference by tests/golden/van_*.pt and
 tests/test_oracle_vs_reference.py): kernel-level parity of the depthwise / gating / layer-scale / generic-BN
 kernels against plain torch fp32, stage-by-stage parity driven with the oracle's boundary tensors, and an end to
 end step.  Layer scales are raised from the 1e-5 initial value to 0.5 in the model-level tests so that the
