@@ -18,6 +18,7 @@ Reference semantics followed: SimpleAICV/classification/backbones/resnet.py:19-4
 import torch
 
 from .. import ops
+from .operands import CONV, STEM, Linear, Operand, rows_wgrad
 
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SILU = 0, 1, 2, 3
 # BatchNorm batch statistics are accumulated by the conv GEMM's epilogue instead of a separate pass over y
@@ -94,18 +95,20 @@ class ConvBN:
         self.kp = _round_up(k, 64)
         self.cp = c if self.is_stem else _round_up(c, 64)
         self.padded = self.kp != k
-        self.kpad = ops.stem_kpad(c, r, s) if self.is_stem else r * s * self.cp
-        self.w_bf16 = None
-        self.w_version = None
+        self.op = Operand(self.conv.weight, STEM if self.is_stem else CONV, kp=self.kp, cp=self.cp)
+        self.kpad = self.op.kpad
         self.sums = None
 
     # ---- parameters
+    @property
+    def w_bf16(self):
+        """The bf16 operand copy of the conv weight ([kp][kpad]; None before the first prep())."""
+        return self.op.w
+
     def prep(self):
-        w = self.conv.weight
         bn = self.bn
-        if self.w_bf16 is None or self.w_bf16.device != w.device:
-            dev = w.device
-            self.w_bf16 = torch.empty(self.kp, self.kpad, device=dev, dtype=torch.bfloat16)
+        dev = self.op.refresh().device
+        if self.sums is None or self.sums.device != dev:
             self.sums = torch.zeros(2, self.kp, device=dev)   # backward scratch (consumed within one bn_bwd)
             if self.padded:
                 self.gamma_p = torch.ones(self.kp, device=dev)
@@ -114,12 +117,6 @@ class ConvBN:
                 self.rv_p = torch.ones(self.kp, device=dev)
                 self.dg_p = torch.empty(self.kp, device=dev)
                 self.db_p = torch.empty(self.kp, device=dev)
-            self.w_version = None
-        ver = (w.data_ptr(), w._version)
-        if ver != self.w_version:
-            ops.prep_conv_weight(w.detach(), self.w_bf16, self.kpad,
-                                 order=ops.ORDER_CRS if self.is_stem else ops.ORDER_RSC, kp=self.kp, cp=self.cp)
-            self.w_version = ver
         if self.padded:
             self.gamma_p[:self.k].copy_(bn.weight.detach())
             self.beta_p[:self.k].copy_(bn.bias.detach())
@@ -149,11 +146,11 @@ class ConvBN:
         tape['stats'] = (stats, ops.gemm_stats_rows(rows, self.kp)) if want_stats else None
         if self.is_stem:
             cols = ops.stem_im2col(a_in, self.r, self.s, self.stride, self.pad, self.kpad)
-            y = ops.linear_fwd(cols, self.w_bf16, stats=stats).view(n, P, Q, self.kp)
+            y = ops.linear_fwd(cols, self.op.w, stats=stats).view(n, P, Q, self.kp)
             tape['cols'] = cols
         else:
             cs = ops.make_conv_shape(n, h, w, self.cp, self.kp, self.r, self.s, self.stride, self.pad)
-            y = ops.conv_fprop(a_in, self.w_bf16, cs, stats=stats)
+            y = ops.conv_fprop(a_in, self.op.w, cs, stats=stats)
             tape['a_in'] = a_in
             tape['cs'] = cs
         tape['in_hw'] = (h, w)
@@ -264,14 +261,14 @@ class ConvBN:
         if not need_dx:
             return None
         if self.stride == 1:
-            return ops.conv_dgrad(dy, self.w_bf16, cs, add=add)
+            return ops.conv_dgrad(dy, self.op.w, cs, add=add)
         assert self.stride == 2
         if self.r == 1:
             assert add is None
-            return 'strided', ops.linear_dgrad(dy.view(-1, self.kp), self.w_bf16).view(n, P, Q, self.cp)
+            return 'strided', ops.linear_dgrad(dy.view(-1, self.kp), self.op.w).view(n, P, Q, self.cp)
         u = ops.zero_upsample2(dy, h, wd)
         cs1 = ops.make_conv_shape(n, h, wd, self.cp, self.kp, self.r, self.s, 1, self.pad)
-        return ops.conv_dgrad(u, self.w_bf16, cs1, add=add)
+        return ops.conv_dgrad(u, self.op.w, cs1, add=add)
 
 
 class ResidualBlockRT:
@@ -397,21 +394,11 @@ class FcHeadRT:
 
     def __init__(self, fc):
         self.fc = fc
-        self.w_bf16 = None
-        self.b_pad = None
-        self.version = None
+        self.lin = Linear(fc)
+        self.op = self.lin.op
 
     def prep(self):
-        w = self.fc.weight
-        ver = (w.data_ptr(), w._version)
-        if self.w_bf16 is None or ver != self.version:
-            npad = _round_up(w.shape[0], 8)
-            if self.w_bf16 is None:
-                self.w_bf16 = torch.zeros(npad, w.shape[1], device=w.device, dtype=torch.bfloat16)
-                self.b_pad = torch.zeros(npad, device=w.device)
-            ops.cast_bf16(w.detach(), self.w_bf16[:w.shape[0]])
-            self.version = ver
-        self.b_pad[:w.shape[0]].copy_(self.fc.bias.detach())
+        self.lin.prep()
 
     def forward(self, a, tape):
         tape['feat_hw'] = (a.shape[1], a.shape[2])
@@ -421,7 +408,7 @@ class FcHeadRT:
             pooled = pooled[:, :feat].contiguous()
         tape['pooled'] = pooled
         ncls = self.fc.weight.shape[0]
-        logits = ops.linear_fwd(pooled, self.w_bf16, bias=self.b_pad, out_f32=True)
+        logits = self.lin.fwd(pooled, out_f32=True)
         if logits.shape[1] != ncls:
             logits = logits[:, :ncls].contiguous()
         return logits
@@ -429,7 +416,7 @@ class FcHeadRT:
     def backward(self, dlogits, tape, sink, cpad):
         """dlogits fp32 [B, num_classes] -> gradient w.r.t. the last feature map (NHWC bf16, cpad channels)."""
         ncls, feat = self.fc.weight.shape
-        npad = self.w_bf16.shape[0]
+        npad = self.op.w.shape[0]
         dlogits = dlogits.contiguous().float()
         bbuf, bacc = sink.begin(self.fc.bias)
         ops.colsum(dlogits, bbuf, accumulate=bacc)
@@ -439,16 +426,8 @@ class FcHeadRT:
             ops.cast_bf16(dlogits, dl)
         else:
             dl[:, :ncls] = dlogits.to(torch.bfloat16)
-        wbuf, wacc = sink.begin(self.fc.weight)
-        part = ops.linear_wgrad(dl, tape['pooled'])
-        if npad == ncls:
-            ops.reduce_partials(part, wbuf, accumulate=wacc)
-        else:
-            tmp = torch.empty(npad, feat, device=dl.device)
-            ops.reduce_partials(part, tmp)
-            wbuf.copy_(tmp[:ncls] + (wbuf if wacc else 0))
-        sink.done(self.fc.weight, wbuf)
-        dpooled = ops.linear_dgrad(dl, self.w_bf16)
+        rows_wgrad(dl, tape['pooled'], self.fc.weight, sink)
+        dpooled = ops.linear_dgrad(dl, self.op.w)
         if cpad != feat:
             full = torch.zeros(dpooled.shape[0], cpad, device=dl.device, dtype=torch.bfloat16)
             full[:, :feat] = dpooled
@@ -464,26 +443,16 @@ class ConvHeadRT:
     def __init__(self, conv):
         self.conv = conv
         assert conv.kernel_size == (1, 1) and conv.bias is not None
-        self.w_bf16 = None
-        self.b_pad = None
-        self.version = None
+        self.lin = Linear(conv)
+        self.op = self.lin.op
 
     def prep(self):
-        w = self.conv.weight
-        ver = (w.data_ptr(), w._version)
-        if self.w_bf16 is None or ver != self.version:
-            npad = _round_up(w.shape[0], 8)
-            if self.w_bf16 is None:
-                self.w_bf16 = torch.zeros(npad, w.shape[1], device=w.device, dtype=torch.bfloat16)
-                self.b_pad = torch.zeros(npad, device=w.device)
-            ops.cast_bf16(w.detach().view(w.shape[0], w.shape[1]), self.w_bf16[:w.shape[0]])
-            self.version = ver
-        self.b_pad[:w.shape[0]].copy_(self.conv.bias.detach())
+        self.lin.prep()
 
     def forward(self, a, tape):
         n, h, w, c = a.shape
         tape['a_in'] = a
-        y = ops.linear_fwd(a.view(n * h * w, c), self.w_bf16, bias=self.b_pad)      # bf16 [N*H*W, npad]
+        y = self.lin.fwd(a.view(n * h * w, c))      # bf16 [N*H*W, npad]
         pooled = ops.avgpool_fwd(y.view(n, h, w, -1))
         return pooled[:, :self.conv.weight.shape[0]].float()
 
@@ -491,24 +460,18 @@ class ConvHeadRT:
         a = tape['a_in']
         n, h, w, c = a.shape
         ncls = self.conv.weight.shape[0]
-        npad = self.w_bf16.shape[0]
+        npad = self.op.w.shape[0]
         dl = torch.zeros(n, npad, device=a.device, dtype=torch.bfloat16)
         dl[:, :ncls] = dlogits.to(torch.bfloat16)
         dy = ops.avgpool_bwd(dl, h, w).view(n * h * w, npad)
-        wt, bias = self.conv.weight, self.conv.bias
-        wbuf, wacc = sink.begin(wt)
-        part = ops.linear_wgrad(dy, a.view(n * h * w, c))
-        tmp = torch.empty(npad, c, device=a.device)
-        ops.reduce_partials(part, tmp)
-        g = tmp[:ncls].view_as(wt)
-        wbuf.copy_(g + wbuf if wacc else g)
-        sink.done(wt, wbuf)
+        bias = self.conv.bias
+        rows_wgrad(dy, a.view(n * h * w, c), self.conv.weight, sink)
         bbuf, bacc = sink.begin(bias)
         full = torch.empty(npad, device=a.device)
         ops.colsum(dy, full)
         bbuf.copy_(full[:ncls] + bbuf if bacc else full[:ncls])
         sink.done(bias, bbuf)
-        return ops.linear_dgrad(dy, self.w_bf16).view(n, h, w, c)
+        return ops.linear_dgrad(dy, self.op.w).view(n, h, w, c)
 
 
 class ResNetRT:
@@ -537,6 +500,7 @@ class ResNetRT:
         self.head = head if head is not None else FcHeadRT(model.fc)
         self.checkpoint = checkpoint
         self.sink = GradSink()
+        self._units = self.units() + [self.head]
 
     def units(self):
         us = [self.stem]
@@ -544,10 +508,12 @@ class ResNetRT:
             us += b.all_units()
         return us
 
+    def operands(self):
+        return [u.op for u in self._units]
+
     def prep(self):
-        for u in self.units():
+        for u in self._units:
             u.prep()
-        self.head.prep()
 
     # The network is run as three stages (stem / residual blocks / head) so that tests can drive
     # each stage with the oracle's tensors (tests/test_resnet_gpu.py, teacher-forced parity).

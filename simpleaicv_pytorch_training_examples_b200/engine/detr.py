@@ -21,12 +21,11 @@ import torch
 
 from .. import ops
 from .convnet import GradSink, ResNetRT
-from .vit import _Linear
+from .operands import Linear, Operand
 
 
 class _NoHead:
-    def prep(self):
-        pass
+    """The DETR backbone has no classifier: DetrRT drives the body's stem and blocks itself."""
 
 
 def _pad_cols_bf16(t, n):
@@ -43,22 +42,14 @@ class _MHA:
         self.mod = mod
         self.C, self.H = mod.embed_dim, mod.num_heads
         self.hd = self.C // self.H
-        self.out = _Linear(mod.out_proj)
-        self.w_bf16 = None
-        self.version = None
+        self.out = Linear(mod.out_proj)
+        self.op = Operand(mod.in_proj_weight)
 
     def prep(self):
-        w = self.mod.in_proj_weight
-        ver = (w.data_ptr(), w._version)
-        if self.w_bf16 is None or ver != self.version:
-            if self.w_bf16 is None or self.w_bf16.device != w.device:
-                self.w_bf16 = torch.empty(w.shape, device=w.device, dtype=torch.bfloat16)
-            ops.cast_bf16(w.detach(), self.w_bf16)
-            self.version = ver
-        self.out.prep()
+        self.op.refresh()
 
     def _proj(self, x, r0, r1):
-        return ops.linear_fwd(x, self.w_bf16[r0:r1], bias=self.mod.in_proj_bias.detach()[r0:r1])
+        return ops.linear_fwd(x, self.op.w[r0:r1], bias=self.mod.in_proj_bias.detach()[r0:r1])
 
     def forward(self, q_in, k_in, v_in, t, B, Lq, Lk, key_bias, p, seed, sb=None):
         """q_in [B*Lq, C], k_in / v_in [B*Lk, C] bf16 operand copies (q_in is k_in for self-attention).
@@ -132,7 +123,7 @@ class _MHA:
 
     def dgrad(self, dy, r0, r1, resid=None):
         """fp32 data gradient of the projection rows r0:r1 (+ resid)."""
-        return ops.linear_dgrad(dy, self.w_bf16[r0:r1], resid=resid, out_f32=True)
+        return ops.linear_dgrad(dy, self.op.w[r0:r1], resid=resid, out_f32=True)
 
 
 def _branch_out(lin, a, resid, p, seed, sb):
@@ -149,11 +140,7 @@ def _branch_grad(dz, dzb, p, seed, sb):
 
 class _FFN:
     def __init__(self, layer):
-        self.l1, self.l2 = _Linear(layer.linear1), _Linear(layer.linear2)
-
-    def prep(self):
-        self.l1.prep()
-        self.l2.prep()
+        self.l1, self.l2 = Linear(layer.linear1), Linear(layer.linear2)
 
     def forward(self, yb, y, t, p, seeds, sb):
         """z = y + dropout(linear2(dropout(relu(linear1(yb)))))"""
@@ -170,7 +157,7 @@ class _FFN:
         if p > 0.:
             ops.dropout(dh, p, seeds[0], out=dh, seed_base=sb)     # survivors' 1 / (1 - p)
         self.l1.bwd(dh, t['ffn_in'], sink, need_dx=False)
-        return ops.linear_dgrad(dh, self.l1.w_bf16, resid=dz, out_f32=True)
+        return ops.linear_dgrad(dh, self.l1.op.w, resid=dz, out_f32=True)
 
 
 def _norm_fwd(norm, z, pos=None, want_y=True, want_yb=True, want_ypb=False):
@@ -194,9 +181,8 @@ class _EncLayer:
         self.attn = _MHA(layer.attention)
         self.ffn = _FFN(layer)
 
-    def prep(self):
-        self.attn.prep()
-        self.ffn.prep()
+    def units(self):
+        return [self.attn, self.attn.out, self.ffn.l1, self.ffn.l2]
 
     def forward(self, x, xb, xpb, t, cx, want_pos_copy):
         """x fp32 stream, xb = bf16(x), xpb = bf16(x + pos).  Returns the same triple for the next layer."""
@@ -228,10 +214,8 @@ class _DecLayer:
         self.ca = _MHA(layer.multihead_attention)
         self.ffn = _FFN(layer)
 
-    def prep(self):
-        self.sa.prep()
-        self.ca.prep()
-        self.ffn.prep()
+    def units(self):
+        return [self.sa, self.sa.out, self.ca, self.ca.out, self.ffn.l1, self.ffn.l2]
 
     def forward(self, x, xb, xqb, memb, mempb, t, cx):
         """x fp32 [B*Q, C] (tgt), xb = bf16(x), xqb = bf16(x + query_pos); memb / mempb: bf16 copies of the encoder
@@ -279,13 +263,12 @@ class _Heads:
     """DETRClsRegHead (head.py:184-213): class logits and the 3-layer box MLP on all decoder outputs at once."""
 
     def __init__(self, head):
-        self.cls = _Linear(head.cls_head)
-        self.r0, self.r2, self.r4 = _Linear(head.reg_head[0]), _Linear(head.reg_head[2]), _Linear(head.reg_head[4])
+        self.cls = Linear(head.cls_head)
+        self.r0, self.r2, self.r4 = Linear(head.reg_head[0]), Linear(head.reg_head[2]), Linear(head.reg_head[4])
         self.ncls = head.cls_head.weight.shape[0]
 
-    def prep(self):
-        for l in (self.cls, self.r0, self.r2, self.r4):
-            l.prep()
+    def units(self):
+        return [self.cls, self.r0, self.r2, self.r4]
 
     def forward(self, hsb, t):
         t['hsb'] = hsb
@@ -296,14 +279,14 @@ class _Heads:
 
     def backward(self, dcls, dreg, t, sink):
         """fp32 gradients of the class logits [rows, ncls] and box logits [rows, 4] -> fp32 gradient of hs."""
-        dcb = _pad_cols_bf16(dcls, self.cls.w_bf16.shape[0])
-        drb = _pad_cols_bf16(dreg, self.r4.w_bf16.shape[0])
+        dcb = _pad_cols_bf16(dcls, self.cls.op.w.shape[0])
+        drb = _pad_cols_bf16(dreg, self.r4.op.w.shape[0])
         dr2 = self.r4.bwd(drb, t['r2'], sink, relu_out=t['r2'])
         dr1 = self.r2.bwd(dr2, t['r1'], sink, relu_out=t['r1'])
         self.r0.bwd(dr1, t['hsb'], sink, need_dx=False)
         self.cls.bwd(dcb, t['hsb'], sink, need_dx=False)
-        dhs = ops.linear_dgrad(dr1, self.r0.w_bf16, out_f32=True)
-        return ops.linear_dgrad(dcb, self.cls.w_bf16, resid=dhs, out_f32=True)
+        dhs = ops.linear_dgrad(dr1, self.r0.op.w, out_f32=True)
+        return ops.linear_dgrad(dcb, self.cls.op.w, resid=dhs, out_f32=True)
 
 
 class DetrRT:
@@ -315,19 +298,20 @@ class DetrRT:
         self.body = ResNetRT(model.backbone, has_maxpool=True, head=_NoHead(),
                              checkpoint=getattr(model.backbone, 'use_gradient_checkpoint', False))
         self.body.sink = self.sink
-        self.proj = _Linear(model.proj_conv)
+        self.proj = Linear(model.proj_conv)
         tr = model.transformer
         self.enc = [_EncLayer(l) for l in tr.encoder_blocks]
         self.dec = [_DecLayer(l) for l in tr.decoder_blocks]
         self.heads = _Heads(model.head)
         self._seed_base = 0
+        self._units = self.body.units() + [self.proj] + [u for l in self.enc + self.dec for u in l.units()] + self.heads.units()
+
+    def operands(self):
+        return [u.op for u in self._units]
 
     def prep(self):
-        self.body.prep()
-        self.proj.prep()
-        for l in self.enc + self.dec:
-            l.prep()
-        self.heads.prep()
+        for u in self._units:
+            u.prep()
 
     def _context(self, B, L, pos, key_bias, training):
         tr = self.model.transformer

@@ -17,7 +17,8 @@ import torch
 
 from .. import ops
 from .convnet import GradSink
-from .vit import _Block, _Linear
+from .operands import Linear, PatchEmbed
+from .vit import _Block, layernorm_bwd
 
 
 class MAERT:
@@ -27,26 +28,18 @@ class MAERT:
         enc, dec = model.encoder, model.decoder
         self.enc_blocks = [_Block(b) for b in enc.blocks]
         self.dec_blocks = [_Block(b) for b in dec.blocks]
-        self.e2d = _Linear(model.encoder_to_decoder)
-        self.fc = _Linear(dec.fc)
+        self.e2d = Linear(model.encoder_to_decoder)
+        self.fc = Linear(dec.fc)
+        self.patch = PatchEmbed(enc.patch_embed.proj)
+        self._units = [lin for b in self.enc_blocks + self.dec_blocks for lin in b.linears()] + [self.e2d, self.fc, self.patch]
         self.sink = GradSink()
-        self.pw_bf16 = None
-        self.pw_version = None
+
+    def operands(self):
+        return [u.op for u in self._units]
 
     def prep(self):
-        for b in self.enc_blocks + self.dec_blocks:
-            for lin in b.linears():
-                lin.prep()
-        self.e2d.prep()
-        self.fc.prep()
-        w = self.model.encoder.patch_embed.proj.weight
-        ver = (w.data_ptr(), w._version)
-        if self.pw_bf16 is None or ver != self.pw_version:
-            self.kpad = ops.stem_kpad(w.shape[1], w.shape[2], w.shape[3])
-            if self.pw_bf16 is None:
-                self.pw_bf16 = torch.empty(w.shape[0], self.kpad, device=w.device, dtype=torch.bfloat16)
-            ops.prep_conv_weight(w.detach(), self.pw_bf16, self.kpad, order=ops.ORDER_CRS)
-            self.pw_version = ver
+        for u in self._units:
+            u.prep()
 
     # ---- masking indices (vit_mae.py:203-225), int32 index tables for the gather kernels
     def masking(self, b, n, dev, noise=None):
@@ -71,12 +64,11 @@ class MAERT:
     def forward(self, x, training, keep_tape, noise=None):
         assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 4
         self.prep()
-        m, enc, dec = self.model, self.model.encoder, self.model.decoder
-        b, p, c, cd = x.shape[0], m.patch_size, enc.embedding_planes, dec.embedding_planes
+        enc, dec = self.model.encoder, self.model.decoder
+        b, c, cd = x.shape[0], enc.embedding_planes, dec.embedding_planes
         tape = {'enc': [dict() for _ in self.enc_blocks], 'dec': [dict() for _ in self.dec_blocks]}
-        cols = tape['cols'] = ops.stem_im2col(x.contiguous(), p, p, p, 0, self.kpad)
-        n = cols.shape[0] // b
-        patch = ops.linear_fwd(cols, self.pw_bf16, bias=enc.patch_embed.proj.bias.detach(), out_f32=True)      # [B*N, C] fp32
+        patch, tape['cols'] = self.patch.fwd(x.contiguous())                                                 # [B*N, C] fp32
+        n = patch.shape[0] // b
         keep_len, mask, enc_idx, enc_pos, dec_idx = self.masking(b, n, x.device, noise)
         le = keep_len + 1
         h = ops.token_gather_fwd(patch.view(b, n, c), enc_idx, enc.cls_token.detach().view(-1),
@@ -107,16 +99,6 @@ class MAERT:
         t.update(ckpt_in=h, ckpt_scales=(scratch['s1'], scratch['s2']), s2=scratch['s2'])
         return out
 
-    def _ln_bwd(self, norm, dy, x, stats):
-        sink = self.sink
-        gbuf, gacc = sink.begin(norm.weight)
-        bbuf, bacc = sink.begin(norm.bias)
-        dxb = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16)
-        dx = ops.layernorm_bwd(dy, x, norm.weight.detach(), stats, gbuf, bbuf, dx_bf16=dxb, accumulate=gacc)
-        sink.done(norm.weight, gbuf)
-        sink.done(norm.bias, bbuf)
-        return dx, dxb
-
     def _blocks_bwd(self, blocks, tapes, dx, dxb, b, l):
         for i in range(len(blocks) - 1, -1, -1):
             t = tapes[i]
@@ -136,7 +118,7 @@ class MAERT:
         dfull = torch.zeros(b, ld, pdim, device=dpred.device, dtype=torch.bfloat16)
         dfull[:, 1:, :] = dpred
         dlnd = self.fc.bwd(dfull.view(b * ld, pdim), tape['lnd'], sink)
-        dx, dxb = self._ln_bwd(dec.norm, dlnd, tape['dec_out'], tape['std'])
+        dx, dxb = layernorm_bwd(dec.norm, dlnd, tape['dec_out'], tape['std'], sink)
         dx, dxb = self._blocks_bwd(self.dec_blocks, tape['dec'], dx, dxb, b, ld)
         # un-shuffle backward: every row of the encoder_to_decoder output is referenced exactly once; mask-token rows sum up
         dy, dmask = ops.token_gather_bwd(dx.view(b, ld, cd), tape['dec_idx'], le, zero=False)
@@ -144,21 +126,14 @@ class MAERT:
         mbuf.view(-1).copy_(dmask + (mbuf.view(-1) if macc else 0))
         sink.done(dec.mask_token, mbuf)
         dlne = self.e2d.bwd(dy.view(b * le, cd), tape['lne'], sink)
-        dx, dxb = self._ln_bwd(enc.norm, dlne, tape['enc_out'], tape['ste'])
+        dx, dxb = layernorm_bwd(enc.norm, dlne, tape['enc_out'], tape['ste'], sink)
         dx, dxb = self._blocks_bwd(self.enc_blocks, tape['enc'], dx, dxb, b, le)
         # gather backward: masked patches get no gradient; the cls rows sum into the cls token (pos_embed is frozen)
         dpatch, dcls = ops.token_gather_bwd(dx.view(b, le, c), tape['enc_idx'], n, zero=True)
         cbuf, cacc = sink.begin(enc.cls_token)
         cbuf.view(-1).copy_(dcls + (cbuf.view(-1) if cacc else 0))
         sink.done(enc.cls_token, cbuf)
-        w, bias = enc.patch_embed.proj.weight, enc.patch_embed.proj.bias
-        wbuf, wacc = sink.begin(w)
-        part = ops.linear_wgrad(dpatch.view(b * n, c), tape['cols'])
-        ops.finish_conv_wgrad(part, wbuf, self.kpad, accumulate=wacc, order=ops.ORDER_CRS)
-        sink.done(w, wbuf)
-        bbuf, bacc = sink.begin(bias)
-        ops.colsum(dpatch.view(b * n, c), bbuf, accumulate=bacc)
-        sink.done(bias, bbuf)
+        self.patch.bwd(dpatch.view(b * n, c), tape['cols'], sink)
         if sink.on_backward_end is not None:
             sink.on_backward_end()
 

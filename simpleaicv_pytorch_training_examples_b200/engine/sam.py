@@ -17,17 +17,8 @@ import torch
 
 from .. import ops
 from .convnet import GradSink
-from .vit import _Linear
-
-
-def _ln_bwd(norm, dy, x, stats, dres, sink, want_bf16=True):
-    gbuf, gacc = sink.begin(norm.weight)
-    bbuf, bacc = sink.begin(norm.bias)
-    dxb = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16) if want_bf16 else None
-    dx = ops.layernorm_bwd(dy, x, norm.weight.detach(), stats, gbuf, bbuf, dres=dres, dx_bf16=dxb, accumulate=gacc)
-    sink.done(norm.weight, gbuf)
-    sink.done(norm.bias, bbuf)
-    return dx, dxb
+from .operands import CONV, Linear, Operand, PatchEmbed
+from .vit import layernorm_bwd
 
 
 class _Block:
@@ -35,8 +26,8 @@ class _Block:
     def __init__(self, blk):
         self.blk = blk
         self.ws = blk.window_size
-        self.qkv, self.proj = _Linear(blk.attn.qkv), _Linear(blk.attn.proj)
-        self.lin1, self.lin2 = _Linear(blk.mlp.lin1), _Linear(blk.mlp.lin2)
+        self.qkv, self.proj = Linear(blk.attn.qkv), Linear(blk.attn.proj)
+        self.lin1, self.lin2 = Linear(blk.mlp.lin1), Linear(blk.mlp.lin2)
         self.heads = blk.attn.head_nums
         self.scale = blk.attn.scale
 
@@ -88,7 +79,7 @@ class _Block:
         # ---- MLP branch
         du = self.lin2.bwd(dxb, t['h'], sink, gelu_pre=t['u'])
         dln2 = self.lin1.bwd(du, t['ln2'], sink)
-        dx, dxb = _ln_bwd(blk.norm2, dln2, t['x_mid'], t['st2'], dx, sink)
+        dx, dxb = layernorm_bwd(blk.norm2, dln2, t['x_mid'], t['st2'], sink, dres=dx)
         # ---- attention branch
         datt_full = self.proj.bwd(dxb, t['att_full'], sink)
         if self.ws > 0:
@@ -117,7 +108,7 @@ class _Block:
             dln1 = ops.window_unpartition(dxw.view(Bw, L, C), B, H, W, self.ws).view(-1, C)
         else:
             dln1 = dxw
-        return _ln_bwd(blk.norm1, dln1, t['x_in'], t['st1'], dx, sink)
+        return layernorm_bwd(blk.norm1, dln1, t['x_in'], t['st1'], sink, dres=dx)
 
 
 class SamEncoderRT:
@@ -126,46 +117,27 @@ class SamEncoderRT:
     def __init__(self, model):
         self.model = model
         self.blocks = [_Block(b) for b in model.blocks]
+        self.patch = PatchEmbed(model.patch_embed.proj)
+        self.n0 = Operand(model.neck[0].weight)             # 1x1 conv, no bias
+        self.n2 = Operand(model.neck[2].weight, CONV)       # 3x3 conv, no bias
+        self._units = [lin for b in self.blocks for lin in b.linears()] + [self.patch]
         self.sink = GradSink()
-        self.pw_bf16 = self.n0_bf16 = self.n2_bf16 = None
-        self.versions = {}
+
+    def operands(self):
+        return [u.op for u in self._units] + [self.n0, self.n2]
 
     def prep(self):
-        m = self.model
-        for b in self.blocks:
-            for lin in b.linears():
-                lin.prep()
-        w = m.patch_embed.proj.weight
-        if self._changed('pw', w):
-            k = w.shape[1] * w.shape[2] * w.shape[3]
-            self.kpad = ops.stem_kpad(w.shape[1], w.shape[2], w.shape[3])
-            if self.pw_bf16 is None:
-                self.pw_bf16 = torch.empty(w.shape[0], self.kpad, device=w.device, dtype=torch.bfloat16)
-            ops.prep_conv_weight(w.detach(), self.pw_bf16, self.kpad, order=ops.ORDER_CRS)
-        w0 = m.neck[0].weight
-        if self._changed('n0', w0):
-            self.n0_bf16 = ops.cast_bf16(w0.detach().view(w0.shape[0], w0.shape[1]), self.n0_bf16)
-        w2 = m.neck[2].weight
-        if self._changed('n2', w2):
-            if self.n2_bf16 is None:
-                self.n2_bf16 = torch.empty(w2.shape[0], 9 * w2.shape[1], device=w2.device, dtype=torch.bfloat16)
-            ops.prep_conv_weight(w2.detach(), self.n2_bf16, 9 * w2.shape[1], order=ops.ORDER_RSC)
-
-    def _changed(self, key, w):
-        ver = (w.data_ptr(), w._version)
-        if self.versions.get(key) != ver:
-            self.versions[key] = ver
-            return True
-        return False
+        for u in self._units:
+            u.prep()
+        self.n0.refresh()
+        self.n2.refresh()
 
     # ---- stages (also driven separately by the teacher-forced parity tests)
     def embed_forward(self, x, tape):
         m = self.model
         B = x.shape[0]
-        ps = m.patch_embed.proj.kernel_size[0]
-        cols = ops.stem_im2col(x, ps, ps, ps, 0, self.kpad)
-        tape['cols'] = cols
-        tok = ops.linear_fwd(cols, self.pw_bf16, bias=m.patch_embed.proj.bias.detach(), out_f32=True)
+        ps = self.patch.p
+        tok, tape['cols'] = self.patch.fwd(x)
         H, W = x.shape[2] // ps, x.shape[3] // ps
         tape['B'], tape['H'], tape['W'] = B, H, W
         ops.add_pos_embed(tok, m.pos_embed.detach())
@@ -176,14 +148,7 @@ class SamEncoderRT:
         pbuf, pacc = sink.begin(m.pos_embed)
         ops.colsum(dx.view(tape['B'], -1), pbuf.view(-1), accumulate=pacc)        # sum over the batch
         sink.done(m.pos_embed, pbuf)
-        w, bias = m.patch_embed.proj.weight, m.patch_embed.proj.bias
-        wbuf, wacc = sink.begin(w)
-        part = ops.linear_wgrad(dxb, tape['cols'])
-        ops.finish_conv_wgrad(part, wbuf, self.kpad, accumulate=wacc, order=ops.ORDER_CRS)
-        sink.done(w, wbuf)
-        bbuf, bacc = sink.begin(bias)
-        ops.colsum(dxb, bbuf, accumulate=bacc)
-        sink.done(bias, bbuf)
+        self.patch.bwd(dxb, tape['cols'], sink)
 
     def neck_forward(self, x, tape):
         """x fp32 [B*H*W, C] -> fp32 NCHW [B, out_planes, H, W]"""
@@ -191,12 +156,12 @@ class SamEncoderRT:
         B, H, W = tape['B'], tape['H'], tape['W']
         n1, n3 = m.neck[1], m.neck[3]
         xb = tape['xb'] = ops.cast_bf16(x)
-        y1 = tape['y1'] = ops.linear_fwd(xb, self.n0_bf16, out_f32=True)                     # 1x1 conv, no bias
+        y1 = tape['y1'] = ops.linear_fwd(xb, self.n0.w, out_f32=True)                     # 1x1 conv, no bias
         oc = y1.shape[1]
         l1, tape['s1'] = ops.layernorm_fwd(y1, n1.weight.detach(), n1.bias.detach(), n1.eps)
         tape['l1'] = l1
         cs = tape['cs'] = ops.make_conv_shape(B, H, W, oc, oc, 3, 3, 1, 1)
-        y2b = ops.conv_fprop(l1.view(B, H, W, oc), self.n2_bf16, cs)
+        y2b = ops.conv_fprop(l1.view(B, H, W, oc), self.n2.w, cs)
         y2 = tape['y2'] = y2b.view(-1, oc).float()
         l2, tape['s2'] = ops.layernorm_fwd(y2, n3.weight.detach(), n3.bias.detach(), n3.eps)
         return l2.view(B, H, W, oc).permute(0, 3, 1, 2).float()
@@ -208,19 +173,19 @@ class SamEncoderRT:
         n1, n3 = m.neck[1], m.neck[3]
         oc = dout.shape[1]
         dl2 = dout.permute(0, 2, 3, 1).reshape(-1, oc).to(torch.bfloat16).contiguous()
-        _, dy2b = _ln_bwd(n3, dl2, tape['y2'], tape['s2'], None, sink)
+        _, dy2b = layernorm_bwd(n3, dl2, tape['y2'], tape['s2'], sink)
         w2 = m.neck[2].weight
         wbuf, wacc = sink.begin(w2)
         part = ops.conv_wgrad(dy2b.view(B, H, W, oc), tape['l1'].view(B, H, W, oc), tape['cs'])
         ops.finish_conv_wgrad(part, wbuf, 9 * oc, accumulate=wacc)
         sink.done(w2, wbuf)
-        dl1 = ops.conv_dgrad(dy2b.view(B, H, W, oc), self.n2_bf16, tape['cs']).view(-1, oc)
-        _, dy1b = _ln_bwd(n1, dl1, tape['y1'], tape['s1'], None, sink)
+        dl1 = ops.conv_dgrad(dy2b.view(B, H, W, oc), self.n2.w, tape['cs']).view(-1, oc)
+        _, dy1b = layernorm_bwd(n1, dl1, tape['y1'], tape['s1'], sink)
         w0 = m.neck[0].weight
         wbuf, wacc = sink.begin(w0)
         ops.reduce_partials(ops.linear_wgrad(dy1b, tape['xb']), wbuf, accumulate=wacc)
         sink.done(w0, wbuf)
-        dx = ops.linear_dgrad(dy1b, self.n0_bf16, out_f32=True)
+        dx = ops.linear_dgrad(dy1b, self.n0.w, out_f32=True)
         return dx, ops.cast_bf16(dx)
 
     def forward(self, x, training, keep_tape):

@@ -17,7 +17,7 @@ import torch
 
 from .. import ops
 from .convnet import FcHeadRT, GradSink
-from .vit import _Linear
+from .operands import CONV, STEM, Linear, Operand
 
 
 def _bn_forward(bn, x, training, out_f32, tape):
@@ -83,9 +83,9 @@ class _Block:
     def __init__(self, blk):
         self.blk = blk
         at, lka, mlp = blk.attn, blk.attn.spatial_gating_unit, blk.mlp
-        self.proj1, self.proj2, self.conv1 = _Linear(at.proj_1), _Linear(at.proj_2), _Linear(lka.conv1)
+        self.proj1, self.proj2, self.conv1 = Linear(at.proj_1), Linear(at.proj_2), Linear(lka.conv1)
         self.conv0, self.conv_sp = _DW(lka.conv0), _DW(lka.conv_spatial)
-        self.fc1, self.fc2, self.dw = _Linear(mlp.fc1), _Linear(mlp.fc2), _DW(mlp.dwconv.dwconv)
+        self.fc1, self.fc2, self.dw = Linear(mlp.fc1), Linear(mlp.fc2), _DW(mlp.dwconv.dwconv)
         self.drop_path = getattr(blk.drop_path, 'drop_path_prob', 0.)
         if getattr(mlp.drop, 'p', 0.) > 0.:
             raise NotImplementedError('VAN dropout_prob > 0 is not implemented by the H100 runtime (0 in every shipped config)')
@@ -164,19 +164,11 @@ class _PatchEmbed:
         self.conv, self.bn = pe.proj, pe.norm
         self.k, self.stride, self.pad = self.conv.kernel_size[0], self.conv.stride[0], self.conv.padding[0]
         self.from_image = self.conv.in_channels % 8 != 0
-        self.w_bf16 = None
-        self.version = None
+        self.op = Operand(self.conv.weight, STEM if self.from_image else CONV)
+        self.kpad = self.op.kpad
 
     def prep(self):
-        w = self.conv.weight
-        ver = (w.data_ptr(), w._version)
-        if self.w_bf16 is None or ver != self.version:
-            k, c = self.k, w.shape[1]
-            self.kpad = ops.stem_kpad(c, k, k) if self.from_image else k * k * c
-            if self.w_bf16 is None:
-                self.w_bf16 = torch.empty(w.shape[0], self.kpad, device=w.device, dtype=torch.bfloat16)
-            ops.prep_conv_weight(w.detach(), self.w_bf16, self.kpad, order=ops.ORDER_CRS if self.from_image else ops.ORDER_RSC)
-            self.version = ver
+        self.op.refresh()
 
     def forward(self, x, t, training):
         """x: NCHW fp32 image (stage 1) or NHWC bf16 -> (bf16 stream [rows, C], (n, P, Q, C))."""
@@ -188,7 +180,7 @@ class _PatchEmbed:
             n, h, w, _ = x.shape
             cols, P, Q = ops.im2col_nhwc(x, self.k, self.stride, self.pad)
         t['cols'], t['in_shape'], t['bn'] = cols, tuple(x.shape), {}
-        y = ops.linear_fwd(cols, self.w_bf16, bias=self.conv.bias.detach())
+        y = ops.linear_fwd(cols, self.op.w, bias=self.conv.bias.detach())
         out = _bn_forward(self.bn, y, training, False, t['bn'])
         return out, (n, P, Q, self.conv.out_channels)
 
@@ -207,7 +199,7 @@ class _PatchEmbed:
         if self.from_image:
             return None
         n, h, ww, c = t['in_shape']
-        dcols = ops.linear_dgrad(dy, self.w_bf16)
+        dcols = ops.linear_dgrad(dy, self.op.w)
         return ops.col2im_nhwc(dcols, n, h, ww, c, self.k, self.stride, self.pad)
 
 
@@ -223,14 +215,14 @@ class VANRT:
             self.stages.append((pe, blocks, getattr(model, f'norm{i + 1}')))
         self.head = FcHeadRT(model.head)
         self.sink = GradSink()
+        self._units = [u for pe, blocks, _ in self.stages for u in [pe] + [lin for b in blocks for lin in b.linears()]] + [self.head]
+
+    def operands(self):
+        return [u.op for u in self._units]
 
     def prep(self):
-        for pe, blocks, _ in self.stages:
-            pe.prep()
-            for b in blocks:
-                for lin in b.linears():
-                    lin.prep()
-        self.head.prep()
+        for u in self._units:
+            u.prep()
 
     # stage-level entry points (also driven by the teacher-forced parity tests)
     def stage_forward(self, i, x, t, training):

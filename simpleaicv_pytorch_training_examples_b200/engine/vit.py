@@ -16,68 +16,28 @@ import torch
 
 from .. import ops
 from .convnet import GradSink
+from .operands import Linear, PatchEmbed, rows_wgrad
 
 
-class _Linear:
-    """bf16 operand copy + forward / backward of one nn.Linear."""
-
-    def __init__(self, mod):
-        self.mod = mod
-        self.w_bf16 = None
-        self.version = None
-
-    def prep(self):
-        w = self.mod.weight
-        ver = (w.data_ptr(), w._version)
-        if self.w_bf16 is None or ver != self.version:
-            if self.w_bf16 is None or self.w_bf16.device != w.device:
-                npad = (w.shape[0] + 7) // 8 * 8
-                self.w_bf16 = torch.zeros(npad, w.shape[1], device=w.device, dtype=torch.bfloat16)
-                self.b_pad = torch.zeros(npad, device=w.device)
-            ops.cast_bf16(w.detach(), self.w_bf16[:w.shape[0]])
-            self.version = ver
-        self.b_pad[:w.shape[0]].copy_(self.mod.bias.detach())
-
-    def fwd(self, x, resid=None, out_f32=False, row_scale=None, rows_per_scale=0):
-        return ops.linear_fwd(x, self.w_bf16, bias=self.b_pad, resid=resid, out_f32=out_f32,
-                              row_scale=row_scale, rows_per_scale=rows_per_scale)
-
-    def fwd_flags(self, x, flags):
-        """Forward with an activation fused in the epilogue (ops.EPI_RELU / ops.EPI_GELU)."""
-        return ops.linear_fwd(x, self.w_bf16, bias=self.b_pad, flags=flags)
-
-    def bwd(self, dy, x, sink, need_dx=True, gelu_pre=None, relu_out=None, add=None):
-        """dy bf16 [M, N], x bf16 [M, K]: writes dW, db through the sink, returns dx bf16
-        (multiplied by gelu'(gelu_pre) when the input of this layer was gelu(gelu_pre), masked by
-        relu_out > 0 when it was a ReLU output, plus `add` when a second gradient joins there)."""
-        w, b = self.mod.weight, self.mod.bias
-        n = w.shape[0]
-        wbuf, wacc = sink.begin(w)
-        part = ops.linear_wgrad(dy, x)
-        if part.shape[1] == n:
-            ops.reduce_partials(part, wbuf, accumulate=wacc)
-        else:  # padded class dimension
-            tmp = torch.empty(part.shape[1], part.shape[2], device=dy.device)
-            ops.reduce_partials(part, tmp)
-            wbuf.copy_(tmp[:n] + (wbuf if wacc else 0))
-        sink.done(w, wbuf)
-        bbuf, bacc = sink.begin(b)
-        if dy.shape[1] == n:
-            ops.colsum(dy, bbuf, accumulate=bacc)
-        else:
-            full = torch.empty(dy.shape[1], device=dy.device)
-            ops.colsum(dy, full)
-            bbuf.copy_(full[:n] + (bbuf if bacc else 0))
-        sink.done(b, bbuf)
-        return ops.linear_dgrad(dy, self.w_bf16, gelu_pre=gelu_pre, relu_out=relu_out, add=add) if need_dx else None
+def layernorm_bwd(norm, dy, x, stats, sink, dres=None, want_bf16=True, scale=None, rows_per_scale=0):
+    """Backward of a row LayerNorm (nn.LayerNorm `norm`): dgamma / dbeta through the sink; returns (dx fp32 (+ dres), its
+    bf16 copy multiplied by the row scale `scale` (one per rows_per_scale rows), or None unless want_bf16)."""
+    gbuf, gacc = sink.begin(norm.weight)
+    bbuf, bacc = sink.begin(norm.bias)
+    dxb = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16) if want_bf16 else None
+    dx = ops.layernorm_bwd(dy, x, norm.weight.detach(), stats, gbuf, bbuf, dres=dres, dx_bf16=dxb, accumulate=gacc,
+                           bf16_row_scale=scale, rows_per_scale=rows_per_scale)
+    sink.done(norm.weight, gbuf)
+    sink.done(norm.bias, bbuf)
+    return dx, dxb
 
 
 class _Block:
 
     def __init__(self, blk):
         self.blk = blk
-        self.qkv, self.proj = _Linear(blk.attn.qkv), _Linear(blk.attn.proj)
-        self.fc1, self.fc2 = _Linear(blk.mlp.fc1), _Linear(blk.mlp.fc2)
+        self.qkv, self.proj = Linear(blk.attn.qkv), Linear(blk.attn.proj)
+        self.fc1, self.fc2 = Linear(blk.mlp.fc1), Linear(blk.mlp.fc2)
         self.heads = blk.attn.head_nums
         self.scale = blk.attn.scale
         self.drop_path = getattr(blk.drop_path, 'drop_path_prob', 0.)
@@ -126,17 +86,6 @@ class _Block:
             return ops.dropout(self.fc2.fwd(t['h']), p, seeds[3], resid=x, row_scale=s2, elems_per_scale=l * c, seed_base=sb)
         return self.fc2.fwd(t['h'], resid=x, out_f32=True, row_scale=s2, rows_per_scale=l)
 
-    def _ln_bwd(self, norm, dy, x, stats, dres, sink, scale, l):
-        """`scale`: drop-path scale of the branch that will consume the bf16 copy of dx."""
-        gbuf, gacc = sink.begin(norm.weight)
-        bbuf, bacc = sink.begin(norm.bias)
-        dxb = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16)
-        dx = ops.layernorm_bwd(dy, x, norm.weight.detach(), stats, gbuf, bbuf, dres=dres, dx_bf16=dxb, accumulate=gacc,
-                               bf16_row_scale=scale, rows_per_scale=l)
-        sink.done(norm.weight, gbuf)
-        sink.done(norm.bias, bbuf)
-        return dx, dxb
-
     def backward(self, dx, dxb, t, b, l, sink, next_scale=None):
         """dx fp32: gradient w.r.t. the block output; dxb: its bf16 copy already multiplied by this
         block's MLP drop-path scale (t['s2']).  Returns (dx_in fp32, bf16 copy multiplied by
@@ -150,7 +99,8 @@ class _Block:
         if p > 0.:
             ops.dropout(du, p, seeds[2], out=du, seed_base=sb)
         dln2 = self.fc1.bwd(du, t['ln2'], sink)
-        dx, dxb = self._ln_bwd(blk.norm2, dln2, t['x_mid'], t['st2'], dx, sink, t['s1'], l)
+        # the bf16 copies of dx carry the drop-path scale of the branch that consumes them
+        dx, dxb = layernorm_bwd(blk.norm2, dln2, t['x_mid'], t['st2'], sink, dres=dx, scale=t['s1'], rows_per_scale=l)
         # ---- attention branch
         g = ops.dropout(dxb, p, seeds[1], seed_base=sb) if p > 0. else dxb
         datt = self.proj.bwd(g, t['att'], sink)
@@ -164,7 +114,7 @@ class _Block:
         else:
             dqkv = ops.attention_bwd(t['qkv'], t['att'], datt, t['lse'], b, l, self.heads, d, self.scale)
         dln1 = self.qkv.bwd(dqkv, t['ln1'], sink)
-        return self._ln_bwd(blk.norm1, dln1, t['x_in'], t['st1'], dx, sink, next_scale, l)
+        return layernorm_bwd(blk.norm1, dln1, t['x_in'], t['st1'], sink, dres=dx, scale=next_scale, rows_per_scale=l)
 
 
 class ViTRT:
@@ -173,35 +123,24 @@ class ViTRT:
     def __init__(self, model):
         self.model = model
         self.blocks = [_Block(b) for b in model.blocks]
-        self.fc = _Linear(model.fc)
+        self.fc = Linear(model.fc)
+        self.patch = PatchEmbed(model.patch_embed.proj)
+        self._units = [lin for b in self.blocks for lin in b.linears()] + [self.fc, self.patch]
         self.sink = GradSink()
-        self.pw_bf16 = None
-        self.pw_version = None
+
+    def operands(self):
+        return [u.op for u in self._units]
 
     def prep(self):
-        for b in self.blocks:
-            for lin in b.linears():
-                lin.prep()
-        self.fc.prep()
-        w = self.model.patch_embed.proj.weight
-        ver = (w.data_ptr(), w._version)
-        if self.pw_bf16 is None or ver != self.pw_version:
-            k = w.shape[1] * w.shape[2] * w.shape[3]
-            self.kpad = ops.stem_kpad(w.shape[1], w.shape[2], w.shape[3])
-            if self.pw_bf16 is None:
-                self.pw_bf16 = torch.empty(w.shape[0], self.kpad, device=w.device, dtype=torch.bfloat16)
-            ops.prep_conv_weight(w.detach(), self.pw_bf16, self.kpad, order=ops.ORDER_CRS)
-            self.pw_version = ver
+        for u in self._units:
+            u.prep()
 
     # ---- stages (driven separately by the teacher-forced parity tests)
     def embed_forward(self, x, tape):
         m = self.model
         b = x.shape[0]
-        p = m.patch_size
-        cols = ops.stem_im2col(x, p, p, p, 0, self.kpad)
-        tape['cols'] = cols
-        patch = ops.linear_fwd(cols, self.pw_bf16, bias=m.patch_embed.proj.bias.detach(), out_f32=True)
-        np_ = cols.shape[0] // b
+        patch, tape['cols'] = self.patch.fwd(x)
+        np_ = patch.shape[0] // b
         c = m.embedding_planes
         tokens = ops.vit_assemble_tokens(patch, m.cls_token.detach().view(-1), m.pos_embed.detach().view(-1, c), b, np_, c)
         tape['b'], tape['l'] = b, np_ + 1
@@ -247,37 +186,19 @@ class ViTRT:
         m, sink = self.model, self.sink
         b, l, c = tape['b'], tape['l'], m.embedding_planes
         ncls = m.fc.weight.shape[0]
-        npad = self.fc.w_bf16.shape[0]
+        npad = self.fc.op.w.shape[0]
         dl = torch.zeros(b, npad, device=dlogits.device, dtype=torch.bfloat16)
         dl[:, :ncls] = dlogits.to(torch.bfloat16)
         # fc bias gradient from the fp32 dlogits
         bbuf, bacc = sink.begin(m.fc.bias)
         ops.colsum(dlogits.contiguous().float(), bbuf, accumulate=bacc)
-        dlnf = self._fc_bwd_nobias(dl, tape['lnf'])
+        rows_wgrad(dl, tape['lnf'], m.fc.weight, sink)
+        dlnf = ops.linear_dgrad(dl, self.fc.op.w)
         sink.done(m.fc.bias, bbuf)
-        gbuf, gacc = sink.begin(m.norm.weight)
-        nbuf, nacc = sink.begin(m.norm.bias)
-        dpooled = ops.layernorm_bwd(dlnf, tape['pooled'], m.norm.weight.detach(), tape['stf'], gbuf, nbuf, accumulate=gacc)
-        sink.done(m.norm.weight, gbuf)
-        sink.done(m.norm.bias, nbuf)
+        dpooled, _ = layernorm_bwd(m.norm, dlnf, tape['pooled'], tape['stf'], sink, want_bf16=False)
         dxb = torch.empty(b * l, c, device=dl.device, dtype=torch.bfloat16)
         dx = ops.token_pool_bwd(dpooled, l, m.global_pool, dx_bf16=dxb.view(b, l, c), bf16_row_scale=next_scale)
         return dx.view(b * l, c), dxb
-
-    def _fc_bwd_nobias(self, dl, x):
-        m, sink = self.model, self.sink
-        w = m.fc.weight
-        n = w.shape[0]
-        wbuf, wacc = sink.begin(w)
-        part = ops.linear_wgrad(dl, x)
-        if part.shape[1] == n:
-            ops.reduce_partials(part, wbuf, accumulate=wacc)
-        else:
-            tmp = torch.empty(part.shape[1], part.shape[2], device=dl.device)
-            ops.reduce_partials(part, tmp)
-            wbuf.copy_(tmp[:n] + (wbuf if wacc else 0))
-        sink.done(w, wbuf)
-        return ops.linear_dgrad(dl, self.fc.w_bf16)
 
     def embed_backward(self, dx, tape):
         m, sink = self.model, self.sink
@@ -289,14 +210,7 @@ class ViTRT:
         ops.vit_assemble_tokens_bwd(dx.view(b, l, c), pbuf, cbuf, dpatch, accumulate=pacc)
         sink.done(m.pos_embed, pbuf)
         sink.done(m.cls_token, cbuf)
-        w, bias = m.patch_embed.proj.weight, m.patch_embed.proj.bias
-        wbuf, wacc = sink.begin(w)
-        part = ops.linear_wgrad(dpatch, tape['cols'])
-        ops.finish_conv_wgrad(part, wbuf, self.kpad, accumulate=wacc, order=ops.ORDER_CRS)
-        sink.done(w, wbuf)
-        bbuf, bacc = sink.begin(bias)
-        ops.colsum(dpatch, bbuf, accumulate=bacc)
-        sink.done(bias, bbuf)
+        self.patch.bwd(dpatch, tape['cols'], sink)
 
     def backward(self, dlogits, tape):
         sink = self.sink

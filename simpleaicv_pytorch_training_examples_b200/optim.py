@@ -3,7 +3,8 @@
 ``FusedSGD`` / ``FusedAdamW`` update ALL parameters of a model with one launch of csrc/capi_optim.cu (torch's foreach
 path: 13 / 45 launches per step), refresh the bf16 GEMM-operand copies of the weights in the same pass (the runtime's
 separate cast / re-layout kernels: 53 per ResNet-50 step, 49 per ViT-B step) and apply the global-norm gradient clip
-without a host sync.  They subclass ``torch.optim.Optimizer``: ``param_groups`` (what ``tools.utils.Scheduler`` rewrites
+without a host sync.  ``attach(model)`` registers the fusable operands the model's runtime lists in ``operands()``
+(engine/operands.py).  They subclass ``torch.optim.Optimizer``: ``param_groups`` (what ``tools.utils.Scheduler`` rewrites
 every iteration), ``state_dict()`` / ``load_state_dict()`` use torch's own keys (``momentum_buffer``; ``step``,
 ``exp_avg``, ``exp_avg_sq``), so checkpoints interchange with the reference's torch.optim.SGD / AdamW
 (/root/reference/tools/utils.py:581-600).
@@ -13,6 +14,7 @@ picks table (device step counter % RING).  Under CUDA-graph capture that copy is
 ``sync_hyper()`` (a pure host write of slot t % RING, called by graph.GraphedTrainStep before each replay) is all a
 per-iteration learning-rate schedule needs, and the host may run RING - 1 steps ahead of the device.
 """
+import collections
 import ctypes
 import math
 
@@ -27,6 +29,9 @@ _TENSOR_DTYPE = np.dtype([('p', '<u8'), ('g', '<u8'), ('s1', '<u8'), ('s2', '<u8
                           ('group', '<i4'), ('rs', '<i4'), ('c', '<i4'), ('cp', '<i4'), ('kpad', '<i4'), ('pad_', '<i4')])
 assert _TENSOR_DTYPE.itemsize == 72   # saicv_opt_tensor (include/saicv_b200.h)
 
+# a registered copy that is one fixed tensor; an engine.operands.Operand has the same two fields
+_Fixed = collections.namedtuple('_Fixed', 'w conv')
+
 
 def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -37,17 +42,17 @@ def _p(t):
 
 
 class _FusedBase(torch.optim.Optimizer):
-    """Shared table building / hyper-parameter plumbing.  Shadows: ``register_shadow(param, bf16_tensor, conv=None)``
-    tells the step to keep ``bf16_tensor`` equal to bf16(param) ([N][K] Linear copy, leading rows) or, with
-    conv=(c, rs, cp, kpad), to the tap-major conv operand layout of saicv_prep_conv_weight (order 0)."""
+    """Shared table building / hyper-parameter plumbing.  ``register_shadow(param, shadow, conv=None)`` tells the step to
+    keep a bf16 copy equal to bf16(param): the leading rows of an [N][K] copy or, with conv=(c, rs, cp, kpad), the
+    tap-major conv operand layout of saicv_prep_conv_weight (order 0)."""
 
     _entry = None       # C-ABI symbol
     _n_state = 1
 
     def __init__(self, params, defaults):
         super().__init__(params, defaults)
-        self._shadows = {}        # id(param) -> (tensor, conv layout or None)
-        self._key = None          # identity of the table (pointers of p / grad / shadow)
+        self._shadows = {}        # id(param) -> copy refreshed by the step: _Fixed or engine.operands.Operand (.w, .conv)
+        self._key = None          # identity of the table (pointers of p / grad / operand copy)
         self._tab = None
         self._t = 0               # optimizer steps taken (AdamW bias correction)
         self._clip = None
@@ -56,29 +61,27 @@ class _FusedBase(torch.optim.Optimizer):
         self._events = [None] * RING   # recorded after the step that read slot i was launched
         self._pending = None
 
-    # ---- shadows (called by the runtimes: engine/convnet.py, engine/vit.py)
-    def register_shadow(self, param, shadow, conv=None, owner=None):
-        """owner: the runtime object whose ``w_bf16`` attribute is this copy; when given, the attribute is re-read before
-        every step, so a copy the runtime re-allocates (device move) is followed instead of silently going stale."""
-        assert shadow.dtype == torch.bfloat16 and shadow.is_contiguous()
-        self._shadows[id(param)] = (shadow, conv, owner)
+    # ---- operand copies
+    def register_shadow(self, param, shadow, conv=None):
+        """`shadow`: a contiguous bf16 tensor (with the layout `conv`), or a fusable engine.operands.Operand of `param`,
+        whose current copy and layout every step reads: a copy the runtime re-allocates (device move) is followed, and
+        one that no refresh() has allocated yet is skipped (its first refresh() casts it)."""
+        if isinstance(shadow, torch.Tensor):
+            assert shadow.dtype == torch.bfloat16 and shadow.is_contiguous()
+            shadow = _Fixed(shadow, conv)
+        else:
+            assert shadow.fusable and shadow.param is param and conv is None
+        self._shadows[id(param)] = shadow
         self._key = None
 
-    def _follow_owners(self):
-        for pid, (shadow, conv, owner) in list(self._shadows.items()):
-            cur = getattr(owner, 'w_bf16', None) if owner is not None else shadow
-            if cur is not None and cur is not shadow:
-                self._shadows[pid] = (cur, conv, owner)
-
     def attach(self, model):
-        """Registers the operand copies of every weight of `model`'s runtime (a no-op for plain torch modules)."""
+        """Registers the fusable operand copies of `model`'s runtime (a no-op for plain torch modules)."""
         m = model if hasattr(model, '_runtime') else getattr(model, 'module', model)
         if hasattr(m, '_runtime'):
-            from .engine import shadows
             mine = {id(p) for g in self.param_groups for p in g['params']}
-            for param, shadow, conv, owner in shadows.collect(m._runtime()):
-                if id(param) in mine:
-                    self.register_shadow(param, shadow, conv, owner=owner)
+            for op in m._runtime().operands():
+                if op.fusable and id(op.param) in mine:
+                    self.register_shadow(op.param, op)
         return self
 
     def load_state_dict(self, state_dict):
@@ -111,14 +114,14 @@ class _FusedBase(torch.optim.Optimizer):
             r['p'], r['g'], r['s1'] = p.data_ptr(), p.grad.data_ptr(), st[0].data_ptr()
             r['s2'] = st[1].data_ptr() if len(st) > 1 else 0
             r['numel'], r['group'] = p.numel(), gi
-            sh = self._shadows.get(id(p))
-            if sh is not None:
-                r['shadow'] = sh[0].data_ptr()
-                if sh[1] is not None:
-                    r['c'], r['rs'], r['cp'], r['kpad'] = sh[1]
-                    assert sh[0].numel() >= (p.numel() // (r['c'] * r['rs'])) * r['kpad']
+            op = self._shadows.get(id(p))
+            if op is not None and op.w is not None:
+                r['shadow'] = op.w.data_ptr()
+                if op.conv is not None:
+                    r['c'], r['rs'], r['cp'], r['kpad'] = op.conv
+                    assert op.w.numel() >= (p.numel() // (r['c'] * r['rs'])) * r['kpad']
                 else:
-                    assert sh[0].numel() >= p.numel()
+                    assert op.w.numel() >= p.numel()
             n = (p.numel() + chunk - 1) // chunk
             ct.extend([i] * n)
             ci.extend(range(n))
@@ -139,9 +142,8 @@ class _FusedBase(torch.optim.Optimizer):
         plist = self._params()
         if not plist:
             return None
-        self._follow_owners()
-        key = tuple((id(p), p.data_ptr(), p.grad.data_ptr(), self._shadows.get(id(p), (None,))[0] is not None and
-                     self._shadows[id(p)][0].data_ptr()) for _, p in plist)
+        copies = {pid: op.w.data_ptr() for pid, op in self._shadows.items() if op.w is not None}
+        key = tuple((id(p), p.data_ptr(), p.grad.data_ptr(), copies.get(id(p), 0)) for _, p in plist)
         if key != self._key:
             self._tab, self._key = self._build(plist), key
         return self._tab

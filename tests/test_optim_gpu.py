@@ -172,47 +172,70 @@ def test_captured_step_follows_the_learning_rate_schedule():
         assert (p - q).abs().max().item() <= 3e-6 * p.abs().max().item() + 1e-7, f'tensor {i}'
 
 
-def test_build_optimizer_fuses_the_runtime_operand_copies():
-    """tools.utils.build_optimizer on a CUDA model returns the fused optimizer with the runtime's bf16 weight copies
-    attached: after a training step the copies equal a fresh cast of the updated parameters, and the next forward
-    launches no cast / re-layout kernel for them."""
+def _family_step(family):
+    """(model on the GPU, a function running one forward and returning a scalar loss) for `family`."""
+    import test_operands_cpu
+    from simpleaicv_pytorch_training_examples_b200.classification import losses
+    model = test_operands_cpu._families()[family]().cuda().train()
+    g = torch.Generator(device='cuda').manual_seed(1)
+    if family == 'resnet18_detr':
+        model.transformer.dropout_prob = 0.0
+        x = torch.randn(2, 3, 128, 160, device='cuda', generator=g)
+        masks = torch.zeros(2, 128, 160, dtype=torch.bool, device='cuda')
+        return model, lambda: sum(o.float().square().mean() for o in model(x, masks))
+    if family == 'sam_encoder':
+        x = torch.randn(1, 3, 320, 320, device='cuda', generator=g)
+        return model, lambda: model(x).float().square().mean()
+    if family == 'mae':
+        x = torch.randn(4, 3, 64, 64, device='cuda', generator=g)
+        return model, lambda: model(x)[0].float().square().mean()
+    side = 32 if family == 'resnet18cifar' else 64
+    x = torch.randn(8, 3, side, side, device='cuda', generator=g)
+    y = torch.randint(0, 10, (8,), device='cuda', generator=g)
+    crit = losses.CELoss()
+    return model, lambda: crit(model(x), y)
+
+
+@pytest.mark.parametrize('family', ['resnet18cifar', 'darknet19', 'darknettiny', 'van_b0', 'vit_base_patch16', 'resnet18_detr',
+                                    'sam_encoder', 'mae'])
+def test_build_optimizer_fuses_the_runtime_operand_copies(family):
+    """tools.utils.build_optimizer on a CUDA model returns the fused optimizer with the runtime's fusable bf16 weight copies
+    attached: after two training steps every one of them equals a fresh cast of its updated parameter, and the next
+    prep() launches a kernel only for the copies the optimizer does not refresh (the stems)."""
     from simpleaicv_pytorch_training_examples_b200 import _lib, optim
-    from simpleaicv_pytorch_training_examples_b200.classification import backbones, losses
+    from simpleaicv_pytorch_training_examples_b200.engine.operands import Operand
     from simpleaicv_pytorch_training_examples_b200.tools import utils as tutils
 
     class Cfg:
         optimizer = ('SGD', {'lr': 0.1, 'momentum': 0.9, 'global_weight_decay': False, 'weight_decay': 1e-4,
                              'no_weight_decay_layer_name_list': []})
     torch.manual_seed(0)
-    model = backbones.resnet18cifar(num_classes=10).cuda().train()
+    model, loss_fn = _family_step(family)
     opt, _ = tutils.build_optimizer(Cfg, model)
-    assert isinstance(opt, optim.FusedSGD) and len(opt._shadows) >= 20
-    x = torch.randn(8, 3, 32, 32, device='cuda')
-    y = torch.randint(0, 10, (8,), device='cuda')
-    crit = losses.CELoss()
+    rt = model._runtime()
+    fusable = [op for op in rt.operands() if op.fusable]
+    assert isinstance(opt, optim.FusedSGD) and len(opt._shadows) == len(fusable)
     for _ in range(2):
-        crit(model(x), y).backward()
+        loss_fn().backward()
         opt.step()
         opt.zero_grad()
-    rt = model._runtime()
-    units = [u for u in rt.units() if not u.is_stem]
-    for u in units:
-        fresh = torch.empty_like(u.w_bf16)
-        from simpleaicv_pytorch_training_examples_b200 import ops
-        ops.prep_conv_weight(u.conv.weight.detach(), fresh, u.kpad, order=ops.ORDER_RSC, kp=u.kp, cp=u.cp)
-        assert torch.equal(fresh, u.w_bf16)
+    for op in fusable:
+        fresh = Operand(op.param, op.layout, kp=op.kp, cp=op.cp) if op.conv else Operand(op.param)
+        assert torch.equal(fresh.refresh(), op.w)
     n0 = _lib.launch_count()
     rt.prep()
     torch.cuda.synchronize()
-    assert _lib.launch_count() - n0 <= 2, 'prep() re-cast weights the optimizer had already refreshed'
+    assert _lib.launch_count() - n0 <= len(rt.operands()) - len(fusable), 'prep() re-cast weights the optimizer had already refreshed'
+    if family != 'resnet18cifar':
+        return
     # and the fused run equals torch.optim.SGD on the same model / data
     torch.manual_seed(0)
-    ref_model = backbones.resnet18cifar(num_classes=10).cuda().train()
+    ref_model, ref_loss_fn = _family_step(family)
     Cfg.optimizer[1]['fused'] = False
     ropt, _ = tutils.build_optimizer(Cfg, ref_model)
     assert isinstance(ropt, torch.optim.SGD)
     for _ in range(2):
-        crit(ref_model(x), y).backward()
+        ref_loss_fn().backward()
         ropt.step()
         ropt.zero_grad()
     for (n, p), q in zip(model.named_parameters(), ref_model.parameters()):
