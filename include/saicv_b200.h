@@ -67,11 +67,13 @@ typedef struct {
  * saicv_linear_fwd). */
 int saicv_conv_fprop(const void* x, const void* w, float* stats_partial, void* y,
                      const saicv_conv_shape* cs, int flags, void* stream);
-/* dx[n,h,w,c] = sum dy[n, h+pad-r, w+pad-s, k] w[k,r,s,c] (+ add[n,h,w,c]): stride-1 data
+/* dx[n,h,w,c] = sum dy[n, h+pad-r, w+pad-s, k] w[k,r,s,c] (+ add[n,h,w,c]) (* mask): stride-1 data
  * gradient; `add` (bf16, may be NULL) is the gradient arriving over the shortcut, fused into the
- * epilogue.  For a stride-2 conv pass the zero-upsampled dy (saicv_zero_upsample2) and stride = 1.
+ * epilogue.  `mask_bits` (may be NULL): the [n*h*w][c/32] ReLU mask written by saicv_bn_apply; the
+ * result (after the add) is multiplied by its bit, i.e. dx is the gradient behind that ReLU.
+ * For a stride-2 conv pass the zero-upsampled dy (saicv_zero_upsample2) and stride = 1.
  * `dy` has spatial extent (h, w).  requires k % 64 == 0, c % 64 == 0. */
-int saicv_conv_dgrad(const void* dy, const void* w, const void* add, void* dx,
+int saicv_conv_dgrad(const void* dy, const void* w, const void* add, const uint32_t* mask_bits, void* dx,
                      const saicv_conv_shape* cs, void* stream);
 /* dw_partial[splits][k][r*s*c] fp32 = sum over output pixels dy[pix,k] * x[patch(pix), (r,s,c)]. */
 int saicv_conv_wgrad(const void* dy, const void* x, float* dw_partial, const saicv_conv_shape* cs,
@@ -126,24 +128,40 @@ int saicv_bn_finalize(const float* partials, int partial_rows, const float* gamm
                       long long rows, int c, float eps, float momentum, void* stream);
 /* out = act(y*scale+shift + res) ; res optional, itself optionally batch-normalised with
  * res_scale_shift (downsample branch).  act: 0 none, 1 ReLU, 2 LeakyReLU(0.1); act | 8: the
- * residual is added after the activation, out = act(y*scale+shift) + res (darknet.py:141-144). */
+ * residual is added after the activation, out = act(y*scale+shift) + res (darknet.py:141-144).
+ * mask_bits (may be NULL; act == 1 and c % 32 == 0): receives the ReLU mask of `out` packed as
+ * uint32 [rows][c/32], bit j of word w set where out[row][32w + j] > 0. */
 int saicv_bn_apply(const void* y, const float* scale_shift, const void* res,
-                   const float* res_scale_shift, void* out, long long rows, int c, int act,
-                   void* stream);
+                   const float* res_scale_shift, void* out, uint32_t* mask_bits, long long rows, int c,
+                   int act, void* stream);
 /* backward reductions: g = dout * act'(out); sums[0][c] = sum g, sums[1][c] = sum g * xhat
  * (xhat from y, saved mean/rstd).  The activation mask comes from `out` (activated output) when
- * it is non-NULL; otherwise, for a unit without residual input, it is recomputed from
- * sign(y*scale+shift) using `scale_shift` (saves reading `out`).  Both may be NULL when act == 0.
+ * it is non-NULL; else from `bits` (the ReLU mask of saicv_bn_apply, act == 1) when it is
+ * non-NULL; otherwise, for a unit without residual input, it is recomputed from
+ * sign(y*scale+shift) using `scale_shift` (saves reading `out`).  All may be NULL when act == 0.
  * `partials`: workspace as above; `sums[2][c]` receives the folded result. */
-int saicv_bn_bwd_reduce(const void* dout, const void* out, const void* y, const float* saved,
-                        const float* scale_shift, float* partials, float* sums, long long rows,
-                        int c, int act, void* stream);
+int saicv_bn_bwd_reduce(const void* dout, const void* out, const uint32_t* bits, const void* y,
+                        const float* saved, const float* scale_shift, float* partials, float* sums,
+                        long long rows, int c, int act, void* stream);
 /* dy = gamma*rstd*(g - sum_g/rows - xhat*sum_gx/rows) bf16; writes dgamma/dbeta (fp32, (+)=)
  * and optionally dres = g (gradient flowing into the residual input). */
-int saicv_bn_bwd_apply(const void* dout, const void* out, const void* y, const float* saved,
-                       const float* gamma, const float* scale_shift, float* sums, void* dy,
-                       void* dres, float* dgamma, float* dbeta, long long rows, int c, int act,
+int saicv_bn_bwd_apply(const void* dout, const void* out, const uint32_t* bits, const void* y,
+                       const float* saved, const float* gamma, const float* scale_shift, float* sums,
+                       void* dy, void* dres, float* dgamma, float* dbeta, long long rows, int c, int act,
                        int accumulate, void* stream);
+/* The same two passes for two BatchNorms A and B with one gradient g and the same rows, c (the last
+ * BatchNorm and the downsample BatchNorm of a residual block): g = g_in * bits (bits may be NULL:
+ * g_in is already masked).  `partials`: SAICV_BN_PARTIAL_ROWS * 4 * c floats; sums[4][c] = A's
+ * sums[2][c] then B's.  Sums, dy and dgamma / dbeta equal two saicv_bn_bwd_reduce /
+ * saicv_bn_bwd_apply calls bit for bit. */
+int saicv_bn_bwd_reduce2(const void* g, const uint32_t* bits, const void* y_a, const void* y_b,
+                         const float* saved_a, const float* saved_b, float* partials, float* sums,
+                         long long rows, int c, void* stream);
+int saicv_bn_bwd_apply2(const void* g, const uint32_t* bits, const void* y_a, const void* y_b,
+                        const float* saved_a, const float* saved_b, const float* gamma_a,
+                        const float* gamma_b, const float* sums, void* dy_a, void* dy_b,
+                        float* dgamma_a, float* dbeta_a, float* dgamma_b, float* dbeta_b,
+                        long long rows, int c, int accumulate_a, int accumulate_b, void* stream);
 /* a = a + b (bf16), used where two gradient paths meet. */
 int saicv_add_bf16(void* a, const void* b, long long n, void* stream);
 

@@ -51,7 +51,7 @@ SIGNATURES = {
     'saicv_linear_wgrad': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_wgrad_splits': [c_int, c_int, c_ll],
     'saicv_conv_fprop': [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_int, c_void_p],
-    'saicv_conv_dgrad': [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_void_p],
+    'saicv_conv_dgrad': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_void_p],
     'saicv_conv_wgrad': [c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_int, c_void_p],
     'saicv_prep_conv_weight': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_finish_conv_wgrad': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
@@ -64,9 +64,11 @@ SIGNATURES = {
     'saicv_add_strided2': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_bn_stats': [c_void_p, c_void_p, c_ll, c_int, c_void_p],
     'saicv_bn_finalize': [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_float, c_float, c_void_p],
-    'saicv_bn_apply': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
-    'saicv_bn_bwd_reduce': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
-    'saicv_bn_bwd_apply': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_void_p],
+    'saicv_bn_apply': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
+    'saicv_bn_bwd_reduce': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
+    'saicv_bn_bwd_apply': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_void_p],
+    'saicv_bn_bwd_reduce2': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p],
+    'saicv_bn_bwd_apply2': [c_void_p] * 15 + [c_ll, c_int, c_int, c_int, c_void_p],
     'saicv_add_bf16': [c_void_p, c_void_p, c_ll, c_void_p],
     'saicv_maxpool3x3s2_fwd': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_maxpool3x3s2_bwd': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],

@@ -80,16 +80,51 @@ struct SlabGeom {
   int ldv;  // row stride in 16-byte vectors (== vpr unless a column chunk of a wider matrix is reduced)
 };
 
+// Tree-folds the ty rows of red[][] that share a channel vector and writes this block's partial row(s):
+// prow[c] = sum s0, and prow[C + c] = sum s1 unless ONLY_S0.  Every BatchNorm reduction folds through here so that the
+// single- and two-BatchNorm backward reductions produce bit-identical partial rows.
+template <bool ONLY_S0>
+__device__ __forceinline__ void fold_slab(float (*red)[17], const float (&s0)[8], const float (&s1)[8], int tx, int ty,
+                                          const SlabGeom& gm, float* __restrict__ prow, int C) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    red[threadIdx.x][i] = s0[i];
+    red[threadIdx.x][8 + i] = s1[i];
+  }
+  __syncthreads();
+  // tree-fold the ty rows that share a channel vector
+  for (int half = gm.ty_count >> 1; half > 0; half >>= 1) {
+    if (ty < half) {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) red[threadIdx.x][i] += red[threadIdx.x + half * gm.tx_count][i];
+    }
+    __syncthreads();
+  }
+  // deterministic: one partial row per block, folded later by fold_partials / bn_finalize
+  if (ty == 0 && tx < gm.vpr) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      prow[tx * 8 + i] = red[threadIdx.x][i];
+      if (!ONLY_S0) prow[C + tx * 8 + i] = red[threadIdx.x][8 + i];
+    }
+  }
+}
+
+// ReLU mask of 8 channels packed as one byte (bit i: channel 8*tx + i, set where the activated output is > 0).  A row of
+// C channels is C/8 bytes, so the bytes of channels 32w .. 32w+31 form the little-endian uint32 word w of the
+// [rows][C/32] mask that bn_apply writes and the data-gradient GEMM epilogue reads (EPI_MASK_BITS).
+__device__ __forceinline__ float mask_bit(uint32_t m, int i) { return ((m >> i) & 1u) ? 1.f : 0.f; }
+
 // MODE 0: sum x, sum x^2 (BN forward statistics)
 // MODE 1: g = dout*act'(.); sum g, sum g*xhat (BN backward reductions)
 // MODE 2: sum x only (bias gradients)
-// Activation mask source for MODE 1: `b` (activated output) when non-null, else recomputed
-// from y with scale/shift `ss` (out = act(y*scale+shift) has the sign of y*scale+shift).
+// Activation mask source for MODE 1: `b` (activated output) when non-null, else the packed ReLU mask `bits` when
+// non-null, else recomputed from y with scale/shift `ss` (out = act(y*scale+shift) has the sign of y*scale+shift).
 template <int MODE, int UNR>
 __global__ void __launch_bounds__(kThreads, 2)
-colreduce_kernel(const void* __restrict__ a, const void* __restrict__ b, const void* __restrict__ y,
-                 const float* __restrict__ saved, const float* __restrict__ ss, float* __restrict__ out,
-                 long long rows, int C, SlabGeom gm, int act) {
+colreduce_kernel(const void* __restrict__ a, const void* __restrict__ b, const uint8_t* __restrict__ bits,
+                 const void* __restrict__ y, const float* __restrict__ saved, const float* __restrict__ ss,
+                 float* __restrict__ out, long long rows, int C, SlabGeom gm, int act) {
   __shared__ float red[kThreads][17];
   const int vpr = gm.vpr;
   const int tx = threadIdx.x % gm.tx_count;
@@ -103,7 +138,8 @@ colreduce_kernel(const void* __restrict__ a, const void* __restrict__ b, const v
   if (r1 > rows) r1 = rows;
   if (tx < vpr) {
     float mean[8], rstd[8], sc[8], sh[8];
-    const bool recompute_mask = (MODE == 1) && act != 0 && b == nullptr;
+    const bool use_bits = (MODE == 1) && act != 0 && b == nullptr && bits != nullptr;
+    const bool recompute_mask = (MODE == 1) && act != 0 && b == nullptr && bits == nullptr;
     if (MODE == 1) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -115,6 +151,7 @@ colreduce_kernel(const void* __restrict__ a, const void* __restrict__ b, const v
     }
     for (long long r = r0 + ty; r < r1; r += (long long)ty_count * UNR) {
       V8 va[UNR], vb[UNR], vy[UNR];
+      uint32_t mb[UNR];
       bool ok[UNR];
 #pragma unroll
       for (int u = 0; u < UNR; ++u) {
@@ -125,7 +162,8 @@ colreduce_kernel(const void* __restrict__ a, const void* __restrict__ b, const v
           va[u] = ldg8(a, vi);
           if (MODE == 1) {
             vy[u] = ldg8(y, vi);
-            if (act != 0 && !recompute_mask) vb[u] = ldg8(b, vi);
+            if (use_bits) mb[u] = __ldg(bits + vi);
+            else if (act != 0 && !recompute_mask) vb[u] = ldg8(b, vi);
           }
         }
       }
@@ -150,6 +188,9 @@ colreduce_kernel(const void* __restrict__ a, const void* __restrict__ b, const v
             if (recompute_mask) {
 #pragma unroll
               for (int i = 0; i < 8; ++i) fa[i] *= act_grad(fy[i] * sc[i] + sh[i], act);
+            } else if (use_bits) {
+#pragma unroll
+              for (int i = 0; i < 8; ++i) fa[i] *= mask_bit(mb[u], i);
             } else {
               float fo[8];
               unpack8(vb[u], fo);
@@ -166,29 +207,80 @@ colreduce_kernel(const void* __restrict__ a, const void* __restrict__ b, const v
       }
     }
   }
+  fold_slab<MODE == 2>(red, s0, s1, tx, ty, gm, out + (long long)blockIdx.x * (MODE == 2 ? C : 2 * C), C);
+}
+
+// Backward reductions of two BatchNorms that share the gradient g and the row geometry (bn3 and the downsample BN of a
+// residual block: both normalise what is summed into the block output).  g is read once; each BatchNorm gets exactly
+// the partial rows colreduce_kernel<1> would write for it: BatchNorm A in out[blk][0 .. 2C), B in out[blk][2C .. 4C).
+// `bits`: ReLU mask applied to g (null: g arrives masked).
+__global__ void __launch_bounds__(kThreads, 2)
+colreduce2_kernel(const void* __restrict__ g, const uint8_t* __restrict__ bits, const void* __restrict__ ya,
+                  const void* __restrict__ yb, const float* __restrict__ saved_a, const float* __restrict__ saved_b,
+                  float* __restrict__ out, long long rows, int C, SlabGeom gm) {
+  // Two rows per pass instead of colreduce_kernel<1>'s four keeps the four accumulator sets in registers.  A thread still
+  // sums rows ty, ty + ty_count, ... in ascending order: the order depends on the slab geometry only.
+  constexpr int UNR = 2;
+  __shared__ float red[kThreads][17];
+  const int vpr = gm.vpr;
+  const int tx = threadIdx.x % gm.tx_count;
+  const int ty = threadIdx.x / gm.tx_count;
+  const int ty_count = gm.ty_count;
+  float sa0[8], sa1[8], sb0[8], sb1[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    red[threadIdx.x][i] = s0[i];
-    red[threadIdx.x][8 + i] = s1[i];
-  }
-  __syncthreads();
-  // tree-fold the ty rows that share a channel vector
-  for (int half = ty_count >> 1; half > 0; half >>= 1) {
-    if (ty < half) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) red[threadIdx.x][i] += red[threadIdx.x + half * gm.tx_count][i];
-    }
-    __syncthreads();
-  }
-  // deterministic: one partial row per block, folded later by fold_partials / bn_finalize
-  if (ty == 0 && tx < vpr) {
-    float* prow = out + (long long)blockIdx.x * (MODE == 2 ? C : 2 * C);
+  for (int i = 0; i < 8; ++i) sa0[i] = sa1[i] = sb0[i] = sb1[i] = 0.f;
+  const long long r0 = (long long)blockIdx.x * gm.rows_per_block;
+  long long r1 = r0 + gm.rows_per_block;
+  if (r1 > rows) r1 = rows;
+  if (tx < vpr) {
+    float ma[8], ra[8], mbn[8], rb[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      prow[tx * 8 + i] = red[threadIdx.x][i];
-      if (MODE != 2) prow[C + tx * 8 + i] = red[threadIdx.x][8 + i];
+      ma[i] = saved_a[tx * 8 + i];
+      ra[i] = saved_a[C + tx * 8 + i];
+      mbn[i] = saved_b[tx * 8 + i];
+      rb[i] = saved_b[C + tx * 8 + i];
+    }
+    for (long long r = r0 + ty; r < r1; r += (long long)ty_count * UNR) {
+      V8 vg[UNR], va[UNR], vb[UNR];
+      uint32_t mk[UNR];
+      bool ok[UNR];
+#pragma unroll
+      for (int u = 0; u < UNR; ++u) {
+        const long long rr = r + (long long)u * ty_count;
+        ok[u] = rr < r1;
+        if (ok[u]) {
+          const long long vi = rr * vpr + tx;
+          vg[u] = ldg8(g, vi);
+          va[u] = ldg8(ya, vi);
+          vb[u] = ldg8(yb, vi);
+          if (bits) mk[u] = __ldg(bits + vi);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < UNR; ++u) {
+        if (!ok[u]) continue;
+        float fg[8], fa[8], fb[8];
+        unpack8(vg[u], fg);
+        unpack8(va[u], fa);
+        unpack8(vb[u], fb);
+        if (bits) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) fg[i] *= mask_bit(mk[u], i);
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          sa0[i] += fg[i];
+          sa1[i] += fg[i] * (fa[i] - ma[i]) * ra[i];
+          sb0[i] += fg[i];
+          sb1[i] += fg[i] * (fb[i] - mbn[i]) * rb[i];
+        }
+      }
     }
   }
+  float* const prow = out + (long long)blockIdx.x * 4 * C;
+  fold_slab<false>(red, sa0, sa1, tx, ty, gm, prow, C);
+  fold_slab<false>(red, sb0, sb1, tx, ty, gm, prow + 2 * C, C);
 }
 
 // out[j] (+)= sum_b partial[b][j]: 8 columns x 32 row groups per block (the <= 264 partial rows are
@@ -237,11 +329,13 @@ bool slab_geom(long long rows, int C, int unroll, SlabGeom* g, int* blocks, int 
 // Writes `*nblk` partial rows into `partials` ([kMaxPartials][2C] or [..][C] for MODE 2).
 template <int MODE>
 int launch_colreduce(const void* a, const void* b, const void* y, const float* saved, const float* ss,
-                     float* partials, long long rows, int C, int act, int* nblk, cudaStream_t st) {
+                     float* partials, long long rows, int C, int act, int* nblk, cudaStream_t st,
+                     const uint32_t* bits = nullptr) {
   SlabGeom g;
   constexpr int UNR = MODE == 1 ? 4 : 8;  // independent 16-byte loads in flight per tensor per thread
   if (!slab_geom(rows, C, UNR, &g, nblk, kMaxPartials)) return 1;
-  colreduce_kernel<MODE, UNR><<<*nblk, kThreads, 0, st>>>(a, b, y, saved, ss, partials, rows, C, g, act);
+  colreduce_kernel<MODE, UNR><<<*nblk, kThreads, 0, st>>>(a, b, reinterpret_cast<const uint8_t*>(bits), y, saved, ss,
+                                                         partials, rows, C, g, act);
   return check_launch("colreduce_kernel");
 }
 int partial_rows(long long rows, int C) {  // must mirror launch_colreduce<0>
@@ -312,8 +406,8 @@ __global__ void bn_finalize_kernel(const float* __restrict__ partials, int nblk,
 template <bool HAS_RES, bool RES_BN>
 __global__ void __launch_bounds__(kThreads, 2)
 bn_apply_kernel(const void* __restrict__ y, const float* __restrict__ ss, const void* __restrict__ res,
-                const float* __restrict__ rss, void* __restrict__ out, long long rows, int C, SlabGeom gm,
-                int act) {
+                const float* __restrict__ rss, void* __restrict__ out, uint8_t* __restrict__ mask, long long rows, int C,
+                SlabGeom gm, int act) {
   const int vpr = gm.vpr;
   const int tx = threadIdx.x % gm.tx_count;
   const int ty = threadIdx.x / gm.tx_count;
@@ -363,25 +457,26 @@ bn_apply_kernel(const void* __restrict__ y, const float* __restrict__ ss, const 
 #pragma unroll
         for (int i = 0; i < 8; ++i) f[i] = act_apply(f[i], act);
       }
-      stg8(out, (r + (long long)u * gm.ty_count) * vpr + tx, pack8(f));
+      const long long vi = (r + (long long)u * gm.ty_count) * vpr + tx;
+      const V8 o = pack8(f);
+      stg8(out, vi, o);
+      if (mask) {   // from the stored bf16 values, so that the mask is exactly (out > 0)
+        float fo[8];
+        unpack8(o, fo);
+        uint32_t m = 0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) m |= (fo[i] > 0.f ? 1u : 0u) << i;
+        mask[vi] = (uint8_t)m;
+      }
     }
   }
 }
 
 // ----------------------------------------------------------------------------- BN backward apply
 // dy = gamma*rstd*(g - sum_g/rows - xhat*sum_gx/rows) = A*g + B*y + K per channel
-template <bool HAS_OUT, bool HAS_DRES>
-__global__ void __launch_bounds__(kThreads, 2)
-bn_bwd_apply_kernel(const void* __restrict__ dout, const void* __restrict__ out, const void* __restrict__ y,
-                    const float* __restrict__ saved, const float* __restrict__ gamma,
-                    const float* __restrict__ sums, const float* __restrict__ ss, void* __restrict__ dy,
-                    void* __restrict__ dres, long long rows, int C, SlabGeom gm, int act, float inv_rows) {
-  const int vpr = gm.vpr;
-  const int tx = threadIdx.x % gm.tx_count;
-  const int ty = threadIdx.x / gm.tx_count;
-  if (tx >= vpr) return;
-  float A[8], B[8], K[8], sc[8], sh[8];
-  const bool recompute_mask = !HAS_OUT && act != 0;
+__device__ __forceinline__ void bwd_apply_coefs(const float* __restrict__ saved, const float* __restrict__ gamma,
+                                                const float* __restrict__ sums, int tx, int C, float inv_rows,
+                                                float (&A)[8], float (&B)[8], float (&K)[8]) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int c = tx * 8 + i;
@@ -391,14 +486,35 @@ bn_bwd_apply_kernel(const void* __restrict__ dout, const void* __restrict__ out,
     A[i] = k1;
     B[i] = -k1 * k3 * rstd;
     K[i] = -k1 * k2 + k1 * k3 * rstd * mean;
-    sc[i] = recompute_mask ? ss[c] : 0.f;
-    sh[i] = recompute_mask ? ss[C + c] : 0.f;
+  }
+}
+
+// Mask source as in colreduce_kernel<1>: `out` (HAS_OUT), else `bits` when non-null, else recomputed from y.
+template <bool HAS_OUT, bool HAS_DRES>
+__global__ void __launch_bounds__(kThreads, 2)
+bn_bwd_apply_kernel(const void* __restrict__ dout, const void* __restrict__ out, const uint8_t* __restrict__ bits,
+                    const void* __restrict__ y, const float* __restrict__ saved, const float* __restrict__ gamma,
+                    const float* __restrict__ sums, const float* __restrict__ ss, void* __restrict__ dy,
+                    void* __restrict__ dres, long long rows, int C, SlabGeom gm, int act, float inv_rows) {
+  const int vpr = gm.vpr;
+  const int tx = threadIdx.x % gm.tx_count;
+  const int ty = threadIdx.x / gm.tx_count;
+  if (tx >= vpr) return;
+  float A[8], B[8], K[8], sc[8], sh[8];
+  const bool use_bits = !HAS_OUT && act != 0 && bits != nullptr;
+  const bool recompute_mask = !HAS_OUT && act != 0 && bits == nullptr;
+  bwd_apply_coefs(saved, gamma, sums, tx, C, inv_rows, A, B, K);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    sc[i] = recompute_mask ? ss[tx * 8 + i] : 0.f;
+    sh[i] = recompute_mask ? ss[C + tx * 8 + i] : 0.f;
   }
   const long long r0 = (long long)blockIdx.x * gm.rows_per_block;
   long long r1 = r0 + gm.rows_per_block;
   if (r1 > rows) r1 = rows;
   for (long long r = r0 + ty; r < r1; r += (long long)gm.ty_count * UNROLL) {
     V8 vg[UNROLL], vo[UNROLL], vy[UNROLL];
+    uint32_t mb[UNROLL];
     bool ok[UNROLL];
 #pragma unroll
     for (int u = 0; u < UNROLL; ++u) {
@@ -409,6 +525,7 @@ bn_bwd_apply_kernel(const void* __restrict__ dout, const void* __restrict__ out,
         vg[u] = ldg8(dout, vi);
         vy[u] = ldg8(y, vi);
         if (HAS_OUT) vo[u] = ldg8(out, vi);
+        else if (use_bits) mb[u] = __ldg(bits + vi);
       }
     }
 #pragma unroll
@@ -423,6 +540,9 @@ bn_bwd_apply_kernel(const void* __restrict__ dout, const void* __restrict__ out,
         unpack8(vo[u], fo);
 #pragma unroll
         for (int i = 0; i < 8; ++i) g[i] *= act_grad(fo[i], act);
+      } else if (use_bits) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) g[i] *= mask_bit(mb[u], i);
       } else if (act != 0) {
 #pragma unroll
         for (int i = 0; i < 8; ++i) g[i] *= act_grad(fy[i] * sc[i] + sh[i], act);
@@ -432,6 +552,61 @@ bn_bwd_apply_kernel(const void* __restrict__ dout, const void* __restrict__ out,
 #pragma unroll
       for (int i = 0; i < 8; ++i) d[i] = A[i] * g[i] + B[i] * fy[i] + K[i];
       stg8(dy, vi, pack8(d));
+    }
+  }
+}
+
+// bn_bwd_apply_kernel for the two BatchNorms of colreduce2_kernel: dya / dyb from one read of g.  sums: [4][C] as
+// folded from colreduce2_kernel's partial rows (A: sums[0..2C), B: sums[2C..4C)).
+__global__ void __launch_bounds__(kThreads, 2)
+bn_bwd_apply2_kernel(const void* __restrict__ g, const uint8_t* __restrict__ bits, const void* __restrict__ ya,
+                     const void* __restrict__ yb, const float* __restrict__ saved_a, const float* __restrict__ saved_b,
+                     const float* __restrict__ gamma_a, const float* __restrict__ gamma_b, const float* __restrict__ sums,
+                     void* __restrict__ dya, void* __restrict__ dyb, long long rows, int C, SlabGeom gm, float inv_rows) {
+  const int vpr = gm.vpr;
+  const int tx = threadIdx.x % gm.tx_count;
+  const int ty = threadIdx.x / gm.tx_count;
+  if (tx >= vpr) return;
+  float Aa[8], Ba[8], Ka[8], Ab[8], Bb[8], Kb[8];
+  bwd_apply_coefs(saved_a, gamma_a, sums, tx, C, inv_rows, Aa, Ba, Ka);
+  bwd_apply_coefs(saved_b, gamma_b, sums + 2 * C, tx, C, inv_rows, Ab, Bb, Kb);
+  const long long r0 = (long long)blockIdx.x * gm.rows_per_block;
+  long long r1 = r0 + gm.rows_per_block;
+  if (r1 > rows) r1 = rows;
+  for (long long r = r0 + ty; r < r1; r += (long long)gm.ty_count * UNROLL) {
+    V8 vg[UNROLL], va[UNROLL], vb[UNROLL];
+    uint32_t mk[UNROLL];
+    bool ok[UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const long long rr = r + (long long)u * gm.ty_count;
+      ok[u] = rr < r1;
+      if (ok[u]) {
+        const long long vi = rr * vpr + tx;
+        vg[u] = ldg8(g, vi);
+        va[u] = ldg8(ya, vi);
+        vb[u] = ldg8(yb, vi);
+        if (bits) mk[u] = __ldg(bits + vi);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      if (!ok[u]) continue;
+      const long long vi = (r + (long long)u * gm.ty_count) * vpr + tx;
+      float fg[8], fa[8], fb[8], d[8];
+      unpack8(vg[u], fg);
+      unpack8(va[u], fa);
+      unpack8(vb[u], fb);
+      if (bits) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) fg[i] *= mask_bit(mk[u], i);
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) d[i] = Aa[i] * fg[i] + Ba[i] * fa[i] + Ka[i];
+      stg8(dya, vi, pack8(d));
+#pragma unroll
+      for (int i = 0; i < 8; ++i) d[i] = Ab[i] * fg[i] + Bb[i] * fb[i] + Kb[i];
+      stg8(dyb, vi, pack8(d));
     }
   }
 }
@@ -853,42 +1028,52 @@ int saicv_bn_finalize(const float* partials, int partial_rows_, const float* gam
 }
 
 int saicv_bn_apply(const void* y, const float* scale_shift, const void* res, const float* res_scale_shift,
-                   void* out, long long rows, int c, int act, void* stream) {
+                   void* out, uint32_t* mask_bits, long long rows, int c, int act, void* stream) {
+  if (mask_bits && (c % 32 || (act & 7) != 1))
+    return set_error("saicv_bn_apply: mask_bits needs c %% 32 == 0 and a ReLU (c=%d act=%d)", c, act);
   SlabGeom g;
   int blocks;
   if (!slab_geom(rows, c, UNROLL, &g, &blocks)) return 1;
+  uint8_t* mask = reinterpret_cast<uint8_t*>(mask_bits);
   if (res == nullptr)
-    bn_apply_kernel<false, false><<<blocks, kThreads, 0, ST>>>(y, scale_shift, res, res_scale_shift, out, rows, c, g, act);
+    bn_apply_kernel<false, false><<<blocks, kThreads, 0, ST>>>(y, scale_shift, res, res_scale_shift, out, mask, rows, c, g, act);
   else if (res_scale_shift == nullptr)
-    bn_apply_kernel<true, false><<<blocks, kThreads, 0, ST>>>(y, scale_shift, res, res_scale_shift, out, rows, c, g, act);
+    bn_apply_kernel<true, false><<<blocks, kThreads, 0, ST>>>(y, scale_shift, res, res_scale_shift, out, mask, rows, c, g, act);
   else
-    bn_apply_kernel<true, true><<<blocks, kThreads, 0, ST>>>(y, scale_shift, res, res_scale_shift, out, rows, c, g, act);
+    bn_apply_kernel<true, true><<<blocks, kThreads, 0, ST>>>(y, scale_shift, res, res_scale_shift, out, mask, rows, c, g, act);
   return check_launch("bn_apply_kernel");
 }
 
-int saicv_bn_bwd_reduce(const void* dout, const void* out, const void* y, const float* saved,
+// the activation-mask source of the backward kernels: `out`, the packed ReLU mask `bits`, or recomputed from y
+static int check_mask_source(const char* fn, const void* out, const uint32_t* bits, const float* scale_shift, int c,
+                             int act) {
+  if (act != 0 && out == nullptr && bits == nullptr && scale_shift == nullptr)
+    return set_error("%s: need the activated output, mask bits or scale_shift to form the activation mask", fn);
+  if ((act & 7) == 3 && out != nullptr) return set_error("%s: SiLU needs the recompute path (out == NULL, scale_shift given)", fn);
+  if (bits != nullptr && (act != 1 || c % 32)) return set_error("%s: mask bits need act == 1 (ReLU) and c %% 32 == 0 (c=%d)", fn, c);
+  return 0;
+}
+
+int saicv_bn_bwd_reduce(const void* dout, const void* out, const uint32_t* bits, const void* y, const float* saved,
                         const float* scale_shift, float* partials, float* sums, long long rows, int c, int act,
                         void* stream) {
-  if (act != 0 && out == nullptr && scale_shift == nullptr)
-    return set_error("saicv_bn_bwd_reduce: need the activated output or scale_shift to form the activation mask");
-  if ((act & 7) == 3 && out != nullptr) return set_error("saicv_bn_bwd_reduce: SiLU needs the recompute path (out == NULL, scale_shift given)");
+  if (int e = check_mask_source("saicv_bn_bwd_reduce", out, bits, scale_shift, c, act)) return e;
   int nblk;
-  if (int e = launch_colreduce<1>(dout, out, y, saved, scale_shift, partials, rows, c, act, &nblk, ST)) return e;
+  if (int e = launch_colreduce<1>(dout, out, y, saved, scale_shift, partials, rows, c, act, &nblk, ST, bits)) return e;
   return fold(partials, sums, nblk, 2 * c, 0, ST);
 }
 
-int saicv_bn_bwd_apply(const void* dout, const void* out, const void* y, const float* saved, const float* gamma,
-                       const float* scale_shift, float* sums, void* dy, void* dres, float* dgamma, float* dbeta,
-                       long long rows, int c, int act, int accumulate, void* stream) {
-  if (act != 0 && out == nullptr && scale_shift == nullptr)
-    return set_error("saicv_bn_bwd_apply: need the activated output or scale_shift to form the activation mask");
-  if ((act & 7) == 3 && out != nullptr) return set_error("saicv_bn_bwd_apply: SiLU needs the recompute path (out == NULL, scale_shift given)");
+int saicv_bn_bwd_apply(const void* dout, const void* out, const uint32_t* bits, const void* y, const float* saved,
+                       const float* gamma, const float* scale_shift, float* sums, void* dy, void* dres, float* dgamma,
+                       float* dbeta, long long rows, int c, int act, int accumulate, void* stream) {
+  if (int e = check_mask_source("saicv_bn_bwd_apply", out, bits, scale_shift, c, act)) return e;
   SlabGeom g;
   int blocks;
   if (!slab_geom(rows, c, UNROLL, &g, &blocks)) return 1;
   const float inv_rows = 1.0f / (float)rows;
+  const uint8_t* mask = reinterpret_cast<const uint8_t*>(bits);
 #define BWD_APPLY(HO, HD) \
-  bn_bwd_apply_kernel<HO, HD><<<blocks, kThreads, 0, ST>>>(dout, out, y, saved, gamma, sums, scale_shift, dy, dres, rows, c, g, act, inv_rows)
+  bn_bwd_apply_kernel<HO, HD><<<blocks, kThreads, 0, ST>>>(dout, out, mask, y, saved, gamma, sums, scale_shift, dy, dres, rows, c, g, act, inv_rows)
   if (out != nullptr && act != 0) {
     if (dres) BWD_APPLY(true, true); else BWD_APPLY(true, false);
   } else {
@@ -897,6 +1082,36 @@ int saicv_bn_bwd_apply(const void* dout, const void* out, const void* y, const f
 #undef BWD_APPLY
   if (int e = check_launch("bn_bwd_apply_kernel")) return e;
   bn_param_grad_kernel<<<(c + 127) / 128, 128, 0, ST>>>(sums, dgamma, dbeta, c, accumulate);
+  return check_launch("bn_param_grad_kernel");
+}
+
+int saicv_bn_bwd_reduce2(const void* g, const uint32_t* bits, const void* y_a, const void* y_b, const float* saved_a,
+                         const float* saved_b, float* partials, float* sums, long long rows, int c, void* stream) {
+  if (bits != nullptr && c % 32) return set_error("saicv_bn_bwd_reduce2: mask bits need c %% 32 == 0 (c=%d)", c);
+  SlabGeom gm;
+  int nblk;
+  if (!slab_geom(rows, c, 4, &gm, &nblk, kMaxPartials)) return 1;   // the geometry of launch_colreduce<1>
+  colreduce2_kernel<<<nblk, kThreads, 0, ST>>>(g, reinterpret_cast<const uint8_t*>(bits), y_a, y_b, saved_a, saved_b,
+                                               partials, rows, c, gm);
+  if (int e = check_launch("colreduce2_kernel")) return e;
+  return fold(partials, sums, nblk, 4 * c, 0, ST);
+}
+
+int saicv_bn_bwd_apply2(const void* g, const uint32_t* bits, const void* y_a, const void* y_b, const float* saved_a,
+                        const float* saved_b, const float* gamma_a, const float* gamma_b, const float* sums, void* dy_a,
+                        void* dy_b, float* dgamma_a, float* dbeta_a, float* dgamma_b, float* dbeta_b, long long rows,
+                        int c, int accumulate_a, int accumulate_b, void* stream) {
+  if (bits != nullptr && c % 32) return set_error("saicv_bn_bwd_apply2: mask bits need c %% 32 == 0 (c=%d)", c);
+  SlabGeom gm;
+  int blocks;
+  if (!slab_geom(rows, c, UNROLL, &gm, &blocks)) return 1;
+  bn_bwd_apply2_kernel<<<blocks, kThreads, 0, ST>>>(g, reinterpret_cast<const uint8_t*>(bits), y_a, y_b, saved_a,
+                                                    saved_b, gamma_a, gamma_b, sums, dy_a, dy_b, rows, c, gm,
+                                                    1.0f / (float)rows);
+  if (int e = check_launch("bn_bwd_apply2_kernel")) return e;
+  bn_param_grad_kernel<<<(c + 127) / 128, 128, 0, ST>>>(sums, dgamma_a, dbeta_a, c, accumulate_a);
+  if (int e = check_launch("bn_param_grad_kernel")) return e;
+  bn_param_grad_kernel<<<(c + 127) / 128, 128, 0, ST>>>(sums + 2 * c, dgamma_b, dbeta_b, c, accumulate_b);
   return check_launch("bn_param_grad_kernel");
 }
 
@@ -1037,8 +1252,8 @@ int saicv_colsum(const void* x, float* partials, float* out, long long rows, int
     int nblk;
     if (!slab_geom(rows, cw, 8, &g, &nblk, kMaxPartials)) return 1;
     g.ldv = c / 8;
-    colreduce_kernel<2, 8><<<nblk, kThreads, 0, ST>>>(reinterpret_cast<const __nv_bfloat16*>(x) + c0, nullptr, nullptr, nullptr,
-                                                   nullptr, partials, rows, cw, g, 0);
+    colreduce_kernel<2, 8><<<nblk, kThreads, 0, ST>>>(reinterpret_cast<const __nv_bfloat16*>(x) + c0, nullptr, nullptr,
+                                                   nullptr, nullptr, nullptr, partials, rows, cw, g, 0);
     if (int e = check_launch("colreduce_kernel")) return e;
     if (int e = fold(partials, out + c0, nblk, cw, accumulate, ST)) return e;
   }

@@ -221,6 +221,8 @@ int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorM
       var = ((p.epi_flags & EPI_STATS) && !getenv("SAICV_GEMM_INLINE_STATS")) ? VAR_STATS_BF16 : VAR_PLAIN_BF16;
     else if (!p.aux_tma && p.out_f32 && !(p.epi_flags & ~GemmVariant<VAR_PLAIN_F32>::kMask)) var = VAR_PLAIN_F32;
   }
+  if ((p.epi_flags & EPI_MASK_BITS) && var != VAR_AUX)
+    return set_error("EPI_MASK_BITS needs the TMA aux-operand epilogue (VAR_AUX): bf16 `add` operand, one split, no overrides");
 #define SAICV_LAUNCH_BN(BN_)                                                         \
   switch (var) {                                                                     \
     case VAR_PLAIN_BF16: return launch<BN_, VAR_PLAIN_BF16>(a, b, d, r, p, st);      \
@@ -369,7 +371,7 @@ int saicv_conv_fprop(const void* x, const void* w, float* stats_partial, void* y
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream);
 }
 
-int saicv_conv_dgrad(const void* dy, const void* w, const void* add, void* dx,
+int saicv_conv_dgrad(const void* dy, const void* w, const void* add, const uint32_t* mask_bits, void* dx,
                      const saicv_conv_shape* cs, void* stream) {
   if (!ensure_init()) return 1;
   if (cs->c % 64 || cs->k % 64 || !aligned16(dy) || !aligned16(w) || !aligned16(dx))
@@ -389,8 +391,10 @@ int saicv_conv_dgrad(const void* dy, const void* w, const void* add, void* dx,
   p.a_mode = A_IM2COL; p.b_mode = B_MN2D; p.flip_taps = 1; p.b_cin = cs->c;
   p.g.P = cs->h; p.g.Q = cs->w; p.g.stride = 1; p.g.lc_h = lc_h; p.g.lc_w = lc_w;
   p.g.R = cs->r; p.g.S = cs->s; p.g.cchunks = cs->k / 64; p.g.n_img = cs->n;
-  p.epi_flags = add ? EPI_RESID_BF16 : 0; p.resid_bf16 = add; p.out_f32 = 0; p.out = dx; p.ldd = cs->c;
+  p.epi_flags = (add ? EPI_RESID_BF16 : 0) | (mask_bits ? EPI_MASK_BITS : 0);
+  p.resid_bf16 = add; p.mask_bits = mask_bits; p.out_f32 = 0; p.out = dx; p.ldd = cs->c;
   if (add && !aligned16(add)) return set_error("saicv_conv_dgrad: unaligned `add`");
+  if (mask_bits && !add) return set_error("saicv_conv_dgrad: mask_bits is applied in the epilogue of the fused `add` only");
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream, add, false);
 }
 

@@ -26,7 +26,7 @@ namespace saicv {
 enum : int { A_K2D = 0, A_IM2COL = 1, A_MN2D = 2 };
 enum : int { B_K2D = 0, B_MN2D = 2, B_IM2COL = 3 };
 enum : int { EPI_BIAS = 1, EPI_RELU = 2, EPI_GELU = 4, EPI_DIRECT = 8, EPI_RESID = 16, EPI_RESID_BF16 = 32,
-              EPI_MUL_DGELU = 64, EPI_ROW_SCALE = 128, EPI_STATS = 256, EPI_MUL_DRELU = 512 };
+              EPI_MUL_DGELU = 64, EPI_ROW_SCALE = 128, EPI_STATS = 256, EPI_MUL_DRELU = 512, EPI_MASK_BITS = 1024 };
 
 constexpr int BM = 128;
 constexpr int BK = 64;
@@ -88,16 +88,18 @@ struct GemmParams {
                        // output's element width and is brought in by TMA (tensor map tmR) INTO the staging
                        // slice, combined in place and stored from there; 0: per-thread global loads
   float* stats_partial;  // EPI_STATS: [gridDim.x][2][N] per-CTA column sums / sums of squares of the bf16 output
+  const uint32_t* mask_bits;  // EPI_MASK_BITS: [M][N/32] ReLU mask (bit j of word w: column 32w + j); applied last as D *= bit
 };
 
 // Kernel variants: the epilogue's feature set is a compile-time mask, so that the common launches run a compact
 // instruction stream (with every feature a run-time branch, branch resolution and instruction fetch take a large share of
 // the issue slots of the short-reduction launches, whose pace the epilogue sets).  VAR_FULL and VAR_AUX spill a few
 // hundred bytes at the 168-register cap of 384 threads (ptxas -v); the other variants do not spill.
-//   VAR_FULL        every flag / output type at run time (GELU forward, EPI_DIRECT, per-thread aux loads)
+//   VAR_FULL        every flag but EPI_MASK_BITS / output type at run time (GELU forward, EPI_DIRECT, per-thread aux loads)
 //   VAR_PLAIN_BF16  bf16 output, optional bias / ReLU / BatchNorm statistics       (conv fprop, plain dgrad, Linear)
 //   VAR_PLAIN_F32   fp32 output, optional bias                                       (split-K weight gradients, fp32 Linear)
-//   VAR_AUX         aux operand by TMA (fp32 residual, bf16 addend / ReLU mask / GELU pre-activation), bias, row scale
+//   VAR_AUX         aux operand by TMA (fp32 residual, bf16 addend / ReLU mask / GELU pre-activation), bias, row scale,
+//                   1-bit ReLU mask (conv dgrad + shortcut gradient, masked by the previous residual block's output ReLU)
 //   VAR_STATS_BF16  VAR_PLAIN_BF16 with the BatchNorm statistics taken by FOUR EXTRA WARPS (512 threads): the column sums of
 //                   a staged slice cost ~2.8x the work of staging it (instruction count), so they are taken off the
 //                   epilogue warps.  The stats warps read the slice from shared memory while the epilogue
@@ -105,10 +107,11 @@ struct GemmParams {
 enum : int { VAR_FULL = 0, VAR_PLAIN_BF16 = 1, VAR_PLAIN_F32 = 2, VAR_AUX = 3, VAR_STATS_BF16 = 4 };
 template <int VAR>
 struct GemmVariant {
-  static constexpr int kMask = VAR == VAR_FULL ? 0x7fffffff
+  static constexpr int kMask = VAR == VAR_FULL ? (0x7fffffff & ~EPI_MASK_BITS)
                                : (VAR == VAR_PLAIN_BF16 || VAR == VAR_STATS_BF16) ? (EPI_BIAS | EPI_RELU | EPI_STATS)
                                : VAR == VAR_PLAIN_F32 ? EPI_BIAS
-                               : (EPI_BIAS | EPI_ROW_SCALE | EPI_RESID | EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU);
+                               : (EPI_BIAS | EPI_ROW_SCALE | EPI_RESID | EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU |
+                                  EPI_MASK_BITS);
   static constexpr int kOut = (VAR == VAR_PLAIN_BF16 || VAR == VAR_STATS_BF16) ? 1 : VAR == VAR_PLAIN_F32 ? 2 : 0;   // 0: run time, 1: bf16, 2: fp32
   static constexpr int kAux = VAR == VAR_FULL ? 0 : VAR == VAR_AUX ? 2 : 1;                // 0: run time, 1: never, 2: always by TMA
   static constexpr bool kStatsWarps = VAR == VAR_STATS_BF16;                               // statistics by warps 12..15
@@ -390,6 +393,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const bool has_rb = (flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU)) && row < p.M;
         float rscale = 1.f;
         if ((flags & EPI_ROW_SCALE) && row < p.M) rscale = __ldg(p.row_scale + row / p.rows_per_scale);
+        uint32_t mbits = 0u;   // the mask word of this thread's row and 32 columns
+        if ((flags & EPI_MASK_BITS) && row < p.M && col0 < p.N) mbits = __ldg(p.mask_bits + row * (p.N >> 5) + (col0 >> 5));
         if (!aux_tma) {
           if (has_rf) {
             const float4* rp = reinterpret_cast<const float4*>(p.resid + row * p.ldd + col0);
@@ -477,6 +482,11 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               }
             }
           }
+        }
+        if (flags & EPI_MASK_BITS) {
+          // a multiply by 0 / 1, not a select: the zeros keep the sign a later (bf16(D) * relu'(out)) would give them
+#pragma unroll
+          for (int j = 0; j < 32; ++j) f[j] *= ((mbits >> j) & 1u) ? 1.f : 0.f;
         }
         if (direct) {
           if (row < p.M) {

@@ -195,55 +195,81 @@ class ConvBN:
             ss[0, :self.k].copy_(scale)
             ss[1, :self.k].copy_(bn.bias.detach() - bn.running_mean * scale)
 
-    def forward(self, a_in, tape, training, res=None, res_ss=None):
+    def forward(self, a_in, tape, training, res=None, res_ss=None, want_mask=False):
         """conv -> BN -> (+res) -> act (or act then +res when res_after_act).  res_ss: BN scale/shift
-        applied to `res` on the fly (downsample branch)."""
+        applied to `res` on the fly (downsample branch).  want_mask: also keep the ReLU mask of the
+        output, packed to one bit per element, as tape['bits']."""
         y = self.conv_fwd(a_in, tape, want_stats=training and FUSE_BN_STATS)
         self.bn_prepare(y, training, tape)
         out = torch.empty_like(y)
         act = self.act | (8 if (self.res_after_act and res is not None) else 0)
-        ops.bn_apply(y, tape['ss'], out, act, res=res, res_scale_shift=res_ss)
+        bits = tape['bits'] = ops.mask_bits_like(y) if want_mask else None
+        ops.bn_apply(y, tape['ss'], out, act, res=res, res_scale_shift=res_ss, mask_bits=bits)
         tape['out'] = out
         return out
 
     # ---- backward
-    def bn_bwd(self, dout, tape, sink, act_out=None, want_dres=False, act=None):
-        """dout: gradient w.r.t. the activated output.  Returns (dy, dres).
-
-        The ReLU mask comes from `act_out` (block output, when a residual was added before the
-        activation) or, for plain conv->BN->act units, is recomputed inside the kernels from
-        sign(y*scale+shift), which saves reading the activated tensor twice."""
-        act = self.act if act is None else act
-        y = tape['y']
-        mask_src = act_out if act != ACT_NONE else None
-        ss = tape['ss'] if (act != ACT_NONE and mask_src is None) else None
-        saved = tape['saved']
-        ops.bn_bwd_reduce(dout, mask_src, y, saved, self.sums, act, scale_shift=ss)
-        dy = torch.empty_like(y)
-        dres = torch.empty_like(y) if want_dres else None
+    def _grad_targets(self, sink):
+        """(gamma, dgamma, dbeta, accumulate) for the BatchNorm backward kernels, and the sink buffers for _grad_done."""
         gbuf, gacc = sink.begin(self.bn.weight)
         bbuf, bacc = sink.begin(self.bn.bias)
         assert gacc == bacc
         if self.padded:
-            ops.bn_bwd_apply(dout, mask_src, y, saved, self.gamma_p, self.sums, dy, dres, self.dg_p, self.db_p,
-                             act, accumulate=False, scale_shift=ss)
-            if gacc:
+            return (self.gamma_p, self.dg_p, self.db_p, False), (gbuf, bbuf, gacc)
+        return (self.bn.weight.detach(), gbuf, bbuf, gacc), (gbuf, bbuf, gacc)
+
+    def _grad_done(self, sink, bufs):
+        gbuf, bbuf, acc = bufs
+        if self.padded:
+            if acc:
                 gbuf.add_(self.dg_p[:self.k])
                 bbuf.add_(self.db_p[:self.k])
             else:
                 gbuf.copy_(self.dg_p[:self.k])
                 bbuf.copy_(self.db_p[:self.k])
-        else:
-            ops.bn_bwd_apply(dout, mask_src, y, saved, self.bn.weight.detach(), self.sums, dy, dres,
-                             gbuf, bbuf, act, accumulate=gacc, scale_shift=ss)
         sink.done(self.bn.weight, gbuf)
         sink.done(self.bn.bias, bbuf)
+
+    def bn_bwd(self, dout, tape, sink, bits=None, want_dres=False, act=None):
+        """dout: gradient w.r.t. the activated output.  Returns (dy, dres).
+
+        The ReLU mask comes from `bits` (the packed mask of a block output, whose residual was added
+        before the activation) or, for plain conv->BN->act units, is recomputed inside the kernels from
+        sign(y*scale+shift), which saves reading the activated tensor twice."""
+        act = self.act if act is None else act
+        y = tape['y']
+        ss = tape['ss'] if (act != ACT_NONE and bits is None) else None
+        saved = tape['saved']
+        ops.bn_bwd_reduce(dout, None, y, saved, self.sums, act, scale_shift=ss, bits=bits)
+        dy = torch.empty_like(y)
+        dres = torch.empty_like(y) if want_dres else None
+        (gamma, dg, db, acc), bufs = self._grad_targets(sink)
+        ops.bn_bwd_apply(dout, None, y, saved, gamma, self.sums, dy, dres, dg, db, act, accumulate=acc,
+                         scale_shift=ss, bits=bits)
+        self._grad_done(sink, bufs)
         return dy, dres
 
-    def conv_bwd(self, dy, tape, sink, need_dx=True, add=None):
+    def bn_bwd_pair(self, other, g, tape, other_tape, sink, bits):
+        """bn_bwd of this unit and of `other` (same rows and channels, no activation of their own) over one gradient:
+        g = dout masked by `bits`, or g = dout when bits is None (it arrived masked).  One reduce and one apply read g
+        once for both.  Returns (dy, dy_other)."""
+        y, yo = tape['y'], other_tape['y']
+        sums = torch.empty(4, self.kp, device=y.device)
+        ops.bn_bwd_reduce2(g, bits, y, yo, tape['saved'], other_tape['saved'], sums)
+        dy, dyo = torch.empty_like(y), torch.empty_like(yo)
+        (ga, dga, dba, acca), bufs_a = self._grad_targets(sink)
+        (gb, dgb, dbb, accb), bufs_b = other._grad_targets(sink)
+        ops.bn_bwd_apply2(g, bits, y, yo, tape['saved'], other_tape['saved'], ga, gb, sums, dy, dyo, dga, dba, dgb, dbb,
+                          accumulate_a=acca, accumulate_b=accb)
+        self._grad_done(sink, bufs_a)
+        other._grad_done(sink, bufs_b)
+        return dy, dyo
+
+    def conv_bwd(self, dy, tape, sink, need_dx=True, add=None, mask_bits=None):
         """dy: gradient w.r.t. the raw conv output [n,P,Q,kp].  Returns the data gradient
-        (NHWC bf16, `add` fused in when given) or None.  A 1x1 stride-2 conv returns
-        ('strided', dd) with the compact gradient dd[n,P,Q,cp] that belongs at the even pixels."""
+        (NHWC bf16, `add` fused in when given, then multiplied by the ReLU mask `mask_bits` when
+        given) or None.  A 1x1 stride-2 conv returns ('strided', dd) with the compact gradient
+        dd[n,P,Q,cp] that belongs at the even pixels."""
         w = self.conv.weight
         wbuf, wacc = sink.begin(w)
         n, P, Q, _ = dy.shape
@@ -261,14 +287,14 @@ class ConvBN:
         if not need_dx:
             return None
         if self.stride == 1:
-            return ops.conv_dgrad(dy, self.op.w, cs, add=add)
+            return ops.conv_dgrad(dy, self.op.w, cs, add=add, mask_bits=mask_bits)
         assert self.stride == 2
         if self.r == 1:
-            assert add is None
+            assert add is None and mask_bits is None
             return 'strided', ops.linear_dgrad(dy.view(-1, self.kp), self.op.w).view(n, P, Q, self.cp)
         u = ops.zero_upsample2(dy, h, wd)
         cs1 = ops.make_conv_shape(n, h, wd, self.cp, self.kp, self.r, self.s, 1, self.pad)
-        return ops.conv_dgrad(u, self.op.w, cs1, add=add)
+        return ops.conv_dgrad(u, self.op.w, cs1, add=add, mask_bits=mask_bits)
 
 
 class ResidualBlockRT:
@@ -291,25 +317,45 @@ class ResidualBlockRT:
         for u, t in zip(self.units[:-1], tapes[:-1]):
             x = u.forward(x, t, training)
         last, tl = self.units[-1], tapes[-1]
+        # the ReLU mask of the block output, one bit per element: the backward applies it instead of reading `out`
         if self.down is not None:
             td = tape.setdefault('d', dict())
             yd = self.down.conv_fwd(a_in, td, want_stats=training and FUSE_BN_STATS)
             self.down.bn_prepare(yd, training, td)
-            out = last.forward(x, tl, training, res=yd, res_ss=td['ss'])
+            out = last.forward(x, tl, training, res=yd, res_ss=td['ss'], want_mask=training)
         else:
-            out = last.forward(x, tl, training, res=a_in)
+            out = last.forward(x, tl, training, res=a_in, want_mask=training)
         return out
 
+    @staticmethod
+    def out_mask(tape):
+        """The packed ReLU mask of the block output kept by forward(), or None (tape of a checkpointed block that has
+        not been re-run)."""
+        tapes = tape.get('u')
+        return tapes[-1].get('bits') if tapes else None
+
     def backward(self, dout, tape, sink):
+        """dout: gradient w.r.t. the block output.  Returns the gradient w.r.t. the block input."""
+        return self.backward_chain(dout, tape, sink)[0]
+
+    def backward_chain(self, dout, tape, sink, dout_masked=False, in_mask=None):
+        """backward() inside a chain of blocks.  dout_masked: dout is already multiplied by the ReLU mask of this block's
+        output (the next block applied it in its data-gradient epilogue).  in_mask: the packed ReLU mask of this block's
+        input (the previous block's output), applied to the input gradient in the epilogue of the data-gradient GEMM that
+        adds the shortcut gradient, when there is one.  Returns (dx, dx_masked): dx_masked tells whether in_mask was
+        applied to dx."""
         tapes = tape['u']
         last, tl = self.units[-1], tapes[-1]
-        out = tl['out']
-        # g = dout * relu'(out) flows to both the last BN and the shortcut
-        dy, g = last.bn_bwd(dout, tl, sink, act_out=out, want_dres=(self.down is None))
-        shortcut, strided = g, None
-        if self.down is not None:
+        # g = dout * relu'(out) flows to both the last BN and the shortcut; with dout_masked, dout is g
+        bits = None if dout_masked else tl['bits']
+        strided = None
+        if self.down is None:
+            dy, g = last.bn_bwd(dout, tl, sink, bits=bits, want_dres=not dout_masked,
+                                act=ACT_NONE if dout_masked else None)
+            shortcut = dout if dout_masked else g
+        else:
             td = tape['d']
-            dyd, _ = self.down.bn_bwd(dout, td, sink, act_out=out, act=ACT_RELU)
+            dy, dyd = last.bn_bwd_pair(self.down, dout, tl, td, sink, bits)
             shortcut = self.down.conv_bwd(dyd, td, sink)
             if isinstance(shortcut, tuple):
                 strided, shortcut = shortcut[1], None
@@ -318,16 +364,42 @@ class ResidualBlockRT:
         # replaces a separate read-read-write pass over the block input (add_bf16: 13 launches, 1.06 ms per ResNet-50 step).
         first_unit = self.units[0]
         fuse = shortcut is not None and not (first_unit.stride == 2 and first_unit.r == 1)   # that case returns a compact gradient
+        # the previous block's ReLU mask rides on the same epilogue: its BatchNorms then read neither its output nor a
+        # masked copy of dx (bit-identical: the mask multiplies by 0 / 1 exactly as their kernels would)
+        mask = in_mask if fuse else None
         n_main = len(self.units) - 1
-        dx = last.conv_bwd(dy, tl, sink, add=shortcut if (fuse and n_main == 0) else None)
+        dx = last.conv_bwd(dy, tl, sink, add=shortcut if (fuse and n_main == 0) else None,
+                           mask_bits=mask if n_main == 0 else None)
         for i, (u, t) in enumerate(zip(reversed(self.units[:-1]), reversed(tapes[:-1]))):
             dy, _ = u.bn_bwd(dx, t, sink)
-            dx = u.conv_bwd(dy, t, sink, add=shortcut if (fuse and i == n_main - 1) else None)
+            dx = u.conv_bwd(dy, t, sink, add=shortcut if (fuse and i == n_main - 1) else None,
+                            mask_bits=mask if i == n_main - 1 else None)
         if shortcut is not None and not fuse:
             ops.add_bf16(dx, shortcut)
         if strided is not None:
             ops.add_strided2(dx, strided)
-        return dx
+        return dx, mask is not None
+
+
+def blocks_backward(blocks, tapes, da, sink):
+    """Backward through a chain of stages (last to first); `da` is the gradient w.r.t. the last stage's output.
+    Re-runs checkpointed stages first (tape['ckpt_in']) and drops each tape once used.  Between two residual blocks the
+    gradient travels masked by the ReLU of the earlier block's output when the later block could apply that mask in its
+    data-gradient epilogue; a checkpointed block's mask does not exist yet at that point, so it is masked by itself."""
+    masked = False
+    for i in reversed(range(len(blocks))):
+        b, t = blocks[i], tapes[i]
+        if 'ckpt_in' in t:
+            b.forward(t.pop('ckpt_in'), t, True)
+        if isinstance(b, ResidualBlockRT):
+            prev = blocks[i - 1] if i > 0 else None
+            in_mask = prev.out_mask(tapes[i - 1]) if isinstance(prev, ResidualBlockRT) else None
+            da, masked = b.backward_chain(da, t, sink, dout_masked=masked, in_mask=in_mask)
+        else:
+            assert not masked
+            da = b.backward(da, t, sink)
+        t.clear()
+    return da
 
 
 class PlainUnitRT:
@@ -564,11 +636,7 @@ class ResNetRT:
         sink = self.sink
         assert tape is not None, 'backward called without a training forward'
         da = self.head_backward(dlogits, tape)
-        for b, t in zip(reversed(self.blocks), reversed(tape['blocks'])):
-            if 'ckpt_in' in t:
-                b.forward(t.pop('ckpt_in'), t, True)
-            da = b.backward(da, t, sink)
-            t.clear()
+        da = blocks_backward(self.blocks, tape['blocks'], da, sink)
         self.stem_backward(da, tape)
         if sink.on_backward_end is not None:
             sink.on_backward_end()

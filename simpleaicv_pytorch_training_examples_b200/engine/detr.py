@@ -20,7 +20,7 @@ csrc/dropout_hash.cuh: the backward recomputes the forward's masks from the per-
 import torch
 
 from .. import ops
-from .convnet import GradSink, ResNetRT
+from .convnet import GradSink, ResNetRT, blocks_backward
 from .operands import Linear, Operand
 
 
@@ -345,11 +345,7 @@ class DetrRT:
 
     def backbone_backward(self, da, tape):
         body, bt = self.body, tape['body']
-        for b, t in zip(reversed(body.blocks), reversed(bt['blocks'])):
-            if 'ckpt_in' in t:
-                b.forward(t.pop('ckpt_in'), t, True)
-            da = b.backward(da, t, self.sink)
-            t.clear()
+        da = blocks_backward(body.blocks, bt['blocks'], da, self.sink)
         body.stem_backward(da, bt)
 
     def transformer_forward(self, src, cx, tape):

@@ -103,12 +103,13 @@ def conv_fprop(x, w, cs, out=None, flags=0, stats=None):
     return out
 
 
-def conv_dgrad(dy, w, cs, out=None, add=None):
+def conv_dgrad(dy, w, cs, out=None, add=None, mask_bits=None):
     """dy: [n, h, w, k] (zero-upsampled for strided convs); cs.stride must be 1.
-    add: optional bf16 [n, h, w, c] tensor summed into the result in the GEMM epilogue."""
+    add: optional bf16 [n, h, w, c] tensor summed into the result in the GEMM epilogue.
+    mask_bits: optional ReLU mask from bn_apply (needs `add`); the sum is multiplied by it."""
     if out is None:
         out = torch.empty(cs.n, cs.h, cs.w, cs.c, device=dy.device, dtype=torch.bfloat16)
-    _lib.call('saicv_conv_dgrad', _p(dy), _p(w), _p(add), _p(out), ctypes.byref(cs), _stream())
+    _lib.call('saicv_conv_dgrad', _p(dy), _p(w), _p(add), _p(mask_bits), _p(out), ctypes.byref(cs), _stream())
     return out
 
 
@@ -229,26 +230,50 @@ def bn_finalize(stats, gamma, beta, rmean, rvar, scale_shift, saved, rows, eps, 
               _p(scale_shift), _p(saved), rows, c, eps, momentum, _stream())
 
 
-def bn_apply(y, scale_shift, out, act, res=None, res_scale_shift=None):
+def mask_bits_like(y):
+    """Buffer for the packed ReLU mask of an activation [..., C]: int32 [rows, C // 32] (bit j of word w is channel
+    32w + j; int32 only because torch has no uint32 arithmetic, the bits are the same)."""
     c = y.shape[-1]
-    _lib.call('saicv_bn_apply', _p(y), _p(scale_shift), _p(res), _p(res_scale_shift), _p(out),
+    return torch.empty(y.numel() // c, c // 32, device=y.device, dtype=torch.int32)
+
+
+def bn_apply(y, scale_shift, out, act, res=None, res_scale_shift=None, mask_bits=None):
+    """mask_bits: optional mask_bits_like(y) buffer that receives (out > 0), packed (ReLU only)."""
+    c = y.shape[-1]
+    _lib.call('saicv_bn_apply', _p(y), _p(scale_shift), _p(res), _p(res_scale_shift), _p(out), _p(mask_bits),
               y.numel() // c, c, act, _stream())
     return out
 
 
-def bn_bwd_reduce(dout, out, y, saved, sums, act, scale_shift=None):
-    """`out` None + scale_shift given: the activation mask is recomputed from y."""
+def bn_bwd_reduce(dout, out, y, saved, sums, act, scale_shift=None, bits=None):
+    """Activation mask from `out`, else from the packed ReLU mask `bits`, else recomputed from y with scale_shift."""
     c = y.shape[-1]
-    _lib.call('saicv_bn_bwd_reduce', _p(dout), _p(out), _p(y), _p(saved), _p(scale_shift),
+    _lib.call('saicv_bn_bwd_reduce', _p(dout), _p(out), _p(bits), _p(y), _p(saved), _p(scale_shift),
               _p(partial_ws(y.device, 2 * c)), _p(sums), y.numel() // c, c, act, _stream())
 
 
 def bn_bwd_apply(dout, out, y, saved, gamma, sums, dy, dres, dgamma, dbeta, act, accumulate=False,
-                 scale_shift=None):
+                 scale_shift=None, bits=None):
     c = y.shape[-1]
-    _lib.call('saicv_bn_bwd_apply', _p(dout), _p(out), _p(y), _p(saved), _p(gamma), _p(scale_shift),
+    _lib.call('saicv_bn_bwd_apply', _p(dout), _p(out), _p(bits), _p(y), _p(saved), _p(gamma), _p(scale_shift),
               _p(sums), _p(dy), _p(dres), _p(dgamma), _p(dbeta), y.numel() // c, c, act,
               int(accumulate), _stream())
+
+
+def bn_bwd_reduce2(g, bits, y_a, y_b, saved_a, saved_b, sums):
+    """bn_bwd_reduce of two BatchNorms over the same gradient g (masked by `bits` unless None): sums [4, C] receives
+    the [2, C] sums of A then of B, bit-identical to two bn_bwd_reduce calls."""
+    c = y_a.shape[-1]
+    _lib.call('saicv_bn_bwd_reduce2', _p(g), _p(bits), _p(y_a), _p(y_b), _p(saved_a), _p(saved_b),
+              _p(partial_ws(g.device, 4 * c)), _p(sums), y_a.numel() // c, c, _stream())
+
+
+def bn_bwd_apply2(g, bits, y_a, y_b, saved_a, saved_b, gamma_a, gamma_b, sums, dy_a, dy_b, dgamma_a, dbeta_a,
+                  dgamma_b, dbeta_b, accumulate_a=False, accumulate_b=False):
+    c = y_a.shape[-1]
+    _lib.call('saicv_bn_bwd_apply2', _p(g), _p(bits), _p(y_a), _p(y_b), _p(saved_a), _p(saved_b), _p(gamma_a),
+              _p(gamma_b), _p(sums), _p(dy_a), _p(dy_b), _p(dgamma_a), _p(dbeta_a), _p(dgamma_b), _p(dbeta_b),
+              y_a.numel() // c, c, int(accumulate_a), int(accumulate_b), _stream())
 
 
 def add_bf16(a, b):
