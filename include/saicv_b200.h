@@ -217,6 +217,18 @@ int saicv_token_pool_bwd(const float* dpooled, float* dx, void* dx_bf16, const f
  * bias fp32 [C] or NULL; relu: fused ReLU (van.py:49-50); flip: mirrored taps = the data gradient. */
 int saicv_dwconv_fwd(const void* x, const float* w, const float* bias, void* y, int n, int h, int wd,
                      int c, int k, int dil, int relu, int flip, void* stream);
+/* ConvFormer SepConv (SimpleAICV/classification/backbones/convformer.py:64-79: dwconv(relu(pwconv1(x)))):
+ * dx = dwconv^T(dy) * (mask > 0), the data gradient of the 7x7 depthwise conv (dilation 1, no bias) masked by
+ * the ReLU in front of it; mask bf16 [n][h][wd][c] = that ReLU's output.  Replaces the autograd pair
+ * conv-backward + threshold_backward of :68-70.  k must be 7. */
+int saicv_dwconv_dgrad_masked(const void* dy, const float* w, const void* mask, void* dx, int n, int h,
+                              int wd, int c, int k, void* stream);
+/* Global average pool of an NHWC stream x [n][hw][c], bf16 or fp32 (x_f32), summed in fp32 and written once
+ * as the head GEMM's bf16 operand y [n][c] (convformer.py:251-254: AdaptiveAvgPool2d of the fp32 or bf16
+ * stream, then autocast's cast for the Linear).  Backward: dx [n][hw][c] (fp32 when dx_f32, else bf16) =
+ * dy [n][c] (bf16) / hw. */
+int saicv_avgpool_stream_fwd(const void* x, int x_f32, void* y, int n, int hw, int c, void* stream);
+int saicv_avgpool_stream_bwd(const void* dy, void* dx, int dx_f32, int n, int hw, int c, void* stream);
 /* dw[C][1][k][k] (+)= sum over pixels dy * shifted x; partial: fp32 workspace
  * [saicv_dwconv_wgrad_blocks(n*h*w)][k*k][C]; fixed-order two-stage reduction. */
 int saicv_dwconv_wgrad_blocks(long long npix);

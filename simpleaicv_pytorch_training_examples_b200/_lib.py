@@ -115,6 +115,9 @@ SIGNATURES = {
     'saicv_heads_pack': [c_void_p, c_int, c_int, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p],
     'saicv_heads_unpack': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p],
     'saicv_dwconv_fwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    'saicv_dwconv_dgrad_masked': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    'saicv_avgpool_stream_fwd': [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p],
+    'saicv_avgpool_stream_bwd': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_dwconv_wgrad_blocks': [c_ll],
     'saicv_dwconv_wgrad': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_mul_bf16': [c_void_p, c_void_p, c_void_p, c_ll, c_void_p],

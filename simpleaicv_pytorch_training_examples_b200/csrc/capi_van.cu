@@ -1,5 +1,7 @@
-// HBM / L1-bound kernels of the VAN hot path (SimpleAICV/classification/backbones/van.py): depthwise
-// convolutions (3x3, 5x5, 7x7 dilation 3; :20-35,59-93) forward / data gradient / weight gradient, the LKA
+// HBM / L1-bound kernels of the VAN and ConvFormer hot paths (SimpleAICV/classification/backbones/van.py,
+// convformer.py): depthwise convolutions (3x3, 5x5, 7x7 dilation 3; :20-35,59-93; ConvFormer's 7x7 with the
+// ReLU-masked data gradient) forward / data gradient / weight gradient, the global average pool of an fp32 or
+// bf16 stream (convformer.py:251-254), the LKA
 // gating multiply (:91), the layer-scale residual update (:183-184), BatchNorm over an fp32 residual stream
 // (:160-165,205-207) and a generic NHWC im2col for the strided patch-embedding convolutions (:189-208).
 // Activations are NHWC bf16 seen as [rows][C]; the residual stream is fp32 (the reference's dtype flow under
@@ -37,10 +39,13 @@ __device__ __forceinline__ void store8(void* p, long long e, bool f32, const flo
 // ----------------------------------------------------------------------------- depthwise convolution
 // Block = 32 pixels x 8 channel vectors (64 channels); blockIdx.y = 64-channel chunk; the chunk's K*K*64
 // weights sit in shared memory as [tap][64] fp32.  flip: taps mirrored (data gradient of a 'same' conv).
-template <int K>
+// MASK (compile-time, appended parameter unused otherwise): y *= (mask > 0) with mask bf16 of y's shape, the
+// ReLU in FRONT of the conv (convformer.py:65-70: dwconv(relu(pwconv1(x)))) applied to its data gradient.
+template <int K, bool MASK = false>
 __global__ void __launch_bounds__(256)
 dwconv_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
-              __nv_bfloat16* __restrict__ y, int N, int H, int W, int C, int dil, int relu, int flip) {
+              __nv_bfloat16* __restrict__ y, int N, int H, int W, int C, int dil, int relu, int flip,
+              const __nv_bfloat16* __restrict__ mask = nullptr) {
   constexpr int KK = K * K;
   __shared__ float sw[KK][64];
   __shared__ float sb[64];
@@ -82,6 +87,12 @@ dwconv_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ w, 
     if (relu) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) acc[i] = fmaxf(acc[i], 0.f);
+    }
+    if (MASK) {
+      float m[8];
+      unpack8(*reinterpret_cast<const V8*>(mask + pix * C + c), m);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] = m[i] > 0.f ? acc[i] : 0.f;
     }
     *reinterpret_cast<V8*>(y + pix * C + c) = pack8(acc);
   }
@@ -143,6 +154,48 @@ __global__ void dwconv_wgrad_fold_kernel(const float* __restrict__ partial, floa
   float s = 0.f;
   for (int b = 0; b < nblk; ++b) s += partial[((long long)b * KK + tap) * C + c];
   grad[i] = accumulate ? grad[i] + s : s;
+}
+
+// ----------------------------------------------------------------------------- global average pool of a stream
+// y[n][c] = bf16(sum_t x[n][t][c] * (1 / HW)), x bf16 or fp32, summed in fp32 in t order (the reference pools the
+// stream in its own dtype and autocast casts the pooled features for the head Linear, convformer.py:251-254)
+__global__ void avgpool_stream_fwd_kernel(const void* __restrict__ x, int x_f32, __nv_bfloat16* __restrict__ y, int N, int HW,
+                                          int C) {
+  const int vpr = C >> 3;
+  const long long total = (long long)N * vpr;
+  const float inv = 1.f / (float)HW;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % vpr);
+    const long long n = i / vpr;
+    float acc[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+    for (int t = 0; t < HW; ++t) {
+      float f[8];
+      load8(x, ((n * HW + t) * vpr + v) * 8, x_f32 != 0, f);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) acc[k] += f[k];
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] *= inv;
+    store8(y, i * 8, false, acc);
+  }
+}
+// dx[n][t][c] = dy[n][c] * (1 / HW), dy bf16, dx fp32 or bf16
+__global__ void avgpool_stream_bwd_kernel(const __nv_bfloat16* __restrict__ dy, void* __restrict__ dx, int dx_f32, int N, int HW,
+                                          int C) {
+  const int vpr = C >> 3;
+  const long long total = (long long)N * HW * vpr;
+  const float inv = 1.f / (float)HW;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % vpr);
+    const long long n = i / ((long long)HW * vpr);
+    float f[8];
+    load8(dy, (n * vpr + v) * 8, false, f);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) f[k] *= inv;
+    store8(dx, i * 8, dx_f32 != 0, f);
+  }
 }
 
 // ----------------------------------------------------------------------------- elementwise
@@ -476,6 +529,33 @@ int saicv_dwconv_fwd(const void* x, const float* w, const float* bias, void* y, 
     default: return set_error("saicv_dwconv_fwd: kernel size %d (3, 5, 7)", k);
   }
   return check_launch("dwconv_kernel");
+}
+
+int saicv_dwconv_dgrad_masked(const void* dy, const float* w, const void* mask, void* dx, int n, int h, int wd, int c, int k,
+                              void* stream) {
+  if (c % 8) return set_error("saicv_dwconv_dgrad_masked: C %% 8 != 0");
+  if (!mask) return set_error("saicv_dwconv_dgrad_masked: mask is NULL");
+  if (k != 7) return set_error("saicv_dwconv_dgrad_masked: kernel size %d (7)", k);
+  const long long npix = (long long)n * h * wd;
+  dim3 grid((unsigned)grid1d(npix, 32, 132 * 8), (unsigned)((c + 63) / 64));
+  dwconv_kernel<7, true><<<grid, 256, 0, ST>>>(reinterpret_cast<const __nv_bfloat16*>(dy), w, nullptr,
+                                               reinterpret_cast<__nv_bfloat16*>(dx), n, h, wd, c, 1, 0, 1,
+                                               reinterpret_cast<const __nv_bfloat16*>(mask));
+  return check_launch("dwconv_kernel");
+}
+
+int saicv_avgpool_stream_fwd(const void* x, int x_f32, void* y, int n, int hw, int c, void* stream) {
+  if (c % 8) return set_error("saicv_avgpool_stream_fwd: C %% 8 != 0");
+  avgpool_stream_fwd_kernel<<<grid1d((long long)n * (c / 8), 128), 128, 0, ST>>>(x, x_f32, reinterpret_cast<__nv_bfloat16*>(y), n,
+                                                                                 hw, c);
+  return check_launch("avgpool_stream_fwd_kernel");
+}
+
+int saicv_avgpool_stream_bwd(const void* dy, void* dx, int dx_f32, int n, int hw, int c, void* stream) {
+  if (c % 8) return set_error("saicv_avgpool_stream_bwd: C %% 8 != 0");
+  avgpool_stream_bwd_kernel<<<grid1d((long long)n * hw * (c / 8)), 256, 0, ST>>>(reinterpret_cast<const __nv_bfloat16*>(dy), dx,
+                                                                                 dx_f32, n, hw, c);
+  return check_launch("avgpool_stream_bwd_kernel");
 }
 
 int saicv_dwconv_wgrad_blocks(long long npix) {

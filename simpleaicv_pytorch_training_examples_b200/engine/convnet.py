@@ -478,6 +478,10 @@ class FcHeadRT:
         feat = self.fc.weight.shape[1]
         if pooled.shape[1] != feat:   # channel-padded feature map (e.g. 16/32-channel stacks)
             pooled = pooled[:, :feat].contiguous()
+        return self.fc_forward(pooled, tape)
+
+    def fc_forward(self, pooled, tape):
+        """pooled bf16 [B, feat] -> fp32 logits [B, num_classes]."""
         tape['pooled'] = pooled
         ncls = self.fc.weight.shape[0]
         logits = self.lin.fwd(pooled, out_f32=True)
@@ -487,7 +491,18 @@ class FcHeadRT:
 
     def backward(self, dlogits, tape, sink, cpad):
         """dlogits fp32 [B, num_classes] -> gradient w.r.t. the last feature map (NHWC bf16, cpad channels)."""
-        ncls, feat = self.fc.weight.shape
+        dpooled = self.fc_backward(dlogits, tape, sink)
+        feat = self.fc.weight.shape[1]
+        if cpad != feat:
+            full = torch.zeros(dpooled.shape[0], cpad, device=dpooled.device, dtype=torch.bfloat16)
+            full[:, :feat] = dpooled
+            dpooled = full
+        h, w = tape['feat_hw']
+        return ops.avgpool_bwd(dpooled, h, w)
+
+    def fc_backward(self, dlogits, tape, sink):
+        """dlogits fp32 [B, num_classes]: writes the Linear's gradients, returns dpooled bf16 [B, feat]."""
+        ncls = self.fc.weight.shape[0]
         npad = self.op.w.shape[0]
         dlogits = dlogits.contiguous().float()
         bbuf, bacc = sink.begin(self.fc.bias)
@@ -499,13 +514,7 @@ class FcHeadRT:
         else:
             dl[:, :ncls] = dlogits.to(torch.bfloat16)
         rows_wgrad(dl, tape['pooled'], self.fc.weight, sink)
-        dpooled = ops.linear_dgrad(dl, self.op.w)
-        if cpad != feat:
-            full = torch.zeros(dpooled.shape[0], cpad, device=dl.device, dtype=torch.bfloat16)
-            full[:, :feat] = dpooled
-            dpooled = full
-        h, w = tape['feat_hw']
-        return ops.avgpool_bwd(dpooled, h, w)
+        return ops.linear_dgrad(dl, self.op.w)
 
 
 class ConvHeadRT:

@@ -72,7 +72,7 @@ def rows_wgrad(dy, x, weight, sink):
 
 
 class Linear:
-    """bf16 operand copy + forward / backward of one nn.Linear (or 1x1 conv with bias)."""
+    """bf16 operand copy + forward / backward of one nn.Linear (or 1x1 conv), with or without bias."""
 
     def __init__(self, mod):
         self.mod = mod
@@ -81,6 +81,8 @@ class Linear:
 
     def prep(self):
         w, b = self.op.refresh(), self.mod.bias
+        if b is None:
+            return
         if self.b_pad is None or self.b_pad.device != w.device:
             self.b_pad = torch.zeros(w.shape[0], device=w.device)
         self.b_pad[:b.shape[0]].copy_(b.detach())
@@ -98,16 +100,17 @@ class Linear:
         (multiplied by gelu'(gelu_pre) when the input of this layer was gelu(gelu_pre), masked by
         relu_out > 0 when it was a ReLU output, plus `add` when a second gradient joins there)."""
         b = self.mod.bias
-        n = b.shape[0]
         rows_wgrad(dy, x, self.mod.weight, sink)
-        bbuf, bacc = sink.begin(b)
-        if dy.shape[1] == n:
-            ops.colsum(dy, bbuf, accumulate=bacc)
-        else:
-            full = torch.empty(dy.shape[1], device=dy.device)
-            ops.colsum(dy, full)
-            bbuf.copy_(full[:n] + (bbuf if bacc else 0))
-        sink.done(b, bbuf)
+        if b is not None:
+            n = b.shape[0]
+            bbuf, bacc = sink.begin(b)
+            if dy.shape[1] == n:
+                ops.colsum(dy, bbuf, accumulate=bacc)
+            else:
+                full = torch.empty(dy.shape[1], device=dy.device)
+                ops.colsum(dy, full)
+                bbuf.copy_(full[:n] + (bbuf if bacc else 0))
+            sink.done(b, bbuf)
         return ops.linear_dgrad(dy, self.op.w, gelu_pre=gelu_pre, relu_out=relu_out, add=add) if need_dx else None
 
 

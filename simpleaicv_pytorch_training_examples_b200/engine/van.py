@@ -156,22 +156,22 @@ class _Block:
         return _bn_backward(blk.norm1, da, t['bn1'], sink, dres=dx1, dx_f32=dx_f32)
 
 
-class _PatchEmbed:
-    """OverlapPatchEmbed (van.py:189-208): conv (with bias) -> BatchNorm; output = the stage's bf16 stream input."""
+class StridedConv:
+    """Square strided conv with bias as explicit im2col + one GEMM: from the NCHW fp32 image (stem im2col, STEM operand)
+    when the input has fewer than 8 channels, else from NHWC bf16 (im2col_nhwc, CONV operand; col2im in the backward)."""
 
-    def __init__(self, pe):
-        self.pe = pe
-        self.conv, self.bn = pe.proj, pe.norm
-        self.k, self.stride, self.pad = self.conv.kernel_size[0], self.conv.stride[0], self.conv.padding[0]
-        self.from_image = self.conv.in_channels % 8 != 0
-        self.op = Operand(self.conv.weight, STEM if self.from_image else CONV)
+    def __init__(self, conv):
+        self.conv = conv
+        self.k, self.stride, self.pad = conv.kernel_size[0], conv.stride[0], conv.padding[0]
+        self.from_image = conv.in_channels % 8 != 0
+        self.op = Operand(conv.weight, STEM if self.from_image else CONV)
         self.kpad = self.op.kpad
 
     def prep(self):
         self.op.refresh()
 
-    def forward(self, x, t, training):
-        """x: NCHW fp32 image (stage 1) or NHWC bf16 -> (bf16 stream [rows, C], (n, P, Q, C))."""
+    def forward(self, x, t):
+        """x: NCHW fp32 image or NHWC bf16 -> (bf16 [rows, C], (n, P, Q, C))."""
         if self.from_image:
             n, _, h, w = x.shape
             cols = ops.stem_im2col(x, self.k, self.k, self.stride, self.pad, self.kpad)
@@ -179,15 +179,12 @@ class _PatchEmbed:
         else:
             n, h, w, _ = x.shape
             cols, P, Q = ops.im2col_nhwc(x, self.k, self.stride, self.pad)
-        t['cols'], t['in_shape'], t['bn'] = cols, tuple(x.shape), {}
+        t['cols'], t['in_shape'] = cols, tuple(x.shape)
         y = ops.linear_fwd(cols, self.op.w, bias=self.conv.bias.detach())
-        out = _bn_forward(self.bn, y, training, False, t['bn'])
-        return out, (n, P, Q, self.conv.out_channels)
+        return y, (n, P, Q, self.conv.out_channels)
 
-    def backward(self, dout, t, sink):
-        """dout: gradient w.r.t. the BN output (bf16 or fp32 [rows, C]).  Returns the NHWC bf16 input gradient
-        (None for the image stage)."""
-        dy = _bn_backward(self.bn, dout, t['bn'], sink, dx_f32=False)
+    def backward(self, dy, t, sink):
+        """dy: bf16 gradient [rows, C] w.r.t. the conv output.  Returns the NHWC bf16 input gradient (None for an image)."""
         w, b = self.conv.weight, self.conv.bias
         wbuf, wacc = sink.begin(w)
         part = ops.linear_wgrad(dy, t['cols'])
@@ -201,6 +198,28 @@ class _PatchEmbed:
         n, h, ww, c = t['in_shape']
         dcols = ops.linear_dgrad(dy, self.op.w)
         return ops.col2im_nhwc(dcols, n, h, ww, c, self.k, self.stride, self.pad)
+
+
+class _PatchEmbed:
+    """OverlapPatchEmbed (van.py:189-208): conv (with bias) -> BatchNorm; output = the stage's bf16 stream input."""
+
+    def __init__(self, pe):
+        self.conv, self.bn = StridedConv(pe.proj), pe.norm
+        self.op = self.conv.op
+
+    def prep(self):
+        self.conv.prep()
+
+    def forward(self, x, t, training):
+        """x: NCHW fp32 image (stage 1) or NHWC bf16 -> (bf16 stream [rows, C], (n, P, Q, C))."""
+        t['bn'] = {}
+        y, shape = self.conv.forward(x, t)
+        return _bn_forward(self.bn, y, training, False, t['bn']), shape
+
+    def backward(self, dout, t, sink):
+        """dout: gradient w.r.t. the BN output (bf16 or fp32 [rows, C]).  Returns the NHWC bf16 input gradient
+        (None for the image stage)."""
+        return self.conv.backward(_bn_backward(self.bn, dout, t['bn'], sink, dx_f32=False), t, sink)
 
 
 class VANRT:

@@ -535,6 +535,33 @@ def dwconv_fwd(x, w, bias, k, dil=1, relu=False, flip=False):
     return out
 
 
+def dwconv_dgrad_masked(dy, w, mask, k=7):
+    """Data gradient of a k x k depthwise 'same' conv (dilation 1) masked by the ReLU in front of it:
+    dwconv^T(dy) * (mask > 0), mask = that ReLU's output (NHWC bf16 like dy)."""
+    n, h, wd, c = dy.shape
+    assert mask.shape == dy.shape and mask.dtype == torch.bfloat16
+    out = torch.empty_like(dy)
+    _lib.call('saicv_dwconv_dgrad_masked', _p(dy), _p(w), _p(mask), _p(out), n, h, wd, c, k, _stream())
+    return out
+
+
+def avgpool_stream_fwd(x):
+    """x: NHWC stream [n, h, w, c] (bf16 or fp32) -> bf16 [n, c] mean over h*w, summed in fp32."""
+    n, h, w, c = x.shape
+    out = torch.empty(n, c, device=x.device, dtype=torch.bfloat16)
+    _lib.call('saicv_avgpool_stream_fwd', _p(x), int(x.dtype == torch.float32), _p(out), n, h * w, c, _stream())
+    return out
+
+
+def avgpool_stream_bwd(dy, h, w, dx_f32=True):
+    """dy bf16 [n, c] -> [n, h, w, c] = dy / (h*w), fp32 (or bf16)."""
+    n, c = dy.shape
+    assert dy.dtype == torch.bfloat16
+    out = torch.empty(n, h, w, c, device=dy.device, dtype=torch.float32 if dx_f32 else torch.bfloat16)
+    _lib.call('saicv_avgpool_stream_bwd', _p(dy), _p(out), int(dx_f32), n, h * w, c, _stream())
+    return out
+
+
 def dwconv_wgrad(dy, x, dw, k, dil=1, accumulate=False):
     n, h, wd, c = x.shape
     nblk = _lib.load().saicv_dwconv_wgrad_blocks(n * h * wd)
