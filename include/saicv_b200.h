@@ -56,6 +56,9 @@ int saicv_linear_dgrad(const void* dy, const void* w, const float* resid, const 
 int saicv_linear_wgrad(const void* dy, const void* x, float* dw_partial, int M, int N, int K,
                        int splits, void* stream);
 int saicv_wgrad_splits(int out_rows, int out_cols, long long reduce_len);
+/* 1 when the weight gradient dW [out_rows, out_cols] is computed as dW^T (fewer padded 128-row tiles: few filters).
+ * saicv_conv_wgrad then writes dw_partial [splits][r*s*c][k]; linear_wgrad callers swap dy and x themselves. */
+int saicv_wgrad_transposed(int out_rows, int out_cols);
 
 /* ---- convolutions: nn.Conv2d inside ConvBnActBlock (resnet.py:33-39, darknet.py:49-56) ---- */
 typedef struct {
@@ -71,11 +74,16 @@ int saicv_conv_fprop(const void* x, const void* w, float* stats_partial, void* y
  * gradient; `add` (bf16, may be NULL) is the gradient arriving over the shortcut, fused into the
  * epilogue.  `mask_bits` (may be NULL): the [n*h*w][c/32] ReLU mask written by saicv_bn_apply; the
  * result (after the add) is multiplied by its bit, i.e. dx is the gradient behind that ReLU.
- * For a stride-2 conv pass the zero-upsampled dy (saicv_zero_upsample2) and stride = 1.
- * `dy` has spatial extent (h, w).  requires k % 64 == 0, c % 64 == 0. */
+ * `dy` has spatial extent (h, w).  requires k % 64 == 0, c % 64 == 0.
+ * stride = 2 (3x3, pad 1, even h and w, w <= 256, no `add` / `mask_bits`): `dy` is the compact [n, h/2, w/2, k]
+ * gradient of the strided conv; each output phase (h mod 2, w mod 2) reduces only the taps that reach it, in the order
+ * the stride-1 path reduces them, so dx equals that path's bit for bit up to the sign of exact zeros.  Other
+ * stride-2 convs: pass the zero-upsampled dy (saicv_zero_upsample2) and stride = 1. */
 int saicv_conv_dgrad(const void* dy, const void* w, const void* add, const uint32_t* mask_bits, void* dx,
                      const saicv_conv_shape* cs, void* stream);
-/* dw_partial[splits][k][r*s*c] fp32 = sum over output pixels dy[pix,k] * x[patch(pix), (r,s,c)]. */
+/* dw_partial[splits][k][r*s*c] fp32 = sum over output pixels dy[pix,k] * x[patch(pix), (r,s,c)]; laid out
+ * [splits][r*s*c][k] (dW^T) when saicv_wgrad_transposed(k, r*s*c).  splits = saicv_wgrad_splits(k, r*s*c, pixels) in
+ * both layouts, so every element is the same sum. */
 int saicv_conv_wgrad(const void* dy, const void* x, float* dw_partial, const saicv_conv_shape* cs,
                      int splits, void* stream);
 
@@ -87,10 +95,10 @@ int saicv_conv_wgrad(const void* dy, const void* x, float* dw_partial, const sai
  * 64 run on channel-padded activations, e.g. DarkNet's 32-channel stem). */
 int saicv_prep_conv_weight(const float* w, void* w_bf16, int k, int c, int r, int s, int kpad,
                            int order, int kp, int cp, void* stream);
-/* sum of fp32 partials [splits][k][kpad] (columns in `order`) -> fp32 grad in torch layout
- * [k][c][r][s]; accumulate != 0 adds to the destination (gradient accumulation). */
+/* sum of fp32 partials [splits][k][kpad] (columns in `order`; transposed != 0: [splits][kpad][k]) -> fp32 grad in
+ * torch layout [k][c][r][s]; accumulate != 0 adds to the destination (gradient accumulation). */
 int saicv_finish_conv_wgrad(const float* partial, float* grad, int splits, int k, int c, int r,
-                            int s, int kpad, int accumulate, int order, int kp, int cp, void* stream);
+                            int s, int kpad, int accumulate, int order, int kp, int cp, int transposed, void* stream);
 /* out[i] (+)= sum_s partial[s][i]; plain reduction for linear wgrad. */
 int saicv_reduce_partials(const float* partial, float* out, int splits, long long n,
                           int accumulate, void* stream);

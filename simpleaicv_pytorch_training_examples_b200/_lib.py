@@ -50,11 +50,12 @@ SIGNATURES = {
     'saicv_linear_dgrad': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_linear_wgrad': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_wgrad_splits': [c_int, c_int, c_ll],
+    'saicv_wgrad_transposed': [c_int, c_int],
     'saicv_conv_fprop': [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_int, c_void_p],
     'saicv_conv_dgrad': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_void_p],
     'saicv_conv_wgrad': [c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_int, c_void_p],
     'saicv_prep_conv_weight': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    'saicv_finish_conv_wgrad': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    'saicv_finish_conv_wgrad': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_reduce_partials': [c_void_p, c_void_p, c_int, c_ll, c_int, c_void_p],
     'saicv_cast_bf16': [c_void_p, c_void_p, c_ll, c_void_p],
     'saicv_nchw_to_nhwc_bf16': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],

@@ -701,7 +701,7 @@ __global__ void prep_conv_weight_kernel(const float* __restrict__ w, __nv_bfloat
 
 __global__ void finish_conv_wgrad_kernel(const float* __restrict__ partial, float* __restrict__ grad, int splits,
                                          int K, int C, int R, int S, int kpad, int accumulate, int order, int Kp,
-                                         int Cp) {
+                                         int Cp, int transposed) {
   const long long total = (long long)K * C * R * S;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
@@ -709,8 +709,8 @@ __global__ void finish_conv_wgrad_kernel(const float* __restrict__ partial, floa
     const long long kc = i / (R * S);
     const int c = (int)(kc % C), k = (int)(kc / C);
     const int S8 = (S + 7) & ~7;
-    const long long src = order == 1 ? (long long)k * kpad + (long long)(c * R + tap / S) * S8 + tap % S
-                                     : (long long)k * kpad + (long long)tap * Cp + c;
+    const long long col = order == 1 ? (long long)(c * R + tap / S) * S8 + tap % S : (long long)tap * Cp + c;
+    const long long src = transposed ? col * Kp + k : (long long)k * kpad + col;   // [Kp][kpad] or dW^T [kpad][Kp]
     float s = accumulate ? grad[i] : 0.f;
     for (int sp = 0; sp < splits; ++sp) s += partial[(long long)sp * Kp * kpad + src];
     grad[i] = s;
@@ -1153,11 +1153,12 @@ int saicv_prep_conv_weight(const float* w, void* w_bf16, int k, int c, int r, in
 }
 
 int saicv_finish_conv_wgrad(const float* partial, float* grad, int splits, int k, int c, int r, int s, int kpad,
-                            int accumulate, int order, int kp, int cp, void* stream) {
+                            int accumulate, int order, int kp, int cp, int transposed, void* stream) {
   if (kp <= 0) kp = k;
   if (cp <= 0) cp = c;
   finish_conv_wgrad_kernel<<<grid_for((long long)k * c * r * s), kThreads, 0, ST>>>(partial, grad, splits, k, c, r,
-                                                                                     s, kpad, accumulate, order, kp, cp);
+                                                                                     s, kpad, accumulate, order, kp, cp,
+                                                                                     transposed);
   return check_launch("finish_conv_wgrad_kernel");
 }
 

@@ -97,6 +97,24 @@ bool encode_out(CUtensorMap* m, const void* ptr, bool f32, uint64_t cols, uint64
   return true;
 }
 
+// Store map of the phase data gradient: dx [n, 2P, 2Q, c] bf16 viewed as {c, b, q, a, n*P + p} for pixel (2p+a, 2q+b);
+// the box {64, 1, Q, 1, rows} is `rows` whole pixel rows of one phase, rows*Q consecutive rows of the staging slice.
+bool encode_out_phases(CUtensorMap* m, void* ptr, uint64_t c, uint64_t np, uint64_t q, uint32_t rows) {
+  cuuint64_t dims[5] = {c, 2, q, 2, np};
+  cuuint64_t strides[4] = {c * 2, 2 * c * 2, 2 * q * c * 2, 4 * q * c * 2};
+  cuuint32_t box[5] = {64u, 1u, (cuuint32_t)q, 1u, rows};
+  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, ptr, dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled(phase out) failed: %d (c=%llu rows=%llu q=%llu box rows=%u)", (int)r,
+              (unsigned long long)c, (unsigned long long)np, (unsigned long long)q, rows);
+    return false;
+  }
+  return true;
+}
+
 // im2col map over an NHWC bf16 tensor.
 bool encode_im2col(CUtensorMap* m, const void* ptr, int n, int h, int w, int c, int lc_h, int lc_w,
                    int uc_h, int uc_w, int stride, uint32_t pixels_per_col) {
@@ -171,8 +189,8 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, con
     if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(smem=%d): %s", Cfg::kSmemBytes, cudaGetErrorString(e));
     attr_set = true;
   }
-  const int num_m = (p.M + BM - 1) / BM, num_n = (p.N + BN - 1) / BN;
-  const long long total = (long long)num_m * num_n * p.splits;
+  const int num_m = (p.M + p.tile_rows - 1) / p.tile_rows, num_n = (p.N + BN - 1) / BN;
+  const long long total = (long long)num_m * num_n * p.splits * p.phases;
   const int grid = (int)(total < g_sm_count ? total : g_sm_count);
   const int stat_bytes = (p.epi_flags & EPI_STATS) ? ((8 * p.N + 15) & ~15) : 0;
   int stages = 0, nb = 1;
@@ -207,6 +225,8 @@ int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorM
              cudaStream_t st, const void* aux = nullptr, bool aux_f32 = false) {
   CUtensorMap r = d;
   p.aux_tma = 0;
+  if (p.tile_rows == 0) p.tile_rows = BM;
+  if (p.phases == 0) p.phases = 1;
   const bool both = (p.epi_flags & EPI_RESID) && (p.epi_flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU));
   if (aux && !both && !(p.epi_flags & EPI_DIRECT) && p.splits == 1 && aux_f32 == (p.out_f32 != 0) && aligned16(aux) &&
       !getenv("SAICV_GEMM_NO_AUX_TMA")) {
@@ -215,7 +235,13 @@ int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorM
   }
   // compile-time epilogue variant (gemm_sm90.cuh GemmVariant); SAICV_GEMM_FULL_VARIANT=1 forces the run-time one
   int var = VAR_FULL;
-  if (!getenv("SAICV_GEMM_FULL_VARIANT")) {
+  if (p.a_mode == A_IM2COL_MN && (p.epi_flags || !p.out_f32 || getenv("SAICV_GEMM_FULL_VARIANT")))
+    return set_error("the transposed conv weight gradient runs on the plain fp32 epilogue (VAR_PLAIN_F32) only");
+  if (p.phases > 1 || p.tile_rows != BM) {
+    if (p.epi_flags || p.aux_tma || p.out_f32 || p.splits != 1)
+      return set_error("the phase data gradient has a plain bf16 epilogue: no epilogue flags, aux operand or split-K");
+    var = VAR_PHASE_BF16;
+  } else if (!getenv("SAICV_GEMM_FULL_VARIANT")) {
     if (p.aux_tma && !(p.epi_flags & ~GemmVariant<VAR_AUX>::kMask)) var = VAR_AUX;
     else if (!p.aux_tma && !p.out_f32 && !(p.epi_flags & ~GemmVariant<VAR_PLAIN_BF16>::kMask))
       var = ((p.epi_flags & EPI_STATS) && !getenv("SAICV_GEMM_INLINE_STATS")) ? VAR_STATS_BF16 : VAR_PLAIN_BF16;
@@ -229,6 +255,7 @@ int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorM
     case VAR_STATS_BF16: return launch<BN_, VAR_STATS_BF16>(a, b, d, r, p, st);      \
     case VAR_PLAIN_F32: return launch<BN_, VAR_PLAIN_F32>(a, b, d, r, p, st);        \
     case VAR_AUX: return launch<BN_, VAR_AUX>(a, b, d, r, p, st);                    \
+    case VAR_PHASE_BF16: return launch<BN_, VAR_PHASE_BF16>(a, b, d, r, p, st);      \
     default: return launch<BN_, VAR_FULL>(a, b, d, r, p, st);                        \
   }
   switch (bn) {
@@ -236,6 +263,47 @@ int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorM
     default: SAICV_LAUNCH_BN(128)
   }
 #undef SAICV_LAUNCH_BN
+}
+
+// Data gradient of a 3x3 / stride 2 / pad 1 convolution on even h, w without the zero-upsampled dy: the four output
+// phases (a, b) = (h mod 2, w mod 2) are stride-1 correlations over the compact dy [n, h/2, w/2, k] (gemm_sm90.cuh,
+// GemmParams::phases).  Phase a of a dimension takes dy offset 0 through tap 1 (a = 0), or offsets 0 and 1 through taps
+// 2 and 0 (a = 1).  The taps of a phase are reduced in the order the stride-1 kernel reduces them over the zero-upsampled
+// dy (offsets ascending, rows outer), so every sum is the same: only the blocks of exact zeros are left out.
+int conv_dgrad_phases(const void* dy, const void* w, const void* add, const uint32_t* mask_bits, void* dx,
+                      const saicv_conv_shape* cs, cudaStream_t st) {
+  if (cs->r != 3 || cs->s != 3 || cs->pad != 1 || cs->h % 2 || cs->w % 2 || cs->w / 2 > BM)
+    return set_error("saicv_conv_dgrad: stride 2 needs a 3x3 pad-1 conv on even h, w with w <= %d (r=%d s=%d pad=%d "
+                     "h=%d w=%d); zero-upsample dy and pass stride 1 otherwise", 2 * BM, cs->r, cs->s, cs->pad, cs->h, cs->w);
+  if (add || mask_bits) return set_error("saicv_conv_dgrad: stride 2 takes no `add` / `mask_bits`");
+  const int P = cs->h / 2, Q = cs->w / 2;
+  const int rows = BM / Q;   // whole dy rows per tile: the 5-D store box cannot wrap inside a row
+  CUtensorMap ta, tb, td;
+  if (!encode_im2col(&ta, dy, cs->n, P, Q, cs->k, 0, 0, 0, 0, 1, 128)) return 2;
+  const int Kw = 9 * cs->c;
+  if (!encode_2d(&tb, w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, Kw, cs->k, Kw, 64, 64)) return 2;
+  if (!encode_out_phases(&td, dx, cs->c, (uint64_t)cs->n * P, Q, rows)) return 2;
+  GemmParams p{};
+  p.M = cs->n * P * Q; p.N = cs->c; p.num_kb = 4 * (cs->k / 64); p.kb_per_split = p.num_kb; p.splits = 1;
+  p.a_mode = A_IM2COL; p.b_mode = B_MN2D; p.b_cin = cs->c;
+  p.g.P = P; p.g.Q = Q; p.g.stride = 1; p.g.lc_h = 0; p.g.lc_w = 0;
+  p.g.R = 3; p.g.S = 3; p.g.cchunks = cs->k / 64; p.g.n_img = cs->n;
+  p.epi_flags = 0; p.out_f32 = 0; p.out = dx; p.ldd = cs->c;
+  p.tile_rows = rows * Q;
+  p.phases = 4;
+  // (weight tap, dy offset) of each output parity along one dimension
+  const int taps1[2][2] = {{1, -1}, {2, 0}};
+  const int order[4] = {3, 1, 2, 0};   // the 4-tap phase first, the 1-tap phase last: the short work items end the launch
+  for (int i = 0; i < 4; ++i) {
+    const int a = order[i] >> 1, b = order[i] & 1;
+    p.ph_out[i] = order[i];
+    p.ph_taps[i] = (1 + a) * (1 + b);
+    int t = 0;
+    for (int dr = 0; dr <= a; ++dr)
+      for (int ds = 0; ds <= b; ++ds)
+        p.ph_tab[i][t++] = (taps1[a][dr] * 3 + taps1[b][ds]) | (dr << 8) | (ds << 9);
+  }
+  return dispatch(pick_bn(cs->c), ta, tb, td, p, st);
 }
 
 }  // namespace
@@ -250,6 +318,14 @@ int saicv_gemm_stats_rows(long long out_rows, int out_cols) {
   const long long tiles = ((out_rows + BM - 1) / BM) * ((out_cols + bn - 1) / bn);
   const int sms = ensure_init() ? g_sm_count : 132;
   return (int)(tiles < sms ? tiles : sms);
+}
+
+int saicv_wgrad_transposed(int out_rows, int out_cols) {
+  // padded tile area of dW [rows, cols] against dW^T: few filters (rows) leave most of every 128-row tile empty
+  const int bn = pick_bn(out_cols), bnt = pick_bn(out_rows);
+  const long long cost = (long long)((out_rows + BM - 1) / BM) * BM * ((out_cols + bn - 1) / bn) * bn;
+  const long long cost_t = (long long)((out_cols + BM - 1) / BM) * BM * ((out_rows + bnt - 1) / bnt) * bnt;
+  return cost_t < cost ? 1 : 0;
 }
 
 int saicv_wgrad_splits(int out_rows, int out_cols, long long reduce_len) {
@@ -376,7 +452,9 @@ int saicv_conv_dgrad(const void* dy, const void* w, const void* add, const uint3
   if (!ensure_init()) return 1;
   if (cs->c % 64 || cs->k % 64 || !aligned16(dy) || !aligned16(w) || !aligned16(dx))
     return set_error("saicv_conv_dgrad: needs c%%64==0 and k%%64==0 (c=%d k=%d)", cs->c, cs->k);
-  if (cs->stride != 1) return set_error("saicv_conv_dgrad: stride must be 1 (zero-upsample dy for strided convs)");
+  if (cs->stride == 2) return conv_dgrad_phases(dy, w, add, mask_bits, dx, cs, (cudaStream_t)stream);
+  if (cs->stride != 1)
+    return set_error("saicv_conv_dgrad: stride %d (1, or 2 for 3x3 pad 1 on even sizes)", cs->stride);
   // dy has spatial extent (h, w) and k channels; output dx [n,h,w,c].
   const long long M = (long long)cs->n * cs->h * cs->w;
   const int Kw = cs->r * cs->s * cs->c;  // weight row length
@@ -406,22 +484,28 @@ int saicv_conv_wgrad(const void* dy, const void* x, float* dw_partial, const sai
   const int P = conv_out(cs->h, cs->pad, cs->r, cs->stride), Q = conv_out(cs->w, cs->pad, cs->s, cs->stride);
   const long long Mpix = (long long)cs->n * P * Q;
   const int Ncols = cs->r * cs->s * cs->c;
-  const int bn = pick_bn(Ncols);
+  // splits: saicv_wgrad_splits in the dW orientation, whichever product runs, so that both reduce the same k-blocks
+  const bool tr = saicv_wgrad_transposed(cs->k, Ncols) != 0;
+  const int bn = pick_bn(tr ? cs->k : Ncols);
   CUtensorMap ta, tb, td;
-  if (!encode_2d(&ta, dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, cs->k, Mpix, cs->k, 64, 64)) return 2;
-  if (!encode_im2col(&tb, x, cs->n, cs->h, cs->w, cs->c, -cs->pad, -cs->pad, cs->pad - (cs->r - 1),
+  CUtensorMap& tdy = tr ? tb : ta;
+  CUtensorMap& tx = tr ? ta : tb;
+  if (!encode_2d(&tdy, dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, cs->k, Mpix, cs->k, 64, 64)) return 2;
+  if (!encode_im2col(&tx, x, cs->n, cs->h, cs->w, cs->c, -cs->pad, -cs->pad, cs->pad - (cs->r - 1),
                      cs->pad - (cs->s - 1), cs->stride, 64))
     return 2;
-  if (!encode_out(&td, dw_partial, true, Ncols, cs->k, Ncols, splits, (uint64_t)cs->k * Ncols)) return 2;
+  if (tr ? !encode_out(&td, dw_partial, true, cs->k, Ncols, cs->k, splits, (uint64_t)cs->k * Ncols)
+         : !encode_out(&td, dw_partial, true, Ncols, cs->k, Ncols, splits, (uint64_t)cs->k * Ncols))
+    return 2;
   GemmParams p{};
-  p.M = cs->k; p.N = Ncols; p.num_kb = (int)((Mpix + BK - 1) / BK);
+  p.M = tr ? Ncols : cs->k; p.N = tr ? cs->k : Ncols; p.num_kb = (int)((Mpix + BK - 1) / BK);
   p.kb_per_split = (p.num_kb + splits - 1) / splits;
   p.splits = (p.num_kb + p.kb_per_split - 1) / p.kb_per_split;
   if (p.splits != splits) return set_error("saicv_conv_wgrad: splits=%d leaves an empty split (use saicv_wgrad_splits)", splits);
-  p.a_mode = A_MN2D; p.b_mode = B_IM2COL;
+  p.a_mode = tr ? A_IM2COL_MN : A_MN2D; p.b_mode = tr ? B_MN2D : B_IM2COL;
   p.g.P = P; p.g.Q = Q; p.g.stride = cs->stride; p.g.lc_h = -cs->pad; p.g.lc_w = -cs->pad;
   p.g.R = cs->r; p.g.S = cs->s; p.g.cchunks = cs->c / 64; p.g.n_img = cs->n;
-  p.epi_flags = 0; p.out_f32 = 1; p.out = dw_partial; p.ldd = Ncols; p.split_stride = (long long)cs->k * Ncols;
+  p.epi_flags = 0; p.out_f32 = 1; p.out = dw_partial; p.ldd = p.N; p.split_stride = (long long)cs->k * Ncols;
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream);
 }
 

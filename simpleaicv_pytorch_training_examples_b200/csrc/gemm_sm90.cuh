@@ -14,6 +14,8 @@
 //   A_K2D    A is a row-major [M, K] matrix                      (linear fwd / dgrad, 1x1 conv)
 //   A_IM2COL A is an NHWC activation tensor read with TMA im2col (conv fprop / dgrad)
 //   A_MN2D   A is stored [K, M] (K = reduction over pixels)      (wgrad: dY^T)
+//   A_IM2COL_MN A is an NHWC tensor read with TMA im2col, [pixels, C] (transposed conv wgrad dW^T = X^T dY, few filters;
+//            VAR_PLAIN_F32 only)
 //   B_K2D    B is a row-major [N, K] matrix                      (weights, fprop)
 //   B_MN2D   B is stored [K, N]                                  (weights for dgrad, x for wgrad)
 //   B_IM2COL B is an NHWC tensor read with TMA im2col, [pixels, C] (wgrad of a conv)
@@ -23,7 +25,7 @@
 
 namespace saicv {
 
-enum : int { A_K2D = 0, A_IM2COL = 1, A_MN2D = 2 };
+enum : int { A_K2D = 0, A_IM2COL = 1, A_MN2D = 2, A_IM2COL_MN = 3 };
 enum : int { B_K2D = 0, B_MN2D = 2, B_IM2COL = 3 };
 enum : int { EPI_BIAS = 1, EPI_RELU = 2, EPI_GELU = 4, EPI_DIRECT = 8, EPI_RESID = 16, EPI_RESID_BF16 = 32,
               EPI_MUL_DGELU = 64, EPI_ROW_SCALE = 128, EPI_STATS = 256, EPI_MUL_DRELU = 512, EPI_MASK_BITS = 1024 };
@@ -89,6 +91,15 @@ struct GemmParams {
                        // slice, combined in place and stored from there; 0: per-thread global loads
   float* stats_partial;  // EPI_STATS: [gridDim.x][2][N] per-CTA column sums / sums of squares of the bf16 output
   const uint32_t* mask_bits;  // EPI_MASK_BITS: [M][N/32] ReLU mask (bit j of word w: column 32w + j); applied last as D *= bit
+  int tile_rows;       // rows of D per work item (BM; the phase dgrad stores whole rows of the compact dy: (BM / Q) * Q)
+  // Data gradient of a 3x3 / stride 2 / pad 1 convolution by output phase: dx pixel (2p+a, 2q+b) only receives dy at
+  // (p, q) + {0, 1}^2 through a fixed subset of the taps, so each phase (a, b) is a stride-1 correlation over the compact
+  // dy with 1, 2 or 4 taps (9 in all).  `phases` (1 otherwise) is the outermost work index; D is stored through a 5-D
+  // map {c, b, q, a, n*P + p} over dx (capi_gemm.cu: saicv_conv_dgrad).
+  int phases;
+  int ph_out[4];       // (a << 1) | b of each phase, in work order
+  int ph_taps[4];      // taps of each phase
+  int ph_tab[4][4];    // per tap, in reduction order: weight tap (r*S + s) | dy row offset << 8 | dy column offset << 9
 };
 
 // Kernel variants: the epilogue's feature set is a compile-time mask, so that the common launches run a compact
@@ -104,17 +115,21 @@ struct GemmParams {
 //                   a staged slice cost ~2.8x the work of staging it (instruction count), so they are taken off the
 //                   epilogue warps.  The stats warps read the slice from shared memory while the epilogue
 //                   warps are already draining the next chunk (handshake: staged / stats-done mbarriers per slice).
-enum : int { VAR_FULL = 0, VAR_PLAIN_BF16 = 1, VAR_PLAIN_F32 = 2, VAR_AUX = 3, VAR_STATS_BF16 = 4 };
+//   VAR_PHASE_BF16  bf16 output, no epilogue operation: the stride-2 data gradient by output phase (GemmParams::phases), a
+//                   variant of its own so that the other launches do not carry its work decomposition
+enum : int { VAR_FULL = 0, VAR_PLAIN_BF16 = 1, VAR_PLAIN_F32 = 2, VAR_AUX = 3, VAR_STATS_BF16 = 4, VAR_PHASE_BF16 = 5 };
 template <int VAR>
 struct GemmVariant {
   static constexpr int kMask = VAR == VAR_FULL ? (0x7fffffff & ~EPI_MASK_BITS)
                                : (VAR == VAR_PLAIN_BF16 || VAR == VAR_STATS_BF16) ? (EPI_BIAS | EPI_RELU | EPI_STATS)
                                : VAR == VAR_PLAIN_F32 ? EPI_BIAS
+                               : VAR == VAR_PHASE_BF16 ? 0
                                : (EPI_BIAS | EPI_ROW_SCALE | EPI_RESID | EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU |
                                   EPI_MASK_BITS);
-  static constexpr int kOut = (VAR == VAR_PLAIN_BF16 || VAR == VAR_STATS_BF16) ? 1 : VAR == VAR_PLAIN_F32 ? 2 : 0;   // 0: run time, 1: bf16, 2: fp32
+  static constexpr int kOut = (VAR == VAR_PLAIN_BF16 || VAR == VAR_STATS_BF16 || VAR == VAR_PHASE_BF16) ? 1 : VAR == VAR_PLAIN_F32 ? 2 : 0;   // 0: run time, 1: bf16, 2: fp32
   static constexpr int kAux = VAR == VAR_FULL ? 0 : VAR == VAR_AUX ? 2 : 1;                // 0: run time, 1: never, 2: always by TMA
   static constexpr bool kStatsWarps = VAR == VAR_STATS_BF16;                               // statistics by warps 12..15
+  static constexpr bool kPhases = VAR == VAR_PHASE_BF16;                                   // GemmParams::phases / tile_rows honoured
   static constexpr int kThreads = kStatsWarps ? kGemmThreads + 128 : kGemmThreads;
 };
 
@@ -160,6 +175,32 @@ __device__ __forceinline__ void gemm_mainloop(float (&acc)[2][32], const uint8_t
   if (prev >= 0) {
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
+  }
+}
+
+// Operand A of the transposed conv weight gradient, im2col patches MN-major: the 64 output pixels kb*64 .. +63
+// (reduction rows) x NCH 64-wide column chunks from chunk cb0 (chunk cb = tap * cchunks + channel chunk), chunk j at
+// +8192 B, the same loads as B_IM2COL.  Chunks past the R*S taps read image n_img, out of bounds: zeros.
+template <int NCH>
+__device__ __forceinline__ void load_patch_chunks(const CUtensorMap* tm, uint64_t* bar, uint8_t* dst, const ConvGeom& g,
+                                                  int cb0, int kb) {
+  const int pix = kb * BK;
+  const int PQ = g.P * g.Q;
+  const int bn_ = pix / PQ;
+  const int rem = pix - bn_ * PQ;
+  const int pp = rem / g.Q;
+  const int bh = pp * g.stride + g.lc_h;
+  const int bw = (rem - pp * g.Q) * g.stride + g.lc_w;
+#pragma unroll
+  for (int j = 0; j < NCH; ++j) {
+    const int cb = cb0 + j;
+    const int tapj = cb / g.cchunks;
+    const int ccj = cb - tapj * g.cchunks;
+    const int rj = tapj / g.S;
+    const int sj = tapj - rj * g.S;
+    const bool valid = tapj < g.R * g.S;
+    tma_load_im2col_4d(tm, bar, dst + j * 8192, ccj * 64, bw, bh, valid ? bn_ : g.n_img, (uint16_t)(valid ? sj : 0),
+                       (uint16_t)(valid ? rj : 0));
   }
 }
 
@@ -216,9 +257,12 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
   __syncthreads();
 
-  const int num_m = (p.M + BM - 1) / BM;
+  const int phases = V::kPhases ? p.phases : 1;
+  const int tile_rows = V::kPhases ? p.tile_rows : BM;
+  const int num_m = (p.M + tile_rows - 1) / tile_rows;
   const int num_n = (p.N + BN - 1) / BN;
-  const int total = num_m * num_n * p.splits;
+  const int per_phase = num_m * num_n * p.splits;
+  const int total = per_phase * phases;
 
   if (warp == 0) {
     // ================================================================ TMA producer
@@ -227,13 +271,15 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       uint32_t phase = 0;
       const int PQ = p.g.P * p.g.Q;
       for (int w = blockIdx.x; w < total; w += gridDim.x) {
-        const int n_blk = w % num_n;
-        const int t = w / num_n;
+        const int ph = V::kPhases ? w / per_phase : 0;
+        const int wp = w - ph * per_phase;
+        const int n_blk = wp % num_n;
+        const int t = wp / num_n;
         const int m_blk = t % num_m;
         const int split = t / num_m;
-        const int m0 = m_blk * BM, n0 = n_blk * BN;
+        const int m0 = m_blk * tile_rows, n0 = n_blk * BN;
         const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
+        const int kb1 = min(phases > 1 ? p.ph_taps[ph] * p.g.cchunks : p.num_kb, kb0 + p.kb_per_split);
         // im2col base pixel of the A tile (fprop / dgrad): fixed for the whole tile
         int a_n = 0, a_h = 0, a_w = 0;
         if (p.a_mode == A_IM2COL) {
@@ -249,18 +295,33 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           mbar_expect_tx(bar, kABytes + kBBytes);
           uint8_t* a_dst = sA + stage * kABytes;
           uint8_t* b_dst = sB + stage * kBBytes;
-          int tap = 0, cc = kb, r = 0, s = 0;
+          int tap = 0, cc = kb, r = 0, s = 0, tapb = 0;   // im2col offsets (r, s) of A, weight tap of B
           if (p.a_mode == A_IM2COL) {
             tap = kb / p.g.cchunks;
             cc = kb - tap * p.g.cchunks;
-            r = tap / p.g.S;
-            s = tap - r * p.g.S;
+            if (phases > 1) {
+              const int e = p.ph_tab[ph][tap];
+              tapb = e & 0xff;
+              r = (e >> 8) & 1;
+              s = (e >> 9) & 1;
+            } else {
+              r = tap / p.g.S;
+              s = tap - r * p.g.S;
+              tapb = p.flip_taps ? (p.g.R * p.g.S - 1 - tap) : tap;
+            }
           }
           // ---- A
           if (p.a_mode == A_K2D) {
             tma_load_2d(&tmA, bar, a_dst, kb * BK, m0);
           } else if (p.a_mode == A_IM2COL) {
             tma_load_im2col_4d(&tmA, bar, a_dst, cc * 64, a_w, a_h, a_n, (uint16_t)s, (uint16_t)r);
+          } else if constexpr (VAR == VAR_PLAIN_F32) {
+            if (p.a_mode == A_IM2COL_MN) {   // transposed conv wgrad: patches [pixels, R*S*C]
+              load_patch_chunks<2>(&tmA, bar, a_dst, p.g, m0 / 64, kb);
+            } else {  // A_MN2D
+              tma_load_2d(&tmA, bar, a_dst, m0, kb * BK);
+              tma_load_2d(&tmA, bar, a_dst + 8192, m0 + 64, kb * BK);
+            }
           } else {  // A_MN2D: [K rows, M cols], two 64-wide column chunks
             tma_load_2d(&tmA, bar, a_dst, m0, kb * BK);
             tma_load_2d(&tmA, bar, a_dst + 8192, m0 + 64, kb * BK);
@@ -270,8 +331,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             tma_load_2d(&tmB, bar, b_dst, kb * BK, n0);
           } else if (p.b_mode == B_MN2D) {
             int col_base = 0, row = kb * BK;
-            if (p.a_mode == A_IM2COL) {  // conv dgrad: weights [Cout, R*S*Cin], mirrored tap
-              const int tapb = p.flip_taps ? (p.g.R * p.g.S - 1 - tap) : tap;
+            if (p.a_mode == A_IM2COL) {  // conv dgrad: weights [Cout, R*S*Cin]
               col_base = tapb * p.b_cin;
               row = cc * 64;
             }
@@ -328,7 +388,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     constexpr int NCH = BN / 32;
     const int c_begin = half ? 2 : 0;
     const int c_end = half ? NCH : 2;
-    const bool a_mn = (p.a_mode == A_MN2D), b_mn = (p.b_mode != B_K2D);
+    const bool a_mn = VAR == VAR_PLAIN_F32 ? (p.a_mode == A_MN2D || p.a_mode == A_IM2COL_MN) : (p.a_mode == A_MN2D);
+    const bool b_mn = (p.b_mode != B_K2D);
     int stage = 0;
     uint32_t phase = 0;
     const int spt = out_f32 ? (c_end - c_begin) : ((c_end - c_begin) >> 1);  // slices per tile of this half
@@ -343,7 +404,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const int m_blk2 = (int)((pf_w / num_n) % num_m);
         const int col = n_blk2 * BN + (out_f32 ? (c_begin + pf_j) * 32 : ((c_begin >> 1) + pf_j) * 64);
         mbar_expect_tx(&abar[pf_b], kStoreBufBytes);   // rows / columns past the matrix are zero-filled and counted
-        tma_load_3d(&tmR, &abar[pf_b], sbase + pf_b * kStoreBufBytes, col, m_blk2 * BM, 0);
+        tma_load_3d(&tmR, &abar[pf_b], sbase + pf_b * kStoreBufBytes, col, m_blk2 * tile_rows, 0);
       }
       if (++pf_j == spt) { pf_j = 0; pf_w += gridDim.x; }
       if (++pf_b == NB) pf_b = 0;
@@ -359,17 +420,19 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       named_bar_sync(3, kStatBarThreads);
     }
     for (int w = blockIdx.x; w < total; w += gridDim.x) {
-      const int n_blk = w % num_n;
-      const int t = w / num_n;
+      const int ph = V::kPhases ? w / per_phase : 0;
+      const int wp = w - ph * per_phase;
+      const int n_blk = wp % num_n;
+      const int t = wp / num_n;
       const int m_blk = t % num_m;
       const int split = t / num_m;
-      const int m0 = m_blk * BM, n0 = n_blk * BN;
+      const int m0 = m_blk * tile_rows, n0 = n_blk * BN;
       const long long row = m0 + row_in_tile;
       if (c_begin >= c_end) continue;   // half 1 of a 64-wide tile: no columns
       float acc[2][32];
       {
         const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
+        const int kb1 = min(phases > 1 ? p.ph_taps[ph] * p.g.cchunks : p.num_kb, kb0 + p.kb_per_split);
         const uint32_t b_off = half * 8192u;   // column 64 of a B stage (K-major: row 64; MN-major: second chunk)
         if (a_mn) gemm_mainloop<BN, 1, 1>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, b_off, lane);
         else if (b_mn) gemm_mainloop<BN, 0, 1>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, b_off, lane);
@@ -538,7 +601,14 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             named_bar_sync(bar_id, 128);
             const int scol = out_f32 ? col0 : col0 - 32;
             if (gtid == 0) {
-              if (scol < p.N) {
+              if (scol < p.N && phases > 1) {
+                const int ab = p.ph_out[ph];
+                asm volatile(
+                    "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(
+                        reinterpret_cast<uint64_t>(&tmD)),
+                    "r"(smem_u32(sbuf)), "r"(scol), "r"(ab & 1), "r"(0), "r"(ab >> 1), "r"(m0 / p.g.Q)
+                    : "memory");
+              } else if (scol < p.N) {
                 asm volatile(
                     "cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
                         reinterpret_cast<uint64_t>(&tmD)),

@@ -273,9 +273,8 @@ class ConvBN:
         w = self.conv.weight
         wbuf, wacc = sink.begin(w)
         n, P, Q, _ = dy.shape
-        h, wd = tape['in_hw']
         if self.is_stem:
-            part = ops.linear_wgrad(dy.view(-1, self.kp), tape['cols'])
+            part = ops.linear_wgrad(dy.view(-1, self.kp), tape['cols'], transposed=ops.wgrad_transposed(self.kp, self.kpad))
             ops.finish_conv_wgrad(part, wbuf, self.kpad, accumulate=wacc, order=ops.ORDER_CRS, kp=self.kp)
             sink.done(w, wbuf)
             assert not need_dx, 'the stem has no data gradient'
@@ -286,15 +285,10 @@ class ConvBN:
         sink.done(w, wbuf)
         if not need_dx:
             return None
-        if self.stride == 1:
-            return ops.conv_dgrad(dy, self.op.w, cs, add=add, mask_bits=mask_bits)
-        assert self.stride == 2
-        if self.r == 1:
+        if self.stride == 2 and self.r == 1:
             assert add is None and mask_bits is None
             return 'strided', ops.linear_dgrad(dy.view(-1, self.kp), self.op.w).view(n, P, Q, self.cp)
-        u = ops.zero_upsample2(dy, h, wd)
-        cs1 = ops.make_conv_shape(n, h, wd, self.cp, self.kp, self.r, self.s, 1, self.pad)
-        return ops.conv_dgrad(u, self.op.w, cs1, add=add, mask_bits=mask_bits)
+        return ops.conv_dgrad(dy, self.op.w, cs, add=add, mask_bits=mask_bits)
 
 
 class ResidualBlockRT:

@@ -75,14 +75,21 @@ def wgrad_splits(out_rows, out_cols, reduce_len):
     return _lib.load().saicv_wgrad_splits(out_rows, out_cols, reduce_len)
 
 
-def linear_wgrad(dy, x, partial=None):
-    """Returns fp32 partials [splits, N, K]; reduce with reduce_partials."""
+def wgrad_transposed(out_rows, out_cols):
+    """Whether the weight gradient dW [out_rows, out_cols] runs as dW^T on fewer padded tiles (few filters)."""
+    return bool(_lib.load().saicv_wgrad_transposed(out_rows, out_cols))
+
+
+def linear_wgrad(dy, x, partial=None, transposed=False):
+    """Returns fp32 partials [splits, N, K] (dW = dy^T x); reduce with reduce_partials.  transposed: partials
+    [splits, K, N] of dW^T = x^T dy over the same splits (every element is the same sum)."""
     M, N = dy.shape
     K = x.shape[1]
     splits = wgrad_splits(N, K, M)
+    a, b, rows, cols = (x, dy, K, N) if transposed else (dy, x, N, K)
     if partial is None:
-        partial = torch.empty(splits, N, K, device=dy.device, dtype=torch.float32)
-    _lib.call('saicv_linear_wgrad', _p(dy), _p(x), _p(partial), M, N, K, splits, _stream())
+        partial = torch.empty(splits, rows, cols, device=dy.device, dtype=torch.float32)
+    _lib.call('saicv_linear_wgrad', _p(a), _p(b), _p(partial), M, rows, cols, splits, _stream())
     return partial
 
 
@@ -103,10 +110,23 @@ def conv_fprop(x, w, cs, out=None, flags=0, stats=None):
     return out
 
 
+def phase_dgrad_ok(cs):
+    """Whether saicv_conv_dgrad takes this stride-2 conv directly (by output phase, on the compact dy): 3x3, pad 1,
+    even h and w, w <= 256 (one 128-row tile holds a whole dy row)."""
+    return (cs.stride == 2 and cs.r == 3 and cs.s == 3 and cs.pad == 1 and cs.h % 2 == 0 and cs.w % 2 == 0
+            and cs.w <= 256)
+
+
 def conv_dgrad(dy, w, cs, out=None, add=None, mask_bits=None):
-    """dy: [n, h, w, k] (zero-upsampled for strided convs); cs.stride must be 1.
+    """dy: [n, P, Q, k], the gradient w.r.t. the conv output; cs: the conv's own shape, stride 1 or 2.
     add: optional bf16 [n, h, w, c] tensor summed into the result in the GEMM epilogue.
-    mask_bits: optional ReLU mask from bn_apply (needs `add`); the sum is multiplied by it."""
+    mask_bits: optional ReLU mask from bn_apply (needs `add`); the sum is multiplied by it.
+    A stride-2 conv that phase_dgrad_ok() rejects, or one with `add`, runs as the stride-1 data gradient of the
+    zero-upsampled dy."""
+    if cs.stride != 1 and not (phase_dgrad_ok(cs) and add is None and mask_bits is None):
+        assert cs.stride == 2, cs.stride
+        dy = zero_upsample2(dy, cs.h, cs.w)
+        cs = make_conv_shape(cs.n, cs.h, cs.w, cs.c, cs.k, cs.r, cs.s, 1, cs.pad)
     if out is None:
         out = torch.empty(cs.n, cs.h, cs.w, cs.c, device=dy.device, dtype=torch.bfloat16)
     _lib.call('saicv_conv_dgrad', _p(dy), _p(w), _p(add), _p(mask_bits), _p(out), ctypes.byref(cs), _stream())
@@ -119,7 +139,9 @@ def conv_wgrad(dy, x, cs, partial=None):
     ncols = cs.r * cs.s * cs.c
     splits = wgrad_splits(cs.k, ncols, cs.n * P * Q)
     if partial is None:
-        partial = torch.empty(splits, cs.k, ncols, device=dy.device, dtype=torch.float32)
+        # [splits, k, ncols], or [splits, ncols, k] when saicv_conv_wgrad computes dW^T (few filters)
+        shape = (splits, ncols, cs.k) if wgrad_transposed(cs.k, ncols) else (splits, cs.k, ncols)
+        partial = torch.empty(shape, device=dy.device, dtype=torch.float32)
     _lib.call('saicv_conv_wgrad', _p(dy), _p(x), _p(partial), ctypes.byref(cs), splits, _stream())
     return partial
 
@@ -135,9 +157,13 @@ def prep_conv_weight(w_f32, out, kpad, order=ORDER_RSC, kp=0, cp=0):
 
 
 def finish_conv_wgrad(partial, grad, kpad, accumulate=False, order=ORDER_RSC, kp=0, cp=0):
+    """partial: [splits, kp, kpad], or [splits, kpad, kp] where conv_wgrad / the stem's linear_wgrad computed dW^T
+    (wgrad_transposed(kp, kpad); never when kp == kpad)."""
     k, c, r, s = grad.shape
+    rows = kp or k
+    transposed = tuple(partial.shape[1:]) == (kpad, rows) and wgrad_transposed(rows, kpad)
     _lib.call('saicv_finish_conv_wgrad', _p(partial), _p(grad), partial.shape[0], k, c, r, s, kpad,
-              int(accumulate), order, kp, cp, _stream())
+              int(accumulate), order, kp, cp, int(transposed), _stream())
     return grad
 
 
