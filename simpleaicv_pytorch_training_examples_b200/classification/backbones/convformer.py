@@ -8,7 +8,7 @@ import numpy as np
 import torch.nn as nn
 
 from ...engine.convformer import ConvFormerRT
-from ...engine.convnet import run_network
+from ...engine.runtime import RuntimeModule
 
 __all__ = ['convformer_s18', 'convformer_s36', 'convformer_m36', 'convformer_b36']
 
@@ -68,7 +68,7 @@ class MetaFormerBlock(nn.Module):
         self.drop_path = DropPathBlock(drop_path_prob) if drop_path_prob > 0. else nn.Identity()
 
 
-class MetaFormer(nn.Module):
+class MetaFormer(RuntimeModule):
 
     def __init__(self, inplanes=3, embedding_planes=[64, 128, 320, 512], block_nums=[2, 2, 6, 2], dropout_prob=0.,
                  drop_path_prob=0., num_classes=1000, use_gradient_checkpoint=False):
@@ -102,20 +102,11 @@ class MetaFormer(nn.Module):
                 nn.init.constant_(m.weight, 1)
                 nn.init.constant_(m.bias, 0)
 
-    def _runtime(self):
-        rt = self.__dict__.get('_rt')
-        if rt is None:
-            rt = ConvFormerRT(self)
-            self.__dict__['_rt'] = rt
-        return rt
-
-    def grad_sink(self):
-        return self._runtime().sink
+    def _build_runtime(self):
+        return ConvFormerRT(self)
 
     def forward(self, x):
-        if not x.is_cuda:
-            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
-        return run_network(self._runtime(), x.float(), self.training)
+        return self._run(x.float())
 
 
 def _metaformer(block_nums, embedding_planes, **kwargs):

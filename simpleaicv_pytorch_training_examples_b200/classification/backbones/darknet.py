@@ -10,8 +10,9 @@ stages (engine.convnet.MaxPoolRT / ConvHeadRT).
 """
 import torch.nn as nn
 
-from ...engine.convnet import (ACT_LEAKY, ACT_RELU, ACT_SILU, ConvBN, ConvHeadRT, DarkBlockRT, MaxPoolRT, PlainUnitRT,
-                               ResNetRT, run_network)
+from ...engine.convnet import ACT_LEAKY, ACT_RELU, ACT_SILU, ConvBN, ConvHeadRT, DarkBlockRT, MaxPoolRT, PlainUnitRT, ResNetRT
+from ...engine.runtime import RuntimeModule
+from .resnet import _init_like_reference  # same initialisation as the reference's darknet.py:218-225,299-306,397-404
 
 __all__ = ['darknettiny', 'darknet19', 'darknet53']
 
@@ -69,32 +70,10 @@ class Darknet53Block(nn.Module):
             ConvBnActBlock(squeezed, inplanes, kernel_size=3, stride=1, padding=1, act_type=act_type))
 
 
-def _init_like_reference(model):  # darknet.py:218-225,299-306,397-404
-    for m in model.modules():
-        if isinstance(m, nn.Conv2d):
-            nn.init.kaiming_normal_(m.weight, mode='fan_out', nonlinearity='relu')
-        elif isinstance(m, (nn.BatchNorm2d, nn.GroupNorm)):
-            nn.init.constant_(m.weight, 1)
-            nn.init.constant_(m.bias, 0)
-
-
-class _DarknetBase(nn.Module):
-
-    def _runtime(self):
-        rt = self.__dict__.get('_rt')
-        if rt is None:
-            rt = self._build_runtime(_ACT[self.act_type])
-            self.__dict__['_rt'] = rt
-        return rt
-
-    def grad_sink(self):
-        return self._runtime().sink
+class _DarknetBase(RuntimeModule):
 
     def forward(self, x):
-        if not x.is_cuda:
-            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU '
-                               '(no CPU fallback exists)')
-        return run_network(self._runtime(), x.float(), self.training)
+        return self._run(x.float())
 
 
 class DarknetTiny(_DarknetBase):
@@ -113,7 +92,8 @@ class DarknetTiny(_DarknetBase):
         self.fc = nn.Linear(512, self.num_classes)
         _init_like_reference(self)
 
-    def _build_runtime(self, act):
+    def _build_runtime(self):
+        act = _ACT[self.act_type]
         stages = [MaxPoolRT(2, 2)]
         for i in range(2, 7):
             stages.append(PlainUnitRT(getattr(self, f'conv{i}'), act))
@@ -141,7 +121,8 @@ class Darknet19(_DarknetBase):
         self.avgpool = nn.AdaptiveAvgPool2d((1, 1))
         _init_like_reference(self)
 
-    def _build_runtime(self, act):
+    def _build_runtime(self):
+        act = _ACT[self.act_type]
         stages = [MaxPoolRT(2, 2)]
         for i in range(2, 7):
             blk = getattr(self, f'layer{i}')
@@ -167,7 +148,8 @@ class Darknet53(_DarknetBase):
         self.fc = nn.Linear(1024, num_classes)
         _init_like_reference(self)
 
-    def _build_runtime(self, act):
+    def _build_runtime(self):
+        act = _ACT[self.act_type]
         stages = []
         for i in range(5):
             stages.append(PlainUnitRT(getattr(self, f'conv{i + 2}'), act))

@@ -11,7 +11,8 @@ is no fallback path.
 import torch
 import torch.nn as nn
 
-from ...engine.convnet import ResNetRT, run_network
+from ...engine.convnet import ResNetRT
+from ...engine.runtime import RuntimeModule
 
 __all__ = ['resnet18', 'resnet34', 'resnet50', 'resnet101', 'resnet152']
 
@@ -71,7 +72,7 @@ def _init_like_reference(model):
             nn.init.constant_(m.bias, 0)
 
 
-class _ResNetBase(nn.Module):
+class _ResNetBase(RuntimeModule):
     """Shared body: 4 stages of residual blocks, global average pool, fc."""
 
     def _build_stages(self, block, layer_nums, inplanes):
@@ -89,23 +90,11 @@ class _ResNetBase(nn.Module):
         self.avgpool = nn.AdaptiveAvgPool2d((1, 1))
         self.fc = nn.Linear(self.planes[3] * self.expansion, self.num_classes)
 
-    def _runtime(self):
-        rt = self.__dict__.get('_rt')
-        if rt is None:
-            rt = ResNetRT(self, has_maxpool=hasattr(self, 'maxpool1'),
-                          checkpoint=getattr(self, 'use_gradient_checkpoint', False))
-            self.__dict__['_rt'] = rt  # not a submodule / not in state_dict
-        return rt
-
-    def grad_sink(self):
-        """Where the runtime deposits parameter gradients (used by distributed.B200DataParallel)."""
-        return self._runtime().sink
+    def _build_runtime(self):
+        return ResNetRT(self, has_maxpool=hasattr(self, 'maxpool1'), checkpoint=getattr(self, 'use_gradient_checkpoint', False))
 
     def forward(self, x):
-        if not x.is_cuda:
-            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU '
-                               '(no CPU fallback exists)')
-        return run_network(self._runtime(), x.float(), self.training)
+        return self._run(x.float())
 
 
 class ResNet(_ResNetBase):

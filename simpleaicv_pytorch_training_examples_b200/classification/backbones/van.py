@@ -10,7 +10,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from ...engine.convnet import run_network
+from ...engine.runtime import RuntimeModule
 from ...engine.van import VANRT
 
 __all__ = ['van_b0', 'van_b1', 'van_b2', 'van_b3', 'van_b4', 'van_b5', 'van_b6']
@@ -86,7 +86,7 @@ class OverlapPatchEmbed(nn.Module):
         self.norm = nn.BatchNorm2d(embedding_planes)
 
 
-class VAN(nn.Module):
+class VAN(RuntimeModule):
 
     def __init__(self, inplanes=3, embedding_planes=[64, 128, 256, 512], mlp_ratios=[4, 4, 4, 4], block_nums=[3, 4, 6, 3],
                  dropout_prob=0., drop_path_prob=0., num_classes=1000, use_gradient_checkpoint=False):
@@ -125,20 +125,11 @@ class VAN(nn.Module):
                 if m.bias is not None:
                     m.bias.data.zero_()
 
-    def _runtime(self):
-        rt = self.__dict__.get('_rt')
-        if rt is None:
-            rt = VANRT(self)
-            self.__dict__['_rt'] = rt
-        return rt
-
-    def grad_sink(self):
-        return self._runtime().sink
+    def _build_runtime(self):
+        return VANRT(self)
 
     def forward(self, x):
-        if not x.is_cuda:
-            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
-        return run_network(self._runtime(), x.float(), self.training)
+        return self._run(x.float())
 
 
 def _van(embedding_planes, mlp_ratios, block_nums, **kwargs):

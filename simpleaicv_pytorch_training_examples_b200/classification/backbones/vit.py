@@ -9,7 +9,7 @@ state_dict keys); ``forward`` hands the batch to the runtime.  CPU tensors raise
 import torch
 import torch.nn as nn
 
-from ...engine.convnet import run_network
+from ...engine.runtime import RuntimeModule
 from ...engine.vit import ViTRT
 
 __all__ = ['vit_base_patch16', 'vit_large_patch16', 'vit_huge_patch14']
@@ -68,7 +68,7 @@ class TransformerEncoderLayer(nn.Module):
         self.drop_path = DropPathBlock(drop_path_prob) if drop_path_prob > 0. else nn.Identity()
 
 
-class ViT(nn.Module):
+class ViT(RuntimeModule):
 
     def __init__(self, patch_size, embedding_planes, block_nums, head_nums, feedforward_ratio, image_size=224,
                  dropout_prob=0., drop_path_prob=0., global_pool=False, num_classes=1000,
@@ -105,21 +105,11 @@ class ViT(nn.Module):
         nn.init.trunc_normal_(self.fc.weight, std=2e-5)
         nn.init.zeros_(self.fc.bias)
 
-    def _runtime(self):
-        rt = self.__dict__.get('_rt')
-        if rt is None:
-            rt = ViTRT(self)
-            self.__dict__['_rt'] = rt
-        return rt
-
-    def grad_sink(self):
-        return self._runtime().sink
+    def _build_runtime(self):
+        return ViTRT(self)
 
     def forward(self, x):
-        if not x.is_cuda:
-            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU '
-                               '(no CPU fallback exists)')
-        return run_network(self._runtime(), x.float(), self.training)
+        return self._run(x.float())
 
 
 def _vit(patch_size, embedding_planes, block_nums, head_nums, feedforward_ratio, **kwargs):

@@ -3,7 +3,7 @@
 Same class names and call signature as SimpleAICV/classification/losses.py:14-28 (CELoss) and
 :78-91 (OneHotLabelCELoss).  They stay plain torch: [B, num_classes] fp32 work is negligible
 next to the backbone and is not a kernel target; its gradient feeds our backward through
-engine.convnet._NetFunction.
+the autograd node of engine.runtime.
 """
 import torch
 import torch.nn as nn

@@ -16,7 +16,8 @@ import torch.nn.functional as F
 from . import backbones
 from .backbones.detr_resnet import PositionEmbeddingBlock
 from .head import DETRClsRegHead
-from ...engine.detr import DetrRT, run_detr
+from ...engine.detr import DetrRT
+from ...engine.runtime import RuntimeModule
 
 __all__ = ['resnet18_detr', 'resnet34_detr', 'resnet50_detr', 'resnet101_detr', 'resnet152_detr']
 
@@ -78,7 +79,7 @@ class DETRTransformer(nn.Module):
                 nn.init.xavier_uniform_(m)
 
 
-class DETR(nn.Module):
+class DETR(RuntimeModule):
 
     def __init__(self, backbone_type, backbone_pretrained_path='', hidden_inplanes=256, query_nums=100, num_classes=80,
                  use_gradient_checkpoint=False):
@@ -94,27 +95,18 @@ class DETR(nn.Module):
         self.query_embed = nn.Embedding(query_nums, hidden_inplanes)
         self.head = DETRClsRegHead(hidden_inplanes, num_classes + 1, num_layers=3)
 
-    def _runtime(self):
-        rt = self.__dict__.get('_rt')
-        if rt is None:
-            rt = DetrRT(self)
-            self.__dict__['_rt'] = rt  # not a submodule / not in state_dict
-        return rt
-
-    def grad_sink(self):
-        return self._runtime().sink
+    def _build_runtime(self):
+        return DetrRT(self)
 
     def forward(self, inputs, masks):
         """inputs fp32 [B, 3, H, W]; masks bool [B, H, W] (True = padding).  Returns [cls_outputs [6, B, Q, classes + 1],
         reg_outputs [6, B, Q, 4]] like the reference (detr.py:309-364)."""
         assert masks is not None
-        if not inputs.is_cuda:
-            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
         fh, fw = _feature_size(inputs.shape[2]), _feature_size(inputs.shape[3])
         fm = F.interpolate(masks.float().unsqueeze(1), size=[fh, fw]).to(torch.bool).squeeze(1)
         pos = self.position_embedding(fm).flatten(2).transpose(1, 2).reshape(-1, self.hidden_inplanes).contiguous()
         key_bias = fm.flatten(1).float().reshape(-1).contiguous()        # float key_padding_mask: +1 on padded keys
-        cls, reg = run_detr(self._runtime(), inputs.float(), pos, key_bias, self.training)
+        cls, reg = self._run(inputs.float(), pos, key_bias)
         return [cls, reg.float().sigmoid()]
 
 

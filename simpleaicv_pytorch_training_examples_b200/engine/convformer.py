@@ -28,8 +28,9 @@ mode, so every BatchNorm receives a second running-statistics momentum update (a
 import torch
 
 from .. import ops
-from .convnet import FcHeadRT, GradSink
+from .convnet import FcHeadRT
 from .operands import Linear
+from .runtime import Runtime
 from .van import StridedConv, _bn_backward, _bn_forward
 
 
@@ -165,7 +166,7 @@ class _Head(FcHeadRT):
         return ops.avgpool_stream_bwd(self.fc_backward(dlogits, tape, sink), h, w).view(-1, c)
 
 
-class ConvFormerRT:
+class ConvFormerRT(Runtime):
     """Whole-network runtime (convformer.py:169-256)."""
 
     def __init__(self, model):
@@ -173,16 +174,8 @@ class ConvFormerRT:
         self.downs = [_Downsampling(d) for d in model.downsample_layers]
         self.stages = [[_Block(b) for b in stage] for stage in model.stages]
         self.head = _Head(model.head)
-        self.sink = GradSink()
-        self._units = [u for d, blocks in zip(self.downs, self.stages) for u in [d] + [lin for b in blocks for lin in b.linears()]]
-        self._units.append(self.head)
-
-    def operands(self):
-        return [u.op for u in self._units]
-
-    def prep(self):
-        for u in self._units:
-            u.prep()
+        super().__init__([u for d, blocks in zip(self.downs, self.stages) for u in [d] + [lin for b in blocks for lin in b.linears()]]
+                         + [self.head])
 
     # layer-level entry points (also driven by the teacher-forced parity tests); stream tensors are [rows, C]
     def stem_forward(self, x, t, training):
@@ -249,5 +242,3 @@ class ConvFormerRT:
                 self.down_forward(i, ck['in'], ck['in_shape'], t, True)
             d = self.down_backward(i, d, t)
             tape['downs'][i] = None
-        if self.sink.on_backward_end is not None:
-            self.sink.on_backward_end()

@@ -19,6 +19,7 @@ import torch
 
 from .. import ops
 from .operands import CONV, STEM, Linear, Operand, rows_wgrad
+from .runtime import GradSink, Runtime  # noqa: F401  GradSink: still importable from here, where it used to live
 
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SILU = 0, 1, 2, 3
 # BatchNorm batch statistics are accumulated by the conv GEMM's epilogue instead of a separate pass over y
@@ -27,37 +28,6 @@ FUSE_BN_STATS = True
 
 def _round_up(v, m):
     return (v + m - 1) // m * m
-
-
-class GradSink:
-    """Where parameter gradients go: ``param.grad`` by default, or bucket views supplied by the
-    data-parallel wrapper (distributed.py) so that the all-reduce runs on flat buffers."""
-
-    def __init__(self):
-        self.views = {}       # id(param) -> fp32 tensor view with the parameter's shape
-        self.on_ready = None  # callback(param) fired as soon as a gradient is complete
-        self.on_backward_end = None  # callback() fired when the whole backward pass is enqueued
-
-    def buffer_for(self, param):
-        v = self.views.get(id(param))
-        if v is None:
-            v = torch.empty_like(param, dtype=torch.float32)
-            self.views[id(param)] = v
-        return v
-
-    def begin(self, param):
-        """Returns (buffer, accumulate): accumulate when param.grad already holds a gradient."""
-        buf = self.buffer_for(param)
-        if param.grad is None:
-            return buf, False
-        if param.grad.data_ptr() != buf.data_ptr():
-            buf.copy_(param.grad)
-        return buf, True
-
-    def done(self, param, buf):
-        param.grad = buf
-        if self.on_ready is not None:
-            self.on_ready(param)
 
 
 # BatchNorm's `num_batches_tracked += 1` of every layer of one network forward, applied by ONE torch._foreach_add_ at the end
@@ -549,7 +519,7 @@ class ConvHeadRT:
         return ops.linear_dgrad(dy, self.op.w).view(n, h, w, c)
 
 
-class ResNetRT:
+class ResNetRT(Runtime):
     """Whole-network runtime for the conv -> BN -> act classifiers: ResNet (resnet.py:158-245),
     ResNetCifar (resnetforcifar.py:27-108), DarknetTiny / Darknet19 / Darknet53 (darknet.py:147-432):
     stem [+ maxpool] + a sequence of stages + head (global average pool + fc, or Darknet19's 1x1-conv
@@ -574,21 +544,13 @@ class ResNetRT:
         self.blocks = blocks
         self.head = head if head is not None else FcHeadRT(model.fc)
         self.checkpoint = checkpoint
-        self.sink = GradSink()
-        self._units = self.units() + [self.head]
+        super().__init__(self.units() + [self.head])
 
     def units(self):
         us = [self.stem]
         for b in self.blocks:
             us += b.all_units()
         return us
-
-    def operands(self):
-        return [u.op for u in self._units]
-
-    def prep(self):
-        for u in self._units:
-            u.prep()
 
     # The network is run as three stages (stem / residual blocks / head) so that tests can drive
     # each stage with the oracle's tensors (tests/test_resnet_gpu.py, teacher-forced parity).
@@ -636,39 +598,7 @@ class ResNetRT:
         self.stem.conv_bwd(dy, tape['stem'], self.sink, need_dx=False)
 
     def backward(self, dlogits, tape):
-        sink = self.sink
         assert tape is not None, 'backward called without a training forward'
         da = self.head_backward(dlogits, tape)
-        da = blocks_backward(self.blocks, tape['blocks'], da, sink)
+        da = blocks_backward(self.blocks, tape['blocks'], da, self.sink)
         self.stem_backward(da, tape)
-        if sink.on_backward_end is not None:
-            sink.on_backward_end()
-
-
-class _NetFunction(torch.autograd.Function):
-    """Couples the runtime to autograd: the criterion (torch) differentiates the logits, this
-    node receives dlogits and runs the whole backward pass on our kernels.  Parameter gradients
-    are produced as a side effect (GradSink), so no parameter is an autograd input.  The tape of
-    saved activations belongs to THIS forward (it lives on ctx), so several forwards of one module
-    may be in flight before their backwards run."""
-
-    @staticmethod
-    def forward(ctx, x, anchor, rt):
-        ctx.rt = rt
-        out, ctx.tape = rt.forward(x, True, True)
-        return out
-
-    @staticmethod
-    def backward(ctx, dlogits):
-        tape, ctx.tape = ctx.tape, None
-        assert tape is not None, 'the graph of this forward pass was already differentiated'
-        ctx.rt.backward(dlogits, tape)
-        return None, None, None
-
-
-def run_network(rt, x, training):
-    if training and torch.is_grad_enabled():
-        anchor = torch.zeros((), device=x.device, requires_grad=True)
-        return _NetFunction.apply(x, anchor, rt)
-    with torch.no_grad():
-        return rt.forward(x, training, False)[0]

@@ -20,8 +20,9 @@ csrc/dropout_hash.cuh: the backward recomputes the forward's masks from the per-
 import torch
 
 from .. import ops
-from .convnet import GradSink, ResNetRT, blocks_backward
+from .convnet import ResNetRT, blocks_backward
 from .operands import Linear, Operand
+from .runtime import Runtime
 
 
 class _NoHead:
@@ -289,29 +290,21 @@ class _Heads:
         return ops.linear_dgrad(dcb, self.cls.op.w, resid=dhs, out_f32=True)
 
 
-class DetrRT:
+class DetrRT(Runtime):
     """Whole-model runtime; `forward` returns (cls [D, B, Q, classes + 1], box logits [D, B, Q, 4], tape)."""
 
     def __init__(self, model):
         self.model = model
-        self.sink = GradSink()
         self.body = ResNetRT(model.backbone, has_maxpool=True, head=_NoHead(),
                              checkpoint=getattr(model.backbone, 'use_gradient_checkpoint', False))
-        self.body.sink = self.sink
         self.proj = Linear(model.proj_conv)
         tr = model.transformer
         self.enc = [_EncLayer(l) for l in tr.encoder_blocks]
         self.dec = [_DecLayer(l) for l in tr.decoder_blocks]
         self.heads = _Heads(model.head)
         self._seed_base = 0
-        self._units = self.body.units() + [self.proj] + [u for l in self.enc + self.dec for u in l.units()] + self.heads.units()
-
-    def operands(self):
-        return [u.op for u in self._units]
-
-    def prep(self):
-        for u in self._units:
-            u.prep()
+        super().__init__(self.body.units() + [self.proj] + [u for l in self.enc + self.dec for u in l.units()] + self.heads.units())
+        self.body.sink = self.sink
 
     def _context(self, B, L, pos, key_bias, training):
         tr = self.model.transformer
@@ -428,37 +421,4 @@ class DetrRT:
         ops.cast_bf16(dsrc, dsb)
         dc5 = self.proj.bwd(dsb, tape['c5'], sink)
         self.backbone_backward(dc5.view(tape['c5_shape']), tape)
-        if sink.on_backward_end is not None:
-            sink.on_backward_end()
 
-
-class _DetrFunction(torch.autograd.Function):
-    """Couples the runtime to autograd (see engine.convnet._NetFunction): the criterion differentiates the two
-    outputs, this node receives their gradients and runs the whole backward pass on our kernels."""
-
-    @staticmethod
-    def forward(ctx, x, anchor, rt, pos, key_bias):
-        ctx.rt = rt
-        cls, reg, ctx.tape = rt.forward(x, pos, key_bias, True, True)
-        ctx.shapes = (cls.shape, reg.shape)
-        return cls, reg
-
-    @staticmethod
-    def backward(ctx, dcls, dreg):
-        tape, ctx.tape = ctx.tape, None
-        assert tape is not None, 'the graph of this forward pass was already differentiated'
-        if dcls is None:
-            dcls = torch.zeros(ctx.shapes[0], device=dreg.device)
-        if dreg is None:
-            dreg = torch.zeros(ctx.shapes[1], device=dcls.device)
-        ctx.rt.backward(dcls.contiguous(), dreg.contiguous(), tape)
-        return None, None, None, None, None
-
-
-def run_detr(rt, x, pos, key_bias, training):
-    if training and torch.is_grad_enabled():
-        anchor = torch.zeros((), device=x.device, requires_grad=True)
-        return _DetrFunction.apply(x, anchor, rt, pos, key_bias)
-    with torch.no_grad():
-        cls, reg, _ = rt.forward(x, pos, key_bias, training, False)
-        return cls, reg

@@ -16,12 +16,13 @@ stream, bf16 GEMM operands.  The mask indices are computed with torch.rand / tor
 import torch
 
 from .. import ops
-from .convnet import GradSink
 from .operands import Linear, PatchEmbed
+from .runtime import Runtime
 from .vit import _Block, layernorm_bwd
 
 
-class MAERT:
+class MAERT(Runtime):
+    non_differentiable_outputs = 1  # the mask
 
     def __init__(self, model):
         self.model = model
@@ -31,15 +32,7 @@ class MAERT:
         self.e2d = Linear(model.encoder_to_decoder)
         self.fc = Linear(dec.fc)
         self.patch = PatchEmbed(enc.patch_embed.proj)
-        self._units = [lin for b in self.enc_blocks + self.dec_blocks for lin in b.linears()] + [self.e2d, self.fc, self.patch]
-        self.sink = GradSink()
-
-    def operands(self):
-        return [u.op for u in self._units]
-
-    def prep(self):
-        for u in self._units:
-            u.prep()
+        super().__init__([lin for b in self.enc_blocks + self.dec_blocks for lin in b.linears()] + [self.e2d, self.fc, self.patch])
 
     # ---- masking indices (vit_mae.py:203-225), int32 index tables for the gather kernels
     def masking(self, b, n, dev, noise=None):
@@ -61,7 +54,7 @@ class MAERT:
         dec_idx = torch.cat([zero, dec_src], dim=1).to(torch.int32).contiguous()
         return keep_len, mask, enc_idx, enc_pos, dec_idx
 
-    def forward(self, x, training, keep_tape, noise=None):
+    def forward(self, x, noise, training, keep_tape):
         assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 4
         self.prep()
         enc, dec = self.model.encoder, self.model.decoder
@@ -134,33 +127,4 @@ class MAERT:
         cbuf.view(-1).copy_(dcls + (cbuf.view(-1) if cacc else 0))
         sink.done(enc.cls_token, cbuf)
         self.patch.bwd(dpatch.view(b * n, c), tape['cols'], sink)
-        if sink.on_backward_end is not None:
-            sink.on_backward_end()
 
-
-class _MAEFunction(torch.autograd.Function):
-    """The loss tail (torch) differentiates the prediction; this node runs the whole backward on the runtime's kernels
-    and deposits the parameter gradients through the GradSink.  The tape lives on ctx (one per forward)."""
-
-    @staticmethod
-    def forward(ctx, x, anchor, rt, noise):
-        ctx.rt = rt
-        pred, mask, ctx.tape = rt.forward(x, True, True, noise)
-        ctx.mark_non_differentiable(mask)
-        return pred, mask
-
-    @staticmethod
-    def backward(ctx, dpred, dmask):
-        tape, ctx.tape = ctx.tape, None
-        assert tape is not None, 'the graph of this forward pass was already differentiated'
-        ctx.rt.backward(dpred.contiguous(), tape)
-        return None, None, None, None
-
-
-def run_mae(rt, x, training, noise=None):
-    if training and torch.is_grad_enabled():
-        anchor = torch.zeros((), device=x.device, requires_grad=True)
-        return _MAEFunction.apply(x, anchor, rt, noise)
-    with torch.no_grad():
-        pred, mask, _ = rt.forward(x, training, False, noise)
-        return pred, mask

@@ -1,0 +1,122 @@
+"""The one boundary between torch and a model runtime.
+
+A runtime (``ResNetRT``, ``ViTRT``, ``DetrRT``, ...) runs a whole model forward and backward on the kernels of
+libsaicv_b200.so; its nn.Module shell (``RuntimeModule``) hands it the batch through ``run``, and the loss tail stays in
+torch.  ``run`` couples the two through one autograd node, and every runtime keeps this contract:
+
+  * ``rt.forward(*inputs, training, keep_tape)`` returns ``(*outputs, tape)``; the tape, which holds what the backward
+    needs, is None unless keep_tape.
+  * ``rt.backward(*grads, tape)`` receives one gradient per differentiable output, each contiguous.  An output that
+    took no part in the loss gets zeros of its shape (autograd materializes them for a Function).
+  * The last ``rt.non_differentiable_outputs`` outputs (MAE's mask) are marked non-differentiable and get no gradient.
+  * Parameter gradients never travel through autograd: the runtime writes them through its ``GradSink``, and the node
+    fires ``sink.on_backward_end()`` once ``rt.backward`` has enqueued the whole backward pass.
+"""
+import torch
+import torch.nn as nn
+
+
+class GradSink:
+    """Where parameter gradients go: ``param.grad`` by default, or bucket views supplied by the
+    data-parallel wrapper (distributed.py) so that the all-reduce runs on flat buffers."""
+
+    def __init__(self):
+        self.views = {}       # id(param) -> fp32 tensor view with the parameter's shape
+        self.on_ready = None  # callback(param) fired as soon as a gradient is complete
+        self.on_backward_end = None  # callback() fired when the whole backward pass is enqueued
+
+    def buffer_for(self, param):
+        v = self.views.get(id(param))
+        if v is None:
+            v = torch.empty_like(param, dtype=torch.float32)
+            self.views[id(param)] = v
+        return v
+
+    def begin(self, param):
+        """Returns (buffer, accumulate): accumulate when param.grad already holds a gradient."""
+        buf = self.buffer_for(param)
+        if param.grad is None:
+            return buf, False
+        if param.grad.data_ptr() != buf.data_ptr():
+            buf.copy_(param.grad)
+        return buf, True
+
+    def done(self, param, buf):
+        param.grad = buf
+        if self.on_ready is not None:
+            self.on_ready(param)
+
+
+class Runtime:
+    """What every runtime owns: its GradSink and the units holding the bf16 weight-operand copies.  ``operands()``
+    lists those copies for the fused optimizer in ``units`` order; ``prep()`` refreshes them before a forward."""
+
+    non_differentiable_outputs = 0
+
+    def __init__(self, units):
+        self.sink = GradSink()
+        self._units = units
+
+    def operands(self):
+        return [u.op for u in self._units]
+
+    def prep(self):
+        for u in self._units:
+            u.prep()
+
+
+class _RuntimeFunction(torch.autograd.Function):
+    """Torch differentiates the outputs; this node receives their gradients and runs the whole backward pass on the
+    runtime's kernels.  No parameter is an input; the zero-dim ``anchor`` requires grad so that the outputs do.  The tape
+    belongs to THIS forward (it lives on ctx), so several forwards of one module may be in flight before their
+    backwards run."""
+
+    @staticmethod
+    def forward(ctx, anchor, rt, *inputs):
+        ctx.rt, ctx.n_inputs = rt, len(inputs)
+        *outs, ctx.tape = rt.forward(*inputs, True, True)
+        if rt.non_differentiable_outputs:
+            ctx.mark_non_differentiable(*outs[-rt.non_differentiable_outputs:])
+        return outs[0] if len(outs) == 1 else tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        tape, ctx.tape = ctx.tape, None
+        assert tape is not None, 'the graph of this forward pass was already differentiated'
+        rt = ctx.rt
+        grads = grads[:len(grads) - rt.non_differentiable_outputs]
+        rt.backward(*(g.contiguous() for g in grads), tape)
+        if rt.sink.on_backward_end is not None:
+            rt.sink.on_backward_end()
+        return (None, None) + (None,) * ctx.n_inputs
+
+
+def run(rt, training, *inputs):
+    """Runs the runtime `rt` on `inputs`: its output, or the tuple of its outputs.  Builds a graph only in training
+    with grad enabled; otherwise the forward keeps no tape."""
+    if training and torch.is_grad_enabled():
+        anchor = torch.zeros((), device=inputs[0].device, requires_grad=True)
+        return _RuntimeFunction.apply(anchor, rt, *inputs)
+    with torch.no_grad():
+        *outs, _ = rt.forward(*inputs, training, False)
+    return outs[0] if len(outs) == 1 else tuple(outs)
+
+
+class RuntimeModule(nn.Module):
+    """Base of the nn.Module shells: parameter containers whose ``forward`` hands the batch to the runtime that the
+    subclass's ``_build_runtime()`` makes."""
+
+    def _runtime(self):
+        rt = self.__dict__.get('_rt')
+        if rt is None:
+            rt = self.__dict__['_rt'] = self._build_runtime()  # not a submodule / not in state_dict
+        return rt
+
+    def grad_sink(self):
+        """Where the runtime deposits parameter gradients (used by distributed.B200DataParallel)."""
+        return self._runtime().sink
+
+    def _run(self, *inputs):
+        if not inputs[0].is_cuda:
+            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
+        return run(self._runtime(), self.training, *inputs)

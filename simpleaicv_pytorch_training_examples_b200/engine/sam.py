@@ -16,8 +16,8 @@ kernel on NHWC rows); the 3x3 conv is the TMA-im2col implicit GEMM.
 import torch
 
 from .. import ops
-from .convnet import GradSink
 from .operands import CONV, Linear, Operand, PatchEmbed
+from .runtime import Runtime
 from .vit import layernorm_bwd
 
 
@@ -111,7 +111,7 @@ class _Block:
         return layernorm_bwd(blk.norm1, dln1, t['x_in'], t['st1'], sink, dres=dx)
 
 
-class SamEncoderRT:
+class SamEncoderRT(Runtime):
     """Whole-encoder runtime (image_encoder.py:313-331)."""
 
     def __init__(self, model):
@@ -120,15 +120,13 @@ class SamEncoderRT:
         self.patch = PatchEmbed(model.patch_embed.proj)
         self.n0 = Operand(model.neck[0].weight)             # 1x1 conv, no bias
         self.n2 = Operand(model.neck[2].weight, CONV)       # 3x3 conv, no bias
-        self._units = [lin for b in self.blocks for lin in b.linears()] + [self.patch]
-        self.sink = GradSink()
+        super().__init__([lin for b in self.blocks for lin in b.linears()] + [self.patch])
 
     def operands(self):
-        return [u.op for u in self._units] + [self.n0, self.n2]
+        return super().operands() + [self.n0, self.n2]
 
     def prep(self):
-        for u in self._units:
-            u.prep()
+        super().prep()
         self.n0.refresh()
         self.n2.refresh()
 
@@ -214,5 +212,3 @@ class SamEncoderRT:
             dx, dxb = self.blocks[i].backward(dx, dxb, t, B, H, W, self.sink)
             t.clear()
         self.embed_backward(dx, dxb, tape)
-        if self.sink.on_backward_end is not None:
-            self.sink.on_backward_end()

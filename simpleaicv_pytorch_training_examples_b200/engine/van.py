@@ -16,8 +16,9 @@ promotes the stream to fp32 after the first block of every stage).
 import torch
 
 from .. import ops
-from .convnet import FcHeadRT, GradSink
+from .convnet import FcHeadRT
 from .operands import CONV, STEM, Linear, Operand
+from .runtime import Runtime
 
 
 def _bn_forward(bn, x, training, out_f32, tape):
@@ -222,7 +223,7 @@ class _PatchEmbed:
         return self.conv.backward(_bn_backward(self.bn, dout, t['bn'], sink, dx_f32=False), t, sink)
 
 
-class VANRT:
+class VANRT(Runtime):
     """Whole-network runtime (van.py:289-310)."""
 
     def __init__(self, model):
@@ -233,15 +234,7 @@ class VANRT:
             blocks = [_Block(b) for b in getattr(model, f'block{i + 1}')]
             self.stages.append((pe, blocks, getattr(model, f'norm{i + 1}')))
         self.head = FcHeadRT(model.head)
-        self.sink = GradSink()
-        self._units = [u for pe, blocks, _ in self.stages for u in [pe] + [lin for b in blocks for lin in b.linears()]] + [self.head]
-
-    def operands(self):
-        return [u.op for u in self._units]
-
-    def prep(self):
-        for u in self._units:
-            u.prep()
+        super().__init__([u for pe, blocks, _ in self.stages for u in [pe] + [lin for b in blocks for lin in b.linears()]] + [self.head])
 
     # stage-level entry points (also driven by the teacher-forced parity tests)
     def stage_forward(self, i, x, t, training):
@@ -278,5 +271,3 @@ class VANRT:
         d = self.head.backward(dlogits, tape['head'], self.sink, tape['head']['feat_c'])
         for i in range(len(self.stages) - 1, -1, -1):
             d = self.stage_backward(i, d, tape['stages'][i])
-        if self.sink.on_backward_end is not None:
-            self.sink.on_backward_end()

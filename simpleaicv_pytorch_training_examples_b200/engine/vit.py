@@ -15,8 +15,8 @@ device (one [B] tensor per branch) and applied to the branch output and to its g
 import torch
 
 from .. import ops
-from .convnet import GradSink
 from .operands import Linear, PatchEmbed, rows_wgrad
+from .runtime import Runtime
 
 
 def layernorm_bwd(norm, dy, x, stats, sink, dres=None, want_bf16=True, scale=None, rows_per_scale=0):
@@ -117,7 +117,7 @@ class _Block:
         return layernorm_bwd(blk.norm1, dln1, t['x_in'], t['st1'], sink, dres=dx, scale=next_scale, rows_per_scale=l)
 
 
-class ViTRT:
+class ViTRT(Runtime):
     """Whole-network runtime (vit.py:239-262)."""
 
     def __init__(self, model):
@@ -125,15 +125,7 @@ class ViTRT:
         self.blocks = [_Block(b) for b in model.blocks]
         self.fc = Linear(model.fc)
         self.patch = PatchEmbed(model.patch_embed.proj)
-        self._units = [lin for b in self.blocks for lin in b.linears()] + [self.fc, self.patch]
-        self.sink = GradSink()
-
-    def operands(self):
-        return [u.op for u in self._units]
-
-    def prep(self):
-        for u in self._units:
-            u.prep()
+        super().__init__([lin for b in self.blocks for lin in b.linears()] + [self.fc, self.patch])
 
     # ---- stages (driven separately by the teacher-forced parity tests)
     def embed_forward(self, x, tape):
@@ -227,5 +219,3 @@ class ViTRT:
         if tape['p'] > 0.:
             ops.dropout(dx, tape['p'], 0, out=dx, seed_base=tape['sb'])
         self.embed_backward(dx, tape)
-        if sink.on_backward_end is not None:
-            sink.on_backward_end()

@@ -6,7 +6,7 @@ score GEMM).  The nn.Modules are parameter containers created in the reference's
 import torch
 import torch.nn as nn
 
-from ....engine.convnet import run_network
+from ....engine.runtime import RuntimeModule
 from ....engine.sam import SamEncoderRT
 
 
@@ -62,7 +62,7 @@ class LayerNorm2d(nn.Module):
         self.eps = eps
 
 
-class ViTImageEncoder(nn.Module):
+class ViTImageEncoder(RuntimeModule):
 
     def __init__(self, image_size=1024, patch_size=16, inplanes=3, embedding_planes=768, block_nums=12, head_nums=12, mlp_ratio=4,
                  out_planes=256, window_size=0, global_attn_indexes=(), use_gradient_checkpoint=False):
@@ -80,18 +80,9 @@ class ViTImageEncoder(nn.Module):
                                   nn.Conv2d(out_planes, out_planes, kernel_size=3, stride=1, padding=1, bias=False),
                                   LayerNorm2d(out_planes))
 
-    def _runtime(self):
-        rt = self.__dict__.get('_rt')
-        if rt is None:
-            rt = SamEncoderRT(self)
-            self.__dict__['_rt'] = rt
-        return rt
-
-    def grad_sink(self):
-        return self._runtime().sink
+    def _build_runtime(self):
+        return SamEncoderRT(self)
 
     def forward(self, x):
         """x: fp32 [B, 3, S, S] -> fp32 [B, out_planes, S/patch, S/patch]"""
-        if not x.is_cuda:
-            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
-        return run_network(self._runtime(), x.float(), self.training)
+        return self._run(x.float())

@@ -12,6 +12,7 @@ import torch
 import torch.nn as nn
 
 from ...classification.backbones.vit import PatchEmbeddingBlock, TransformerEncoderLayer
+from ...engine.runtime import RuntimeModule
 
 __all__ = ['vit_base_patch16_224_mae_pretrain_model', 'vit_large_patch16_224_mae_pretrain_model',
            'vit_huge_patch14_224_mae_pretrain_model']
@@ -88,7 +89,7 @@ class VITMAEPretrainModelDecoder(nn.Module):
         _xavier_linears(self)
 
 
-class VITMAEPretrainModel(nn.Module):
+class VITMAEPretrainModel(RuntimeModule):
 
     def __init__(self, patch_size=16, image_size=224, mask_ratio=0.75, encoder_embedding_planes=768, encoder_block_nums=12,
                  encoder_head_nums=12, encoder_feedforward_ratio=4, encoder_dropout_prob=0., decoder_embedding_planes=384,
@@ -108,24 +109,14 @@ class VITMAEPretrainModel(nn.Module):
         if encoder_dropout_prob > 0. or decoder_dropout_prob > 0.:
             raise NotImplementedError('MAE on the H100 runtime: dropout_prob > 0 is not wired (the shipped MAE configs use 0)')
 
-    def _runtime(self):
-        rt = self.__dict__.get('_rt')
-        if rt is None:
-            from ...engine.mae import MAERT
-            rt = MAERT(self)
-            self.__dict__['_rt'] = rt
-        return rt
-
-    def grad_sink(self):
-        return self._runtime().sink
+    def _build_runtime(self):
+        from ...engine.mae import MAERT
+        return MAERT(self)
 
     def forward(self, x, noise=None):
         """x: fp32 [B, 3, H, W] on the GPU.  noise: optional [B, L] uniform draws that decide the masking (the reference
         draws them with torch.rand inside random_masking, vit_mae.py:203-225; tests pass them in to pin the masks)."""
-        if not x.is_cuda:
-            raise RuntimeError('this model runs on H100 kernels only; move the batch to the GPU (no CPU fallback exists)')
-        from ...engine.mae import run_mae
-        return run_mae(self._runtime(), x.float(), self.training, noise)
+        return self._run(x.float(), noise)
 
     def images_to_patch(self, images):
         """(N, 3, H, W) -> (N, L, patch_size**2 * 3), vit_mae.py:437-449."""

@@ -16,7 +16,7 @@ class _FakeNet(nn.Module):
         self.a = nn.Linear(300, 70)
         self.b = nn.Linear(70, 9)
         self.unused = nn.Parameter(torch.ones(5))
-        from simpleaicv_pytorch_training_examples_b200.engine.convnet import GradSink
+        from simpleaicv_pytorch_training_examples_b200.engine.runtime import GradSink
         self.__dict__['_sink'] = GradSink()
 
     def grad_sink(self):
