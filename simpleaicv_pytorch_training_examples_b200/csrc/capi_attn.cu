@@ -238,17 +238,31 @@ int bwd_for(const saicv_attn_bwd_args* a, cudaStream_t st) {
 
 #define SAICV_ATTN_SHAPES(X) X(32, 32) X(48, 32) X(64, 64) X(80, 80) X(96, 64) X(112, 64) X(112, 80) X(128, 80) X(192, 64) X(208, 80)
 
+// The refusals of both entries, checked before either launches anything: a refused backward leaves delta and the
+// gradient buffers untouched.
+int check_args(const saicv_attn_args* a, const char* who) {
+  if (a->lq < 1 || a->lk < 1 || a->b < 1 || a->h < 1) return set_error("%s: empty problem", who);
+  if (!(a->scale > 0.f)) return set_error("%s: the softmax scale must be positive", who);
+  if (!(a->dropout_p >= 0.f && a->dropout_p < 1.f)) return set_error("%s: dropout_p must be in [0, 1)", who);
+  if (a->key_mask_bits && a->mask_words * 32 < ((a->lk + 127) / 128) * 128)
+    return set_error("%s: mask_words must cover lk rounded up to 128 keys", who);
+  bool known = false, drop = false;
+#define X(Q, V) if (a->dqk == Q && a->dv == V) { known = true; drop = kDropoutShape<Q, V>; }
+  SAICV_ATTN_SHAPES(X)
+#undef X
+  if (!known) return set_error("%s: unsupported (score width, value width) = (%d, %d)", who, a->dqk, a->dv);
+  if (a->dropout_p > 0.f && !drop)
+    return set_error("attention dropout is not compiled for (score width, value width) = (%d, %d)", a->dqk, a->dv);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
 
 int saicv_attn_fwd(const saicv_attn_args* a, void* stream) {
   if (!ensure()) return 1;
-  if (a->lq < 1 || a->lk < 1 || a->b < 1 || a->h < 1) return set_error("saicv_attn_fwd: empty problem");
-  if (!(a->scale > 0.f)) return set_error("saicv_attn_fwd: the softmax scale must be positive");
-  if (!(a->dropout_p >= 0.f && a->dropout_p < 1.f)) return set_error("saicv_attn_fwd: dropout_p must be in [0, 1)");
-  if (a->key_mask_bits && a->mask_words * 32 < ((a->lk + 127) / 128) * 128)
-    return set_error("saicv_attn_fwd: mask_words must cover lk rounded up to 128 keys");
+  if (int e = check_args(a, "saicv_attn_fwd")) return e;
 #define X(Q, V) if (a->dqk == Q && a->dv == V) return fwd_for<Q, V>(a, (cudaStream_t)stream);
   SAICV_ATTN_SHAPES(X)
 #undef X
@@ -258,6 +272,7 @@ int saicv_attn_fwd(const saicv_attn_args* a, void* stream) {
 int saicv_attn_bwd(const saicv_attn_bwd_args* a, void* stream) {
   if (!ensure()) return 1;
   const saicv_attn_args* f = &a->fwd;
+  if (int e = check_args(f, "saicv_attn_bwd")) return e;
   if (a->dk_cols < 0 || a->dk_cols > f->dqk || (a->dk_cols % 16)) return set_error("saicv_attn_bwd: bad dk_cols %d", a->dk_cols);
   {
     const long long rows = (long long)f->b * f->h * f->lq;

@@ -1,8 +1,9 @@
 """GPU parity of the wgmma attention family (csrc/attn_sm90.cuh) through the general C-ABI entry
 (saicv_attn_fwd / saicv_attn_bwd) against plain fp32 torch attention on the same bf16-representable inputs:
-every supported (score width, value width), long sequences (several key blocks / row tiles), cross attention
-(Lq != Lk), key-padding masks and strided (packed / head-major) layouts.  Tolerances: outputs 2e-2 abs,
-gradients relative L2 2e-2 (bf16 P / dS operands, fp32 accumulation)."""
+the (score width, value width) pairs the ViT, SAM and DETR runtimes use, long sequences (several key blocks / row
+tiles), cross attention (Lq != Lk), key-padding masks and strided (packed / head-major) layouts.  Tolerances: outputs
+2e-2 abs, gradients relative L2 2e-2 (bf16 P / dS operands, fp32 accumulation).  Element-wise conformance of every
+compiled width against float64 interval references is in test_attn_conformance_gpu.py."""
 import math
 
 import pytest

@@ -35,7 +35,7 @@ def hash_keep(seed, a, b, p):
     x = x ^ (x >> 15)
     x = x * 0x846CA68B & M
     x = x ^ (x >> 16)
-    t = min(int(p * 4294967296.0), 0xFFFFFFFF)
+    t = min(int(torch.tensor(p, dtype=torch.float32).item() * 4294967296.0), 0xFFFFFFFF)   # the C ABI takes p as a float
     return x >= t
 
 
