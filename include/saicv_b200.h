@@ -459,6 +459,18 @@ int saicv_token_fill_slabs(long long rows);
 int saicv_token_gather_bwd(const float* dout, const int* idx, void* dsrc, int dsrc_bf16, long long src_rows,
                            float* fill_partial, int b, int r, int c, void* stream);
 
+/* ---- DINOv3 ViT (SimpleAICV/detection/models/backbones/dinov3vit.py; csrc/capi_dinov3.cu) ----------------------------
+ * Rotary position embedding in place on the q and k slices of packed qkv bf16 [b*l][3][heads][hd] (:347-367 apply_rope):
+ * x <- bf16(x*cos + rotate_half(x)*sin) in fp32 with two rounded products and one add (bit-identical to the reference's
+ * torch expression), sin / cos fp32 [l][hd].  The backward applies the transposed rotation to the dq / dk slices of
+ * dqkv: g <- bf16(g*cos + rotate_half^T(g*sin)).  hd %% 8 == 0, any l and number of heads. */
+int saicv_rope_qk_fwd(void* qkv, const float* sin_t, const float* cos_t, int b, int l, int heads, int hd, void* stream);
+int saicv_rope_qk_bwd(void* dqkv, const float* sin_t, const float* cos_t, int b, int l, int heads, int hd, void* stream);
+/* SwiGLU gate (:134-141): h = bf16(bf16(silu(a)) * b); backward db = bf16(dh * bf16(silu(a))),
+ * da = bf16(bf16(dh * b) * silu'(a)), autocast's rounding points.  bf16, n %% 8 == 0. */
+int saicv_swiglu_fwd(const void* a, const void* b, void* h, long long n, void* stream);
+int saicv_swiglu_bwd(const void* dh, const void* a, const void* b, void* da, void* db, long long n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

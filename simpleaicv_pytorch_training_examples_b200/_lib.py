@@ -131,6 +131,10 @@ SIGNATURES = {
     'saicv_bn_bwd_generic': [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
     'saicv_im2col_nhwc': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_col2im_nhwc': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    'saicv_rope_qk_fwd': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
+    'saicv_rope_qk_bwd': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
+    'saicv_swiglu_fwd': [c_void_p, c_void_p, c_void_p, c_ll, c_void_p],
+    'saicv_swiglu_bwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p],
 }
 
 _lib = None

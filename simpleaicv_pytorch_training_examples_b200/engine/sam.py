@@ -111,6 +111,58 @@ class _Block:
         return layernorm_bwd(blk.norm1, dln1, t['x_in'], t['st1'], sink, dres=dx)
 
 
+class Neck:
+    """The image-encoder neck (image_encoder.py:299-311, also the DINOv3 encoder's, dinov3_image_encoder.py:53-65) on
+    NHWC rows: 1x1 conv -> LayerNorm2d -> 3x3 conv -> LayerNorm2d.  It owns the bf16 operand copies of its two convs."""
+
+    def __init__(self, neck):
+        self.mod = neck
+        self.n0 = Operand(neck[0].weight)             # 1x1 conv, no bias
+        self.n2 = Operand(neck[2].weight, CONV)       # 3x3 conv, no bias
+
+    def operands(self):
+        return [self.n0, self.n2]
+
+    def prep(self):
+        self.n0.refresh()
+        self.n2.refresh()
+
+    def forward(self, xb, B, H, W, tape):
+        """xb bf16 [B*H*W, C] -> fp32 NCHW [B, out_planes, H, W]"""
+        m = self.mod
+        n1, n3 = m[1], m[3]
+        tape['xb'] = xb
+        y1 = tape['y1'] = ops.linear_fwd(xb, self.n0.w, out_f32=True)                     # 1x1 conv, no bias
+        oc = y1.shape[1]
+        l1, tape['s1'] = ops.layernorm_fwd(y1, n1.weight.detach(), n1.bias.detach(), n1.eps)
+        tape['l1'] = l1
+        cs = tape['cs'] = ops.make_conv_shape(B, H, W, oc, oc, 3, 3, 1, 1)
+        y2b = ops.conv_fprop(l1.view(B, H, W, oc), self.n2.w, cs)
+        y2 = tape['y2'] = y2b.view(-1, oc).float()
+        l2, tape['s2'] = ops.layernorm_fwd(y2, n3.weight.detach(), n3.bias.detach(), n3.eps)
+        return l2.view(B, H, W, oc).permute(0, 3, 1, 2).float()
+
+    def backward(self, dout, tape, sink, out_f32):
+        """dout fp32 NCHW -> dx [B*H*W, C] w.r.t. xb (fp32 when out_f32, else bf16)"""
+        m = self.mod
+        B, oc, H, W = dout.shape
+        n1, n3 = m[1], m[3]
+        dl2 = dout.permute(0, 2, 3, 1).reshape(-1, oc).to(torch.bfloat16).contiguous()
+        _, dy2b = layernorm_bwd(n3, dl2, tape['y2'], tape['s2'], sink)
+        w2 = m[2].weight
+        wbuf, wacc = sink.begin(w2)
+        part = ops.conv_wgrad(dy2b.view(B, H, W, oc), tape['l1'].view(B, H, W, oc), tape['cs'])
+        ops.finish_conv_wgrad(part, wbuf, 9 * oc, accumulate=wacc)
+        sink.done(w2, wbuf)
+        dl1 = ops.conv_dgrad(dy2b.view(B, H, W, oc), self.n2.w, tape['cs']).view(-1, oc)
+        _, dy1b = layernorm_bwd(n1, dl1, tape['y1'], tape['s1'], sink)
+        w0 = m[0].weight
+        wbuf, wacc = sink.begin(w0)
+        ops.reduce_partials(ops.linear_wgrad(dy1b, tape['xb']), wbuf, accumulate=wacc)
+        sink.done(w0, wbuf)
+        return ops.linear_dgrad(dy1b, self.n0.w, out_f32=out_f32)
+
+
 class SamEncoderRT(Runtime):
     """Whole-encoder runtime (image_encoder.py:313-331)."""
 
@@ -118,17 +170,15 @@ class SamEncoderRT(Runtime):
         self.model = model
         self.blocks = [_Block(b) for b in model.blocks]
         self.patch = PatchEmbed(model.patch_embed.proj)
-        self.n0 = Operand(model.neck[0].weight)             # 1x1 conv, no bias
-        self.n2 = Operand(model.neck[2].weight, CONV)       # 3x3 conv, no bias
+        self.neck = Neck(model.neck)
         super().__init__([lin for b in self.blocks for lin in b.linears()] + [self.patch])
 
     def operands(self):
-        return super().operands() + [self.n0, self.n2]
+        return super().operands() + self.neck.operands()
 
     def prep(self):
         super().prep()
-        self.n0.refresh()
-        self.n2.refresh()
+        self.neck.prep()
 
     # ---- stages (also driven separately by the teacher-forced parity tests)
     def embed_forward(self, x, tape):
@@ -150,40 +200,11 @@ class SamEncoderRT(Runtime):
 
     def neck_forward(self, x, tape):
         """x fp32 [B*H*W, C] -> fp32 NCHW [B, out_planes, H, W]"""
-        m = self.model
-        B, H, W = tape['B'], tape['H'], tape['W']
-        n1, n3 = m.neck[1], m.neck[3]
-        xb = tape['xb'] = ops.cast_bf16(x)
-        y1 = tape['y1'] = ops.linear_fwd(xb, self.n0.w, out_f32=True)                     # 1x1 conv, no bias
-        oc = y1.shape[1]
-        l1, tape['s1'] = ops.layernorm_fwd(y1, n1.weight.detach(), n1.bias.detach(), n1.eps)
-        tape['l1'] = l1
-        cs = tape['cs'] = ops.make_conv_shape(B, H, W, oc, oc, 3, 3, 1, 1)
-        y2b = ops.conv_fprop(l1.view(B, H, W, oc), self.n2.w, cs)
-        y2 = tape['y2'] = y2b.view(-1, oc).float()
-        l2, tape['s2'] = ops.layernorm_fwd(y2, n3.weight.detach(), n3.bias.detach(), n3.eps)
-        return l2.view(B, H, W, oc).permute(0, 3, 1, 2).float()
+        return self.neck.forward(ops.cast_bf16(x), tape['B'], tape['H'], tape['W'], tape)
 
     def neck_backward(self, dout, tape):
         """dout fp32 NCHW -> (dx fp32 [B*H*W, C], its bf16 copy)"""
-        m, sink = self.model, self.sink
-        B, H, W = tape['B'], tape['H'], tape['W']
-        n1, n3 = m.neck[1], m.neck[3]
-        oc = dout.shape[1]
-        dl2 = dout.permute(0, 2, 3, 1).reshape(-1, oc).to(torch.bfloat16).contiguous()
-        _, dy2b = layernorm_bwd(n3, dl2, tape['y2'], tape['s2'], sink)
-        w2 = m.neck[2].weight
-        wbuf, wacc = sink.begin(w2)
-        part = ops.conv_wgrad(dy2b.view(B, H, W, oc), tape['l1'].view(B, H, W, oc), tape['cs'])
-        ops.finish_conv_wgrad(part, wbuf, 9 * oc, accumulate=wacc)
-        sink.done(w2, wbuf)
-        dl1 = ops.conv_dgrad(dy2b.view(B, H, W, oc), self.n2.w, tape['cs']).view(-1, oc)
-        _, dy1b = layernorm_bwd(n1, dl1, tape['y1'], tape['s1'], sink)
-        w0 = m.neck[0].weight
-        wbuf, wacc = sink.begin(w0)
-        ops.reduce_partials(ops.linear_wgrad(dy1b, tape['xb']), wbuf, accumulate=wacc)
-        sink.done(w0, wbuf)
-        dx = ops.linear_dgrad(dy1b, self.n0.w, out_f32=True)
+        dx = self.neck.backward(dout, tape, self.sink, out_f32=True)
         return dx, ops.cast_bf16(dx)
 
     def forward(self, x, training, keep_tape):
@@ -196,8 +217,8 @@ class SamEncoderRT(Runtime):
             if ckpt:
                 t['ckpt_in'] = h
                 h = blk.forward(h, {}, tape['B'], tape['H'], tape['W'])
-            else:
-                h = blk.forward(h, t, tape['B'], tape['H'], tape['W'])
+            else:   # without a tape each block's intermediates are freed as soon as the next block starts
+                h = blk.forward(h, t if keep_tape else {}, tape['B'], tape['H'], tape['W'])
         out = self.neck_forward(h, tape)
         return out, (tape if keep_tape else None)
 

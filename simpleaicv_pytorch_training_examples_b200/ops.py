@@ -827,3 +827,30 @@ def sam_loss_bwd(logits, targets, coef, alpha, gamma):
     _lib.call('saicv_sam_loss_bwd', _p(logits), int(logits.dtype == torch.bfloat16), _p(targets), _p(coef.contiguous()), _p(dl),
               int(logits.dtype == torch.bfloat16), b, m, n, float(alpha), float(gamma), _stream())
     return dl
+
+
+# ----------------------------------------------------------------------------- DINOv3 kernels
+def rope_qk(qkv, sin, cos, b, l, heads, hd, backward=False):
+    """In place on the q and k slices of packed qkv bf16 [b*l, 3*heads*hd]: the rotary embedding with the fp32 table
+    sin / cos [l, hd] (backward=True: its transpose, applied to dq / dk of a dqkv buffer)."""
+    assert qkv.dtype == torch.bfloat16 and qkv.shape == (b * l, 3 * heads * hd)
+    assert sin.dtype == cos.dtype == torch.float32 and sin.shape == cos.shape == (l, hd)
+    _lib.call('saicv_rope_qk_bwd' if backward else 'saicv_rope_qk_fwd', _p(qkv), _p(sin), _p(cos), b, l, heads, hd, _stream())
+    return qkv
+
+
+def swiglu_fwd(a, b, out=None):
+    """h = silu(a) * b (bf16)."""
+    assert a.dtype == b.dtype == torch.bfloat16 and a.shape == b.shape
+    if out is None:
+        out = torch.empty_like(a)
+    _lib.call('saicv_swiglu_fwd', _p(a), _p(b), _p(out), a.numel(), _stream())
+    return out
+
+
+def swiglu_bwd(dh, a, b):
+    """Returns (da, db) of h = silu(a) * b."""
+    assert dh.dtype == a.dtype == b.dtype == torch.bfloat16 and dh.shape == a.shape == b.shape
+    da, db = torch.empty_like(a), torch.empty_like(b)
+    _lib.call('saicv_swiglu_bwd', _p(dh), _p(a), _p(b), _p(da), _p(db), a.numel(), _stream())
+    return da, db
