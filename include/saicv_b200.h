@@ -194,7 +194,7 @@ int saicv_colsum(const void* x, float* partials, float* out, long long rows, int
 
 /* ---- ViT blocks (SimpleAICV/classification/backbones/vit.py) --------------------------------- */
 /* nn.LayerNorm(eps=1e-6) (vit.py:147,151,225): x fp32 [rows][c] -> y bf16; stats[2][rows] =
- * (mean, rstd) kept for the backward.  c in {128, 256, 768, 1024, 1280}. */
+ * (mean, rstd) kept for the backward.  c in {128, 256, 384, 512, 768, 1024, 1280}. */
 int saicv_layernorm_fwd(const float* x, const float* gamma, const float* beta, void* y,
                         float* stats, long long rows, int c, float eps, void* stream);
 /* dx (fp32) = dres + LN'(dy) with dres the residual-stream gradient (may be NULL); optional bf16
