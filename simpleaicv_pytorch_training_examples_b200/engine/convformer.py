@@ -32,6 +32,7 @@ from .convnet import FcHeadRT
 from .operands import Linear
 from .runtime import Runtime
 from .van import StridedConv, _bn_backward, _bn_forward
+from .vit import drop_path_scale
 
 
 def _bf16_scaled(d, scale, rows_per_scale):
@@ -65,16 +66,7 @@ class _Block:
     def draw_scales(self, n, training, dev):
         """The two per-sample drop-path scales (token mixer, then MLP), drawn on the device in the reference's order
         (convformer.py:131-135: bernoulli_(keep) / keep), or (None, None) when drop path is off."""
-        if not training or self.drop_path == 0.:
-            return None, None
-        keep = 1. - self.drop_path
-        out = []
-        for _ in range(2):
-            s = torch.empty(n, device=dev).bernoulli_(keep)
-            if keep > 0.:
-                s.div_(keep)
-            out.append(s)
-        return tuple(out)
+        return drop_path_scale(self.drop_path, n, training, dev), drop_path_scale(self.drop_path, n, training, dev)
 
     def _residual(self, lin, x, h, scale, hw):
         """x + scale * lin(h): fp32 in the GEMM epilogue on an fp32 stream, else bf16(x + bf16(lin(h)))."""
@@ -109,9 +101,8 @@ class _Block:
         dx1 = _bn_backward(self.blk.norm2, dn2, t['bn2'], sink, dres=dx2)
         ddd = self.pw2.bwd(_bf16_scaled(dx1, t['s1'], hw), t['dd'], sink).view(n, h, w, 2 * c)
         r1 = t['r1'].view(n, h, w, 2 * c)
-        wbuf, wacc = sink.begin(self.dw.weight)
-        ops.dwconv_wgrad(ddd, r1, wbuf, 7, 1, accumulate=wacc)
-        sink.done(self.dw.weight, wbuf)
+        with sink.grad(self.dw.weight) as (acc, buf):
+            ops.dwconv_wgrad(ddd, r1, buf, 7, 1, accumulate=acc)
         dh = ops.dwconv_dgrad_masked(ddd, self.dw.weight.detach(), r1, 7)        # * relu'(pwconv1 output)
         dn1 = self.pw1.bwd(dh.view(-1, 2 * c), t['n1'], sink)
         return _bn_backward(self.blk.norm1, dn1, t['bn1'], sink, dres=dx1)

@@ -15,11 +15,13 @@ out through ``grad_buffer_of``), not returned through autograd.
 Reference semantics followed: SimpleAICV/classification/backbones/resnet.py:19-48 (ConvBnActBlock),
 :51-97 (BasicBlock), :100-155 (Bottleneck), :226-245 (ResNet.forward), resnetforcifar.py:98-108.
 """
+import contextlib
+
 import torch
 
 from .. import ops
 from .operands import CONV, STEM, Linear, Operand, rows_wgrad
-from .runtime import GradSink, Runtime  # noqa: F401  GradSink: still importable from here, where it used to live
+from .runtime import Runtime
 
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SILU = 0, 1, 2, 3
 # BatchNorm batch statistics are accumulated by the conv GEMM's epilogue instead of a separate pass over y
@@ -179,26 +181,17 @@ class ConvBN:
         return out
 
     # ---- backward
-    def _grad_targets(self, sink):
-        """(gamma, dgamma, dbeta, accumulate) for the BatchNorm backward kernels, and the sink buffers for _grad_done."""
-        gbuf, gacc = sink.begin(self.bn.weight)
-        bbuf, bacc = sink.begin(self.bn.bias)
-        assert gacc == bacc
+    @contextlib.contextmanager
+    def _bn_grad(self, sink):
+        """(gamma, dgamma, dbeta, accumulate) for a BatchNorm backward kernel.  A channel-padded unit's kernel writes kp
+        channels of scratch, whose first k go through the sink on exit."""
         if self.padded:
-            return (self.gamma_p, self.dg_p, self.db_p, False), (gbuf, bbuf, gacc)
-        return (self.bn.weight.detach(), gbuf, bbuf, gacc), (gbuf, bbuf, gacc)
-
-    def _grad_done(self, sink, bufs):
-        gbuf, bbuf, acc = bufs
-        if self.padded:
-            if acc:
-                gbuf.add_(self.dg_p[:self.k])
-                bbuf.add_(self.db_p[:self.k])
-            else:
-                gbuf.copy_(self.dg_p[:self.k])
-                bbuf.copy_(self.db_p[:self.k])
-        sink.done(self.bn.weight, gbuf)
-        sink.done(self.bn.bias, bbuf)
+            yield self.gamma_p, self.dg_p, self.db_p, False
+            sink.add(self.bn.weight, self.dg_p[:self.k])
+            sink.add(self.bn.bias, self.db_p[:self.k])
+        else:
+            with sink.grad(self.bn.weight, self.bn.bias) as (acc, dg, db):
+                yield self.bn.weight.detach(), dg, db, acc
 
     def bn_bwd(self, dout, tape, sink, bits=None, want_dres=False, act=None):
         """dout: gradient w.r.t. the activated output.  Returns (dy, dres).
@@ -213,10 +206,9 @@ class ConvBN:
         ops.bn_bwd_reduce(dout, None, y, saved, self.sums, act, scale_shift=ss, bits=bits)
         dy = torch.empty_like(y)
         dres = torch.empty_like(y) if want_dres else None
-        (gamma, dg, db, acc), bufs = self._grad_targets(sink)
-        ops.bn_bwd_apply(dout, None, y, saved, gamma, self.sums, dy, dres, dg, db, act, accumulate=acc,
-                         scale_shift=ss, bits=bits)
-        self._grad_done(sink, bufs)
+        with self._bn_grad(sink) as (gamma, dg, db, acc):
+            ops.bn_bwd_apply(dout, None, y, saved, gamma, self.sums, dy, dres, dg, db, act, accumulate=acc,
+                             scale_shift=ss, bits=bits)
         return dy, dres
 
     def bn_bwd_pair(self, other, g, tape, other_tape, sink, bits):
@@ -227,12 +219,10 @@ class ConvBN:
         sums = torch.empty(4, self.kp, device=y.device)
         ops.bn_bwd_reduce2(g, bits, y, yo, tape['saved'], other_tape['saved'], sums)
         dy, dyo = torch.empty_like(y), torch.empty_like(yo)
-        (ga, dga, dba, acca), bufs_a = self._grad_targets(sink)
-        (gb, dgb, dbb, accb), bufs_b = other._grad_targets(sink)
-        ops.bn_bwd_apply2(g, bits, y, yo, tape['saved'], other_tape['saved'], ga, gb, sums, dy, dyo, dga, dba, dgb, dbb,
-                          accumulate_a=acca, accumulate_b=accb)
-        self._grad_done(sink, bufs_a)
-        other._grad_done(sink, bufs_b)
+        # nested this way round so that this unit's gradients are reported before other's (the inner block exits first)
+        with other._bn_grad(sink) as (gb, dgb, dbb, accb), self._bn_grad(sink) as (ga, dga, dba, acca):
+            ops.bn_bwd_apply2(g, bits, y, yo, tape['saved'], other_tape['saved'], ga, gb, sums, dy, dyo, dga, dba, dgb, dbb,
+                              accumulate_a=acca, accumulate_b=accb)
         return dy, dyo
 
     def conv_bwd(self, dy, tape, sink, need_dx=True, add=None, mask_bits=None):
@@ -240,19 +230,16 @@ class ConvBN:
         (NHWC bf16, `add` fused in when given, then multiplied by the ReLU mask `mask_bits` when
         given) or None.  A 1x1 stride-2 conv returns ('strided', dd) with the compact gradient
         dd[n,P,Q,cp] that belongs at the even pixels."""
-        w = self.conv.weight
-        wbuf, wacc = sink.begin(w)
         n, P, Q, _ = dy.shape
         if self.is_stem:
-            part = ops.linear_wgrad(dy.view(-1, self.kp), tape['cols'], transposed=ops.wgrad_transposed(self.kp, self.kpad))
-            ops.finish_conv_wgrad(part, wbuf, self.kpad, accumulate=wacc, order=ops.ORDER_CRS, kp=self.kp)
-            sink.done(w, wbuf)
+            with sink.grad(self.conv.weight) as (acc, buf):
+                part = ops.linear_wgrad(dy.view(-1, self.kp), tape['cols'], transposed=ops.wgrad_transposed(self.kp, self.kpad))
+                ops.finish_conv_wgrad(part, buf, self.kpad, accumulate=acc, order=ops.ORDER_CRS, kp=self.kp)
             assert not need_dx, 'the stem has no data gradient'
             return None
         cs = tape['cs']
-        part = ops.conv_wgrad(dy, tape['a_in'], cs)
-        ops.finish_conv_wgrad(part, wbuf, self.kpad, accumulate=wacc, kp=self.kp, cp=self.cp)
-        sink.done(w, wbuf)
+        with sink.grad(self.conv.weight) as (acc, buf):
+            ops.finish_conv_wgrad(ops.conv_wgrad(dy, tape['a_in'], cs), buf, self.kpad, accumulate=acc, kp=self.kp, cp=self.cp)
         if not need_dx:
             return None
         if self.stride == 2 and self.r == 1:
@@ -469,10 +456,9 @@ class FcHeadRT:
         ncls = self.fc.weight.shape[0]
         npad = self.op.w.shape[0]
         dlogits = dlogits.contiguous().float()
-        bbuf, bacc = sink.begin(self.fc.bias)
-        ops.colsum(dlogits, bbuf, accumulate=bacc)
-        sink.done(self.fc.bias, bbuf)
-        dl = torch.zeros(dlogits.shape[0], npad, device=dlogits.device, dtype=torch.bfloat16)
+        with sink.grad(self.fc.bias) as (acc, buf):
+            ops.colsum(dlogits, buf, accumulate=acc)
+        dl =torch.zeros(dlogits.shape[0], npad, device=dlogits.device, dtype=torch.bfloat16)
         if npad == ncls:
             ops.cast_bf16(dlogits, dl)
         else:
@@ -509,13 +495,10 @@ class ConvHeadRT:
         dl = torch.zeros(n, npad, device=a.device, dtype=torch.bfloat16)
         dl[:, :ncls] = dlogits.to(torch.bfloat16)
         dy = ops.avgpool_bwd(dl, h, w).view(n * h * w, npad)
-        bias = self.conv.bias
         rows_wgrad(dy, a.view(n * h * w, c), self.conv.weight, sink)
-        bbuf, bacc = sink.begin(bias)
         full = torch.empty(npad, device=a.device)
         ops.colsum(dy, full)
-        bbuf.copy_(full[:ncls] + bbuf if bacc else full[:ncls])
-        sink.done(bias, bbuf)
+        sink.add(self.conv.bias, full[:ncls])
         return ops.linear_dgrad(dy, self.op.w).view(n, h, w, c)
 
 
@@ -561,6 +544,16 @@ class ResNetRT(Runtime):
             a, tape['argmax'] = ops.maxpool3x3s2_fwd(a)
         return a
 
+    def blocks_forward(self, a, tapes, training, checkpoint):
+        """Runs the blocks on the stem output `a`, one tape each; with checkpoint a tape keeps only its block's input."""
+        for b, t in zip(self.blocks, tapes):
+            if checkpoint:
+                t['ckpt_in'] = a
+                a = b.forward(a, {}, training)
+            else:
+                a = b.forward(a, t, training)
+        return a
+
     def head_forward(self, a, tape):
         tape['feat_c'] = a.shape[3]
         return self.head.forward(a, tape)
@@ -575,13 +568,7 @@ class ResNetRT(Runtime):
         _NBT_BATCH = [] if training else None
         try:
             a = self.stem_forward(x, tape, training)
-            ckpt = self.checkpoint and keep_tape
-            for b, t in zip(self.blocks, tape['blocks']):
-                if ckpt:
-                    t['ckpt_in'] = a
-                    a = b.forward(a, {}, training)
-                else:
-                    a = b.forward(a, t, training)
+            a = self.blocks_forward(a, tape['blocks'], training, self.checkpoint and keep_tape)
             logits = self.head_forward(a, tape)
         finally:
             _flush_nbt()

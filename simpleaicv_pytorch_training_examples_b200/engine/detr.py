@@ -110,16 +110,13 @@ class _MHA:
             dkv = dk_dst.view(B, Lk, -1)[:, :, dk0:dk0 + C].unflatten(2, (H, hd)).permute(0, 2, 1, 3)
             ops.attn_bwd(t['qe'], t['ke'], t['vv'], t['ov'], t['lse'], dov, t['kscale'], dqv, dkv, dvv,
                          dropout_p=t['p'], dropout_seed=t['seed'], dropout_seed_base=t['sb'])
-        w, b = self.mod.in_proj_weight, self.mod.in_proj_bias
-        wbuf, wacc = sink.begin(w)
-        bbuf, bacc = sink.begin(b)
         pieces = [(dq_dst, t['q_in'], 0, 2 * C)] if same else [(dq_dst, t['q_in'], 0, C), (dk_dst, t['k_in'], C, 2 * C)]
         pieces.append((dv, t['v_in'], 2 * C, 3 * C))
-        for dy, x, r0, r1 in pieces:
-            ops.reduce_partials(ops.linear_wgrad(dy, x), wbuf[r0:r1], accumulate=wacc)
-            ops.colsum(dy, bbuf[r0:r1], accumulate=bacc)
-        sink.done(w, wbuf)
-        sink.done(b, bbuf)
+        # the weight's block is the inner one so that the weight is reported before the bias
+        with sink.grad(self.mod.in_proj_bias) as (bacc, bbuf), sink.grad(self.mod.in_proj_weight) as (wacc, wbuf):
+            for dy, x, r0, r1 in pieces:
+                ops.reduce_partials(ops.linear_wgrad(dy, x), wbuf[r0:r1], accumulate=wacc)
+                ops.colsum(dy, bbuf[r0:r1], accumulate=bacc)
         return (dq_dst, None, dv) if same else (dq_dst, dk_dst, dv)
 
     def dgrad(self, dy, r0, r1, resid=None):
@@ -167,13 +164,9 @@ def _norm_fwd(norm, z, pos=None, want_y=True, want_yb=True, want_ypb=False):
 
 
 def _norm_bwd(norm, dy, z, stats, sink, dres=None, want_dz=True, want_dzb=True):
-    gbuf, gacc = sink.begin(norm.weight)
-    bbuf, bacc = sink.begin(norm.bias)
-    dz, dzb = ops.postln_bwd(dy, z, norm.weight.detach(), stats, gbuf, bbuf, dres=dres, want_dz=want_dz, want_dzb=want_dzb,
-                             accumulate=gacc)
-    sink.done(norm.weight, gbuf)
-    sink.done(norm.bias, bbuf)
-    return dz, dzb
+    with sink.grad(norm.weight, norm.bias) as (acc, dg, db):
+        return ops.postln_bwd(dy, z, norm.weight.detach(), stats, dg, db, dres=dres, want_dz=want_dz, want_dzb=want_dzb,
+                              accumulate=acc)
 
 
 class _EncLayer:
@@ -326,15 +319,7 @@ class DetrRT(Runtime):
     def backbone_forward(self, x, tape, training, keep_tape):
         body = self.body
         tape['body'] = bt = {'stem': {}, 'blocks': [dict() for _ in body.blocks]}
-        a = body.stem_forward(x, bt, training)
-        ckpt = body.checkpoint and keep_tape
-        for b, t in zip(body.blocks, bt['blocks']):
-            if ckpt:
-                t['ckpt_in'] = a
-                a = b.forward(a, {}, training)
-            else:
-                a = b.forward(a, t, training)
-        return a
+        return body.blocks_forward(body.stem_forward(x, bt, training), bt['blocks'], training, body.checkpoint and keep_tape)
 
     def backbone_backward(self, da, tape):
         body, bt = self.body, tape['body']
@@ -375,22 +360,17 @@ class DetrRT(Runtime):
         C = dhs.shape[1]
         dhs = dhs.view(D, B * Q, C)
         norm = self.model.transformer.decoder_norm
-        gbuf, gacc = sink.begin(norm.weight)
-        bbuf, bacc = sink.begin(norm.bias)
         dy, dmem, dqpos = None, None, None
-        for i in reversed(range(D)):
-            z, stats = tape['inter'][i]
-            # gradient through decoder_norm of this layer's output, plus what the next layer sent back
-            dy, _ = ops.postln_bwd(dhs[i], z, norm.weight.detach(), stats, gbuf, bbuf, dres=dy, want_dzb=False,
-                                   accumulate=gacc or i != D - 1)
-            dy, dmem, dqpos = self.dec[i].backward(dy, tape['dec'][i], sink, cx, dmem, dqpos, need_dx=i > 0)
-            tape['dec'][i].clear()
-        sink.done(norm.weight, gbuf)
-        sink.done(norm.bias, bbuf)
-        qe = self.model.query_embed.weight
-        qbuf, qacc = sink.begin(qe)
-        ops.colsum(dqpos.view(B, -1), qbuf.view(-1), accumulate=qacc)      # sum over the batch of the broadcast rows
-        sink.done(qe, qbuf)
+        with sink.grad(norm.weight, norm.bias) as (acc, dg, db):
+            for i in reversed(range(D)):
+                z, stats = tape['inter'][i]
+                # gradient through decoder_norm of this layer's output, plus what the next layer sent back
+                dy, _ = ops.postln_bwd(dhs[i], z, norm.weight.detach(), stats, dg, db, dres=dy, want_dzb=False,
+                                       accumulate=acc or i != D - 1)
+                dy, dmem, dqpos = self.dec[i].backward(dy, tape['dec'][i], sink, cx, dmem, dqpos, need_dx=i > 0)
+                tape['dec'][i].clear()
+        with sink.grad(self.model.query_embed.weight) as (acc, buf):
+            ops.colsum(dqpos.view(B, -1), buf.view(-1), accumulate=acc)      # sum over the batch of the broadcast rows
         dx = dmem
         for l, t in zip(reversed(self.enc), reversed(tape['enc'])):
             dx = l.backward(dx, t, sink, cx)

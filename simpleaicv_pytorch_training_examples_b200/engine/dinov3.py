@@ -67,13 +67,9 @@ class _MaskedQKV(Linear):
     def bwd(self, dy, x, sink):
         m = self.mod
         rows_wgrad(dy, x, m.weight, sink)
-        n = m.bias.shape[0]
-        bbuf, bacc = sink.begin(m.bias)
         full = torch.empty(dy.shape[1], device=dy.device)
         ops.colsum(dy, full)
-        g = full[:n] * m.bias_mask.to(full.dtype)
-        bbuf.copy_(g + bbuf if bacc else g)
-        sink.done(m.bias, bbuf)
+        sink.add(m.bias, full[:m.bias.shape[0]] * m.bias_mask.to(full.dtype))
         return ops.linear_dgrad(dy, self.op.w)
 
 
@@ -124,9 +120,8 @@ class _Block:
         d = dx.shape[1] // self.heads
         # ---- MLP branch
         ls2 = blk.ls2.gamma
-        lbuf, lacc = sink.begin(ls2)
-        df = ops.ls_residual_bwd(dx, t['f'], None, ls2.detach(), lbuf, accumulate=lacc)
-        sink.done(ls2, lbuf)
+        with sink.grad(ls2) as (acc, buf):
+            df = ops.ls_residual_bwd(dx, t['f'], None, ls2.detach(), buf, accumulate=acc)
         if self.swiglu:
             w1, w2, w3 = self.ffn
             dh = w3.bwd(df, t['h'], sink)
@@ -139,9 +134,8 @@ class _Block:
         dx, _ = layernorm_bwd(blk.norm2, dln2, t['x_mid'], t['st2'], sink, dres=dx, want_bf16=False)
         # ---- attention branch
         ls1 = blk.ls1.gamma
-        lbuf, lacc = sink.begin(ls1)
-        dpa = ops.ls_residual_bwd(dx, t['pa'], None, ls1.detach(), lbuf, accumulate=lacc)
-        sink.done(ls1, lbuf)
+        with sink.grad(ls1) as (acc, buf):
+            dpa = ops.ls_residual_bwd(dx, t['pa'], None, ls1.detach(), buf, accumulate=acc)
         datt = self.proj.bwd(dpa, t['att'], sink)
         dqkv = ops.attention_bwd(t['qkv'], t['att'], datt, t['lse'], b, l, self.heads, d, self.scale)
         ops.rope_qk(dqkv, rope[0], rope[1], b, l, self.heads, d, backward=True)

@@ -115,16 +115,12 @@ class MAERT(Runtime):
         dx, dxb = self._blocks_bwd(self.dec_blocks, tape['dec'], dx, dxb, b, ld)
         # un-shuffle backward: every row of the encoder_to_decoder output is referenced exactly once; mask-token rows sum up
         dy, dmask = ops.token_gather_bwd(dx.view(b, ld, cd), tape['dec_idx'], le, zero=False)
-        mbuf, macc = sink.begin(dec.mask_token)
-        mbuf.view(-1).copy_(dmask + (mbuf.view(-1) if macc else 0))
-        sink.done(dec.mask_token, mbuf)
+        sink.add(dec.mask_token, dmask.view_as(dec.mask_token))
         dlne = self.e2d.bwd(dy.view(b * le, cd), tape['lne'], sink)
         dx, dxb = layernorm_bwd(enc.norm, dlne, tape['enc_out'], tape['ste'], sink)
         dx, dxb = self._blocks_bwd(self.enc_blocks, tape['enc'], dx, dxb, b, le)
         # gather backward: masked patches get no gradient; the cls rows sum into the cls token (pos_embed is frozen)
         dpatch, dcls = ops.token_gather_bwd(dx.view(b, le, c), tape['enc_idx'], n, zero=True)
-        cbuf, cacc = sink.begin(enc.cls_token)
-        cbuf.view(-1).copy_(dcls + (cbuf.view(-1) if cacc else 0))
-        sink.done(enc.cls_token, cbuf)
+        sink.add(enc.cls_token, dcls.view_as(enc.cls_token))
         self.patch.bwd(dpatch.view(b * n, c), tape['cols'], sink)
 

@@ -59,16 +59,14 @@ def rows_wgrad(dy, x, weight, sink):
     """Weight gradient of a GEMM with a ``rows`` operand: dy bf16 [M, N8] (N8 = the padded rows), x bf16 [M, K].  Writes
     the [N, K] gradient of `weight` through the sink."""
     n = weight.shape[0]
-    wbuf, wacc = sink.begin(weight)
     part = ops.linear_wgrad(dy, x)
     if part.shape[1] == n:
-        ops.reduce_partials(part, wbuf, accumulate=wacc)
+        with sink.grad(weight) as (acc, buf):
+            ops.reduce_partials(part, buf, accumulate=acc)
     else:
         tmp = torch.empty(part.shape[1], part.shape[2], device=dy.device)
         ops.reduce_partials(part, tmp)
-        g = tmp[:n].view_as(wbuf)
-        wbuf.copy_(g + wbuf if wacc else g)
-    sink.done(weight, wbuf)
+        sink.add(weight, tmp[:n].view_as(weight))
 
 
 class Linear:
@@ -103,14 +101,13 @@ class Linear:
         rows_wgrad(dy, x, self.mod.weight, sink)
         if b is not None:
             n = b.shape[0]
-            bbuf, bacc = sink.begin(b)
             if dy.shape[1] == n:
-                ops.colsum(dy, bbuf, accumulate=bacc)
+                with sink.grad(b) as (acc, buf):
+                    ops.colsum(dy, buf, accumulate=acc)
             else:
                 full = torch.empty(dy.shape[1], device=dy.device)
                 ops.colsum(dy, full)
-                bbuf.copy_(full[:n] + (bbuf if bacc else 0))
-            sink.done(b, bbuf)
+                sink.add(b, full[:n])
         return ops.linear_dgrad(dy, self.op.w, gelu_pre=gelu_pre, relu_out=relu_out, add=add) if need_dx else None
 
 
@@ -133,11 +130,7 @@ class PatchEmbed:
 
     def bwd(self, dy, cols, sink):
         """dy bf16 [B*P*Q, C]: writes the weight and bias gradients through the sink."""
-        w, b = self.conv.weight, self.conv.bias
-        wbuf, wacc = sink.begin(w)
-        part = ops.linear_wgrad(dy, cols)
-        ops.finish_conv_wgrad(part, wbuf, self.op.kpad, accumulate=wacc, order=ops.ORDER_CRS)
-        sink.done(w, wbuf)
-        bbuf, bacc = sink.begin(b)
-        ops.colsum(dy, bbuf, accumulate=bacc)
-        sink.done(b, bbuf)
+        with sink.grad(self.conv.weight) as (acc, buf):
+            ops.finish_conv_wgrad(ops.linear_wgrad(dy, cols), buf, self.op.kpad, accumulate=acc, order=ops.ORDER_CRS)
+        with sink.grad(self.conv.bias) as (acc, buf):
+            ops.colsum(dy, buf, accumulate=acc)

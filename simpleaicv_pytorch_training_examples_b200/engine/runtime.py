@@ -12,6 +12,8 @@ torch.  ``run`` couples the two through one autograd node, and every runtime kee
   * Parameter gradients never travel through autograd: the runtime writes them through its ``GradSink``, and the node
     fires ``sink.on_backward_end()`` once ``rt.backward`` has enqueued the whole backward pass.
 """
+import contextlib
+
 import torch
 import torch.nn as nn
 
@@ -25,26 +27,40 @@ class GradSink:
         self.on_ready = None  # callback(param) fired as soon as a gradient is complete
         self.on_backward_end = None  # callback() fired when the whole backward pass is enqueued
 
-    def buffer_for(self, param):
-        v = self.views.get(id(param))
-        if v is None:
-            v = torch.empty_like(param, dtype=torch.float32)
-            self.views[id(param)] = v
-        return v
-
-    def begin(self, param):
-        """Returns (buffer, accumulate): accumulate when param.grad already holds a gradient."""
-        buf = self.buffer_for(param)
-        if param.grad is None:
-            return buf, False
-        if param.grad.data_ptr() != buf.data_ptr():
+    def _buffer(self, param):
+        """The buffer the gradient of `param` is written into; it holds param.grad when there is one."""
+        buf = self.views.get(id(param))
+        if buf is None:
+            buf = self.views[id(param)] = torch.empty_like(param, dtype=torch.float32)
+        if param.grad is not None and param.grad.data_ptr() != buf.data_ptr():
             buf.copy_(param.grad)
-        return buf, True
+        return buf
 
-    def done(self, param, buf):
-        param.grad = buf
-        if self.on_ready is not None:
-            self.on_ready(param)
+    @contextlib.contextmanager
+    def grad(self, *params):
+        """``with sink.grad(*params) as (accumulate, *buffers):`` the body writes the gradient of each parameter into its
+        buffer (parameter shape, fp32), adding to what the buffer holds when `accumulate`: a gradient is already there.
+        The parameters share one flag because one kernel writes them, so they must agree on it.  On normal exit each buffer
+        becomes its parameter's .grad and on_ready fires, in argument order; if the body raises, neither happens."""
+        accumulate = params[0].grad is not None
+        if any((p.grad is not None) != accumulate for p in params):
+            raise RuntimeError('parameters whose gradients one kernel writes must all have a gradient or all have none; '
+                               f'.grad is set on {[tuple(p.shape) for p in params if p.grad is not None]} only')
+        bufs = [self._buffer(p) for p in params]
+        yield (accumulate, *bufs)
+        for p, buf in zip(params, bufs):
+            p.grad = buf
+            if self.on_ready is not None:
+                self.on_ready(p)
+
+    def add(self, param, g):
+        """Writes `g`, a gradient computed in the parameter's shape: copied into the buffer, or added to the gradient
+        already there."""
+        with self.grad(param) as (accumulate, buf):
+            if accumulate:
+                buf.add_(g)
+            else:
+                buf.copy_(g)
 
 
 class Runtime:

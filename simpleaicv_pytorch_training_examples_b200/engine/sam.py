@@ -96,13 +96,9 @@ class _Block:
                      t['lse'], datt.view(Bw, L, self.heads, hd).permute(0, 2, 1, 3), 1.0, dqe,
                      d5[:, :, 1].permute(0, 2, 1, 3), d5[:, :, 2].permute(0, 2, 1, 3), dk_cols=hd)
         rph, rpw = blk.attn.rel_pos_h, blk.attn.rel_pos_w
-        hbuf, hacc = sink.begin(rph)
-        wbuf, wacc = sink.begin(rpw)
-        assert hacc == wacc
-        ops.relpos_bwd(dqe, qkv, rph.detach(), rpw.detach(), dqkv, hbuf, wbuf, Bw, self.heads, hd, Sh, Sw, self.scale, accumulate=hacc,
-                       aux=t.get('rp_aux'))
-        sink.done(rph, hbuf)
-        sink.done(rpw, wbuf)
+        with sink.grad(rph, rpw) as (acc, hbuf, wbuf):
+            ops.relpos_bwd(dqe, qkv, rph.detach(), rpw.detach(), dqkv, hbuf, wbuf, Bw, self.heads, hd, Sh, Sw, self.scale,
+                           accumulate=acc, aux=t.get('rp_aux'))
         dxw = self.qkv.bwd(dqkv, t['xw'], sink)
         if self.ws > 0:
             dln1 = ops.window_unpartition(dxw.view(Bw, L, C), B, H, W, self.ws).view(-1, C)
@@ -149,17 +145,13 @@ class Neck:
         n1, n3 = m[1], m[3]
         dl2 = dout.permute(0, 2, 3, 1).reshape(-1, oc).to(torch.bfloat16).contiguous()
         _, dy2b = layernorm_bwd(n3, dl2, tape['y2'], tape['s2'], sink)
-        w2 = m[2].weight
-        wbuf, wacc = sink.begin(w2)
-        part = ops.conv_wgrad(dy2b.view(B, H, W, oc), tape['l1'].view(B, H, W, oc), tape['cs'])
-        ops.finish_conv_wgrad(part, wbuf, 9 * oc, accumulate=wacc)
-        sink.done(w2, wbuf)
+        with sink.grad(m[2].weight) as (acc, buf):
+            part = ops.conv_wgrad(dy2b.view(B, H, W, oc), tape['l1'].view(B, H, W, oc), tape['cs'])
+            ops.finish_conv_wgrad(part, buf, 9 * oc, accumulate=acc)
         dl1 = ops.conv_dgrad(dy2b.view(B, H, W, oc), self.n2.w, tape['cs']).view(-1, oc)
         _, dy1b = layernorm_bwd(n1, dl1, tape['y1'], tape['s1'], sink)
-        w0 = m[0].weight
-        wbuf, wacc = sink.begin(w0)
-        ops.reduce_partials(ops.linear_wgrad(dy1b, tape['xb']), wbuf, accumulate=wacc)
-        sink.done(w0, wbuf)
+        with sink.grad(m[0].weight) as (acc, buf):
+            ops.reduce_partials(ops.linear_wgrad(dy1b, tape['xb']), buf, accumulate=acc)
         return ops.linear_dgrad(dy1b, self.n0.w, out_f32=out_f32)
 
 
@@ -193,9 +185,8 @@ class SamEncoderRT(Runtime):
 
     def embed_backward(self, dx, dxb, tape):
         m, sink = self.model, self.sink
-        pbuf, pacc = sink.begin(m.pos_embed)
-        ops.colsum(dx.view(tape['B'], -1), pbuf.view(-1), accumulate=pacc)        # sum over the batch
-        sink.done(m.pos_embed, pbuf)
+        with sink.grad(m.pos_embed) as (acc, buf):
+            ops.colsum(dx.view(tape['B'], -1), buf.view(-1), accumulate=acc)        # sum over the batch
         self.patch.bwd(dxb, tape['cols'], sink)
 
     def neck_forward(self, x, tape):

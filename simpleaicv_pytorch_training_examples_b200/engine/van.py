@@ -19,6 +19,7 @@ from .. import ops
 from .convnet import FcHeadRT
 from .operands import CONV, STEM, Linear, Operand
 from .runtime import Runtime
+from .vit import drop_path_scale
 
 
 def _bn_forward(bn, x, training, out_f32, tape):
@@ -45,13 +46,8 @@ def _bn_forward(bn, x, training, out_f32, tape):
 
 
 def _bn_backward(bn, g, tape, sink, dres=None, dx_f32=True):
-    gbuf, gacc = sink.begin(bn.weight)
-    bbuf, bacc = sink.begin(bn.bias)
-    assert gacc == bacc
-    dx = ops.bn_bwd_generic(tape['x'], g, tape['saved'], bn.weight.detach(), gbuf, bbuf, dres=dres, dx_f32=dx_f32, accumulate=gacc)
-    sink.done(bn.weight, gbuf)
-    sink.done(bn.bias, bbuf)
-    return dx
+    with sink.grad(bn.weight, bn.bias) as (acc, dg, db):
+        return ops.bn_bwd_generic(tape['x'], g, tape['saved'], bn.weight.detach(), dg, db, dres=dres, dx_f32=dx_f32, accumulate=acc)
 
 
 class _DW:
@@ -69,14 +65,11 @@ class _DW:
 
     def bwd(self, dy, x, sink):
         """dy: gradient w.r.t. the conv output (pre-ReLU), x: the conv input.  Returns dx."""
-        w, b = self.conv.weight, self.conv.bias
-        wbuf, wacc = sink.begin(w)
-        ops.dwconv_wgrad(dy, x, wbuf, self.k, self.dil, accumulate=wacc)
-        sink.done(w, wbuf)
-        bbuf, bacc = sink.begin(b)
-        ops.colsum(dy.view(-1, dy.shape[-1]), bbuf, accumulate=bacc)
-        sink.done(b, bbuf)
-        return ops.dwconv_fwd(dy, w.detach(), None, self.k, self.dil, flip=True)
+        with sink.grad(self.conv.weight) as (acc, buf):
+            ops.dwconv_wgrad(dy, x, buf, self.k, self.dil, accumulate=acc)
+        with sink.grad(self.conv.bias) as (acc, buf):
+            ops.colsum(dy.view(-1, dy.shape[-1]), buf, accumulate=acc)
+        return ops.dwconv_fwd(dy, self.conv.weight.detach(), None, self.k, self.dil, flip=True)
 
 
 class _Block:
@@ -94,15 +87,6 @@ class _Block:
     def linears(self):
         return [self.proj1, self.proj2, self.conv1, self.fc1, self.fc2]
 
-    def _path_scale(self, n, training, dev):
-        if not training or self.drop_path == 0.:
-            return None
-        keep = 1. - self.drop_path
-        s = torch.empty(n, device=dev).bernoulli_(keep)
-        if keep > 0.:
-            s.div_(keep)
-        return s
-
     def forward(self, x, t, shape, training):
         """x: stream [rows, C] (bf16 for the first block of a stage, fp32 afterwards) -> fp32 [rows, C]."""
         n, h, w, c = shape
@@ -115,7 +99,7 @@ class _Block:
         c1 = t['c1'] = self.conv1.fwd(cs.view(-1, c))
         g = t['g'] = ops.mul_bf16(p1, c1)
         p2 = t['p2'] = self.proj2.fwd(g)
-        s1 = t['s1'] = self._path_scale(n, training, x.device)
+        s1 = t['s1'] = drop_path_scale(self.drop_path, n, training, x.device)
         ls1 = blk.layer_scale_1.detach().view(-1)
         x1 = t['x1'] = ops.ls_residual_fwd(x, p2, a, ls1, s1, h * w)
         m = t['m'] = _bn_forward(blk.norm2, x1, training, False, t['bn2'])
@@ -123,7 +107,7 @@ class _Block:
         hid = f1.shape[1]
         d = t['d'] = self.dw.fwd(f1.view(n, h, w, hid), relu=True)
         f2 = t['f2'] = self.fc2.fwd(d.view(-1, hid))
-        s2 = t['s2'] = self._path_scale(n, training, x.device)
+        s2 = t['s2'] = drop_path_scale(self.drop_path, n, training, x.device)
         return ops.ls_residual_fwd(x1, f2, None, blk.layer_scale_2.detach().view(-1), s2, h * w)
 
     def backward(self, dx2, t, shape, sink, dx_f32=True):
@@ -133,20 +117,18 @@ class _Block:
         blk = self.blk
         hw = h * w
         # ---- MLP branch
-        lbuf, lacc = sink.begin(blk.layer_scale_2)
-        df2 = ops.ls_residual_bwd(dx2, t['f2'], None, blk.layer_scale_2.detach().view(-1), lbuf.view(-1), accumulate=lacc,
-                                  row_scale=t['s2'], rows_per_scale=hw)
-        sink.done(blk.layer_scale_2, lbuf)
+        with sink.grad(blk.layer_scale_2) as (acc, buf):
+            df2 = ops.ls_residual_bwd(dx2, t['f2'], None, blk.layer_scale_2.detach().view(-1), buf.view(-1), accumulate=acc,
+                                      row_scale=t['s2'], rows_per_scale=hw)
         hid = t['f1'].shape[1]
         dpre = self.fc2.bwd(df2, t['d'].view(-1, hid), sink, relu_out=t['d'].view(-1, hid))     # masked by relu'(d)
         df1 = self.dw.bwd(dpre.view(n, h, w, hid), t['f1'].view(n, h, w, hid), sink)
         dm = self.fc1.bwd(df1.view(-1, hid), t['m'], sink)
         dx1 = _bn_backward(blk.norm2, dm, t['bn2'], sink, dres=dx2)
         # ---- attention branch
-        lbuf, lacc = sink.begin(blk.layer_scale_1)
-        dy = ops.ls_residual_bwd(dx1, t['p2'], t['a'], blk.layer_scale_1.detach().view(-1), lbuf.view(-1), accumulate=lacc,
-                                 row_scale=t['s1'], rows_per_scale=hw)
-        sink.done(blk.layer_scale_1, lbuf)
+        with sink.grad(blk.layer_scale_1) as (acc, buf):
+            dy = ops.ls_residual_bwd(dx1, t['p2'], t['a'], blk.layer_scale_1.detach().view(-1), buf.view(-1), accumulate=acc,
+                                     row_scale=t['s1'], rows_per_scale=hw)
         dg = self.proj2.bwd(dy, t['g'], sink)
         dc1 = ops.mul_bf16(dg, t['p1'])
         dcs = self.conv1.bwd(dc1, t['cs'].view(-1, c), sink)
@@ -186,14 +168,11 @@ class StridedConv:
 
     def backward(self, dy, t, sink):
         """dy: bf16 gradient [rows, C] w.r.t. the conv output.  Returns the NHWC bf16 input gradient (None for an image)."""
-        w, b = self.conv.weight, self.conv.bias
-        wbuf, wacc = sink.begin(w)
-        part = ops.linear_wgrad(dy, t['cols'])
-        ops.finish_conv_wgrad(part, wbuf, self.kpad, accumulate=wacc, order=ops.ORDER_CRS if self.from_image else ops.ORDER_RSC)
-        sink.done(w, wbuf)
-        bbuf, bacc = sink.begin(b)
-        ops.colsum(dy, bbuf, accumulate=bacc)
-        sink.done(b, bbuf)
+        with sink.grad(self.conv.weight) as (acc, buf):
+            ops.finish_conv_wgrad(ops.linear_wgrad(dy, t['cols']), buf, self.kpad, accumulate=acc,
+                                  order=ops.ORDER_CRS if self.from_image else ops.ORDER_RSC)
+        with sink.grad(self.conv.bias) as (acc, buf):
+            ops.colsum(dy, buf, accumulate=acc)
         if self.from_image:
             return None
         n, h, ww, c = t['in_shape']

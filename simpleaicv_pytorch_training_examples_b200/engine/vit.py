@@ -22,14 +22,23 @@ from .runtime import Runtime
 def layernorm_bwd(norm, dy, x, stats, sink, dres=None, want_bf16=True, scale=None, rows_per_scale=0):
     """Backward of a row LayerNorm (nn.LayerNorm `norm`): dgamma / dbeta through the sink; returns (dx fp32 (+ dres), its
     bf16 copy multiplied by the row scale `scale` (one per rows_per_scale rows), or None unless want_bf16)."""
-    gbuf, gacc = sink.begin(norm.weight)
-    bbuf, bacc = sink.begin(norm.bias)
     dxb = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16) if want_bf16 else None
-    dx = ops.layernorm_bwd(dy, x, norm.weight.detach(), stats, gbuf, bbuf, dres=dres, dx_bf16=dxb, accumulate=gacc,
-                           bf16_row_scale=scale, rows_per_scale=rows_per_scale)
-    sink.done(norm.weight, gbuf)
-    sink.done(norm.bias, bbuf)
+    with sink.grad(norm.weight, norm.bias) as (acc, dg, db):
+        dx = ops.layernorm_bwd(dy, x, norm.weight.detach(), stats, dg, db, dres=dres, dx_bf16=dxb, accumulate=acc,
+                               bf16_row_scale=scale, rows_per_scale=rows_per_scale)
     return dx, dxb
+
+
+def drop_path_scale(p, n, training, dev):
+    """The per-sample drop-path scale [n] of drop probability `p`, drawn on the device as the reference draws it
+    (bernoulli_(keep) / keep), or None when drop path is off."""
+    if not training or p == 0.:
+        return None
+    keep = 1. - p
+    s = torch.empty(n, device=dev).bernoulli_(keep)
+    if keep > 0.:
+        s.div_(keep)
+    return s
 
 
 class _Block:
@@ -44,15 +53,6 @@ class _Block:
 
     def linears(self):
         return [self.qkv, self.proj, self.fc1, self.fc2]
-
-    def _path_scale(self, b, l, training, dev):
-        if not training or self.drop_path == 0.:
-            return None
-        keep = 1. - self.drop_path
-        s = torch.empty(b, device=dev).bernoulli_(keep)
-        if keep > 0.:
-            s.div_(keep)
-        return s
 
     def forward(self, x, t, b, l, training, p=0., seeds=None, scales=None, sb=None):
         """x: fp32 [B*L, C] -> fp32 [B*L, C].  p: dropout probability of this pass (vit.py:59,73-78,90-97: attention
@@ -70,7 +70,7 @@ class _Block:
                                        dropout_p=p, dropout_seed=seeds[0], dropout_seed_base=sb)
         else:
             t['att'], t['lse'] = ops.attention_fwd(t['qkv'], b, l, self.heads, d, self.scale)
-        s1 = t['s1'] = scales[0] if scales is not None else self._path_scale(b, l, training, x.device)
+        s1 = t['s1'] = scales[0] if scales is not None else drop_path_scale(self.drop_path, b, training, x.device)
         if p > 0.:
             x = ops.dropout(self.proj.fwd(t['att']), p, seeds[1], resid=x, row_scale=s1, elems_per_scale=l * c, seed_base=sb)
         else:
@@ -81,7 +81,7 @@ class _Block:
         t['h'] = ops.gelu_fwd(t['u'])
         if p > 0.:
             ops.dropout(t['h'], p, seeds[2], out=t['h'], seed_base=sb)
-        s2 = t['s2'] = scales[1] if scales is not None else self._path_scale(b, l, training, x.device)
+        s2 = t['s2'] = scales[1] if scales is not None else drop_path_scale(self.drop_path, b, training, x.device)
         if p > 0.:
             return ops.dropout(self.fc2.fwd(t['h']), p, seeds[3], resid=x, row_scale=s2, elems_per_scale=l * c, seed_base=sb)
         return self.fc2.fwd(t['h'], resid=x, out_f32=True, row_scale=s2, rows_per_scale=l)
@@ -182,11 +182,10 @@ class ViTRT(Runtime):
         dl = torch.zeros(b, npad, device=dlogits.device, dtype=torch.bfloat16)
         dl[:, :ncls] = dlogits.to(torch.bfloat16)
         # fc bias gradient from the fp32 dlogits
-        bbuf, bacc = sink.begin(m.fc.bias)
-        ops.colsum(dlogits.contiguous().float(), bbuf, accumulate=bacc)
-        rows_wgrad(dl, tape['lnf'], m.fc.weight, sink)
-        dlnf = ops.linear_dgrad(dl, self.fc.op.w)
-        sink.done(m.fc.bias, bbuf)
+        with sink.grad(m.fc.bias) as (acc, buf):
+            ops.colsum(dlogits.contiguous().float(), buf, accumulate=acc)
+            rows_wgrad(dl, tape['lnf'], m.fc.weight, sink)
+            dlnf = ops.linear_dgrad(dl, self.fc.op.w)
         dpooled, _ = layernorm_bwd(m.norm, dlnf, tape['pooled'], tape['stf'], sink, want_bf16=False)
         dxb = torch.empty(b * l, c, device=dl.device, dtype=torch.bfloat16)
         dx = ops.token_pool_bwd(dpooled, l, m.global_pool, dx_bf16=dxb.view(b, l, c), bf16_row_scale=next_scale)
@@ -195,13 +194,9 @@ class ViTRT(Runtime):
     def embed_backward(self, dx, tape):
         m, sink = self.model, self.sink
         b, l, c = tape['b'], tape['l'], m.embedding_planes
-        pbuf, pacc = sink.begin(m.pos_embed)
-        cbuf, cacc = sink.begin(m.cls_token)
-        assert pacc == cacc
         dpatch = torch.empty(b * (l - 1), c, device=dx.device, dtype=torch.bfloat16)
-        ops.vit_assemble_tokens_bwd(dx.view(b, l, c), pbuf, cbuf, dpatch, accumulate=pacc)
-        sink.done(m.pos_embed, pbuf)
-        sink.done(m.cls_token, cbuf)
+        with sink.grad(m.pos_embed, m.cls_token) as (acc, pbuf, cbuf):
+            ops.vit_assemble_tokens_bwd(dx.view(b, l, c), pbuf, cbuf, dpatch, accumulate=acc)
         self.patch.bwd(dpatch, tape['cols'], sink)
 
     def backward(self, dlogits, tape):

@@ -25,13 +25,7 @@ class _FakeNet(nn.Module):
     def fake_backward(self, rank, scale=1.0):
         sink = self._sink
         for i, p in enumerate(reversed([self.a.weight, self.a.bias, self.b.weight, self.b.bias])):
-            buf, acc = sink.begin(p)
-            g = torch.full_like(p, (rank + 1) * (i + 1) * scale)
-            if acc:
-                buf.add_(g)
-            else:
-                buf.copy_(g)
-            sink.done(p, buf)
+            sink.add(p, torch.full_like(p, (rank + 1) * (i + 1) * scale))
         if sink.on_backward_end is not None:
             sink.on_backward_end()
 
@@ -78,7 +72,7 @@ def _worker(rank, world, port, q):
         dist.destroy_process_group()
 
 
-def test_bucketed_allreduce_gloo_world2():
+def test_bucketed_allreduce_gloo_world2_gradients_written_through_sink_add():
     s = socket.socket()
     s.bind(('127.0.0.1', 0))
     port = s.getsockname()[1]

@@ -1,9 +1,10 @@
 """The autograd boundary of engine/runtime.py, driven on the CPU by a stand-in runtime made of plain torch ops that
-keeps the runtime contract: forward(*inputs, training, keep_tape) -> (*outputs, tape), backward(*grads, tape)."""
+keeps the runtime contract: forward(*inputs, training, keep_tape) -> (*outputs, tape), backward(*grads, tape); and the
+GradSink that every runtime writes its parameter gradients through."""
 import pytest
 import torch
 
-from simpleaicv_pytorch_training_examples_b200.engine.runtime import Runtime, run
+from simpleaicv_pytorch_training_examples_b200.engine.runtime import GradSink, Runtime, run
 
 
 class _FakeRT(Runtime):
@@ -83,3 +84,70 @@ def test_eval_and_no_grad_keep_no_tape_and_build_no_graph(training, grad):
         outs = run(rt, training, torch.randn(3, 4), torch.tensor(2.))
     assert rt.events == [('forward', training, False, False)]
     assert len(outs) == 3 and all(o.grad_fn is None and not o.requires_grad for o in outs)
+
+
+def _recording_sink():
+    sink, ready = GradSink(), []
+    sink.on_ready = ready.append
+    return sink, ready
+
+
+def test_grad_becomes_the_sink_buffer_and_each_parameter_is_reported_once_in_order():
+    sink, ready = _recording_sink()
+    w, b = torch.nn.Parameter(torch.ones(3, 2)), torch.nn.Parameter(torch.ones(3))
+    with sink.grad(w, b) as (acc, wbuf, bbuf):
+        assert not acc and wbuf.shape == w.shape and bbuf.shape == b.shape and wbuf.dtype == torch.float32
+        assert w.grad is None and not ready        # nothing is published before the body has written the gradients
+        wbuf.fill_(2.)
+        bbuf.fill_(3.)
+    assert w.grad is wbuf and b.grad is bbuf
+    assert w.grad is sink.views[id(w)] and b.grad is sink.views[id(b)]
+    assert [id(p) for p in ready] == [id(w), id(b)]
+
+
+def test_accumulates_onto_an_existing_grad_held_in_another_tensor():
+    sink, ready = _recording_sink()
+    w = torch.nn.Parameter(torch.zeros(4))
+    prev = torch.arange(4.)
+    w.grad = prev
+    with sink.grad(w) as (acc, buf):
+        assert acc and buf is not prev and torch.equal(buf, prev)
+        buf.add_(1.)
+    assert w.grad is buf and torch.equal(w.grad, torch.arange(4.) + 1) and torch.equal(prev, torch.arange(4.))
+    with sink.grad(w) as (acc, buf2):               # .grad is now the buffer itself: accumulate in place
+        assert acc and buf2 is buf
+        buf2.add_(1.)
+    assert torch.equal(w.grad, torch.arange(4.) + 2) and len(ready) == 2
+
+
+def test_a_raising_body_publishes_nothing():
+    sink, ready = _recording_sink()
+    w, b = torch.nn.Parameter(torch.ones(2)), torch.nn.Parameter(torch.ones(2))
+    with pytest.raises(ValueError, match='kernel failed'):
+        with sink.grad(w, b) as (_, wbuf, bbuf):
+            wbuf.zero_()
+            raise ValueError('kernel failed')
+    assert w.grad is None and b.grad is None and not ready
+
+
+@pytest.mark.parametrize('with_grad', ['first', 'second'])
+def test_parameters_written_by_one_kernel_must_agree_on_accumulate(with_grad):
+    sink, ready = _recording_sink()
+    w, b = torch.nn.Parameter(torch.ones(2)), torch.nn.Parameter(torch.ones(2))
+    has, other = (w, b) if with_grad == 'first' else (b, w)
+    has.grad = torch.full((2,), 5.)
+    with pytest.raises(RuntimeError, match='all have a gradient or all have none'):
+        with sink.grad(w, b):
+            pass
+    assert other.grad is None and torch.equal(has.grad, torch.full((2,), 5.)) and not ready
+
+
+def test_add_copies_the_first_gradient_and_adds_the_next():
+    sink, ready = _recording_sink()
+    w = torch.nn.Parameter(torch.ones(3))
+    g = torch.tensor([-0., 1., 2.])
+    sink.add(w, g)
+    assert w.grad is sink.views[id(w)] and w.grad is not g
+    assert torch.equal(w.grad, g) and torch.signbit(w.grad[0])     # a copy: -0.0 stays -0.0
+    sink.add(w, g)
+    assert torch.equal(w.grad, 2 * g) and [id(p) for p in ready] == [id(w)] * 2
