@@ -152,12 +152,12 @@ void tune_override(int* bn, int* stages, int* nb) {
   if (nb && c > 0) *nb = c;
 }
 
-// Split of the 227 KB between the operand ring (stages) and the epilogue staging slices (nb per half)
-// (tests/profile_gemm_tune.py sweeps it):
-//  * no aux operand: two slices per half whenever >= 3 stages remain (>= 4 for reductions of 4+ k-blocks) - a TMA store
+// Split of the 227 KB between the operand ring (stages) and the epilogue staging slices (2 * nb, used round-robin by the
+// tile's consecutive 64-column bf16 / 32-column fp32 slices) (tests/profile_gemm_tune.py sweeps it):
+//  * no aux operand: nb = 2 whenever >= 3 stages remain (>= 4 for reductions of 4+ k-blocks) - a TMA store
 //    is then not waited for right after it was issued;
 //  * aux operand by TMA: the slices are also the landing buffers of the next aux tiles, so depth matters more than ring
-//    stages while the reduction is short: <= 4 k-blocks -> 3 slices / 2+ stages, fp32 tiles of <= 16 k-blocks -> 2 slices /
+//    stages while the reduction is short: <= 4 k-blocks -> nb = 3 / 2+ stages, fp32 tiles of <= 16 k-blocks -> nb = 2 /
 //    3 stages; everything longer keeps 4 stages first.
 template <int BN>
 void pick_smem_split(const GemmParams& p, int stat_bytes, int* stages_out, int* nb_out) {
@@ -206,7 +206,8 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, con
 }
 
 // Tile width with the least padded columns (ties -> wider tile).  128 is the widest: each of the two consumer
-// warpgroups keeps a 128 x 64 fp32 accumulator in registers next to its epilogue.
+// warpgroups keeps the 64 x BN fp32 accumulator of its 64 rows (one m64nBN wgmma per k16 step) in registers next to its
+// epilogue, 64 registers a thread at BN = 128.
 int pick_bn(int N) {
   const int cand[2] = {128, 64};
   int best = 128;

@@ -5,9 +5,10 @@
 // One CTA per SM, 384 threads:
 //   warp 0      TMA producer (one lane)        global -> 128B-swizzled smem ring
 //   warps 1..3  idle (keep the consumers on aligned warpgroups)
-//   warps 4..11 two consumer warpgroups; warpgroup h owns columns h*64 .. h*64+63 of the 128 x BN tile:
-//               wgmma (two m64n64 row blocks) -> registers -> per-warp transpose through shared memory so that a
-//               thread owns one row -> (bias/act/residual) -> smem -> TMA store
+//   warps 4..11 two consumer warpgroups; warpgroup h owns rows h*64 .. h*64+63 and all BN columns of the 128 x BN tile:
+//               wgmma (one m64nBN per k16 step) -> registers -> per-warp transpose through shared memory so that a
+//               thread owns 16 columns of one row -> (bias/act/residual) -> smem slice shared by both warpgroups ->
+//               TMA store by one thread
 //
 // Operand feeding modes (runtime, so that fprop / dgrad / wgrad of linear layers and of NHWC
 // convolutions all go through this one kernel):
@@ -34,16 +35,16 @@ constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int kGemmThreads = 384;  // 4 control warps (TMA producer + 3 idle) + 8 consumer / epilogue warps
 constexpr int kStoreBufBytes = 16384;  // one staging slice: 128 rows x 128 B
-constexpr int kMaxStoreBufs = 3;       // staging slices per epilogue half (runtime 1..3, GemmParams::store_bufs)
+constexpr int kMaxStoreBufs = 3;       // GemmParams::store_bufs (runtime 1..3): the tile's staging pool is 2 * store_bufs slices
 constexpr int kSmemTotal = 232448;     // dynamic shared memory every launch asks for (227 KB)
 constexpr int kXposeStride = 33;       // floats per row of a warp's transpose buffer (32 columns + 1: conflict-free rows)
-constexpr int kXposeBytes = 8 * 32 * kXposeStride * 4;   // one 32 x 32 fp32 buffer per consumer warp
+constexpr int kXposeBytes = 8 * 32 * kXposeStride * 4;   // two 16 x 32 fp32 buffers (alternating chunks) per consumer warp
 constexpr int kSmemBudget = kSmemTotal - 1024 /*align slack*/ - 512 /*barriers*/ - kXposeBytes;
 
 // The split of shared memory between the operand ring and the epilogue staging slices is a launch
-// parameter (capi_gemm.cu: pick_smem_split): long reductions want >= 4 ring stages and get one slice
-// per half, short reductions (the epilogue-bound 1x1 convolutions, K = 64..256) trade ring stages
-// for 2-3 slices so that a TMA store (and the TMA load of the next aux slice) is never waited for
+// parameter (capi_gemm.cu: pick_smem_split): long reductions want >= 4 ring stages and get two
+// slices, short reductions (the epilogue-bound 1x1 convolutions, K = 64..256) trade ring stages
+// for 4-6 slices so that a TMA store (and the TMA load of the next aux slice) is never waited for
 // right after it was issued.
 template <int BN>
 struct GemmCfg {
@@ -51,8 +52,8 @@ struct GemmCfg {
   static constexpr int kStagesRaw = (kSmemBudget - 2 * kStoreBufBytes) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;   // upper bound of the ring depth
   static constexpr int kSmemBytes = kSmemTotal;
-  static_assert(BN == 64 || BN == 128, "a consumer warpgroup owns 64 columns: BN is 64 (one warpgroup) or 128 (two)");
-  static constexpr int kConsumerWGs = BN / 64;
+  static_assert(BN == 64 || BN == 128, "a consumer warpgroup reduces 64 rows x BN columns with one m64nBN wgmma: BN is 64 or 128");
+  static constexpr int kConsumerWGs = 2;   // rows 0..63 and 64..127 of every tile
 };
 
 struct ConvGeom {
@@ -85,7 +86,7 @@ struct GemmParams {
   long long ldd;       // leading dimension of D in elements
   long long split_stride;  // elements between split-K partial outputs
   int num_stages;      // smem ring depth actually used (<= GemmCfg::kStages)
-  int store_bufs;      // staging slices per epilogue half (1..kMaxStoreBufs)
+  int store_bufs;      // 1..kMaxStoreBufs: the epilogue rotates through 2 * store_bufs staging slices
   int aux_tma;         // 1: the aux operand of the epilogue (resid when out_f32, resid_bf16 otherwise) has the
                        // output's element width and is brought in by TMA (tensor map tmR) INTO the staging
                        // slice, combined in place and stored from there; 0: per-thread global loads
@@ -104,8 +105,8 @@ struct GemmParams {
 
 // Kernel variants: the epilogue's feature set is a compile-time mask, so that the common launches run a compact
 // instruction stream (with every feature a run-time branch, branch resolution and instruction fetch take a large share of
-// the issue slots of the short-reduction launches, whose pace the epilogue sets).  VAR_FULL and VAR_AUX spill a few
-// hundred bytes at the 168-register cap of 384 threads (ptxas -v); the other variants do not spill.
+// the issue slots of the short-reduction launches, whose pace the epilogue sets).  No variant spills (ptxas -v); VAR_FULL
+// and VAR_AUX at BN = 128 sit at the 168-register cap of 384 threads.
 //   VAR_FULL        every flag but EPI_MASK_BITS / output type at run time (GELU forward, EPI_DIRECT, per-thread aux loads)
 //   VAR_PLAIN_BF16  bf16 output, optional bias / ReLU / BatchNorm statistics       (conv fprop, plain dgrad, Linear)
 //   VAR_PLAIN_F32   fp32 output, optional bias                                       (split-K weight gradients, fp32 Linear)
@@ -133,35 +134,35 @@ struct GemmVariant {
   static constexpr int kThreads = kStatsWarps ? kGemmThreads + 128 : kGemmThreads;
 };
 
-// Reduction of one tile by one consumer warpgroup: acc[blk] = rows blk*64 .. +63 x the warpgroup's 64 columns
-// (`b_off`: byte offset of its first column in a B stage).  Both operand layouts put row / column 64 at +8192 bytes.
+// Reduction of one tile by one consumer warpgroup: acc = its 64 rows (`a_off`: byte offset of the first one in an A
+// stage; both operand layouts put row 64 at +8192 bytes) x all BN columns, one m64nBN wgmma per k16 step.  A K-major B
+// stage is BN rows of 128 B; an MN-major one is BN / 64 chunks of 64 columns 8192 B apart, which is the descriptor's LBO.
 // A stage is handed back to the producer (one arrival per warp) once the wgmma group that read it has retired.
 template <int BN, int TA, int TB>
-__device__ __forceinline__ void gemm_mainloop(float (&acc)[2][32], const uint8_t* sA, const uint8_t* sB, uint64_t* full_bar,
+__device__ __forceinline__ void gemm_mainloop(float (&acc)[BN / 2], const uint8_t* sA, const uint8_t* sB, uint64_t* full_bar,
                                               uint64_t* empty_bar, int nstages, int& stage, uint32_t& phase, int kb0, int kb1,
-                                              uint32_t b_off, int lane) {
+                                              uint32_t a_off, int lane) {
   constexpr int kABytes = BM * BK * 2, kBBytes = BN * BK * 2;
   constexpr uint32_t a_lbo = TA ? 8192u : 16u, b_lbo = TB ? 8192u : 16u;
   constexpr uint32_t a_kstep = TA ? 2048u : 32u, b_kstep = TB ? 2048u : 32u;   // bytes per k16 step
   int prev = -1;
   for (int kb = kb0; kb < kb1; ++kb) {
     mbar_wait(&full_bar[stage], phase);
-    const uint32_t a_addr = smem_u32(sA + stage * kABytes);
-    const uint32_t b_addr = smem_u32(sB + stage * kBBytes) + b_off;
-    wgmma_fence_regs(acc[0]);
-    wgmma_fence_regs(acc[1]);
+    const uint32_t a_addr = smem_u32(sA + stage * kABytes) + a_off;
+    const uint32_t b_addr = smem_u32(sB + stage * kBBytes);
+    wgmma_fence_regs(acc);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t da = make_smem_desc(a_addr + k * a_kstep, a_lbo, 1024);
       const uint64_t db = make_smem_desc(b_addr + k * b_kstep, b_lbo, 1024);
       const int acc_in = (kb > kb0 || k > 0) ? 1 : 0;
-      wgmma_m64n64<TA, TB>(acc[0], make_smem_desc(a_addr + k * a_kstep, a_lbo, 1024), db, acc_in);
-      wgmma_m64n64<TA, TB>(acc[1], make_smem_desc(a_addr + 8192 + k * a_kstep, a_lbo, 1024), db, acc_in);
+      if constexpr (BN == 128) wgmma_m64n128<TA, TB>(acc, da, db, acc_in);
+      else wgmma_m64n64<TA, TB>(acc, da, db, acc_in);
     }
     wgmma_commit();
     wgmma_wait<1>();   // the group of the previous stage has retired: its operands may be overwritten
-    wgmma_fence_regs(acc[0]);
-    wgmma_fence_regs(acc[1]);
+    wgmma_fence_regs(acc);
     if (prev >= 0) {
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
@@ -170,8 +171,7 @@ __device__ __forceinline__ void gemm_mainloop(float (&acc)[2][32], const uint8_t
     if (++stage == nstages) { stage = 0; phase ^= 1; }
   }
   wgmma_wait<0>();
-  wgmma_fence_regs(acc[0]);
-  wgmma_fence_regs(acc[1]);
+  wgmma_fence_regs(acc);
   if (prev >= 0) {
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
@@ -215,8 +215,9 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr int kBBytes = BN * BK * 2;
 
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
+  // 1024-byte alignment by an offset from the __shared__ symbol (not by integer arithmetic on the pointer value), so that
+  // the compiler still knows every access below is to shared memory and emits 32-bit LDS / STS instead of generic ones
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   using V = GemmVariant<VAR>;
   const int flags = p.epi_flags & V::kMask;          // bits outside the variant's mask are known zeros
   const bool out_f32 = V::kOut == 0 ? (p.out_f32 != 0) : (V::kOut == 2);
@@ -229,10 +230,10 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   float* sStat = reinterpret_cast<float*>(sD + 2 * NB * kStoreBufBytes);  // [2][N] when EPI_STATS
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(sD + 2 * NB * kStoreBufBytes + (do_stats ? ((8 * p.N + 15) & ~15) : 0));
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* aux_bar = empty_bar + kStages;   // [2 halves][kMaxStoreBufs]: aux slice landed in staging slice b
-  uint64_t* staged_bar = aux_bar + 2 * kMaxStoreBufs;    // [2][kMaxStoreBufs] VAR_STATS_BF16: slice b of the half is staged
-  uint64_t* sdone_bar = staged_bar + 2 * kMaxStoreBufs;  // [2][kMaxStoreBufs] the four stats warps have read slice b
-  float* sXpose = reinterpret_cast<float*>(smem + kSmemTotal - 1024 - kXposeBytes);   // [8 warps][32][kXposeStride]
+  uint64_t* aux_bar = empty_bar + kStages;   // [2 * kMaxStoreBufs]: aux slice landed in staging slice b
+  uint64_t* staged_bar = aux_bar + 2 * kMaxStoreBufs;    // [2 * kMaxStoreBufs] VAR_STATS_BF16: staging slice b is staged
+  uint64_t* sdone_bar = staged_bar + 2 * kMaxStoreBufs;  // [2 * kMaxStoreBufs] the four stats warps have read slice b
+  float* sXpose = reinterpret_cast<float*>(smem + kSmemTotal - 1024 - kXposeBytes);   // [8 warps][2][16][kXposeStride]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -365,53 +366,50 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     __syncwarp();
   } else if (warp >= 4 && warp < 12) {
     // ================================================================ consumers: wgmma + epilogue
-    // 8 warps: warpgroup `half` = e/4 reduces and drains columns half*64 .. +63 of every tile.  Warp e%4 of it holds
-    // the accumulators of rows (e%4)*16 .. +15 and 64 + (e%4)*16 .. +15; after the reduction it transposes each
-    // 32-column chunk through its own shared-memory buffer so that lane l owns one row.  Each half owns NB 16 KB staging slices
-    // (128 rows x 128 B = 64 bf16 or 32 fp32 columns, 128B-swizzled) used round-robin and its own
-    // TMA-store bulk groups: slice s is written while the store of slice s-1 is still reading.
-    // With aux_tma the half's thread 0 also TMA-loads the aux operand of slice s+LA (LA = max(1, NB-1))
-    // into the slice that store s-1 has released; every thread combines its own row in place.
+    // 8 warps: warpgroup `half` = e/4 reduces and drains rows half*64 .. +63 of every tile, all BN columns.  Warp e%4 of it
+    // holds the accumulators of rows half*64 + (e%4)*16 .. +15; after the reduction it transposes each 32-column chunk
+    // through its own shared-memory buffer so that lane l owns columns (l/16)*16 .. +15 of row l%16.  The tile's 2*NB
+    // 16 KB staging slices (128 rows x 128 B = 64 bf16 or 32 fp32 columns, 128B-swizzled) are used round-robin in
+    // ascending column order; both warpgroups write their rows of the same slice, one 256-thread barrier closes it and
+    // the first consumer thread issues its TMA store: slice s is written while the stores of earlier slices still read.
+    // With aux_tma that thread also TMA-loads the aux operand of slice s+LA (LA = 2*NB - 1) into the slice
+    // that store s-1 has released; every thread combines its own piece of a row in place.
     const int e = warp - 4;
     const int q = e & 3;
     const int half = e >> 2;
-    const int gtid = threadIdx.x - 128 - half * 128;  // 0..127 inside the half
-    const int row_in_tile = (lane < 16 ? 0 : 48) + q * 16 + lane;   // lanes 0..15: rows q*16.., 16..31: rows 64 + q*16..
+    const bool leader = threadIdx.x == 128;           // issues the TMA stores and the aux requests of the tile
+    const int hh = lane >> 4;                         // which 16 columns of a 32-column chunk this thread owns
+    const int row_in_tile = half * 64 + q * 16 + (lane & 15);
     const int rsw = row_in_tile & 7;                  // 128B-swizzle phase of this thread's staging row
-    const uint32_t bar_id = 1 + half;
-    uint8_t* const sbase = sD + half * NB * kStoreBufBytes;
-    uint64_t* const abar = aux_bar + half * kMaxStoreBufs;
+    const uint32_t bar_id = 1;
+    const int NBT = 2 * NB;                           // staging slices of the tile
     float* const xp = sXpose + e * 32 * kXposeStride;
     const bool direct = (flags & EPI_DIRECT) != 0;
     const bool aux_tma = V::kAux == 0 ? (p.aux_tma != 0) : (V::kAux == 2);
-    // chunk (32 columns) range of this half: its 64 columns (one bf16 slice or two fp32 slices); none for half 1 of BN = 64
-    constexpr int NCH = BN / 32;
-    const int c_begin = half ? 2 : 0;
-    const int c_end = half ? NCH : 2;
+    constexpr int NCH = BN / 32;                      // 32-column chunks of a tile
     const bool a_mn = VAR == VAR_PLAIN_F32 ? (p.a_mode == A_MN2D || p.a_mode == A_IM2COL_MN) : (p.a_mode == A_MN2D);
     const bool b_mn = (p.b_mode != B_K2D);
     int stage = 0;
     uint32_t phase = 0;
-    const int spt = out_f32 ? (c_end - c_begin) : ((c_end - c_begin) >> 1);  // slices per tile of this half
+    const int spt = out_f32 ? NCH : (NCH >> 1);       // slices per tile
     int bufi = 0;             // staging slice of the current output slice
-    uint32_t aux_phase = 0;   // bit b: parity to wait for on abar[b]
-    // aux prefetch cursor (thread 0 of the half): next slice to request = slice pf_j of work item pf_w
+    uint32_t aux_phase = 0;   // bit b: parity to wait for on aux_bar[b]
+    // aux prefetch cursor (leader): next slice to request = slice pf_j of work item pf_w
     long long pf_w = blockIdx.x;
     int pf_j = 0, pf_b = 0;
     auto request_aux = [&]() {
       if (pf_w < total) {
         const int n_blk2 = (int)(pf_w % num_n);
         const int m_blk2 = (int)((pf_w / num_n) % num_m);
-        const int col = n_blk2 * BN + (out_f32 ? (c_begin + pf_j) * 32 : ((c_begin >> 1) + pf_j) * 64);
-        mbar_expect_tx(&abar[pf_b], kStoreBufBytes);   // rows / columns past the matrix are zero-filled and counted
-        tma_load_3d(&tmR, &abar[pf_b], sbase + pf_b * kStoreBufBytes, col, m_blk2 * tile_rows, 0);
+        const int col = n_blk2 * BN + pf_j * (out_f32 ? 32 : 64);
+        mbar_expect_tx(&aux_bar[pf_b], kStoreBufBytes);   // rows / columns past the matrix are zero-filled and counted
+        tma_load_3d(&tmR, &aux_bar[pf_b], sD + pf_b * kStoreBufBytes, col, m_blk2 * tile_rows, 0);
       }
       if (++pf_j == spt) { pf_j = 0; pf_w += gridDim.x; }
-      if (++pf_b == NB) pf_b = 0;
+      if (++pf_b == NBT) pf_b = 0;
     };
-    if (aux_tma && gtid == 0 && spt > 0) {
-      const int la = NB > 1 ? NB - 1 : 1;
-      for (int i = 0; i < la; ++i) request_aux();
+    if (aux_tma && leader) {
+      for (int i = 0; i < NBT - 1; ++i) request_aux();
     }
     constexpr int kStatBarThreads = V::kStatsWarps ? 384 : 256;
     uint32_t sd_phase = 0;     // VAR_STATS_BF16: bit b = parity of the stats-done barrier of staging slice b
@@ -428,179 +426,171 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int split = t / num_m;
       const int m0 = m_blk * tile_rows, n0 = n_blk * BN;
       const long long row = m0 + row_in_tile;
-      if (c_begin >= c_end) continue;   // half 1 of a 64-wide tile: no columns
-      float acc[2][32];
+      float acc[BN / 2];
       {
         const int kb0 = split * p.kb_per_split;
         const int kb1 = min(phases > 1 ? p.ph_taps[ph] * p.g.cchunks : p.num_kb, kb0 + p.kb_per_split);
-        const uint32_t b_off = half * 8192u;   // column 64 of a B stage (K-major: row 64; MN-major: second chunk)
-        if (a_mn) gemm_mainloop<BN, 1, 1>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, b_off, lane);
-        else if (b_mn) gemm_mainloop<BN, 0, 1>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, b_off, lane);
-        else gemm_mainloop<BN, 0, 0>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, b_off, lane);
+        const uint32_t a_off = half * 8192u;   // row 64 of an A stage (K-major: row 64; MN-major: second chunk)
+        if (a_mn) gemm_mainloop<BN, 1, 1>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, a_off, lane);
+        else if (b_mn) gemm_mainloop<BN, 0, 1>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, a_off, lane);
+        else gemm_mainloop<BN, 0, 0>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, a_off, lane);
       }
 #pragma unroll
-      for (int ci = 0; ci < 2; ++ci) {
-        const int c = c_begin + ci;
+      for (int c = 0; c < NCH; ++c) {
         const int col0 = n0 + c * 32;
-        const int part = out_f32 ? 0 : ((c - c_begin) & 1);   // bf16: which 32-column half of the 64-column slice
+        const int tcol = col0 + hh * 16;                      // first of this thread's 16 columns
+        const int part = out_f32 ? 0 : (c & 1);               // bf16: which 32-column half of the 64-column slice
         const bool s_begin = out_f32 || part == 0;
         const bool s_end = out_f32 || part == 1;
-        uint8_t* const sbuf = sbase + bufi * kStoreBufBytes;
+        uint8_t* const sbuf = sD + bufi * kStoreBufBytes;
         uint8_t* const buf = sbuf + row_in_tile * 128;
+        const int u0 = out_f32 ? hh * 4 : part * 4 + hh * 2;  // first 16-byte unit of this thread's columns in the slice row
         // operands of the epilogue are requested before the accumulator transpose so their latency overlaps it
         float bv = 0.f;
         if ((flags & EPI_BIAS) && col0 + lane < p.N) bv = __ldg(p.bias + col0 + lane);
-        float4 rf[8];
-        uint4 rb[4];
+        float4 rf[4];
+        uint4 rb[2];
         const bool has_rf = (flags & EPI_RESID) && row < p.M;
         const bool has_rb = (flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU)) && row < p.M;
         float rscale = 1.f;
         if ((flags & EPI_ROW_SCALE) && row < p.M) rscale = __ldg(p.row_scale + row / p.rows_per_scale);
-        uint32_t mbits = 0u;   // the mask word of this thread's row and 32 columns
-        if ((flags & EPI_MASK_BITS) && row < p.M && col0 < p.N) mbits = __ldg(p.mask_bits + row * (p.N >> 5) + (col0 >> 5));
+        uint32_t mbits = 0u;   // this thread's 16 bits of the mask word of its row and the chunk's 32 columns
+        if ((flags & EPI_MASK_BITS) && row < p.M && col0 < p.N)
+          mbits = __ldg(p.mask_bits + row * (p.N >> 5) + (col0 >> 5)) >> (hh * 16);
         if (!aux_tma) {
           if (has_rf) {
-            const float4* rp = reinterpret_cast<const float4*>(p.resid + row * p.ldd + col0);
+            const float4* rp = reinterpret_cast<const float4*>(p.resid + row * p.ldd + tcol);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) rf[j] = (col0 + 4 * j < p.N) ? __ldg(rp + j) : make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int j = 0; j < 4; ++j) rf[j] = (tcol + 4 * j < p.N) ? __ldg(rp + j) : make_float4(0.f, 0.f, 0.f, 0.f);
           }
           if (has_rb) {
             const uint4* rp = reinterpret_cast<const uint4*>(
-                reinterpret_cast<const __nv_bfloat16*>(p.resid_bf16) + row * p.ldd + col0);
+                reinterpret_cast<const __nv_bfloat16*>(p.resid_bf16) + row * p.ldd + tcol);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) rb[j] = (col0 + 8 * j < p.N) ? __ldg(rp + j) : make_uint4(0, 0, 0, 0);
+            for (int j = 0; j < 2; ++j) rb[j] = (tcol + 8 * j < p.N) ? __ldg(rp + j) : make_uint4(0, 0, 0, 0);
           }
         }
-        // columns c*32 .. +31 of the warp's 32 rows: fragment layout -> lane = row (see ptx.cuh, wgmma)
-        __syncwarp();
+        // columns c*32 .. +31 of the warp's 16 rows: fragment layout -> lane = (row, 16-column half) (see ptx.cuh, wgmma).
+        // Consecutive chunks alternate between the warp's two buffers, so one barrier per chunk orders writes and reads.
+        float* const xc = xp + (c & 1) * 16 * kXposeStride;
 #pragma unroll
-        for (int blk = 0; blk < 2; ++blk) {
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = ci * 4 + jj;
-            float* const dst = xp + (blk * 16 + (lane >> 2)) * kXposeStride + jj * 8 + 2 * (lane & 3);
-            dst[0] = acc[blk][4 * j];
-            dst[1] = acc[blk][4 * j + 1];
-            dst[8 * kXposeStride] = acc[blk][4 * j + 2];
-            dst[8 * kXposeStride + 1] = acc[blk][4 * j + 3];
-          }
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = c * 4 + jj;
+          float* const dst = xc + (lane >> 2) * kXposeStride + jj * 8 + 2 * (lane & 3);
+          dst[0] = acc[4 * j];
+          dst[1] = acc[4 * j + 1];
+          dst[8 * kXposeStride] = acc[4 * j + 2];
+          dst[8 * kXposeStride + 1] = acc[4 * j + 3];
         }
         __syncwarp();
-        float f[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] = xp[lane * kXposeStride + j];
-        if (aux_tma) {
-          // the aux slice was TMA-loaded into this staging slice; each thread reads its own (swizzled) row
-          if (s_begin) mbar_wait(&abar[bufi], (aux_phase >> bufi) & 1u);
-          if (out_f32) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) rf[j] = *reinterpret_cast<const float4*>(buf + ((j ^ rsw) << 4));
-          } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) rb[j] = *reinterpret_cast<const uint4*>(buf + (((part * 4 + j) ^ rsw) << 4));
-          }
-        }
-        if (flags & EPI_BIAS) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] += __shfl_sync(0xffffffffu, bv, j);
-        }
-        if (flags & EPI_GELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = gelu_erf(f[j]);
-        }
-        if (flags & EPI_RELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
-        }
-        if (flags & EPI_ROW_SCALE) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] *= rscale;
-        }
-        if (flags & EPI_RESID) {
-          if (aux_tma || has_rf) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              f[4 * j] += rf[j].x; f[4 * j + 1] += rf[j].y; f[4 * j + 2] += rf[j].z; f[4 * j + 3] += rf[j].w;
+        if (aux_tma && s_begin) mbar_wait(&aux_bar[bufi], (aux_phase >> bufi) & 1u);   // the aux slice has landed in this staging slice
+        if (!direct && s_begin && !aux_tma) {
+          // the store that last read this staging slice (2*NB slices ago) must have drained it (and the stats warps too)
+          if (leader) {
+            tma_store_wait_read_n(NBT - 1);
+            if (V::kStatsWarps && do_stats) {
+              mbar_wait(&sdone_bar[bufi], ((sd_phase >> bufi) & 1u) ^ 1u);
+              sd_phase ^= (1u << bufi);
             }
           }
+          named_bar_sync(bar_id, 256);
         }
-        if (flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU)) {
-          if (aux_tma || has_rb) {
+        // the thread's 16 columns in two runs of 8 (one 16-byte unit of bf16 output): fewer values live at a time
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint32_t wv[4] = {rb[j].x, rb[j].y, rb[j].z, rb[j].w};
+        for (int g = 0; g < 2; ++g) {
+          float f[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) f[j] = xc[(lane & 15) * kXposeStride + hh * 16 + g * 8 + j];
+          if (aux_tma) {
+            // each thread reads its own piece of its (swizzled) row of the aux slice
+            if (out_f32) {
+#pragma unroll
+              for (int j = 0; j < 2; ++j) rf[2 * g + j] = *reinterpret_cast<const float4*>(buf + (((u0 + 2 * g + j) ^ rsw) << 4));
+            } else {
+              rb[g] = *reinterpret_cast<const uint4*>(buf + (((u0 + g) ^ rsw) << 4));
+            }
+          }
+          if (flags & EPI_BIAS) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[j] += __shfl_sync(0xffffffffu, bv, hh * 16 + g * 8 + j);
+          }
+          if (flags & EPI_GELU) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[j] = gelu_erf(f[j]);
+          }
+          if (flags & EPI_RELU) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[j] = fmaxf(f[j], 0.f);
+          }
+          if (flags & EPI_ROW_SCALE) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[j] *= rscale;
+          }
+          if (flags & EPI_RESID) {
+            if (aux_tma || has_rf) {
+#pragma unroll
+              for (int j = 0; j < 2; ++j) {
+                const float4 r4 = rf[2 * g + j];
+                f[4 * j] += r4.x; f[4 * j + 1] += r4.y; f[4 * j + 2] += r4.z; f[4 * j + 3] += r4.w;
+              }
+            }
+          }
+          if (flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU)) {
+            if (aux_tma || has_rb) {
+              const uint32_t wv[4] = {rb[g].x, rb[g].y, rb[g].z, rb[g].w};
 #pragma unroll
               for (int u = 0; u < 4; ++u) {
                 const float2 ab = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wv[u]));
                 if (flags & EPI_MUL_DGELU) {
-                  f[8 * j + 2 * u] *= gelu_erf_grad(ab.x);
-                  f[8 * j + 2 * u + 1] *= gelu_erf_grad(ab.y);
+                  f[2 * u] *= gelu_erf_grad(ab.x);
+                  f[2 * u + 1] *= gelu_erf_grad(ab.y);
                 } else if (flags & EPI_MUL_DRELU) {   // resid_bf16 = ReLU output: pass the gradient where it is > 0
-                  f[8 * j + 2 * u] = ab.x > 0.f ? f[8 * j + 2 * u] : 0.f;
-                  f[8 * j + 2 * u + 1] = ab.y > 0.f ? f[8 * j + 2 * u + 1] : 0.f;
+                  f[2 * u] = ab.x > 0.f ? f[2 * u] : 0.f;
+                  f[2 * u + 1] = ab.y > 0.f ? f[2 * u + 1] : 0.f;
                 } else {
-                  f[8 * j + 2 * u] += ab.x;
-                  f[8 * j + 2 * u + 1] += ab.y;
+                  f[2 * u] += ab.x;
+                  f[2 * u + 1] += ab.y;
                 }
               }
             }
           }
-        }
-        if (flags & EPI_MASK_BITS) {
-          // a multiply by 0 / 1, not a select: the zeros keep the sign a later (bf16(D) * relu'(out)) would give them
+          if (flags & EPI_MASK_BITS) {
+            // a multiply by 0 / 1, not a select: the zeros keep the sign a later (bf16(D) * relu'(out)) would give them
 #pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] *= ((mbits >> j) & 1u) ? 1.f : 0.f;
-        }
-        if (direct) {
-          if (row < p.M) {
-            if (out_f32) {
-              float* o = reinterpret_cast<float*>(p.out) + split * p.split_stride + row * p.ldd + col0;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                if (col0 + j < p.N)
-                  *reinterpret_cast<float4*>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-            } else {
-              __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + split * p.split_stride +
-                                 row * p.ldd + col0;
-#pragma unroll
-              for (int j = 0; j < 32; j += 8)
-                if (col0 + j < p.N)
-                  *reinterpret_cast<uint4*>(o + j) =
-                      make_uint4(pack_bf16x2(f[j], f[j + 1]), pack_bf16x2(f[j + 2], f[j + 3]),
-                                 pack_bf16x2(f[j + 4], f[j + 5]), pack_bf16x2(f[j + 6], f[j + 7]));
-            }
+            for (int j = 0; j < 8; ++j) f[j] *= ((mbits >> (g * 8 + j)) & 1u) ? 1.f : 0.f;
           }
-        } else {
-          if (s_begin && !aux_tma) {
-            // the store that last read this staging slice (NB slices ago) must have drained it (and the stats warps too)
-            if (gtid == 0) {
-              tma_store_wait_read_n(NB - 1);
-              if (V::kStatsWarps && do_stats) {
-                mbar_wait(&sdone_bar[half * kMaxStoreBufs + bufi], ((sd_phase >> bufi) & 1u) ^ 1u);
-                sd_phase ^= (1u << bufi);
+          if (direct) {
+            if (row < p.M && tcol + g * 8 < p.N) {
+              if (out_f32) {
+                float* o = reinterpret_cast<float*>(p.out) + split * p.split_stride + row * p.ldd + tcol + g * 8;
+                *reinterpret_cast<float4*>(o) = make_float4(f[0], f[1], f[2], f[3]);
+                if (tcol + g * 8 + 4 < p.N) *reinterpret_cast<float4*>(o + 4) = make_float4(f[4], f[5], f[6], f[7]);
+              } else {
+                __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + split * p.split_stride +
+                                   row * p.ldd + tcol + g * 8;
+                *reinterpret_cast<uint4*>(o) = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]),
+                                                          pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
               }
             }
-            named_bar_sync(bar_id, 128);
-          }
-          if (out_f32) {
+          } else if (out_f32) {
             // one 128 B (32 x fp32) slice per TMA store
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-              *reinterpret_cast<float4*>(buf + ((j ^ rsw) << 4)) =
+            for (int j = 0; j < 2; ++j)
+              *reinterpret_cast<float4*>(buf + (((u0 + 2 * g + j) ^ rsw) << 4)) =
                   make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
           } else {
             // bf16: two 32-column chunks make one 128 B (64 x bf16) slice
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<uint4*>(buf + (((part * 4 + j) ^ rsw) << 4)) =
-                  make_uint4(pack_bf16x2(f[8 * j], f[8 * j + 1]), pack_bf16x2(f[8 * j + 2], f[8 * j + 3]),
-                             pack_bf16x2(f[8 * j + 4], f[8 * j + 5]), pack_bf16x2(f[8 * j + 6], f[8 * j + 7]));
+            *reinterpret_cast<uint4*>(buf + (((u0 + g) ^ rsw) << 4)) =
+                make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]),
+                           pack_bf16x2(f[6], f[7]));
           }
+        }
+        if (!direct) {
           if (s_end) {
             fence_proxy_async_smem();
-            named_bar_sync(bar_id, 128);
+            named_bar_sync(bar_id, 256);
             const int scol = out_f32 ? col0 : col0 - 32;
-            if (gtid == 0) {
+            if (leader) {
               if (scol < p.N && phases > 1) {
                 const int ab = p.ph_out[ph];
                 asm volatile(
@@ -618,22 +608,23 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               tma_store_commit();
               if (aux_tma) {
                 // the slice that store s-1 read becomes the landing buffer of aux slice s + LA
-                tma_store_wait_read_n(NB > 1 ? 1 : 0);
+                tma_store_wait_read_n(1);
                 request_aux();
               }
             }
             if (V::kStatsWarps && do_stats) {
-              if (gtid == 0) mbar_arrive(&staged_bar[half * kMaxStoreBufs + bufi]);   // hand the slice to the stats warps
-            } else if (do_stats) {
+              if (leader) mbar_arrive(&staged_bar[bufi]);   // hand the slice to the stats warps
+            } else if (do_stats && half == (bufi & 1)) {   // 2*NB slices in rotation: the slice count's parity
               // BatchNorm statistics of the slice just staged (the bf16 values as stored), read back
               // from the swizzled buffer (conflict free: a warp reads the 128 contiguous bytes of one
               // row) concurrently with the TMA store of the same buffer.  Rows >= M / cols >= N are zero.
-              // Fixed summation order (bit-reproducible, no atomics): warp wq of the half owns columns
-              // wq*16..+15 of the slice for all 128 rows.  Lane l reads 8 bytes (4 columns) of row
+              // Fixed summation order (bit-reproducible, no atomics): the warpgroups take alternate slices;
+              // warp wq of the one whose turn it is owns columns wq*16..+15 of the slice for all 128 rows.
+              // Lane l reads 8 bytes (4 columns) of row
               // i*8 + l/4: the 8 rows of one load hit 8 distinct swizzled 16-byte chunks, so the
               // 256-byte request is conflict free.  The 8 row-lanes are then folded by shuffles and
               // lanes 0..3 add to the accumulators they alone own.
-              const int wq = gtid >> 5;
+              const int wq = q;
               const int piece = lane & 3;
               const int chunk = wq * 2 + (piece >> 1);
               const int r0 = lane >> 2;        // row of load i is i*8 + r0: its swizzle phase (row & 7) is r0 for every i
@@ -667,12 +658,12 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               }
             }
             aux_phase ^= (1u << bufi);
-            if (++bufi == NB) bufi = 0;
+            if (++bufi == NBT) bufi = 0;
           }
         }
       }
     }
-    if (gtid == 0) tma_store_wait<0>();
+    if (leader) tma_store_wait<0>();
     if (do_stats) {
       named_bar_sync(3, kStatBarThreads);
       float* dst = p.stats_partial + (long long)blockIdx.x * 2 * p.N;
@@ -680,7 +671,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   } else if (V::kStatsWarps && warp >= 12) {
     // ================================================================ statistics warps (VAR_STATS_BF16)
-    // Warp wq owns columns wq*16 .. +15 of every staged 64-column slice of BOTH epilogue halves for all 128 rows (fixed
+    // Warp wq owns columns wq*16 .. +15 of every staged 64-column slice for all 128 rows (fixed
     // ownership and summation order: bit-reproducible, no atomics).  Lane l reads 8 bytes (4 columns) of row i*8 + l/4;
     // the 8 row-lanes are folded by shuffles and lanes 0..3 add to the shared-memory accumulators they alone own.
     if (do_stats) {
@@ -689,55 +680,48 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int chunk = wq * 2 + (piece >> 1);
       const int r0 = lane >> 2;
       const int soff = r0 * 128 + ((chunk ^ r0) << 4) + (piece & 1) * 8;
-      constexpr int NCH = BN / 32;
-      constexpr int split_at = 2 * ((BN / 64 + 1) / 2);
-      constexpr int spt_h[2] = {split_at / 2, (NCH - split_at) / 2};
-      int sb[2] = {0, 0};
-      uint32_t st_phase[2] = {0u, 0u};
+      const int NBT = 2 * NB;
+      int b = 0;                         // staging slice of the next output slice (the epilogue's rotation)
+      uint32_t st_phase = 0u;
       named_bar_sync(3, 384);            // accumulators zeroed by the epilogue warps
       for (int w = blockIdx.x; w < total; w += gridDim.x) {
         const int n0 = (w % num_n) * BN;
 #pragma unroll 1
-        for (int j = 0; j < spt_h[0]; ++j) {
-#pragma unroll 1
-          for (int h = 0; h < 2; ++h) {
-            if (j >= spt_h[h]) continue;
-            const int b = sb[h];
-            mbar_wait(&staged_bar[h * kMaxStoreBufs + b], (st_phase[h] >> b) & 1u);
-            const uint8_t* const sp = sD + (h * NB + b) * kStoreBufBytes + soff;
-            float sx[4] = {0.f, 0.f, 0.f, 0.f}, sq[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int j = 0; j < BN / 64; ++j) {
+          mbar_wait(&staged_bar[b], (st_phase >> b) & 1u);
+          const uint8_t* const sp = sD + b * kStoreBufBytes + soff;
+          float sx[4] = {0.f, 0.f, 0.f, 0.f}, sq[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const uint2 w2 = *reinterpret_cast<const uint2*>(sp + i * 1024);
-              const float a0 = __uint_as_float(w2.x << 16), a1 = __uint_as_float(w2.x & 0xffff0000u);
-              const float b0 = __uint_as_float(w2.y << 16), b1 = __uint_as_float(w2.y & 0xffff0000u);
-              sx[0] += a0; sq[0] = fmaf(a0, a0, sq[0]);
-              sx[1] += a1; sq[1] = fmaf(a1, a1, sq[1]);
-              sx[2] += b0; sq[2] = fmaf(b0, b0, sq[2]);
-              sx[3] += b1; sq[3] = fmaf(b1, b1, sq[3]);
-            }
-            // the slice is read: the epilogue may reuse it (after its TMA store has drained it too)
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sdone_bar[h * kMaxStoreBufs + b]);
-#pragma unroll
-            for (int o = 4; o < 32; o <<= 1) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                sx[k] += __shfl_xor_sync(0xffffffffu, sx[k], o);
-                sq[k] += __shfl_xor_sync(0xffffffffu, sq[k], o);
-              }
-            }
-            const int gcol = n0 + ((h ? split_at : 0) / 2 + j) * 64 + wq * 16 + piece * 4;
-            if (lane < 4 && gcol < p.N) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                sStat[gcol + k] += sx[k];
-                sStat[p.N + gcol + k] += sq[k];
-              }
-            }
-            st_phase[h] ^= (1u << b);
-            sb[h] = (b + 1 == NB) ? 0 : b + 1;
+          for (int i = 0; i < 16; ++i) {
+            const uint2 w2 = *reinterpret_cast<const uint2*>(sp + i * 1024);
+            const float a0 = __uint_as_float(w2.x << 16), a1 = __uint_as_float(w2.x & 0xffff0000u);
+            const float b0 = __uint_as_float(w2.y << 16), b1 = __uint_as_float(w2.y & 0xffff0000u);
+            sx[0] += a0; sq[0] = fmaf(a0, a0, sq[0]);
+            sx[1] += a1; sq[1] = fmaf(a1, a1, sq[1]);
+            sx[2] += b0; sq[2] = fmaf(b0, b0, sq[2]);
+            sx[3] += b1; sq[3] = fmaf(b1, b1, sq[3]);
           }
+          // the slice is read: the epilogue may reuse it (after its TMA store has drained it too)
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&sdone_bar[b]);
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              sx[k] += __shfl_xor_sync(0xffffffffu, sx[k], o);
+              sq[k] += __shfl_xor_sync(0xffffffffu, sq[k], o);
+            }
+          }
+          const int gcol = n0 + j * 64 + wq * 16 + piece * 4;
+          if (lane < 4 && gcol < p.N) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              sStat[gcol + k] += sx[k];
+              sStat[p.N + gcol + k] += sq[k];
+            }
+          }
+          st_phase ^= (1u << b);
+          b = (b + 1 == NBT) ? 0 : b + 1;
         }
       }
       named_bar_sync(3, 384);            // all slices accumulated: the epilogue warps write the partial row
