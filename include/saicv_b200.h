@@ -59,6 +59,14 @@ int saicv_wgrad_splits(int out_rows, int out_cols, long long reduce_len);
 /* 1 when the weight gradient dW [out_rows, out_cols] is computed as dW^T (fewer padded 128-row tiles: few filters).
  * saicv_conv_wgrad then writes dw_partial [splits][r*s*c][k]; linear_wgrad callers swap dy and x themselves. */
 int saicv_wgrad_transposed(int out_rows, int out_cols);
+/* One product of a quintic Newton-Schulz iteration (the Muon optimizer) over `batch` bf16 matrices stored back to back,
+ * one launch; fp32 accumulation, one rounding to bf16:
+ *   mode 0  out[b][m][m] = x x^T                      (x [b][m][n])
+ *   mode 1  out[b][m][m] = alpha x x + beta x          (x [b][m][m]; the product is x x, not x x^T)
+ *   mode 2  out[b][m][n] = alpha x y + beta y          (x [b][m][m], y [b][m][n])
+ * m, n multiples of 8 (zero padding is exact under the iteration); out aliases neither x nor y. */
+int saicv_ns_gemm(int mode, const void* x, const void* y, void* out, int batch, int m, int n, float alpha, float beta,
+                  void* stream);
 
 /* ---- convolutions: nn.Conv2d inside ConvBnActBlock (resnet.py:33-39, darknet.py:49-56) ---- */
 typedef struct {
@@ -438,6 +446,31 @@ int saicv_multi_tensor_adamw(const void* tensors, const int* chunk_tensor, const
 /* partial: fp32 [n_chunks] workspace; clip = {min(1, max_norm / (norm + 1e-6)), norm}; fixed summation order. */
 int saicv_multi_tensor_clip_coef(const void* tensors, const int* chunk_tensor, const int* chunk_index, int n_chunks,
                                  float max_norm, float* partial, float* clip, void* stream);
+/* Muon (the reference's tools/muon_optimizer.py): one saicv_muon_tensor per saicv_opt_tensor row.  Muon rows (slot >= 0):
+ * s1 = momentum buffer; AdamW rows (slot < 0): s1 / s2 = moment1 / moment2, step_idx = their per-parameter step count.
+ * hyper rows {lr, weight_decay, momentum, nesterov, beta1, beta2, eps, 0}.
+ *   saicv_muon_prep   buf = momentum buf + g; u = nesterov ? g + momentum buf : buf; writes bf16(u / (||u||_F + 1e-7))
+ *                     into the tensor's slot of `ns` ([min(r,c)][ld], transposed when r > c; r x c = shape[0] x rest);
+ *                     partial: fp32 [n_chunks] workspace (per-chunk sums, folded in a fixed order)
+ *   saicv_muon_apply  Muon rows p = p (1 - lr wd) - lr adj U (U read back from the slot); AdamW rows moments by lerp,
+ *                     p = p (1 - lr wd) - lr sqrt(1 - beta2^t) / (1 - beta1^t) m / (eps + sqrt(v)) with
+ *                     t = adam_steps[step_idx] + 1; then advances adam_steps of the table's AdamW rows and *step.
+ * Both refresh the bf16 operand copies like the SGD / AdamW steps. */
+typedef struct {
+  long long slot;      /* element offset of the tensor's slot in the Newton-Schulz buffer; -1: AdamW row */
+  int rows, cols;      /* 2-D view [shape[0], numel / shape[0]] */
+  int ld;              /* columns of the slot */
+  int transposed;      /* the slot holds the transpose (rows > cols) */
+  int chunk0, nchunks; /* the tensor's chunks in launch order */
+  int step_idx;        /* AdamW rows: index into adam_steps */
+  float adj;           /* 0.2 * sqrt(max(shape[0], shape[1])) */
+} saicv_muon_tensor;
+int saicv_muon_prep(const void* tensors, const void* muon, const int* chunk_tensor, const int* chunk_index, int n_chunks,
+                    const float* hyper, int n_groups, const int* step, const float* clip, float* partial, void* ns,
+                    void* stream);
+int saicv_muon_apply(const void* tensors, const void* muon, const int* chunk_tensor, const int* chunk_index, int n_chunks,
+                     int n_tensors, const float* hyper, int n_groups, int* step, const float* clip, const void* ns,
+                     int* adam_steps, void* stream);
 
 /* ---- input-pipeline edge (SURVEY.md 8 f3; csrc/capi_input.cu) ---------------------------------------------------------
  * out fp32 [n][3][h][w] = (float(in uint8 [n][h][w][3]) / 255 - mean[c]) / std[c]: ToTensor + Normalize of

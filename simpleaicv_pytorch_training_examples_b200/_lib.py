@@ -51,6 +51,7 @@ SIGNATURES = {
     'saicv_linear_wgrad': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_wgrad_splits': [c_int, c_int, c_ll],
     'saicv_wgrad_transposed': [c_int, c_int],
+    'saicv_ns_gemm': [c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_void_p],
     'saicv_conv_fprop': [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_int, c_void_p],
     'saicv_conv_dgrad': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_void_p],
     'saicv_conv_wgrad': [c_void_p, c_void_p, c_void_p, ctypes.POINTER(ConvShape), c_int, c_void_p],
@@ -109,6 +110,8 @@ SIGNATURES = {
     'saicv_multi_tensor_sgd': [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p],
     'saicv_multi_tensor_adamw': [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p],
     'saicv_multi_tensor_clip_coef': [c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p],
+    'saicv_muon_prep': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    'saicv_muon_apply': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     'saicv_postln_fwd': [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_void_p],
     'saicv_postln_bwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
     'saicv_add_pos_cast': [c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_void_p],

@@ -190,7 +190,7 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, con
     attr_set = true;
   }
   const int num_m = (p.M + p.tile_rows - 1) / p.tile_rows, num_n = (p.N + BN - 1) / BN;
-  const long long total = (long long)num_m * num_n * p.splits * p.phases;
+  const long long total = (long long)num_m * num_n * p.splits * p.phases * (GemmVariant<VAR>::kBatch ? p.batch : 1);
   const int grid = (int)(total < g_sm_count ? total : g_sm_count);
   const int stat_bytes = (p.epi_flags & EPI_STATS) ? ((8 * p.N + 15) & ~15) : 0;
   int stages = 0, nb = 1;
@@ -305,6 +305,24 @@ int conv_dgrad_phases(const void* dy, const void* w, const void* add, const uint
         p.ph_tab[i][t++] = (taps1[a][dr] * 3 + taps1[b][ds]) | (dr << 8) | (ds << 9);
   }
   return dispatch(pick_bn(cs->c), ta, tb, td, p, st);
+}
+
+// 3-D map over `batch` row-major [rows][cols] bf16 matrices stored back to back, 128B swizzle.
+bool encode_batched(CUtensorMap* m, const void* ptr, uint64_t cols, uint64_t rows, uint64_t batch, uint32_t box_cols,
+                    uint32_t box_rows) {
+  cuuint64_t dims[3] = {cols, rows, batch};
+  cuuint64_t strides[2] = {cols * 2, rows * cols * 2};
+  cuuint32_t box[3] = {box_cols, box_rows, 1u};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled(batched) failed: %d (cols=%llu rows=%llu batch=%llu box=%u,%u ptr=%p)", (int)r,
+              (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)batch, box_cols, box_rows, ptr);
+    return false;
+  }
+  return true;
 }
 
 }  // namespace
@@ -508,6 +526,46 @@ int saicv_conv_wgrad(const void* dy, const void* x, float* dw_partial, const sai
   p.g.R = cs->r; p.g.S = cs->s; p.g.cchunks = cs->c / 64; p.g.n_img = cs->n;
   p.epi_flags = 0; p.out_f32 = 1; p.out = dw_partial; p.ldd = p.N; p.split_stride = (long long)cs->k * Ncols;
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream);
+}
+
+// One product of a quintic Newton-Schulz iteration over `batch` matrices stacked in one buffer, one launch:
+//   mode 0  out[m][m] = x x^T                        x [m][n]   (both operands K-major from x)
+//   mode 1  out[m][m] = alpha x x + beta x            x [m][m]   (second operand MN-major: x x^T would be wrong, the
+//                                                                 computed x is not bitwise symmetric)
+//   mode 2  out[m][n] = alpha x y + beta y            x [m][m], y [m][n]
+// m and n are multiples of 8 (pad with zeros: zero rows / columns stay zero).  out must not alias x or y.
+int saicv_ns_gemm(int mode, const void* x, const void* y, void* out, int batch, int m, int n, float alpha, float beta,
+                  void* stream) {
+  if (!ensure_init()) return 1;
+  if (mode < 0 || mode > 2 || batch <= 0 || m <= 0 || n <= 0 || (m % 8) || (n % 8) || !aligned16(x) || !aligned16(out) ||
+      (mode == 2 && (!y || !aligned16(y))))
+    return set_error("saicv_ns_gemm: bad arguments (mode=%d batch=%d m=%d n=%d; m, n must be multiples of 8, pointers "
+                     "16-byte aligned)", mode, batch, m, n);
+  const int out_cols = mode == 2 ? n : m;
+  const int red = mode == 0 ? n : m;
+  const int bn = pick_bn(out_cols);
+  CUtensorMap ta, tb, td, tr;
+  if (!encode_batched(&ta, x, red, m, batch, 64, 128)) return 2;
+  if (mode == 0) {
+    if (!encode_batched(&tb, x, n, m, batch, 64, bn)) return 2;
+  } else if (!encode_batched(&tb, mode == 1 ? x : y, out_cols, m, batch, 64, 64)) {
+    return 2;
+  }
+  if (!encode_out(&td, out, false, out_cols, m, out_cols, batch, (uint64_t)m * out_cols)) return 2;
+  tr = td;
+  GemmParams p{};
+  p.M = m; p.N = out_cols; p.num_kb = (red + BK - 1) / BK; p.kb_per_split = p.num_kb; p.splits = 1;
+  p.a_mode = A_K2D; p.b_mode = mode == 0 ? B_K2D : B_MN2D;
+  p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
+  p.out_f32 = 0; p.out = out; p.ldd = out_cols; p.tile_rows = BM; p.phases = 1;
+  p.batch = batch; p.alpha = alpha; p.beta = beta;
+  if (mode != 0) {
+    const void* aux = mode == 1 ? x : y;
+    if (!encode_out(&tr, aux, false, out_cols, m, out_cols, batch, (uint64_t)m * out_cols)) return 2;
+    p.epi_flags = EPI_AXPBY; p.aux_tma = 1;
+  }
+  const cudaStream_t st = (cudaStream_t)stream;
+  return bn == 64 ? launch<64, VAR_NS>(ta, tb, td, tr, p, st) : launch<128, VAR_NS>(ta, tb, td, tr, p, st);
 }
 
 }  // extern "C"

@@ -201,6 +201,146 @@ clip_coef_kernel(const float* __restrict__ partial, int n, float max_norm, float
 
 __global__ void opt_advance_kernel(int* step) { *step += 1; }
 
+// ---- Muon (tools/muon_optimizer.py of the reference; optim.FusedMuon).  A row of saicv_muon_tensor goes with each
+// OptTensor row: s1 is the momentum buffer (Muon rows) or moment1 (AdamW rows), s2 moment2.  Muon rows own a bf16 slot
+// [min(r, c)][ld] of the Newton-Schulz buffer holding X (transposed when r > c, as the reference does).
+struct MuonTensor {
+  long long slot;   // element offset of the slot; < 0: AdamW row
+  int rows, cols;   // 2-D view of the parameter: [shape[0], numel / shape[0]]
+  int ld;           // columns of the slot
+  int transposed;   // slot = X^T (rows > cols)
+  int chunk0, nchunks;   // chunks of this tensor in launch order (norm partials)
+  int step_idx;     // AdamW rows: per-parameter step counter
+  float adj;        // 0.2 * sqrt(max(shape[0], shape[1]))
+};
+static_assert(sizeof(MuonTensor) == sizeof(saicv_muon_tensor) && sizeof(MuonTensor) == 40, "saicv_muon_tensor layout");
+
+__device__ __forceinline__ long long muon_slot_index(const MuonTensor& m, long long i) {
+  const long long r = i / m.cols, c = i - r * m.cols;
+  return m.slot + (m.transposed ? c * m.ld + r : r * m.ld + c);
+}
+
+__device__ __forceinline__ float block_sum(float s, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  float tot = 0.f;
+  for (int i = 0; i < kOptThreads / 32; ++i) tot += red[i];
+  return tot;
+}
+
+// hyper[group] = {lr, weight_decay, momentum, nesterov, beta1, beta2, eps, -}
+// buf = momentum * buf + g; u = nesterov ? g + momentum * buf : buf; partial[chunk] = sum of bf16(u)^2 over the chunk.
+__global__ void __launch_bounds__(kOptThreads)
+muon_momentum_kernel(const OptTensor* __restrict__ tensors, const MuonTensor* __restrict__ muon,
+                     const int* __restrict__ chunk_tensor, const int* __restrict__ chunk_index, const float* __restrict__ hyper,
+                     int n_groups, const int* __restrict__ step, const float* __restrict__ clip, float* __restrict__ partial) {
+  const int ti = chunk_tensor[blockIdx.x];
+  if (muon[ti].slot < 0) return;
+  const OptTensor t = tensors[ti];
+  const long long base = (long long)chunk_index[blockIdx.x] * kChunk;
+  const int n = (int)min((long long)kChunk, t.numel - base);
+  const float* h = hyper + ((long long)(*step % SAICV_OPT_RING) * n_groups + t.group) * 8;
+  const float mom = h[2];
+  const bool nesterov = h[3] != 0.f;
+  const float gs = clip ? clip[0] : 1.f;
+  float s = 0.f;
+  for (int i = threadIdx.x; i < n; i += kOptThreads) {
+    const float g = t.g[base + i] * gs;
+    const float b = mom * t.s1[base + i] + g;
+    t.s1[base + i] = b;
+    const float u = __bfloat162float(__float2bfloat16_rn(nesterov ? g + mom * b : b));
+    s = fmaf(u, u, s);
+  }
+  __shared__ float red[kOptThreads / 32];
+  const float tot = block_sum(s, red);
+  if (threadIdx.x == 0) partial[blockIdx.x] = tot;
+}
+
+// X = bf16(u / (||bf16(u)||_F + 1e-7)) into the slot; the norm folds the tensor's chunk partials in a fixed order, so every
+// block of a tensor computes the same value.
+__global__ void __launch_bounds__(kOptThreads)
+muon_cast_kernel(const OptTensor* __restrict__ tensors, const MuonTensor* __restrict__ muon,
+                 const int* __restrict__ chunk_tensor, const int* __restrict__ chunk_index, const float* __restrict__ hyper,
+                 int n_groups, const int* __restrict__ step, const float* __restrict__ clip, const float* __restrict__ partial,
+                 __nv_bfloat16* __restrict__ ns) {
+  const int ti = chunk_tensor[blockIdx.x];
+  const MuonTensor m = muon[ti];
+  if (m.slot < 0) return;
+  const OptTensor t = tensors[ti];
+  __shared__ double dred[kOptThreads];
+  double ds = 0.0;
+  for (int i = threadIdx.x; i < m.nchunks; i += kOptThreads) ds += (double)partial[m.chunk0 + i];
+  dred[threadIdx.x] = ds;
+  __syncthreads();
+  for (int o = kOptThreads / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) dred[threadIdx.x] += dred[threadIdx.x + o];
+    __syncthreads();
+  }
+  const float inv = 1.f / ((float)sqrt(dred[0]) + 1e-7f);
+  const long long base = (long long)chunk_index[blockIdx.x] * kChunk;
+  const int n = (int)min((long long)kChunk, t.numel - base);
+  const float* h = hyper + ((long long)(*step % SAICV_OPT_RING) * n_groups + t.group) * 8;
+  const float mom = h[2];
+  const bool nesterov = h[3] != 0.f;
+  const float gs = clip ? clip[0] : 1.f;
+  for (int i = threadIdx.x; i < n; i += kOptThreads) {
+    const float b = t.s1[base + i];
+    const float u = __bfloat162float(__float2bfloat16_rn(nesterov ? t.g[base + i] * gs + mom * b : b));
+    ns[muon_slot_index(m, base + i)] = __float2bfloat16_rn(u * inv);
+  }
+}
+
+// Muon rows: p = p (1 - lr wd) - lr adj U.  AdamW rows (the reference's formula, not torch's AdamW): moments by lerp,
+// p = p (1 - lr wd) - (lr sqrt(bc2) / bc1) m / (eps + sqrt(v)) with the parameter's own step count t = steps[idx] + 1.
+__global__ void __launch_bounds__(kOptThreads)
+muon_apply_kernel(const OptTensor* __restrict__ tensors, const MuonTensor* __restrict__ muon,
+                  const int* __restrict__ chunk_tensor, const int* __restrict__ chunk_index, const float* __restrict__ hyper,
+                  int n_groups, const int* __restrict__ step, const float* __restrict__ clip,
+                  const __nv_bfloat16* __restrict__ ns, const int* __restrict__ adam_steps) {
+  const int ti = chunk_tensor[blockIdx.x];
+  const OptTensor t = tensors[ti];
+  const MuonTensor m = muon[ti];
+  const long long base = (long long)chunk_index[blockIdx.x] * kChunk;
+  const int n = (int)min((long long)kChunk, t.numel - base);
+  const float* h = hyper + ((long long)(*step % SAICV_OPT_RING) * n_groups + t.group) * 8;
+  const float lr = h[0], wd = h[1], b1 = h[4], b2 = h[5], eps = h[6];
+  const float decay = 1.f - lr * wd;
+  if (m.slot >= 0) {
+    const float a = lr * m.adj;
+    for (int i = threadIdx.x; i < n; i += kOptThreads) {
+      const float p = t.p[base + i] * decay - a * __bfloat162float(ns[muon_slot_index(m, base + i)]);
+      t.p[base + i] = p;
+      if (t.shadow) write_shadow(t, base + i, p);
+    }
+    return;
+  }
+  const int st = adam_steps[m.step_idx] + 1;
+  const double bc1 = 1.0 - pow((double)b1, st), bc2 = 1.0 - pow((double)b2, st);
+  const float a = (float)((double)lr * sqrt(bc2) / bc1);
+  const float gs = clip ? clip[0] : 1.f;
+  for (int i = threadIdx.x; i < n; i += kOptThreads) {
+    const float g = t.g[base + i] * gs;
+    float mv = t.s1[base + i], vv = t.s2[base + i];
+    mv = mv + (g - mv) * (1.f - b1);
+    vv = vv + (g * g - vv) * (1.f - b2);
+    const float p = t.p[base + i] * decay - a * (mv / (eps + sqrtf(vv)));
+    t.p[base + i] = p;
+    t.s1[base + i] = mv;
+    t.s2[base + i] = vv;
+    if (t.shadow) write_shadow(t, base + i, p);
+  }
+}
+
+// Advances the step count of every AdamW row of the table (parameters with a gradient) and the ring step.
+__global__ void muon_advance_kernel(const MuonTensor* __restrict__ muon, int n_tensors, int* __restrict__ adam_steps,
+                                    int* __restrict__ step) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_tensors && muon[i].slot < 0) adam_steps[muon[i].step_idx] += 1;
+  if (i == 0) *step += 1;
+}
+
 }  // namespace
 }  // namespace saicv
 
@@ -238,6 +378,32 @@ int saicv_multi_tensor_clip_coef(const void* tensors, const int* chunk_tensor, c
   if (check_launch("multi_sqnorm_kernel")) return 1;
   clip_coef_kernel<<<1, kOptThreads, 0, ST>>>(partial, n_chunks, max_norm, clip);
   return check_launch("clip_coef_kernel");
+}
+
+int saicv_muon_prep(const void* tensors, const void* muon, const int* chunk_tensor, const int* chunk_index, int n_chunks,
+                    const float* hyper, int n_groups, const int* step, const float* clip, float* partial, void* ns,
+                    void* stream) {
+  if (n_chunks <= 0) return 0;
+  const OptTensor* t = reinterpret_cast<const OptTensor*>(tensors);
+  const MuonTensor* m = reinterpret_cast<const MuonTensor*>(muon);
+  muon_momentum_kernel<<<n_chunks, kOptThreads, 0, ST>>>(t, m, chunk_tensor, chunk_index, hyper, n_groups, step, clip, partial);
+  if (check_launch("muon_momentum_kernel")) return 1;
+  muon_cast_kernel<<<n_chunks, kOptThreads, 0, ST>>>(t, m, chunk_tensor, chunk_index, hyper, n_groups, step, clip, partial,
+                                                     reinterpret_cast<__nv_bfloat16*>(ns));
+  return check_launch("muon_cast_kernel");
+}
+
+int saicv_muon_apply(const void* tensors, const void* muon, const int* chunk_tensor, const int* chunk_index, int n_chunks,
+                     int n_tensors, const float* hyper, int n_groups, int* step, const float* clip, const void* ns,
+                     int* adam_steps, void* stream) {
+  if (n_chunks <= 0) return 0;
+  const MuonTensor* m = reinterpret_cast<const MuonTensor*>(muon);
+  muon_apply_kernel<<<n_chunks, kOptThreads, 0, ST>>>(reinterpret_cast<const OptTensor*>(tensors), m, chunk_tensor, chunk_index,
+                                                      hyper, n_groups, step, clip,
+                                                      reinterpret_cast<const __nv_bfloat16*>(ns), adam_steps);
+  if (check_launch("muon_apply_kernel")) return 1;
+  muon_advance_kernel<<<(n_tensors + 255) / 256, 256, 0, ST>>>(m, n_tensors, adam_steps, step);
+  return check_launch("muon_advance_kernel");
 }
 
 }  // extern "C"

@@ -29,7 +29,8 @@ namespace saicv {
 enum : int { A_K2D = 0, A_IM2COL = 1, A_MN2D = 2, A_IM2COL_MN = 3 };
 enum : int { B_K2D = 0, B_MN2D = 2, B_IM2COL = 3 };
 enum : int { EPI_BIAS = 1, EPI_RELU = 2, EPI_GELU = 4, EPI_DIRECT = 8, EPI_RESID = 16, EPI_RESID_BF16 = 32,
-              EPI_MUL_DGELU = 64, EPI_ROW_SCALE = 128, EPI_STATS = 256, EPI_MUL_DRELU = 512, EPI_MASK_BITS = 1024 };
+              EPI_MUL_DGELU = 64, EPI_ROW_SCALE = 128, EPI_STATS = 256, EPI_MUL_DRELU = 512, EPI_MASK_BITS = 1024,
+              EPI_AXPBY = 2048 };
 
 constexpr int BM = 128;
 constexpr int BK = 64;
@@ -101,6 +102,10 @@ struct GemmParams {
   int ph_out[4];       // (a << 1) | b of each phase, in work order
   int ph_taps[4];      // taps of each phase
   int ph_tab[4][4];    // per tap, in reduction order: weight tap (r*S + s) | dy row offset << 8 | dy column offset << 9
+  // VAR_NS: `batch` same-shape matrices stacked in one buffer; the matrix is the outermost work index and the third
+  // coordinate of the 3-D operand, aux and output maps.  EPI_AXPBY: D = alpha * acc + beta * aux.
+  int batch;
+  float alpha, beta;
 };
 
 // Kernel variants: the epilogue's feature set is a compile-time mask, so that the common launches run a compact
@@ -118,19 +123,23 @@ struct GemmParams {
 //                   warps are already draining the next chunk (handshake: staged / stats-done mbarriers per slice).
 //   VAR_PHASE_BF16  bf16 output, no epilogue operation: the stride-2 data gradient by output phase (GemmParams::phases), a
 //                   variant of its own so that the other launches do not carry its work decomposition
-enum : int { VAR_FULL = 0, VAR_PLAIN_BF16 = 1, VAR_PLAIN_F32 = 2, VAR_AUX = 3, VAR_STATS_BF16 = 4, VAR_PHASE_BF16 = 5 };
+//   VAR_NS          bf16 output over a batch of matrices (GemmParams::batch), optional D = alpha * acc + beta * aux with a
+//                   bf16 aux operand by TMA: the Newton-Schulz products of the Muon optimizer (capi_gemm.cu: saicv_ns_gemm)
+enum : int { VAR_FULL = 0, VAR_PLAIN_BF16 = 1, VAR_PLAIN_F32 = 2, VAR_AUX = 3, VAR_STATS_BF16 = 4, VAR_PHASE_BF16 = 5, VAR_NS = 6 };
 template <int VAR>
 struct GemmVariant {
   static constexpr int kMask = VAR == VAR_FULL ? (0x7fffffff & ~EPI_MASK_BITS)
                                : (VAR == VAR_PLAIN_BF16 || VAR == VAR_STATS_BF16) ? (EPI_BIAS | EPI_RELU | EPI_STATS)
                                : VAR == VAR_PLAIN_F32 ? EPI_BIAS
                                : VAR == VAR_PHASE_BF16 ? 0
+                               : VAR == VAR_NS ? EPI_AXPBY
                                : (EPI_BIAS | EPI_ROW_SCALE | EPI_RESID | EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU |
                                   EPI_MASK_BITS);
-  static constexpr int kOut = (VAR == VAR_PLAIN_BF16 || VAR == VAR_STATS_BF16 || VAR == VAR_PHASE_BF16) ? 1 : VAR == VAR_PLAIN_F32 ? 2 : 0;   // 0: run time, 1: bf16, 2: fp32
-  static constexpr int kAux = VAR == VAR_FULL ? 0 : VAR == VAR_AUX ? 2 : 1;                // 0: run time, 1: never, 2: always by TMA
+  static constexpr int kOut = (VAR == VAR_PLAIN_BF16 || VAR == VAR_STATS_BF16 || VAR == VAR_PHASE_BF16 || VAR == VAR_NS) ? 1 : VAR == VAR_PLAIN_F32 ? 2 : 0;   // 0: run time, 1: bf16, 2: fp32
+  static constexpr int kAux = (VAR == VAR_FULL || VAR == VAR_NS) ? 0 : VAR == VAR_AUX ? 2 : 1;   // 0: run time, 1: never, 2: always by TMA
   static constexpr bool kStatsWarps = VAR == VAR_STATS_BF16;                               // statistics by warps 12..15
   static constexpr bool kPhases = VAR == VAR_PHASE_BF16;                                   // GemmParams::phases / tile_rows honoured
+  static constexpr bool kBatch = VAR == VAR_NS;                                            // GemmParams::batch honoured
   static constexpr int kThreads = kStatsWarps ? kGemmThreads + 128 : kGemmThreads;
 };
 
@@ -263,7 +272,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int num_m = (p.M + tile_rows - 1) / tile_rows;
   const int num_n = (p.N + BN - 1) / BN;
   const int per_phase = num_m * num_n * p.splits;
-  const int total = per_phase * phases;
+  const int total = per_phase * phases * (V::kBatch ? p.batch : 1);
 
   if (warp == 0) {
     // ================================================================ TMA producer
@@ -272,7 +281,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       uint32_t phase = 0;
       const int PQ = p.g.P * p.g.Q;
       for (int w = blockIdx.x; w < total; w += gridDim.x) {
-        const int ph = V::kPhases ? w / per_phase : 0;
+        const int ph = (V::kPhases || V::kBatch) ? w / per_phase : 0;   // output phase, or matrix of the batch
         const int wp = w - ph * per_phase;
         const int n_blk = wp % num_n;
         const int t = wp / num_n;
@@ -310,6 +319,17 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               s = tap - r * p.g.S;
               tapb = p.flip_taps ? (p.g.R * p.g.S - 1 - tap) : tap;
             }
+          }
+          if constexpr (V::kBatch) {   // A K-major; B K-major or MN-major; coordinate 2 = matrix
+            tma_load_3d(&tmA, bar, a_dst, kb * BK, m0, ph);
+            if (p.b_mode == B_K2D) {
+              tma_load_3d(&tmB, bar, b_dst, kb * BK, n0, ph);
+            } else {
+#pragma unroll
+              for (int j = 0; j < BN / 64; ++j) tma_load_3d(&tmB, bar, b_dst + j * 8192, n0 + j * 64, kb * BK, ph);
+            }
+            if (++stage == nstages) { stage = 0; phase ^= 1; }
+            continue;
           }
           // ---- A
           if (p.a_mode == A_K2D) {
@@ -403,7 +423,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const int m_blk2 = (int)((pf_w / num_n) % num_m);
         const int col = n_blk2 * BN + pf_j * (out_f32 ? 32 : 64);
         mbar_expect_tx(&aux_bar[pf_b], kStoreBufBytes);   // rows / columns past the matrix are zero-filled and counted
-        tma_load_3d(&tmR, &aux_bar[pf_b], sD + pf_b * kStoreBufBytes, col, m_blk2 * tile_rows, 0);
+        tma_load_3d(&tmR, &aux_bar[pf_b], sD + pf_b * kStoreBufBytes, col, m_blk2 * tile_rows,
+                    V::kBatch ? (int)(pf_w / per_phase) : 0);
       }
       if (++pf_j == spt) { pf_j = 0; pf_w += gridDim.x; }
       if (++pf_b == NBT) pf_b = 0;
@@ -418,7 +439,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       named_bar_sync(3, kStatBarThreads);
     }
     for (int w = blockIdx.x; w < total; w += gridDim.x) {
-      const int ph = V::kPhases ? w / per_phase : 0;
+      const int ph = (V::kPhases || V::kBatch) ? w / per_phase : 0;
       const int wp = w - ph * per_phase;
       const int n_blk = wp % num_n;
       const int t = wp / num_n;
@@ -554,6 +575,15 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               }
             }
           }
+          if (flags & EPI_AXPBY) {
+            const uint32_t wv[4] = {rb[g].x, rb[g].y, rb[g].z, rb[g].w};
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+              const float2 ab = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wv[u]));
+              f[2 * u] = fmaf(p.beta, ab.x, p.alpha * f[2 * u]);
+              f[2 * u + 1] = fmaf(p.beta, ab.y, p.alpha * f[2 * u + 1]);
+            }
+          }
           if (flags & EPI_MASK_BITS) {
             // a multiply by 0 / 1, not a select: the zeros keep the sign a later (bf16(D) * relu'(out)) would give them
 #pragma unroll
@@ -602,7 +632,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 asm volatile(
                     "cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
                         reinterpret_cast<uint64_t>(&tmD)),
-                    "r"(smem_u32(sbuf)), "r"(scol), "r"(m0), "r"(split)
+                    "r"(smem_u32(sbuf)), "r"(scol), "r"(m0), "r"(V::kBatch ? ph : split)
                     : "memory");
               }
               tma_store_commit();

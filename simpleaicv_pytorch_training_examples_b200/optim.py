@@ -204,8 +204,7 @@ class _FusedBase(torch.optim.Optimizer):
         capturing = torch.cuda.is_current_stream_capturing()
         slot = self._publish()
         self._hyper_dev.copy_(self._hyper_host, non_blocking=True)
-        _lib.call(self._entry, _p(tab['tensors']), _p(tab['ct']), _p(tab['ci']), tab['n'], _p(self._hyper_dev),
-                  len(self.param_groups), _p(self._step_dev), _p(self._clip) if self._use_clip else None, _stream())
+        self._launch(tab, _p(self._clip) if self._use_clip else None)
         self._use_clip = False
         if capturing:
             self._t -= 1          # recorded, not executed: the first replay publishes this step's table again
@@ -217,6 +216,10 @@ class _FusedBase(torch.optim.Optimizer):
             if id(p) not in self._shadows:
                 torch.autograd.graph.increment_version(p)
         return loss
+
+    def _launch(self, tab, clip):
+        _lib.call(self._entry, _p(tab['tensors']), _p(tab['ct']), _p(tab['ci']), tab['n'], _p(self._hyper_dev),
+                  len(self.param_groups), _p(self._step_dev), clip, _stream())
 
 
 class FusedSGD(_FusedBase):
@@ -270,3 +273,165 @@ class FusedAdamW(_FusedBase):
         self._key = None
         if self._hyper_host is not None:
             self._step_dev.fill_(self._t)
+
+
+_MUON_DTYPE = np.dtype([('slot', '<i8'), ('rows', '<i4'), ('cols', '<i4'), ('ld', '<i4'), ('transposed', '<i4'),
+                        ('chunk0', '<i4'), ('nchunks', '<i4'), ('step_idx', '<i4'), ('adj', '<f4')])
+assert _MUON_DTYPE.itemsize == 40   # saicv_muon_tensor (include/saicv_b200.h)
+
+NS_COEFFS = (3.4445, -4.7750, 2.0315)   # quintic Newton-Schulz coefficients of the reference
+
+
+def _round8(n):
+    return (n + 7) // 8 * 8
+
+
+def newton_schulz(x, steps, t0, t1, a, b):
+    """`steps` quintic Newton-Schulz iterations, in place, on x: bf16 [batch, m, n], m <= n, both multiples of 8, already
+    scaled to Frobenius norm <= 1.  Each iteration is three batched GEMM launches (csrc/capi_gemm.cu saicv_ns_gemm):
+    A = X X^T, B = b A + c A A, X' = a X + B X.  t0 / t1 (as large as x) and a / b ([batch, m, m]) are workspaces; the
+    intermediate iterates alternate between t0 and t1 so that no product writes an operand it reads."""
+    batch, m, n = x.shape
+    ca, cb, cc = NS_COEFFS
+    st = _stream()
+    for s in range(steps):
+        src = x if s == 0 else (t0, t1)[(s - 1) % 2]
+        dst = x if s == steps - 1 and steps > 1 else (t0, t1)[s % 2]
+        _lib.call('saicv_ns_gemm', 0, _p(src), None, _p(a), batch, m, n, ctypes.c_float(1.), ctypes.c_float(0.), st)
+        _lib.call('saicv_ns_gemm', 1, _p(a), None, _p(b), batch, m, m, ctypes.c_float(cc), ctypes.c_float(cb), st)
+        _lib.call('saicv_ns_gemm', 2, _p(b), _p(src), _p(dst), batch, m, n, ctypes.c_float(1.), ctypes.c_float(ca), st)
+    if steps == 1:
+        x.copy_(t0)
+    return x
+
+
+class FusedMuon(_FusedBase):
+    """The reference's Muon (tools/muon_optimizer.py): SGD-momentum (Nesterov by default) whose update of every >= 2-D
+    weight is orthogonalised by quintic Newton-Schulz iterations in bf16, and an AdamW backup for the other parameters.
+
+    One step is: a multi-tensor prep (momentum, Nesterov, bf16 cast into each matrix's slot of its shape class, transposed
+    when rows > cols, Frobenius normalisation), per shape class the Newton-Schulz iterations as batched GEMMs over all of
+    its matrices, and one multi-tensor apply (Muon and AdamW rows, bf16 operand copies refreshed).  The Newton-Schulz
+    buffers are allocated at the first step; after it nothing is allocated and nothing waits for the device, so the step
+    can be captured in a CUDA graph.  State keys and shapes are the reference's (``use_muon``; ``momentum_buffer`` 2-D;
+    ``step`` int, ``moment1``, ``moment2``), so checkpoints interchange.  One parameter group (tools.utils.Scheduler
+    rewrites its ``lr``)."""
+
+    def __init__(self, lr=1e-3, wd=0.1, muon_params=None, momentum=0.95, nesterov=True, ns_steps=5, adamw_params=None,
+                 adamw_betas=(0.9, 0.999), adamw_eps=1e-8):
+        muon_params = list(muon_params) if muon_params is not None else []
+        adamw_params = list(adamw_params) if adamw_params is not None else []
+        for p in muon_params + adamw_params:
+            if not p.is_cuda:
+                raise RuntimeError('FusedMuon runs on the GPU only: move the model to CUDA before building the optimizer '
+                                   '(there is no CPU implementation)')
+        super().__init__(muon_params + adamw_params, dict(lr=lr, wd=wd, momentum=momentum, nesterov=nesterov,
+                                                          ns_steps=ns_steps, adamw_betas=adamw_betas, adamw_eps=adamw_eps))
+        for p in muon_params:
+            assert p.ndim >= 2, f'Muon requires parameters with ndim >= 2, got {p.ndim}'
+            self.state[p]['use_muon'] = True
+        for p in adamw_params:
+            self.state[p]['use_muon'] = False
+        self._adam_index = {id(p): i for i, p in enumerate(adamw_params)}
+        self._adam_steps = None     # device int32 [len(adamw_params)]: per-parameter AdamW step counts
+        # Newton-Schulz slots: shape class (m, n) -> its matrices; every Muon parameter owns one slot whether or not it
+        # has a gradient in a given step, so the layout never changes
+        self._slots, self._classes = {}, []
+        off = 0
+        classes = collections.OrderedDict()
+        for p in muon_params:
+            r, c = p.shape[0], p.numel() // p.shape[0]
+            classes.setdefault((min(r, c), max(r, c)), []).append(p)
+        for (m, n), ps in classes.items():
+            mp, np_ = _round8(m), _round8(n)
+            self._classes.append((off, len(ps), mp, np_))
+            for j, p in enumerate(ps):
+                self._slots[id(p)] = (off + j * mp * np_, np_)
+            off += len(ps) * mp * np_
+        self._ns_elems = off
+        self._ns = None
+
+    def _state_tensors(self, p):
+        st = self.state[p]
+        if st['use_muon']:
+            if 'momentum_buffer' not in st:
+                st['momentum_buffer'] = torch.zeros(p.shape[0], p.numel() // p.shape[0], device=p.device)
+            return (st['momentum_buffer'],)
+        if 'moment1' not in st:
+            st['step'] = 0
+            st['moment1'] = torch.zeros_like(p)
+            st['moment2'] = torch.zeros_like(p)
+        return st['moment1'], st['moment2']
+
+    def _hyper_row(self, g, t):
+        b1, b2 = g['adamw_betas']
+        return (g['lr'], g['wd'], g['momentum'], 1. if g['nesterov'] else 0., b1, b2, g['adamw_eps'])
+
+    def _build(self, plist):
+        tab = super()._build(plist)
+        dev = tab['dev']
+        chunk = _lib.load().saicv_opt_chunk()
+        rows = np.zeros(len(plist), dtype=_MUON_DTYPE)
+        c0 = 0
+        for i, (_, p) in enumerate(plist):
+            r = rows[i]
+            r['rows'], r['cols'] = p.shape[0], p.numel() // p.shape[0]
+            r['chunk0'], r['nchunks'] = c0, (p.numel() + chunk - 1) // chunk
+            c0 += int(r['nchunks'])
+            if self.state[p]['use_muon']:
+                r['slot'], r['ld'] = self._slots[id(p)]
+                r['transposed'] = int(r['rows'] > r['cols'])
+                r['adj'] = 0.2 * math.sqrt(max(p.shape[0], p.shape[1]))
+            else:
+                r['slot'], r['step_idx'] = -1, self._adam_index[id(p)]
+        tab['muon'] = torch.from_numpy(rows.view(np.uint8).copy()).to(dev)
+        tab['n_tensors'] = len(plist)
+        if self._ns is None:
+            big_x = max((b * mp * np_ for _, b, mp, np_ in self._classes), default=0)
+            big_a = max((b * mp * mp for _, b, mp, _ in self._classes), default=0)
+            self._ns = torch.zeros(max(self._ns_elems, 8), dtype=torch.bfloat16, device=dev)
+            self._ns_work = [torch.empty(max(k, 8), dtype=torch.bfloat16, device=dev) for k in (big_x, big_x, big_a, big_a)]
+        if self._adam_steps is None:
+            self._adam_steps = torch.zeros(max(len(self._adam_index), 1), dtype=torch.int32, device=dev)
+            self._load_adam_steps()
+        return tab
+
+    def _launch(self, tab, clip):
+        common = (_p(tab['tensors']), _p(tab['muon']), _p(tab['ct']), _p(tab['ci']), tab['n'])
+        hyper = (_p(self._hyper_dev), len(self.param_groups), _p(self._step_dev), clip)
+        _lib.call('saicv_muon_prep', *common, *hyper, _p(tab['partial']), _p(self._ns), _stream())
+        steps = int(self.param_groups[0]['ns_steps'])
+        t0, t1, a, b = self._ns_work
+        for off, batch, mp, np_ in self._classes:
+            x = self._ns[off:off + batch * mp * np_].view(batch, mp, np_)
+            newton_schulz(x, steps, t0[:x.numel()].view_as(x), t1[:x.numel()].view_as(x),
+                          a[:batch * mp * mp].view(batch, mp, mp), b[:batch * mp * mp].view(batch, mp, mp))
+        _lib.call('saicv_muon_apply', *common, tab['n_tensors'], *hyper, _p(self._ns), _p(self._adam_steps), _stream())
+
+    def _load_adam_steps(self):
+        if self._adam_steps is None:
+            return
+        host = torch.zeros(self._adam_steps.numel(), dtype=torch.int32)
+        for g in self.param_groups:
+            for p in g['params']:
+                i = self._adam_index.get(id(p))
+                if i is not None and 'step' in self.state[p]:
+                    host[i] = int(self.state[p]['step'])
+        self._adam_steps.copy_(host)
+
+    def state_dict(self):
+        if self._adam_steps is not None:
+            host = self._adam_steps.cpu()
+            for g in self.param_groups:
+                for p in g['params']:
+                    i = self._adam_index.get(id(p))
+                    if i is not None and 'step' in self.state[p]:
+                        self.state[p]['step'] = int(host[i])
+        return super().state_dict()
+
+    def load_state_dict(self, state_dict):
+        super().load_state_dict(state_dict)
+        for st in self.state.values():
+            if 'momentum_buffer' in st:
+                st['momentum_buffer'] = st['momentum_buffer'].contiguous()
+        self._load_adam_steps()

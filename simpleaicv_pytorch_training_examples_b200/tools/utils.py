@@ -2,7 +2,7 @@
 
   get_logger            tools/utils.py:66-92   (rank-0 file + stderr logging)
   set_seed              tools/utils.py:95-107
-  build_optimizer       tools/utils.py:292-600 (param groups by weight decay / lr / layer decay)
+  build_optimizer       tools/utils.py:292-680 (param groups by weight decay / lr / layer decay; Muon split)
   Scheduler             tools/utils.py:205-289 (per-iteration MultiStep / Cosine / Poly LR, warm-up)
   build_training_mode   tools/utils.py:175-202 (DDP wrap -> distributed.B200DataParallel)
   EmaModel              tools/utils.py:145-172
@@ -97,10 +97,45 @@ def param_group_table(config, model):
     return rows
 
 
+MUON_EXCLUDE = ('position_encoding', 'cls_token', 'patch_embedding')
+
+
+def muon_split(opt, model):
+    """(muon [(name, param)], adamw [(name, param)], description list) of the trainable parameters for the optimizer
+    config `opt`: Muon takes the >= 2-D ones whose name contains none of MUON_EXCLUDE + exclude_muon_layer_name_list
+    (the reference's rule, tools/utils.py:609-655)."""
+    extra = opt['exclude_muon_layer_name_list'] if isinstance(opt.get('exclude_muon_layer_name_list'), list) else []
+    names = list(MUON_EXCLUDE) + extra
+    muon, adamw = [], []
+    for name, p in model.named_parameters():
+        if not p.requires_grad:
+            continue
+        (muon if p.ndim >= 2 and not any(e in name for e in names) else adamw).append((name, p))
+    info = [{'name': [n for n, _ in ps], 'optimizer': kind, 'lr': opt['lr'], 'weight_decay': opt['weight_decay']}
+            for kind, ps in (('Muon', muon), ('AdamW', adamw)) if ps]
+    return muon, adamw, info
+
+
+def _build_muon(opt, model):
+    """The reference's Muon branch: one lr / weight decay for every parameter (per-layer lr / wd, layer decay and
+    no-weight-decay lists are ignored, as there)."""
+    muon, adamw, info = muon_split(opt, model)
+    lr, wd = opt['lr'], opt['weight_decay']
+    from ..optim import FusedMuon   # raises a RuntimeError on CPU parameters: there is no CPU implementation
+    optimizer = FusedMuon(lr=lr, wd=wd, muon_params=[p for _, p in muon], adamw_params=[p for _, p in adamw],
+                          momentum=opt.get('momentum', 0.95), nesterov=opt.get('nesterov', True),
+                          ns_steps=opt.get('ns_steps', 5),
+                          adamw_betas=(opt.get('adamw_beta1', 0.9), opt.get('adamw_beta2', 0.999)),
+                          adamw_eps=opt.get('adamw_eps', 1e-8)).attach(model)
+    return optimizer, info
+
+
 def build_optimizer(config, model):
     """Returns (optimizer, group description list) like the reference."""
     name, opt = config.optimizer
-    assert name in ('SGD', 'AdamW'), 'Unsupported optimizer!'
+    assert name in ('SGD', 'AdamW', 'Muon'), 'Unsupported optimizer!'
+    if name == 'Muon':
+        return _build_muon(opt, model)
     rows = param_group_table(config, model)
     groups, descr = {}, {}
     for r in rows:
