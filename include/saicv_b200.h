@@ -410,6 +410,25 @@ int saicv_sam_loss_sums(const void* logits, int logits_bf16, const float* target
 int saicv_sam_loss_bwd(const void* logits, int logits_bf16, const float* targets, const float* coef, void* dlogits,
                        int dl_bf16, int b, int m, long long n, float alpha, float gamma, void* stream);
 
+/* ---- SemanticSoftmaxLoss / SemanticSoftmaxMeter of ImageNet-21K semantic-tree training (classification/losses.py:94-140,
+ * common.py:712-757; csrc/capi_loss.cu) -------------------------------------------------------------------------------
+ * logits: fp32 or bf16 [b][n]; labels: int64 [b][levels] semantic labels (position within the level, or -1);
+ * level_cols: int32, the ascending columns of level 0, then level 1, ...; level_off: int32 [levels + 1] offsets into it;
+ * col_level: int32 [n], the level of each column or -1; factors: fp32 [levels]; 1 <= levels <= 16.
+ * fwd: lse fp32 [b][levels] = log-sum-exp over each level's columns (kept for bwd); terms fp32 [b][levels] workspace;
+ * loss fp32 [1] = sum_l factors[l] * mean_b(v * sum_c -((1-s) [c == y] + s/n_l) log_softmax(x)_c), folded in a fixed
+ * order.  bwd: dlogits fp32 [b][n] = grad[0] * factors[l] / b * v * (exp(x - lse) - s/n_l - (1-s) [c == y]), exactly 0
+ * in columns of no level and in (row, level) pairs whose label is -1.  accuracy: counts int32 [levels][2] = {rows whose
+ * first argmax over the level's columns (NaN largest) equals the label, rows with a label >= 0}, cleared first. */
+int saicv_semantic_softmax_fwd(const void* logits, int logits_bf16, const long long* labels, const int* level_cols,
+                               const int* level_off, const float* factors, float* lse, float* terms, float* loss, int b, int n,
+                               int levels, float smoothing, void* stream);
+int saicv_semantic_softmax_bwd(const void* logits, int logits_bf16, const long long* labels, const int* col_level,
+                               const int* level_cols, const int* level_off, const float* factors, const float* lse,
+                               const float* grad, float* dlogits, int b, int n, int levels, float smoothing, void* stream);
+int saicv_semantic_accuracy(const void* logits, int logits_bf16, const long long* labels, const int* level_cols,
+                            const int* level_off, int* counts, int b, int n, int levels, void* stream);
+
 /* ---- multi-tensor optimizer step (SURVEY.md 8 f2; csrc/capi_optim.cu) --------------------------------------------------
  * Replaces torch.optim.SGD / torch.optim.AdamW as the reference builds them (tools/utils.py:292-600, stepped at
  * tools/scripts.py:209-248) with ONE launch over all parameters, the refresh of the bf16 GEMM-operand copies and the

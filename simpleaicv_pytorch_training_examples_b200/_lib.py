@@ -102,6 +102,9 @@ SIGNATURES = {
     'saicv_sam_loss_partial_floats': [c_int, c_int, c_ll],
     'saicv_sam_loss_sums': [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_ll, c_float, c_float, c_float, c_void_p],
     'saicv_sam_loss_bwd': [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_float, c_float, c_void_p],
+    'saicv_semantic_softmax_fwd': [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p],
+    'saicv_semantic_softmax_bwd': [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p],
+    'saicv_semantic_accuracy': [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     'saicv_u8_nhwc_to_nchw_norm': [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p],
     'saicv_token_gather_fwd': [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     'saicv_token_fill_slabs': [c_ll],

@@ -94,6 +94,44 @@ class AccMeter:
         self.acc5 = float(self.acc5_correct_num) / self.sample_num if self.sample_num != 0 else 0
 
 
+class SemanticSoftmaxMeter:
+    """common.py:712-757 of the reference: accuracy over the semantic tree's levels, counting every (row, level) pair that
+    has a label.  compute_per_batch runs one kernel (csrc/capi_loss.cu: first argmax per level, torch.argmax's NaN rule)
+    on the SemanticOutputs' full logits and returns (correct, valid) as int64 device scalars: the reference's
+    ``result = sum_l mean_valid(correct) * n_valid`` is that integer.  The counts stay on the device until compute()."""
+
+    def __init__(self):
+        self.reset()
+
+    def reset(self):
+        self.acc1 = 0
+        self.sum = 0
+        self.count = 0
+
+    def compute_per_batch(self, semantic_outputs, semantic_labels):
+        from .. import ops
+        from .semantic import SemanticOutputs
+        if not isinstance(semantic_outputs, SemanticOutputs):
+            raise TypeError('SemanticSoftmaxMeter takes the SemanticOutputs of SemanticTree.convert_outputs_to_semantic_outputs')
+        logits = semantic_outputs.logits
+        if not logits.is_cuda:
+            raise RuntimeError('SemanticSoftmaxMeter runs on H100 kernels only; move the logits to the GPU')
+        if logits.dtype not in (torch.float32, torch.bfloat16):
+            logits = logits.float()
+        t = semantic_outputs.tree.tables(logits.device)
+        counts = ops.semantic_accuracy(logits.contiguous(), semantic_labels.long().contiguous(), t.level_cols, t.level_off)
+        total = counts.sum(dim=0, dtype=torch.int64)
+        return total[0], total[1]
+
+    def update_per_batch(self, result, num_valids_total):
+        self.sum += result
+        self.count += num_valids_total
+
+    def compute(self):
+        count = int(self.count)
+        self.acc1 = float(self.sum) / count if count != 0 else 0
+
+
 def get_amp_type(model):
     """The autocast dtype the reference's loop would select for the device ``model`` lives on.
 

@@ -829,6 +829,41 @@ def sam_loss_bwd(logits, targets, coef, alpha, gamma):
     return dl
 
 
+# ----------------------------------------------------------------------------- SemanticSoftmaxLoss
+def semantic_softmax_fwd(logits, labels, level_cols, level_off, factors, smoothing):
+    """logits fp32 / bf16 [B, N], semantic labels int64 [B, L], level tables int32 (include/saicv_b200.h), factors fp32 [L]
+    -> (loss fp32 [], lse fp32 [B, L])."""
+    b, n = logits.shape
+    levels = labels.shape[1]
+    assert labels.dtype == torch.int64 and labels.shape[0] == b and factors.dtype == torch.float32 and factors.numel() >= levels
+    lse = torch.empty(b, levels, device=logits.device, dtype=torch.float32)
+    terms = torch.empty(b, levels, device=logits.device, dtype=torch.float32)
+    loss = torch.empty((), device=logits.device, dtype=torch.float32)
+    _lib.call('saicv_semantic_softmax_fwd', _p(logits), int(logits.dtype == torch.bfloat16), _p(labels), _p(level_cols), _p(level_off),
+              _p(factors), _p(lse), _p(terms), _p(loss), b, n, levels, float(smoothing), _stream())
+    return loss, lse
+
+
+def semantic_softmax_bwd(logits, labels, col_level, level_cols, level_off, factors, lse, grad, smoothing):
+    """Gradient fp32 [B, N] of grad (fp32 device scalar) * loss w.r.t. the logits."""
+    b, n = logits.shape
+    dl = torch.empty(b, n, device=logits.device, dtype=torch.float32)
+    _lib.call('saicv_semantic_softmax_bwd', _p(logits), int(logits.dtype == torch.bfloat16), _p(labels), _p(col_level), _p(level_cols),
+              _p(level_off), _p(factors), _p(lse), _p(grad), _p(dl), b, n, labels.shape[1], float(smoothing), _stream())
+    return dl
+
+
+def semantic_accuracy(logits, labels, level_cols, level_off):
+    """int32 [L, 2]: per level, rows whose first argmax over the level's columns equals the label, and rows with a label."""
+    b, n = logits.shape
+    levels = labels.shape[1]
+    assert labels.dtype == torch.int64 and labels.shape[0] == b
+    counts = torch.empty(levels, 2, device=logits.device, dtype=torch.int32)
+    _lib.call('saicv_semantic_accuracy', _p(logits), int(logits.dtype == torch.bfloat16), _p(labels), _p(level_cols), _p(level_off),
+              _p(counts), b, n, levels, _stream())
+    return counts
+
+
 # ----------------------------------------------------------------------------- DINOv3 kernels
 def rope_qk(qkv, sin, cos, b, l, heads, hd, backward=False):
     """In place on the q and k slices of packed qkv bf16 [b*l, 3*heads*hd]: the rotary embedding with the fp32 table

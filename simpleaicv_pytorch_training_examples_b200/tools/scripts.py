@@ -1,5 +1,6 @@
 """train / test loops of the classification task with the call signatures of the reference's
-tools/scripts.py:36-113 (test_classification), :116-275 (train_classification) and :1774-1934 (train_mae_self_supervised_learning).
+tools/scripts.py:36-113 (test_classification), :116-275 (train_classification) and :1774-1934 (train_mae_self_supervised_learning),
+and of tools/train_imagenet21k_classification_model.py:27-237 (ImageNet-21K semantic-softmax training).
 
 Arithmetic per step is the reference's: forward, criterion, backward (gradient average across
 ranks), optional clipping, optimizer step, per-iteration LR.  Control flow is tightened for the
@@ -9,7 +10,8 @@ small all-reduce and ONE device->host read per step; there is no per-step barrie
 import torch
 import torch.distributed as dist
 
-from ..classification.common import AccMeter, AverageMeter
+from ..classification.common import AccMeter, AverageMeter, SemanticSoftmaxMeter
+from ..classification.semantic import SemanticTree
 
 
 def _world():
@@ -101,6 +103,19 @@ def train_mae_self_supervised_learning(train_loader, model, criterion, optimizer
         outputs, masks = model(images)
         return criterion(outputs, labels, masks)
     return train_classification(train_loader, model, criterion, optimizer, scheduler, epoch, logger, config, compute_loss=mae_loss)
+
+
+def train_imagenet21k_classification(train_loader, model, criterion, optimizer, scheduler, epoch, logger, config):
+    """tools/train_imagenet21k_classification_model.py:94-237 of the reference: `criterion(semantic outputs, semantic labels)`
+    with the guards / accumulation / clipping / per-iteration LR of train_classification.  The tree of config.train_dataset
+    is built once; label conversion is a device gather, so the step keeps its one host sync."""
+    tree = SemanticTree.of(config.train_dataset)
+
+    def semantic_loss(model, criterion, images, labels):
+        outputs = model(images)
+        return criterion(tree.convert_outputs_to_semantic_outputs(outputs), tree.convert_single_labels_to_semantic_labels(labels))
+    return train_classification(train_loader, model, criterion, optimizer, scheduler, epoch, logger, config,
+                                compute_loss=semantic_loss)
 
 
 def train_epoch_with_loss_terms(train_loader, model, criterion, optimizer, scheduler, epoch, logger, config, compute,
@@ -235,3 +250,26 @@ def test_classification(test_loader, model, criterion, config):
         [meter.acc1_correct_num, meter.acc5_correct_num, meter.sample_num, loss_sum], dist.ReduceOp.SUM, group)
     meter.compute()
     return meter.acc1 * 100, meter.acc5 * 100, loss_sum / meter.sample_num
+
+
+@torch.no_grad()
+def test_imagenet21k_classification(test_loader, model, criterion, config):
+    """tools/train_imagenet21k_classification_model.py:27-91 of the reference: returns (acc1 %, mean loss) over the semantic
+    levels (SemanticSoftmaxMeter).  Loss and accuracy counts accumulate on the device and cross the host, and the ranks, in
+    one all-reduce at the end of the evaluation."""
+    model.eval()
+    tree = SemanticTree.of(config.test_dataset)
+    group = getattr(config, 'group', None)
+    accs = SemanticSoftmaxMeter()
+    loss_sum, samples = 0., 0
+    for data in test_loader:
+        images, labels = data['image'].cuda(non_blocking=True), data['label'].cuda(non_blocking=True)
+        outputs = tree.convert_outputs_to_semantic_outputs(model(images))
+        labels = tree.convert_single_labels_to_semantic_labels(labels)
+        loss_sum = loss_sum + criterion(outputs, labels).detach().double() * images.size(0)
+        accs.update_per_batch(*accs.compute_per_batch(outputs, labels))
+        samples += images.size(0)
+    accs.sum, accs.count, loss_sum, samples = all_reduce_operation_in_group_for_variables(
+        [accs.sum, accs.count, loss_sum, samples], dist.ReduceOp.SUM, group)
+    accs.compute()
+    return accs.acc1 * 100, (loss_sum / samples if samples else 0.)

@@ -4,7 +4,9 @@ Drop-in for the reference's tools/train_classification_model.py:33-283: reads ``
 ``<work-dir>/train_config.py`` (the same python-class config; only its ``backbones`` / ``losses``
 imports point at this package), builds loaders / optimizer / scheduler, wraps the model for data
 parallelism, resumes from ``checkpoints/latest.pth``, trains and evaluates every epoch and saves
-``latest.pth`` / ``best.pth`` with the reference's checkpoint keys.
+``latest.pth`` / ``best.pth`` with the reference's checkpoint keys.  ``main(train_fn, test_fn)`` is shared by the entry
+points whose epoch bodies differ (train_imagenet21k_classification_model); ``test_fn`` returns (acc1, acc5, loss) or
+(acc1, loss).
 """
 import argparse
 import os
@@ -26,7 +28,7 @@ def parse_args():
     return parser.parse_args()
 
 
-def main():
+def main(train_fn=train_classification, test_fn=test_classification):
     assert torch.cuda.is_available(), 'need at least one H100 to train'
     args = parse_args()
     sys.path.append(args.work_dir)
@@ -89,12 +91,14 @@ def main():
         t0 = time.time()
         if train_sampler is not None:
             train_sampler.set_epoch(epoch)
-        train_loss = train_classification(train_loader, model, train_criterion, optimizer, scheduler, epoch, logger, config)
+        train_loss = train_fn(train_loader, model, train_criterion, optimizer, scheduler, epoch, logger, config)
         eval_model = config.ema_model.ema_model if config.ema_model is not None else model
-        acc1, acc5, test_loss = test_classification(test_loader, eval_model, test_criterion, config)
+        result = test_fn(test_loader, eval_model, test_criterion, config)
+        acc1, test_loss = result[0], result[-1]
+        acc5 = f'acc5 {result[1]:.3f}%, ' if len(result) == 3 else ''
         train_time += (time.time() - t0) / 3600
         if master:
-            logger.info(f'epoch {epoch:0>3d}: train loss {train_loss:.4f}, acc1 {acc1:.3f}%, acc5 {acc5:.3f}%, '
+            logger.info(f'epoch {epoch:0>3d}: train loss {train_loss:.4f}, acc1 {acc1:.3f}%, {acc5}'
                         f'test loss {test_loss:.4f}, {(time.time() - t0) / 3600:.3f} h')
             if best_acc1 < acc1 <= 100:
                 best_acc1 = acc1
