@@ -498,6 +498,21 @@ int saicv_muon_apply(const void* tensors, const void* muon, const int* chunk_ten
 int saicv_u8_nhwc_to_nchw_norm(const void* in, float* out, int n, int h, int w, const float* mean3, const float* std3,
                                void* stream);
 
+/* The same edge for the recipes that end in RandomErasing(mode='pixel') and MixupCutmixClassificationCollater(mode='batch')
+ * (classification/common.py:597-642, mixupcutmixclassificationcollator.py:140-167,269-284), from the draws the host made:
+ *   v(s, c, y, x) = (y, x) in rect s ? noise[noise_off[s] + ((y - top_s) * w_s + (x - left_s)) * 3 + c] : the norm above
+ *   mode 0: out[b] = v(b);  mode 2 (cutmix): out[b] = (y, x) in box ? v(n-1-b) : v(b);
+ *   mode 1 (mixup): out[b] = fadd(fmul(v(b), (float)lam), fmul(v(n-1-b), (float)(1 - lam)))
+ *   soft fp32 [n][num_classes] = fadd(fmul(y1, (float)lam), fmul(y2, (float)(1 - lam))), y1 / y2 = on_value at
+ *   labels[b] / labels[n-1-b] (device int64 [n]), off_value elsewhere.
+ * rects: HOST int32 [n][4] (top, left, h, w; h == 0 or w == 0: not erased); noise_off: HOST int64 [n]; noise: device fp32
+ * [noise_len]; box4: HOST int32 {y0, y1, x0, x1} (mode 2).  n even, 2 <= n <= 1024.  Rectangles or a box outside the
+ * image, noise past noise_len and a non-finite lam are rejected before any launch. */
+int saicv_u8_mix_erase_norm(const void* in, float* out, int n, int h, int w, const float* mean3, const float* std3,
+                            const int* rects, const long long* noise_off, const float* noise, long long noise_len, int mode,
+                            const int* box4, double lam, const long long* labels, float* soft, int num_classes,
+                            float on_value, float off_value, void* stream);
+
 /* ---- token gather / scatter for masked-token models (SURVEY.md 8 f4; csrc/capi_tokens.cu) -----------------------------
  * out fp32 [b][r][c] = (idx[b][r] >= 0 ? src[b][idx[b][r]][:] : fill[:]) + (pos ? pos[pos_idx ? pos_idx[b][r] : r][:] : 0);
  * src fp32 [b][src_rows][c].  One call is the torch.gather + cat(cls / mask token) + position-encoding add of

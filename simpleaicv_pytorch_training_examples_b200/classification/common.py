@@ -1,7 +1,11 @@
 """Host-side helpers of the classification hot path with the reference's names
 (SimpleAICV/classification/common.py:668-685 AverageMeter, :688-709 AccMeter, :843-881 get_amp_type) and the
 input-pipeline edge of SURVEY.md 8 f3: ``Uint8ClassificationCollater`` + ``DeviceNormalize`` move the batch over PCIe as
-uint8 pixels and normalise on the device.  The per-sample transforms / datasets stay CPU data code (SURVEY.md section 2)."""
+uint8 pixels and normalise on the device; ``Uint8RandomErasing`` + ``Uint8MixupCutmixClassificationCollater`` do the same for
+the recipes that end in RandomErasing and Mixup / CutMix, with the random draws on the host and the pixel and label
+arithmetic on the device.  The per-sample transforms / datasets stay CPU data code (SURVEY.md section 2)."""
+import math
+
 import numpy as np
 import torch
 
@@ -38,6 +42,169 @@ class Uint8ClassificationCollater:
         if self.pin_memory and torch.cuda.is_available():
             images, labels = images.pin_memory(), labels.pin_memory()
         return {'image': images, 'label': labels}
+
+
+MIX_NONE, MIX_MIXUP, MIX_CUTMIX = 0, 1, 2
+
+
+class MixupEraseRecord:
+    """The host's draws for one batch of ``Uint8MixupCutmixClassificationCollater``; the device applies them
+    (ops.u8_mix_erase_normalize, csrc/capi_input.cu).
+
+    rects int32 [B, 4]: (top, left, h, w) of image b's erase rectangle, h = w = 0 when it was not erased;
+    offsets int64 [B]: where image b's fp32 [h, w, 3] noise starts in ``noise`` (fp32, the rectangles' noise concatenated);
+    mode: MIX_NONE / MIX_MIXUP / MIX_CUTMIX; box: the CutMix box (y0, y1, x0, x1); lam: the (corrected) float64 lambda;
+    on_value / off_value: the smoothed one-hot values, computed in float64 as the reference does."""
+
+    def __init__(self, rects, offsets, noise, mode, box, lam, num_classes, on_value, off_value):
+        self.rects, self.offsets, self.noise = rects, offsets, noise
+        self.mode, self.box, self.lam = mode, box, lam
+        self.num_classes, self.on_value, self.off_value = num_classes, on_value, off_value
+
+    def pin_memory(self):
+        """Called by DataLoader(pin_memory=True): only the noise is copied to the device, the rest is read on the host."""
+        self.noise = self.noise.pin_memory()
+        return self
+
+
+class Uint8RandomErasing:
+    """Takes the place of ``TorchMeanStdNormalize(mean, std), RandomErasing(...)`` at the end of a transform list
+    (SimpleAICV/classification/common.py:228-248,560-642) when the batch is collated by
+    ``Uint8MixupCutmixClassificationCollater``: the image stays uint8 [H, W, 3] and the erase rectangle and its noise go
+    into the sample ('erase_rect', 'erase_noise') instead of into the pixels.
+
+    The np.random calls are RandomErasing's, in its order: uniform(0, 1) against ``prob``; then up to 10 tries of
+    uniform(min_area, max_area), uniform(log aspect range), and, when the rectangle fits, randint(top), randint(left) and
+    normal(size=(h, w, 3)).  The noise is kept as float32, the value the reference's assignment into its float32 image
+    stores.  Only the shipped setting (mode='pixel', one rectangle) is implemented."""
+
+    def __init__(self, prob=0.25, min_area=0.02, max_area=1 / 3, min_aspect=0.3, max_aspect=None, mode='pixel',
+                 min_count=1, max_count=None):
+        max_count = max_count if max_count else min_count
+        if mode != 'pixel':
+            raise NotImplementedError(f"Uint8RandomErasing mode={mode!r}: only mode='pixel' (the shipped configs') is implemented")
+        if min_count != 1 or max_count != 1:
+            raise NotImplementedError(f'Uint8RandomErasing min_count={min_count}, max_count={max_count}: only one rectangle '
+                                      '(the shipped configs\' max_count=1) is implemented')
+        self.prob = prob
+        self.min_area = min_area
+        self.max_area = max_area
+        max_aspect = max_aspect if max_aspect else 1 / min_aspect
+        self.log_aspect_ratio = (math.log(min_aspect), math.log(max_aspect))
+
+    def __call__(self, sample):
+        image = np.asarray(sample['image'])
+        if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+            raise ValueError(f'Uint8RandomErasing expects a PIL RGB image or a uint8 [H, W, 3] array, got {image.dtype} {image.shape}')
+        image_h, image_w = image.shape[:2]
+        rect, noise = np.zeros(4, dtype=np.int32), np.zeros(0, dtype=np.float32)
+        if np.random.uniform(0, 1) < self.prob:
+            area = image_h * image_w
+            for _ in range(10):
+                target_area = np.random.uniform(self.min_area, self.max_area) * area
+                aspect_ratio = math.exp(np.random.uniform(*self.log_aspect_ratio))
+                h = int(round(math.sqrt(target_area * aspect_ratio)))
+                w = int(round(math.sqrt(target_area / aspect_ratio)))
+                if w < image_w and h < image_h:
+                    top = np.random.randint(0, image_h - h)
+                    left = np.random.randint(0, image_w - w)
+                    noise = np.random.normal(loc=0.0, scale=1.0, size=(h, w, 3)).astype(np.float32).reshape(-1)
+                    rect[:] = (top, left, h, w)
+                    break
+        sample['image'], sample['erase_rect'], sample['erase_noise'] = image, rect, noise
+        return sample
+
+
+class Uint8MixupCutmixClassificationCollater:
+    """Counterpart of MixupCutmixClassificationCollater (SimpleAICV/classification/mixupcutmixclassificationcollator.py:
+    99-284) for samples from ``Uint8RandomErasing`` (or any uint8 [H, W, 3] samples): stacks the images into one pinned
+    uint8 [B, H, W, 3] tensor as ``Uint8ClassificationCollater`` does and adds a ``MixupEraseRecord`` under 'mixup'.
+    tools.utils.CudaPrefetcher(normalize=(mean, std)) turns the batch into the reference's {'image': fp32 [B, 3, H, W],
+    'label': fp32 [B, num_classes]}, bit for bit.
+
+    The batch-mode draws are the reference's, in its order: rand() against mixup_cutmix_prob; with both alphas > 0, rand()
+    against switch_to_cutmix_prob; beta(alpha, alpha); for CutMix randint(0, H) for the box centre row and randint(0, W)
+    for its column.  The corrected lambda is 1 - box area / (H * W) in float64; when lambda is 1 nothing is mixed.
+    Only the shipped setting (use_mixup=True, mode='batch', cutmix_minmax=None) is implemented."""
+
+    def __init__(self, use_mixup=True, mixup_alpha=0.8, cutmix_alpha=1.0, cutmix_minmax=None, mixup_cutmix_prob=1.0,
+                 switch_to_cutmix_prob=0.5, mode='batch', correct_lam=True, label_smoothing=0.1, num_classes=1000,
+                 pin_memory=True):
+        if not use_mixup:
+            raise NotImplementedError('Uint8MixupCutmixClassificationCollater use_mixup=False: use Uint8ClassificationCollater '
+                                      '(the shipped configs use use_mixup=True)')
+        if mode != 'batch':
+            raise NotImplementedError(f"Uint8MixupCutmixClassificationCollater mode={mode!r}: only mode='batch' (the shipped "
+                                      "configs') is implemented")
+        if cutmix_minmax is not None:
+            raise NotImplementedError('Uint8MixupCutmixClassificationCollater cutmix_minmax: only cutmix_minmax=None (the '
+                                      'shipped configs\') is implemented')
+        if not (mixup_alpha > 0. or cutmix_alpha > 0.):
+            raise ValueError('one of mixup_alpha > 0, cutmix_alpha > 0 must hold')
+        self.mixup_alpha = mixup_alpha
+        self.cutmix_alpha = cutmix_alpha
+        self.mixup_cutmix_prob = mixup_cutmix_prob
+        self.switch_to_cutmix_prob = switch_to_cutmix_prob
+        self.correct_lam = correct_lam
+        self.label_smoothing = label_smoothing
+        self.num_classes = num_classes
+        self.pin_memory = pin_memory
+
+    def _params_per_batch(self):
+        lam, use_cutmix = 1., False
+        if np.random.rand() < self.mixup_cutmix_prob:
+            if self.mixup_alpha > 0. and self.cutmix_alpha > 0.:
+                use_cutmix = np.random.rand() < self.switch_to_cutmix_prob
+                alpha = self.cutmix_alpha if use_cutmix else self.mixup_alpha
+            elif self.mixup_alpha > 0.:
+                alpha = self.mixup_alpha
+            else:
+                use_cutmix, alpha = True, self.cutmix_alpha
+            lam = float(np.random.beta(alpha, alpha))
+        return lam, use_cutmix
+
+    def __call__(self, data):
+        shape = np.shape(data[0]['image'])
+        for s in data:
+            img = s['image']
+            if np.shape(img) != shape or len(shape) != 3 or shape[2] != 3 or np.asarray(img).dtype != np.uint8:
+                raise ValueError(f'expects uint8 [H, W, 3] images of one shape, got {np.asarray(img).dtype} {np.shape(img)} '
+                                 f'next to {shape}')
+        b, (h, w) = len(data), shape[:2]
+        if b % 2 != 0:
+            raise ValueError(f'Mixup / CutMix pairs image b with image B-1-b: the batch size must be even (got {b})')
+        labels = np.array([s['label'] for s in data]).astype(np.float32).astype(np.int64)
+        if labels.min() < 0 or labels.max() >= self.num_classes:
+            raise ValueError(f'labels must lie in [0, {self.num_classes}), got {labels.min()}..{labels.max()}')
+        images = np.stack([np.ascontiguousarray(s['image']) for s in data])
+        rects = np.stack([s.get('erase_rect', np.zeros(4, np.int32)) for s in data]).astype(np.int32)
+        noises = [np.asarray(s.get('erase_noise', np.zeros(0, np.float32)), dtype=np.float32).reshape(-1) for s in data]
+        offsets = np.zeros(b, dtype=np.int64)
+        offsets[1:] = np.cumsum([len(n) for n in noises])[:-1]
+
+        lam, use_cutmix = self._params_per_batch()
+        mode, box = MIX_NONE, (0, 0, 0, 0)
+        if lam != 1.:
+            if use_cutmix:
+                ratio = np.sqrt(1 - lam)
+                cut_h, cut_w = int(h * ratio), int(w * ratio)
+                cy = np.random.randint(0, h)
+                cx = np.random.randint(0, w)
+                yl, yh = int(np.clip(cy - cut_h // 2, 0, h)), int(np.clip(cy + cut_h // 2, 0, h))
+                xl, xh = int(np.clip(cx - cut_w // 2, 0, w)), int(np.clip(cx + cut_w // 2, 0, w))
+                if self.correct_lam:
+                    lam = 1. - (yh - yl) * (xh - xl) / float(h * w)
+                mode, box = MIX_CUTMIX, (yl, yh, xl, xh)
+            else:
+                mode = MIX_MIXUP
+        off_value = self.label_smoothing / self.num_classes
+        record = MixupEraseRecord(torch.from_numpy(rects), torch.from_numpy(offsets),
+                                  torch.from_numpy(np.concatenate(noises)),
+                                  mode, box, lam, self.num_classes, 1. - self.label_smoothing + off_value, off_value)
+        images, labels = torch.from_numpy(images), torch.from_numpy(labels)
+        if self.pin_memory and torch.cuda.is_available():
+            images, labels, record = images.pin_memory(), labels.pin_memory(), record.pin_memory()
+        return {'image': images, 'label': labels, 'mixup': record}
 
 
 class DeviceNormalize:

@@ -188,6 +188,33 @@ def u8_normalize(images, mean, std, out=None):
     return out
 
 
+def u8_mix_erase_normalize(images, labels, mean, std, record, noise, out=None, soft=None):
+    """The uint8 edge of the Mixup / CutMix + RandomErasing recipes: images uint8 [N, H, W, 3] and labels int64 [N] (device)
+    -> (fp32 [N, 3, H, W], fp32 soft labels [N, num_classes]) as TorchMeanStdNormalize + RandomErasing +
+    MixupCutmixClassificationCollater compute them on the host, bit-identical.  record: the batch's
+    classification.common.MixupEraseRecord (read on the host); noise: device fp32 whose first record.noise.numel()
+    floats hold record.noise."""
+    assert images.is_cuda and images.dtype == torch.uint8 and images.dim() == 4 and images.shape[3] == 3 and images.is_contiguous()
+    n, h, w, _ = images.shape
+    assert labels.is_cuda and labels.dtype == torch.int64 and tuple(labels.shape) == (n,)
+    rects, offsets = record.rects, record.offsets
+    assert rects.dtype == torch.int32 and tuple(rects.shape) == (n, 4) and not rects.is_cuda and rects.is_contiguous()
+    assert offsets.dtype == torch.int64 and tuple(offsets.shape) == (n,) and not offsets.is_cuda and offsets.is_contiguous()
+    used = record.noise.numel()
+    assert noise.dtype == torch.float32 and noise.numel() >= used
+    if out is None:
+        out = torch.empty(n, 3, h, w, device=images.device, dtype=torch.float32)
+    if soft is None:
+        soft = torch.empty(n, record.num_classes, device=images.device, dtype=torch.float32)
+    m3 = (ctypes.c_float * 3)(*[float(v) for v in mean])
+    s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
+    box = (ctypes.c_int * 4)(*[int(v) for v in record.box])
+    _lib.call('saicv_u8_mix_erase_norm', _p(images), _p(out), n, h, w, m3, s3, ctypes.c_void_p(rects.data_ptr()),
+              ctypes.c_void_p(offsets.data_ptr()), _p(noise), used, int(record.mode), box, float(record.lam), _p(labels),
+              _p(soft), int(record.num_classes), float(record.on_value), float(record.off_value), _stream())
+    return out, soft
+
+
 def nchw_to_nhwc_bf16(x, out=None):
     n, c, h, w = x.shape
     if out is None:

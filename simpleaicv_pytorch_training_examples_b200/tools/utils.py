@@ -242,7 +242,10 @@ class CudaPrefetcher:
     def __init__(self, loader, device=None, copy_streams=4, normalize=None):
         """normalize=(mean, std): batches whose 'image' is a uint8 [B, H, W, 3] tensor (classification.common.
         Uint8ClassificationCollater) are copied as uint8 - a quarter of the bytes - and turned into the fp32 NCHW
-        normalised batch on the device, on the copy stream (SURVEY.md 8 f3; csrc/capi_input.cu).
+        normalised batch on the device, on the copy stream (SURVEY.md 8 f3; csrc/capi_input.cu).  Batches that also carry a
+        'mixup' record (classification.common.Uint8MixupCutmixClassificationCollater) get the reference's RandomErasing and
+        Mixup / CutMix applied by the same pass and are yielded as {'image': fp32 [B, 3, H, W], 'label': fp32 [B, classes]};
+        such a batch without ``normalize`` raises.
         copy_streams > 1: tensors of 32 MB and more are copied in that many chunks on separate streams, so that the copy of
         the next batch keeps its bandwidth while the current step's kernels run (tests/profile_h2d.py measures it)."""
         self.loader = loader
@@ -260,12 +263,18 @@ class CudaPrefetcher:
         batch = next(it, None)
         if batch is None:
             return None
+        rec = batch.get('mixup')
+        if rec is not None and self.normalize is None:
+            raise RuntimeError("a batch with a 'mixup' record (Uint8MixupCutmixClassificationCollater) needs "
+                               'CudaPrefetcher(normalize=(mean, std)): its uint8 pixels are not the model input')
         slot = self._slots[k & 1]
         with torch.cuda.stream(self.stream):
             if self._free[k & 1] is not None:
                 self.stream.wait_event(self._free[k & 1])
             out = {}
             for name, v in batch.items():
+                if name == 'mixup':
+                    continue
                 if not torch.is_tensor(v):
                     out[name] = v
                     continue
@@ -292,10 +301,27 @@ class CudaPrefetcher:
                 nb = slot.get('image_f32')
                 if nb is None or nb.shape[0] != img.shape[0] or nb.shape[2:] != img.shape[1:3]:
                     nb = slot['image_f32'] = torch.empty(img.shape[0], 3, img.shape[1], img.shape[2], device=self.device)
-                out['image'] = ops.u8_normalize(img, self.normalize[0], self.normalize[1], out=nb)
+                if rec is None:
+                    out['image'] = ops.u8_normalize(img, self.normalize[0], self.normalize[1], out=nb)
+                else:
+                    out['image'], out['label'] = self._mix(slot, img, out['label'], rec, nb)
             ev = torch.cuda.Event()
             ev.record(self.stream)
         return out, ev
+
+    def _mix(self, slot, img, labels, rec, out):
+        from .. import ops
+        used = rec.noise.numel()
+        noise = slot.get('mixup_noise')
+        if noise is None or noise.numel() < used:
+            # the noise length changes every batch: the buffer only grows, to powers of two, so it is rarely re-allocated
+            noise = slot['mixup_noise'] = torch.empty(1 << max(used - 1, 0).bit_length(), device=self.device)
+        if used:
+            noise[:used].copy_(rec.noise, non_blocking=True)
+        soft = slot.get('mixup_label')
+        if soft is None or tuple(soft.shape) != (img.shape[0], rec.num_classes):
+            soft = slot['mixup_label'] = torch.empty(img.shape[0], rec.num_classes, device=self.device)
+        return ops.u8_mix_erase_normalize(img, labels, self.normalize[0], self.normalize[1], rec, noise, out=out, soft=soft)
 
     def __iter__(self):
         it = iter(self.loader)
