@@ -356,12 +356,6 @@ typedef struct {
   int dk_cols;
 } saicv_attn_bwd_args;
 int saicv_attn_bwd(const saicv_attn_bwd_args* a, void* stream);
-/* ViT convenience entries (vit.py:66-76): qkv bf16 [b][l][3][h][d] -> out bf16 [b][l][h*d]; lse [b][h][l];
- * backward writes dqkv in the layout of qkv; delta: fp32 workspace [b][h][l]. */
-int saicv_attention_fwd(const void* qkv, void* out, float* lse, int b, int l, int h, int d,
-                        float scale, void* stream);
-int saicv_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse,
-                        float* delta, void* dqkv, int b, int l, int h, int d, float scale, void* stream);
 
 /* ---- DETR transformer glue (SimpleAICV/detection/models/detr.py:44-180; csrc/capi_detr.cu) -------------------
  * Post-LayerNorm on the fp32 token stream: y = LN(z) (nullable), yb = bf16(y) (nullable),

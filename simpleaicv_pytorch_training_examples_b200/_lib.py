@@ -87,8 +87,6 @@ SIGNATURES = {
     'saicv_vit_assemble_tokens_bwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_token_pool_fwd': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_token_pool_bwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
-    'saicv_attention_fwd': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p],
-    'saicv_attention_bwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p],
     'saicv_attn_fwd': [ctypes.POINTER(AttnArgs), c_void_p],
     'saicv_attn_bwd': [ctypes.POINTER(AttnBwdArgs), c_void_p],
     'saicv_window_partition': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],

@@ -1,8 +1,4 @@
 // Host side of the wgmma attention family (attn_sm90.cuh): tensor maps, template dispatch, launches.
-#include <cudaTypedefs.h>
-
-#include <mutex>
-
 #include "../../include/saicv_b200.h"
 #include "attn_sm90.cuh"
 #include "host_util.h"
@@ -10,38 +6,6 @@
 using namespace saicv;
 
 namespace {
-
-PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
-int g_sms = 0;
-std::once_flag g_once;
-bool g_ok = false;
-
-void init() {
-  cudaDriverEntryPointQueryResult qres;
-  void* fn = nullptr;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess || fn == nullptr) {
-    set_error("cuTensorMapEncodeTiled not available (no CUDA driver?)");
-    return;
-  }
-  g_encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
-  int dev = 0;
-  cudaDeviceProp prop;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) {
-    set_error("cudaGetDeviceProperties failed");
-    return;
-  }
-  if (prop.major != 9) {
-    set_error("libsaicv_b200 requires an sm_90 (H100) device, found sm_%d%d", prop.major, prop.minor);
-    return;
-  }
-  g_sms = prop.multiProcessorCount;
-  g_ok = true;
-}
-bool ensure() {
-  std::call_once(g_once, init);
-  return g_ok;
-}
 
 // [B][H][L][D] view with arbitrary (16-byte aligned) strides; box = 64 columns x `rows` rows, 128B swizzle,
 // out-of-range rows / columns read as zero.
@@ -55,9 +19,9 @@ bool encode_4d(CUtensorMap* m, const void* ptr, int D, int L, int H, int B, cons
     set_error("attention operand not 16-byte aligned (ptr %p strides %lld %lld %lld elements)", ptr, strides[0], strides[1], strides[2]);
     return false;
   }
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, st, box, es,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = device()->encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, st, box, es,
+                                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled(attention 4d) failed: %d (D=%d L=%d H=%d B=%d strides %lld %lld %lld)", (int)r, D, L, H, B,
               strides[0], strides[1], strides[2]);
@@ -75,7 +39,7 @@ int persistent_grid(K kernel, int minb, long long total) {
     cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     carve = true;
   }
-  const long long g = (long long)g_sms * minb;
+  const long long g = (long long)device()->sms * minb;
   return (int)(total < g ? total : g);
 }
 
@@ -261,7 +225,7 @@ int check_args(const saicv_attn_args* a, const char* who) {
 extern "C" {
 
 int saicv_attn_fwd(const saicv_attn_args* a, void* stream) {
-  if (!ensure()) return 1;
+  if (!device()) return 1;
   if (int e = check_args(a, "saicv_attn_fwd")) return e;
 #define X(Q, V) if (a->dqk == Q && a->dv == V) return fwd_for<Q, V>(a, (cudaStream_t)stream);
   SAICV_ATTN_SHAPES(X)
@@ -270,16 +234,15 @@ int saicv_attn_fwd(const saicv_attn_args* a, void* stream) {
 }
 
 int saicv_attn_bwd(const saicv_attn_bwd_args* a, void* stream) {
-  if (!ensure()) return 1;
+  if (!device()) return 1;
   const saicv_attn_args* f = &a->fwd;
   if (int e = check_args(f, "saicv_attn_bwd")) return e;
   if (a->dk_cols < 0 || a->dk_cols > f->dqk || (a->dk_cols % 16)) return set_error("saicv_attn_bwd: bad dk_cols %d", a->dk_cols);
   {
     const long long rows = (long long)f->b * f->h * f->lq;
     if (f->dv % 8 || f->dv > 128) return set_error("saicv_attn_bwd: the value width must be a multiple of 8, <= 128 (got %d)", f->dv);
-    long long blocks = (rows + 15) / 16;               // 16 rows per 256-thread block
-    if (blocks > (long long)g_sms * 16) blocks = (long long)g_sms * 16;
-    attn_delta_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+    // 16 rows per 256-thread block
+    attn_delta_kernel<<<grid_1d(rows, 16, device()->sms * 16), 256, 0, (cudaStream_t)stream>>>(
         reinterpret_cast<const __nv_bfloat16*>(f->out), reinterpret_cast<const __nv_bfloat16*>(a->dout), a->delta, f->b, f->h,
         f->lq, f->dv, f->o_strides[0], f->o_strides[1], f->o_strides[2]);
     if (int e = check_launch("attn_delta_kernel")) return e;
@@ -288,36 +251,6 @@ int saicv_attn_bwd(const saicv_attn_bwd_args* a, void* stream) {
   SAICV_ATTN_SHAPES(X)
 #undef X
   return set_error("saicv_attn_bwd: unsupported (score width, value width) = (%d, %d)", f->dqk, f->dv);
-}
-
-// ---- packed-qkv convenience entries used by the ViT runtime: qkv [B, L, 3, H, d], out [B, L, H*d]
-static void fill_packed(saicv_attn_args* a, const void* qkv, void* out, float* lse, int b, int l, int h, int d, float scale) {
-  const __nv_bfloat16* base = reinterpret_cast<const __nv_bfloat16*>(qkv);
-  const long long sl = 3LL * h * d, sb = (long long)l * sl;
-  a->q = base; a->k = base + (long long)h * d; a->v = base + 2LL * h * d;
-  a->out = out; a->lse = lse;
-  for (auto* s : {a->q_strides, a->k_strides, a->v_strides}) { s[0] = sb; s[1] = d; s[2] = sl; }
-  a->o_strides[0] = (long long)l * h * d; a->o_strides[1] = d; a->o_strides[2] = (long long)h * d;
-  a->key_mask_bits = nullptr; a->mask_words = 0;
-  a->b = b; a->h = h; a->lq = l; a->lk = l; a->dqk = d; a->dv = d; a->scale = scale;
-}
-
-int saicv_attention_fwd(const void* qkv, void* out, float* lse, int b, int l, int h, int d, float scale, void* stream) {
-  saicv_attn_args a{};
-  fill_packed(&a, qkv, out, lse, b, l, h, d, scale);
-  return saicv_attn_fwd(&a, stream);
-}
-
-int saicv_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* delta, void* dqkv, int b,
-                        int l, int h, int d, float scale, void* stream) {
-  saicv_attn_bwd_args a{};
-  fill_packed(&a.fwd, qkv, const_cast<void*>(out), const_cast<float*>(lse), b, l, h, d, scale);
-  a.dout = dout; a.delta = delta;
-  __nv_bfloat16* g = reinterpret_cast<__nv_bfloat16*>(dqkv);
-  a.dq = g; a.dk = g + (long long)h * d; a.dv = g + 2LL * h * d;
-  for (auto* s : {a.dq_strides, a.dk_strides, a.dv_strides}) { s[0] = a.fwd.q_strides[0]; s[1] = d; s[2] = a.fwd.q_strides[2]; }
-  a.dk_cols = d;
-  return saicv_attn_bwd(&a, stream);
 }
 
 }  // extern "C"

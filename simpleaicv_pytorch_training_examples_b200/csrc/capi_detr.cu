@@ -83,7 +83,7 @@ postln_fwd_kernel(const float* __restrict__ z, const float* __restrict__ gamma, 
 }
 
 // dz = dres + rstd*(dxhat - mean(dxhat) - xhat*mean(dxhat*xhat)), dxhat = dy*gamma, dy fp32; dgamma / dbeta as
-// per-block partial rows ([gridDim.x][2][C]) folded in a fixed order by postln_fold_kernel (bit-reproducible).
+// per-block partial rows ([gridDim.x][2][C]) folded in a fixed order by fold_partials (bit-reproducible).
 template <int NCH>
 __global__ void __launch_bounds__(256)
 postln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ z, const float* __restrict__ gamma,
@@ -142,24 +142,6 @@ postln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ z, con
       partials[((long long)blockIdx.x * 2 + pass) * C + c] = s;
     }
   }
-}
-
-__global__ void postln_fold_kernel(const float* __restrict__ partials, float* __restrict__ dgamma, float* __restrict__ dbeta,
-                                   int nblk, int C, int accumulate) {
-  __shared__ float sm[32][9];                            // 8 columns x 32 row groups per block, fixed summation order
-  const int cl = threadIdx.x & 7, grp = threadIdx.x >> 3;
-  const int j = blockIdx.x * 8 + cl;  // 0 .. 2C-1
-  float s = 0.f;
-  if (j < 2 * C)
-    for (int b = grp; b < nblk; b += 32) s += partials[(long long)b * 2 * C + j];
-  sm[grp][cl] = s;
-  __syncthreads();
-  if (grp != 0 || j >= 2 * C) return;
-  float t = 0.f;
-#pragma unroll
-  for (int g = 0; g < 32; ++g) t += sm[g][cl];
-  float* dst = j < C ? dgamma + j : dbeta + (j - C);
-  *dst = accumulate ? *dst + t : t;
 }
 
 // xb = bf16(x); xpb = bf16(x + pos[row % pos_rows])   (4 columns per thread)
@@ -273,13 +255,6 @@ __global__ void heads_unpack_kernel(const __nv_bfloat16* __restrict__ src, __nv_
   }
 }
 
-int grid_1d(long long items, int per_block = 256, int cap = 132 * 16) {
-  long long b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > cap) b = cap;
-  return (int)b;
-}
-
 }  // namespace
 }  // namespace saicv
 
@@ -318,8 +293,7 @@ int saicv_postln_bwd(const float* dy, const float* z, const float* gamma, const 
     default: return set_error("saicv_postln_bwd: unsupported width %d", c);
   }
   if (int e = check_launch("postln_bwd_kernel")) return e;
-  postln_fold_kernel<<<(2 * c + 7) / 8, 256, 0, ST>>>(partials, dgamma, dbeta, grid, c, accumulate);
-  return check_launch("postln_fold_kernel");
+  return fold_partials(partials, grid, 2 * c, dgamma, dbeta, c, accumulate, ST);
 }
 
 int saicv_add_pos_cast(const float* x, const float* pos, long long pos_rows, void* xb, void* xpb, long long rows, int c,

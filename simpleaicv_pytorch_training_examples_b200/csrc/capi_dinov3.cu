@@ -105,13 +105,6 @@ __global__ void swiglu_bwd_kernel(const V8* __restrict__ dh, const V8* __restric
   }
 }
 
-int grid_1d(long long items) {
-  long long b = (items + 255) / 256;
-  if (b < 1) b = 1;
-  if (b > 132 * 16) b = 132 * 16;
-  return (int)b;
-}
-
 int rope_launch(bool bwd, void* qkv, const float* sin_t, const float* cos_t, int b, int l, int heads, int hd, void* stream) {
   const char* name = bwd ? "saicv_rope_qk_bwd" : "saicv_rope_qk_fwd";
   if (hd <= 0 || hd % 8) return set_error("%s: head size %d must be a positive multiple of 8", name, hd);

@@ -5,36 +5,11 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
-#include <atomic>
-#include <cstdarg>
-#include <cstdio>
-
 #include "../../include/saicv_b200.h"
 #include "host_util.h"
 #include "vec8.cuh"
 
 namespace saicv {
-
-static thread_local char g_err[512] = "";
-int set_error(const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_err, sizeof(g_err), fmt, ap);
-  va_end(ap);
-  return 1;
-}
-static std::atomic<long long> g_launches{0};
-void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-int check_launch(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("%s: %s", what, cudaGetErrorString(e));
-  count_launch(1);
-  return 0;
-}
-long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
-const char* last_error() { return g_err; }
-long long launch_count();
-
 namespace {
 
 constexpr int kThreads = 256;
@@ -53,18 +28,6 @@ __device__ __forceinline__ float act_grad(float out, int act) {
     return sg * (1.f + out * (1.f - sg));
   }
   return act == 1 ? (out > 0.f ? 1.f : 0.f) : (act == 2 ? (out > 0.f ? 1.f : 0.1f) : 1.f);
-}
-
-int grid_for(long long work_items, int per_block = kThreads, int max_blocks = 132 * 16) {
-  long long b = (work_items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return (int)b;
-}
-int next_pow2(int v) {
-  int p = 1;
-  while (p < v) p <<= 1;
-  return p;
 }
 
 // ----------------------------------------------------------------------------- slab kernels
@@ -283,10 +246,10 @@ colreduce2_kernel(const void* __restrict__ g, const uint8_t* __restrict__ bits, 
   fold_slab<false>(red, sb0, sb1, tx, ty, gm, prow + 2 * C, C);
 }
 
-// out[j] (+)= sum_b partial[b][j]: 8 columns x 32 row groups per block (the <= 264 partial rows are
-// spread over 32 threads per column so the fold is a handful of loads deep)
-__global__ void fold_partials_kernel(const float* __restrict__ partial, float* __restrict__ out, int nblk, int ncols,
-                                     int accumulate) {
+// out0[j] (+)= sum_b partial[b][j] for j < split, out1[j - split] for the columns after: 8 columns x 32 row groups per
+// block (the <= 264 partial rows are spread over 32 threads per column so the fold is a handful of loads deep)
+__global__ void fold_partials_kernel(const float* __restrict__ partial, float* __restrict__ out0, float* __restrict__ out1,
+                                     int split, int nblk, int ncols, int accumulate) {
   __shared__ float sm[32][9];
   const int cl = threadIdx.x & 7, grp = threadIdx.x >> 3;
   const int col = blockIdx.x * 8 + cl;
@@ -299,7 +262,8 @@ __global__ void fold_partials_kernel(const float* __restrict__ partial, float* _
     float t = 0.f;
 #pragma unroll
     for (int g = 0; g < 32; ++g) t += sm[g][cl];
-    out[col] = accumulate ? out[col] + t : t;
+    float* dst = col < split ? out0 + col : out1 + (col - split);
+    *dst = accumulate ? *dst + t : t;
   }
 }
 
@@ -313,7 +277,7 @@ bool slab_geom(long long rows, int C, int unroll, SlabGeom* g, int* blocks, int 
   }
   g->vpr = C / 8;
   g->ldv = C / 8;
-  g->tx_count = next_pow2(g->vpr) > kThreads ? kThreads : next_pow2(g->vpr);
+  g->tx_count = pow2_ge(g->vpr) > kThreads ? kThreads : pow2_ge(g->vpr);
   g->ty_count = kThreads / g->tx_count;
   long long b = (rows + (long long)g->ty_count * min_rows_per_thread - 1) / ((long long)g->ty_count * min_rows_per_thread);
   if (b > max_blocks) b = max_blocks;
@@ -343,10 +307,6 @@ int partial_rows(long long rows, int C) {  // must mirror launch_colreduce<0>
   int n = 0;
   slab_geom(rows, C, 8, &g, &n, kMaxPartials);
   return n;
-}
-int fold(const float* partials, float* out, int nblk, int ncols, int accumulate, cudaStream_t st) {
-  fold_partials_kernel<<<(ncols + 7) / 8, 256, 0, st>>>(partials, out, nblk, ncols, accumulate);
-  return check_launch("fold_partials_kernel");
 }
 
 // fp32 column sums (fc bias gradient from fp32 dlogits): small, one thread per column
@@ -1001,6 +961,17 @@ __global__ void avgpool_bwd_kernel(const void* __restrict__ dy, void* __restrict
 }
 
 }  // namespace
+
+int fold_partials(const float* partials, int nblk, int ncols, float* out0, float* out1, int split, int accumulate,
+                  cudaStream_t st) {
+  fold_partials_kernel<<<(ncols + 7) / 8, 256, 0, st>>>(partials, out0, out1, split, nblk, ncols, accumulate);
+  return check_launch("fold_partials_kernel");
+}
+int bn_param_grad(const float* sums, float* dgamma, float* dbeta, int c, int accumulate, cudaStream_t st) {
+  bn_param_grad_kernel<<<(c + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, c, accumulate);
+  return check_launch("bn_param_grad_kernel");
+}
+
 }  // namespace saicv
 
 using namespace saicv;
@@ -1010,8 +981,6 @@ using namespace saicv;
 extern "C" {
 
 int saicv_version(void) { return 100; }
-long long saicv_launch_count(void) { return saicv::launch_count(); }
-const char* saicv_last_error(void) { return saicv::last_error(); }
 
 int saicv_bn_stats(const void* y, float* partials, long long rows, int c, void* stream) {
   int nblk;
@@ -1060,7 +1029,7 @@ int saicv_bn_bwd_reduce(const void* dout, const void* out, const uint32_t* bits,
   if (int e = check_mask_source("saicv_bn_bwd_reduce", out, bits, scale_shift, c, act)) return e;
   int nblk;
   if (int e = launch_colreduce<1>(dout, out, y, saved, scale_shift, partials, rows, c, act, &nblk, ST, bits)) return e;
-  return fold(partials, sums, nblk, 2 * c, 0, ST);
+  return fold_partials(partials, nblk, 2 * c, sums, nullptr, 2 * c, 0, ST);
 }
 
 int saicv_bn_bwd_apply(const void* dout, const void* out, const uint32_t* bits, const void* y, const float* saved,
@@ -1081,8 +1050,7 @@ int saicv_bn_bwd_apply(const void* dout, const void* out, const uint32_t* bits, 
   }
 #undef BWD_APPLY
   if (int e = check_launch("bn_bwd_apply_kernel")) return e;
-  bn_param_grad_kernel<<<(c + 127) / 128, 128, 0, ST>>>(sums, dgamma, dbeta, c, accumulate);
-  return check_launch("bn_param_grad_kernel");
+  return bn_param_grad(sums, dgamma, dbeta, c, accumulate, ST);
 }
 
 int saicv_bn_bwd_reduce2(const void* g, const uint32_t* bits, const void* y_a, const void* y_b, const float* saved_a,
@@ -1094,7 +1062,7 @@ int saicv_bn_bwd_reduce2(const void* g, const uint32_t* bits, const void* y_a, c
   colreduce2_kernel<<<nblk, kThreads, 0, ST>>>(g, reinterpret_cast<const uint8_t*>(bits), y_a, y_b, saved_a, saved_b,
                                                partials, rows, c, gm);
   if (int e = check_launch("colreduce2_kernel")) return e;
-  return fold(partials, sums, nblk, 4 * c, 0, ST);
+  return fold_partials(partials, nblk, 4 * c, sums, nullptr, 4 * c, 0, ST);
 }
 
 int saicv_bn_bwd_apply2(const void* g, const uint32_t* bits, const void* y_a, const void* y_b, const float* saved_a,
@@ -1109,35 +1077,33 @@ int saicv_bn_bwd_apply2(const void* g, const uint32_t* bits, const void* y_a, co
                                                     saved_b, gamma_a, gamma_b, sums, dy_a, dy_b, rows, c, gm,
                                                     1.0f / (float)rows);
   if (int e = check_launch("bn_bwd_apply2_kernel")) return e;
-  bn_param_grad_kernel<<<(c + 127) / 128, 128, 0, ST>>>(sums, dgamma_a, dbeta_a, c, accumulate_a);
-  if (int e = check_launch("bn_param_grad_kernel")) return e;
-  bn_param_grad_kernel<<<(c + 127) / 128, 128, 0, ST>>>(sums + 2 * c, dgamma_b, dbeta_b, c, accumulate_b);
-  return check_launch("bn_param_grad_kernel");
+  if (int e = bn_param_grad(sums, dgamma_a, dbeta_a, c, accumulate_a, ST)) return e;
+  return bn_param_grad(sums + 2 * c, dgamma_b, dbeta_b, c, accumulate_b, ST);
 }
 
 int saicv_add_bf16(void* a, const void* b, long long n, void* stream) {
   if (n % 8) return set_error("saicv_add_bf16: n %% 8 != 0");
-  add_bf16_kernel<<<grid_for(n / 8), kThreads, 0, ST>>>(a, b, n / 8);
+  add_bf16_kernel<<<grid_1d(n / 8), kThreads, 0, ST>>>(a, b, n / 8);
   return check_launch("add_bf16_kernel");
 }
 
 int saicv_cast_bf16(const float* src, void* dst, long long n, void* stream) {
   if (n % 8 == 0 && ((uintptr_t)src & 15) == 0 && ((uintptr_t)dst & 15) == 0) {
-    cast_bf16_vec_kernel<<<grid_for(n / 8), kThreads, 0, ST>>>(reinterpret_cast<const float4*>(src), reinterpret_cast<uint4*>(dst), n / 8);
+    cast_bf16_vec_kernel<<<grid_1d(n / 8), kThreads, 0, ST>>>(reinterpret_cast<const float4*>(src), reinterpret_cast<uint4*>(dst), n / 8);
     return check_launch("cast_bf16_vec_kernel");
   }
-  cast_bf16_kernel<<<grid_for(n), kThreads, 0, ST>>>(src, reinterpret_cast<__nv_bfloat16*>(dst), n);
+  cast_bf16_kernel<<<grid_1d(n), kThreads, 0, ST>>>(src, reinterpret_cast<__nv_bfloat16*>(dst), n);
   return check_launch("cast_bf16_kernel");
 }
 
 int saicv_reduce_partials(const float* partial, float* out, int splits, long long n, int accumulate,
                           void* stream) {
   if (n % 4 == 0 && ((uintptr_t)partial & 15) == 0 && ((uintptr_t)out & 15) == 0) {
-    reduce_partials_vec_kernel<<<grid_for(n / 4), kThreads, 0, ST>>>(reinterpret_cast<const float4*>(partial), reinterpret_cast<float4*>(out),
+    reduce_partials_vec_kernel<<<grid_1d(n / 4), kThreads, 0, ST>>>(reinterpret_cast<const float4*>(partial), reinterpret_cast<float4*>(out),
                                                                     splits, n / 4, accumulate);
     return check_launch("reduce_partials_vec_kernel");
   }
-  reduce_partials_kernel<<<grid_for(n), kThreads, 0, ST>>>(partial, out, splits, n, accumulate);
+  reduce_partials_kernel<<<grid_1d(n), kThreads, 0, ST>>>(partial, out, splits, n, accumulate);
   return check_launch("reduce_partials_kernel");
 }
 
@@ -1147,7 +1113,7 @@ int saicv_prep_conv_weight(const float* w, void* w_bf16, int k, int c, int r, in
   if (cp <= 0) cp = c;
   if (kpad % 8 || kpad < r * s * (order == 1 ? c : cp) || kp < k || cp < c)
     return set_error("saicv_prep_conv_weight: bad padding (kpad %d kp %d cp %d)", kpad, kp, cp);
-  prep_conv_weight_kernel<<<grid_for((long long)kp * kpad), kThreads, 0, ST>>>(
+  prep_conv_weight_kernel<<<grid_1d((long long)kp * kpad), kThreads, 0, ST>>>(
       w, reinterpret_cast<__nv_bfloat16*>(w_bf16), k, c, r, s, kpad, order, kp, cp);
   return check_launch("prep_conv_weight_kernel");
 }
@@ -1156,14 +1122,14 @@ int saicv_finish_conv_wgrad(const float* partial, float* grad, int splits, int k
                             int accumulate, int order, int kp, int cp, int transposed, void* stream) {
   if (kp <= 0) kp = k;
   if (cp <= 0) cp = c;
-  finish_conv_wgrad_kernel<<<grid_for((long long)k * c * r * s), kThreads, 0, ST>>>(partial, grad, splits, k, c, r,
+  finish_conv_wgrad_kernel<<<grid_1d((long long)k * c * r * s), kThreads, 0, ST>>>(partial, grad, splits, k, c, r,
                                                                                      s, kpad, accumulate, order, kp, cp,
                                                                                      transposed);
   return check_launch("finish_conv_wgrad_kernel");
 }
 
 int saicv_nchw_to_nhwc_bf16(const float* x, void* y, int n, int c, int h, int w, void* stream) {
-  nchw_to_nhwc_kernel<<<grid_for((long long)n * h * w), kThreads, 0, ST>>>(x, reinterpret_cast<__nv_bfloat16*>(y),
+  nchw_to_nhwc_kernel<<<grid_1d((long long)n * h * w), kThreads, 0, ST>>>(x, reinterpret_cast<__nv_bfloat16*>(y),
                                                                            n, c, h, w);
   return check_launch("nchw_to_nhwc_kernel");
 }
@@ -1186,13 +1152,13 @@ int saicv_stem_im2col(const float* x, void* cols, int n, int c, int h, int w, in
 
 int saicv_zero_upsample2(const void* dy, void* u, int n, int p, int q, int h, int w, int c, void* stream) {
   if (c % 8) return set_error("saicv_zero_upsample2: C %% 8 != 0");
-  zero_upsample2_kernel<<<grid_for((long long)n * h * w * (c / 8)), kThreads, 0, ST>>>(dy, u, n, p, q, h, w, c);
+  zero_upsample2_kernel<<<grid_1d((long long)n * h * w * (c / 8)), kThreads, 0, ST>>>(dy, u, n, p, q, h, w, c);
   return check_launch("zero_upsample2_kernel");
 }
 
 int saicv_add_strided2(void* dx, const void* dd, int n, int p, int q, int h, int w, int c, void* stream) {
   if (c % 8) return set_error("saicv_add_strided2: C %% 8 != 0");
-  add_strided2_kernel<<<grid_for((long long)n * p * q * (c / 8)), kThreads, 0, ST>>>(dx, dd, n, p, q, h, w, c);
+  add_strided2_kernel<<<grid_1d((long long)n * p * q * (c / 8)), kThreads, 0, ST>>>(dx, dd, n, p, q, h, w, c);
   return check_launch("add_strided2_kernel");
 }
 
@@ -1201,7 +1167,7 @@ int saicv_maxpool_fwd(const void* x, void* y, uint8_t* argmax, int n, int h, int
   if (c % 8) return set_error("saicv_maxpool_fwd: C %% 8 != 0");
   if (k < 1 || k > 15 || stride < 1) return set_error("saicv_maxpool_fwd: unsupported window %d / stride %d", k, stride);
   const int P = (h + pad + pad_hi - k) / stride + 1, Q = (w + pad + pad_hi - k) / stride + 1;
-  const int grid = grid_for((long long)n * P * Q * (c / 8));
+  const int grid = grid_1d((long long)n * P * Q * (c / 8));
   if (k == 3) maxpool_fwd_kernel<3><<<grid, kThreads, 0, ST>>>(x, y, argmax, n, h, w, c, P, Q, k, stride, pad, oob_zero);
   else if (k == 2) maxpool_fwd_kernel<2><<<grid, kThreads, 0, ST>>>(x, y, argmax, n, h, w, c, P, Q, k, stride, pad, oob_zero);
   else maxpool_fwd_kernel<0><<<grid, kThreads, 0, ST>>>(x, y, argmax, n, h, w, c, P, Q, k, stride, pad, oob_zero);
@@ -1212,7 +1178,7 @@ int saicv_maxpool_bwd(const void* dy, const uint8_t* argmax, void* dx, int n, in
                       int pad, int pad_hi, void* stream) {
   if (c % 8) return set_error("saicv_maxpool_bwd: C %% 8 != 0");
   const int P = (h + pad + pad_hi - k) / stride + 1, Q = (w + pad + pad_hi - k) / stride + 1;
-  const int grid = grid_for((long long)n * h * w * (c / 8));
+  const int grid = grid_1d((long long)n * h * w * (c / 8));
   if (k <= 2 * stride && k >= stride) maxpool_bwd_kernel<true><<<grid, kThreads, 0, ST>>>(dy, argmax, dx, n, h, w, c, P, Q, k, stride, pad);
   else maxpool_bwd_kernel<false><<<grid, kThreads, 0, ST>>>(dy, argmax, dx, n, h, w, c, P, Q, k, stride, pad);
   return check_launch("maxpool_bwd_kernel");
@@ -1229,13 +1195,13 @@ int saicv_maxpool3x3s2_bwd(const void* dy, const uint8_t* argmax, void* dx, int 
 
 int saicv_avgpool_fwd(const void* x, void* y, int n, int hw, int c, void* stream) {
   if (c % 8) return set_error("saicv_avgpool_fwd: C %% 8 != 0");
-  avgpool_fwd_kernel<<<grid_for((long long)n * (c / 8), 128), 128, 0, ST>>>(x, y, n, hw, c);
+  avgpool_fwd_kernel<<<grid_1d((long long)n * (c / 8), 128), 128, 0, ST>>>(x, y, n, hw, c);
   return check_launch("avgpool_fwd_kernel");
 }
 
 int saicv_avgpool_bwd(const void* dy, void* dx, int n, int hw, int c, void* stream) {
   if (c % 8) return set_error("saicv_avgpool_bwd: C %% 8 != 0");
-  avgpool_bwd_kernel<<<grid_for((long long)n * hw * (c / 8)), kThreads, 0, ST>>>(dy, dx, n, hw, c);
+  avgpool_bwd_kernel<<<grid_1d((long long)n * hw * (c / 8)), kThreads, 0, ST>>>(dy, dx, n, hw, c);
   return check_launch("avgpool_bwd_kernel");
 }
 
@@ -1256,7 +1222,7 @@ int saicv_colsum(const void* x, float* partials, float* out, long long rows, int
     colreduce_kernel<2, 8><<<nblk, kThreads, 0, ST>>>(reinterpret_cast<const __nv_bfloat16*>(x) + c0, nullptr, nullptr,
                                                    nullptr, nullptr, nullptr, partials, rows, cw, g, 0);
     if (int e = check_launch("colreduce_kernel")) return e;
-    if (int e = fold(partials, out + c0, nblk, cw, accumulate, ST)) return e;
+    if (int e = fold_partials(partials, nblk, cw, out + c0, nullptr, cw, accumulate, ST)) return e;
   }
   return 0;
 }

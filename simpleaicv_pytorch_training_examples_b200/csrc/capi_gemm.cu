@@ -6,7 +6,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <mutex>
 
 #include "../../include/saicv_b200.h"
 #include "gemm_sm90.cuh"
@@ -16,47 +15,6 @@ using namespace saicv;
 
 namespace {
 
-PFN_cuTensorMapEncodeTiled_v12000 g_encode_tiled = nullptr;
-PFN_cuTensorMapEncodeIm2col_v12000 g_encode_im2col = nullptr;
-int g_sm_count = 0;
-int g_driver_version = 0;
-std::once_flag g_once;
-bool g_init_ok = false;
-
-void init_driver() {
-  cudaDriverEntryPointQueryResult qres;
-  void* fn = nullptr;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess || fn == nullptr) {
-    set_error("cuTensorMapEncodeTiled not available (no CUDA driver?)");
-    return;
-  }
-  g_encode_tiled = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
-  fn = nullptr;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &fn, cudaEnableDefault, &qres) != cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess || fn == nullptr) {
-    set_error("cuTensorMapEncodeIm2col not available");
-    return;
-  }
-  g_encode_im2col = reinterpret_cast<PFN_cuTensorMapEncodeIm2col_v12000>(fn);
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) { set_error("cudaGetDevice failed"); return; }
-  cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) { set_error("cudaGetDeviceProperties failed"); return; }
-  if (prop.major != 9) {
-    set_error("libsaicv_b200 requires an sm_90 (H100) device, found sm_%d%d", prop.major, prop.minor);
-    return;
-  }
-  g_sm_count = prop.multiProcessorCount;
-  cudaDriverGetVersion(&g_driver_version);
-  g_init_ok = true;
-}
-
-bool ensure_init() {
-  std::call_once(g_once, init_driver);
-  return g_init_ok;
-}
-
 // 2-D tiled map over a row-major [rows][cols] matrix, 128B swizzle.
 bool encode_2d(CUtensorMap* m, const void* ptr, CUtensorMapDataType dt, int esz, uint64_t cols,
                uint64_t rows, uint64_t row_stride_elems, uint32_t box_cols, uint32_t box_rows) {
@@ -64,9 +22,9 @@ bool encode_2d(CUtensorMap* m, const void* ptr, CUtensorMapDataType dt, int esz,
   cuuint64_t strides[1] = {row_stride_elems * (uint64_t)esz};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode_tiled(m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = device()->encode_tiled(m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled(2d) failed: %d (cols=%llu rows=%llu stride=%llu box=%u,%u ptr=%p)",
               (int)r, (unsigned long long)cols, (unsigned long long)rows,
@@ -84,10 +42,10 @@ bool encode_out(CUtensorMap* m, const void* ptr, bool f32, uint64_t cols, uint64
   cuuint64_t strides[2] = {ldd * esz, (splits > 1 ? split_stride : ldd * rows) * esz};
   cuuint32_t box[3] = {f32 ? 32u : 64u, 128u, 1u};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = g_encode_tiled(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3,
-                              const_cast<void*>(ptr), dims, strides, box, estr,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = device()->encode_tiled(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3,
+                                      const_cast<void*>(ptr), dims, strides, box, estr,
+                                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled(out) failed: %d (cols=%llu rows=%llu ldd=%llu splits=%llu)", (int)r,
               (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)ldd,
@@ -104,9 +62,9 @@ bool encode_out_phases(CUtensorMap* m, void* ptr, uint64_t c, uint64_t np, uint6
   cuuint64_t strides[4] = {c * 2, 2 * c * 2, 2 * q * c * 2, 4 * q * c * 2};
   cuuint32_t box[5] = {64u, 1u, (cuuint32_t)q, 1u, rows};
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, ptr, dims, strides, box, estr,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = device()->encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, ptr, dims, strides, box, estr,
+                                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled(phase out) failed: %d (c=%llu rows=%llu q=%llu box rows=%u)", (int)r,
               (unsigned long long)c, (unsigned long long)np, (unsigned long long)q, rows);
@@ -123,10 +81,10 @@ bool encode_im2col(CUtensorMap* m, const void* ptr, int n, int h, int w, int c, 
   int lower[2] = {lc_w, lc_h};
   int upper[2] = {uc_w, uc_h};
   cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-  CUresult r = g_encode_im2col(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides,
-                               lower, upper, 64, pixels_per_col, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = device()->encode_im2col(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides,
+                                       lower, upper, 64, pixels_per_col, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeIm2col failed: %d (n=%d h=%d w=%d c=%d lc=%d,%d uc=%d,%d stride=%d ppc=%u)",
               (int)r, n, h, w, c, lc_h, lc_w, uc_h, uc_w, stride, pixels_per_col);
@@ -134,7 +92,7 @@ bool encode_im2col(CUtensorMap* m, const void* ptr, int n, int h, int w, int c, 
   }
   // Same driver quirk CUTLASS works around (cute/atom/copy_traits_sm90_im2col.hpp): tensors
   // smaller than 128 KiB need bit 21 of the second descriptor word cleared on drivers <= 13.1.
-  if (g_driver_version <= 13010 && (uint64_t)n * h * w * c * 2 < 131072)
+  if (device()->driver_version <= 13010 && (uint64_t)n * h * w * c * 2 < 131072)
     reinterpret_cast<uint64_t*>(m)[1] &= ~(1ull << 21);
   return true;
 }
@@ -191,7 +149,8 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, con
   }
   const int num_m = (p.M + p.tile_rows - 1) / p.tile_rows, num_n = (p.N + BN - 1) / BN;
   const long long total = (long long)num_m * num_n * p.splits * p.phases * (GemmVariant<VAR>::kBatch ? p.batch : 1);
-  const int grid = (int)(total < g_sm_count ? total : g_sm_count);
+  const int sms = device()->sms;
+  const int grid = (int)(total < sms ? total : sms);
   const int stat_bytes = (p.epi_flags & EPI_STATS) ? ((8 * p.N + 15) & ~15) : 0;
   int stages = 0, nb = 1;
   pick_smem_split<BN>(p, stat_bytes, &stages, &nb);
@@ -314,9 +273,9 @@ bool encode_batched(CUtensorMap* m, const void* ptr, uint64_t cols, uint64_t row
   cuuint64_t strides[2] = {cols * 2, rows * cols * 2};
   cuuint32_t box[3] = {box_cols, box_rows, 1u};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = device()->encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr,
+                                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled(batched) failed: %d (cols=%llu rows=%llu batch=%llu box=%u,%u ptr=%p)", (int)r,
               (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)batch, box_cols, box_rows, ptr);
@@ -329,13 +288,11 @@ bool encode_batched(CUtensorMap* m, const void* ptr, uint64_t cols, uint64_t row
 
 extern "C" {
 
-int saicv_sm_count(void) { return ensure_init() ? g_sm_count : 0; }
-
 int saicv_gemm_stats_rows(long long out_rows, int out_cols) {
   // number of partial rows a stats-fused forward GEMM writes = its grid size
   const int bn = pick_bn(out_cols);
   const long long tiles = ((out_rows + BM - 1) / BM) * ((out_cols + bn - 1) / bn);
-  const int sms = ensure_init() ? g_sm_count : 132;
+  const int sms = saicv_sm_count();
   return (int)(tiles < sms ? tiles : sms);
 }
 
@@ -351,7 +308,7 @@ int saicv_wgrad_splits(int out_rows, int out_cols, long long reduce_len) {
   const int bn = pick_bn(out_cols);
   const long long tiles = (long long)((out_rows + BM - 1) / BM) * ((out_cols + bn - 1) / bn);
   const long long num_kb = (reduce_len + BK - 1) / BK;
-  const int sms = g_sm_count > 0 ? g_sm_count : 132;
+  const int sms = saicv_sm_count();
   long long want = (2LL * sms + tiles - 1) / tiles;      // ~2 work items per SM
   long long max_by_k = num_kb / 8 > 0 ? num_kb / 8 : 1;  // at least 8 k-blocks per split
   long long s = want < max_by_k ? want : max_by_k;
@@ -366,7 +323,7 @@ int saicv_wgrad_splits(int out_rows, int out_cols, long long reduce_len) {
 int saicv_linear_fwd(const void* x, const void* w, const float* bias, const float* resid,
                      const float* row_scale, int rows_per_scale, float* stats_partial, void* y, int M, int N,
                      int K, int flags, int out_f32, void* stream) {
-  if (!ensure_init()) return 1;
+  if (!device()) return 1;
   if (!aligned16(x) || !aligned16(w) || !aligned16(y) || (K % 8) || (N % (out_f32 ? 4 : 8)))
     return set_error("saicv_linear_fwd: unaligned operand (M=%d N=%d K=%d)", M, N, K);
   const int bn = pick_bn(N);
@@ -393,7 +350,7 @@ int saicv_linear_fwd(const void* x, const void* w, const float* bias, const floa
 
 int saicv_linear_dgrad(const void* dy, const void* w, const float* resid, const void* gelu_pre, void* dx,
                        int M, int N, int K, int flags, int out_f32, void* stream) {
-  if (!ensure_init()) return 1;
+  if (!device()) return 1;
   if (!aligned16(dy) || !aligned16(w) || !aligned16(dx) || (K % 8) || (N % 8))
     return set_error("saicv_linear_dgrad: unaligned operand (M=%d N=%d K=%d)", M, N, K);
   // GEMM: D[M, K] = dy[M, N] * W[N, K]; reduction over N; B = W stored [N(red)][K(out)] -> MN-major
@@ -416,7 +373,7 @@ int saicv_linear_dgrad(const void* dy, const void* w, const float* resid, const 
 
 int saicv_linear_wgrad(const void* dy, const void* x, float* dw_partial, int M, int N, int K,
                        int splits, void* stream) {
-  if (!ensure_init()) return 1;
+  if (!device()) return 1;
   if (!aligned16(dy) || !aligned16(x) || !aligned16(dw_partial) || (K % 8) || (N % 8))
     return set_error("saicv_linear_wgrad: unaligned operand (M=%d N=%d K=%d)", M, N, K);
   // GEMM: D[N, K] = dy[M, N]^T * x[M, K]; reduction over M; both operands MN-major
@@ -440,7 +397,7 @@ static int conv_out(int in, int pad, int r, int stride) { return (in + 2 * pad -
 
 int saicv_conv_fprop(const void* x, const void* w, float* stats_partial, void* y, const saicv_conv_shape* cs,
                      int flags, void* stream) {
-  if (!ensure_init()) return 1;
+  if (!device()) return 1;
   if (cs->c % 64 || cs->k % 8 || !aligned16(x) || !aligned16(w) || !aligned16(y))
     return set_error("saicv_conv_fprop: needs c%%64==0, k%%8==0 and 16B-aligned pointers (c=%d k=%d)", cs->c, cs->k);
   const int P = conv_out(cs->h, cs->pad, cs->r, cs->stride), Q = conv_out(cs->w, cs->pad, cs->s, cs->stride);
@@ -468,7 +425,7 @@ int saicv_conv_fprop(const void* x, const void* w, float* stats_partial, void* y
 
 int saicv_conv_dgrad(const void* dy, const void* w, const void* add, const uint32_t* mask_bits, void* dx,
                      const saicv_conv_shape* cs, void* stream) {
-  if (!ensure_init()) return 1;
+  if (!device()) return 1;
   if (cs->c % 64 || cs->k % 64 || !aligned16(dy) || !aligned16(w) || !aligned16(dx))
     return set_error("saicv_conv_dgrad: needs c%%64==0 and k%%64==0 (c=%d k=%d)", cs->c, cs->k);
   if (cs->stride == 2) return conv_dgrad_phases(dy, w, add, mask_bits, dx, cs, (cudaStream_t)stream);
@@ -497,7 +454,7 @@ int saicv_conv_dgrad(const void* dy, const void* w, const void* add, const uint3
 
 int saicv_conv_wgrad(const void* dy, const void* x, float* dw_partial, const saicv_conv_shape* cs,
                      int splits, void* stream) {
-  if (!ensure_init()) return 1;
+  if (!device()) return 1;
   if (cs->c % 64 || cs->k % 8 || !aligned16(dy) || !aligned16(x) || !aligned16(dw_partial))
     return set_error("saicv_conv_wgrad: needs c%%64==0, k%%8==0 (c=%d k=%d)", cs->c, cs->k);
   const int P = conv_out(cs->h, cs->pad, cs->r, cs->stride), Q = conv_out(cs->w, cs->pad, cs->s, cs->stride);
@@ -536,7 +493,7 @@ int saicv_conv_wgrad(const void* dy, const void* x, float* dw_partial, const sai
 // m and n are multiples of 8 (pad with zeros: zero rows / columns stay zero).  out must not alias x or y.
 int saicv_ns_gemm(int mode, const void* x, const void* y, void* out, int batch, int m, int n, float alpha, float beta,
                   void* stream) {
-  if (!ensure_init()) return 1;
+  if (!device()) return 1;
   if (mode < 0 || mode > 2 || batch <= 0 || m <= 0 || n <= 0 || (m % 8) || (n % 8) || !aligned16(x) || !aligned16(out) ||
       (mode == 2 && (!y || !aligned16(y))))
     return set_error("saicv_ns_gemm: bad arguments (mode=%d batch=%d m=%d n=%d; m, n must be multiples of 8, pointers "

@@ -174,10 +174,6 @@ mix_soft_label_kernel(const long long* __restrict__ labels, float* __restrict__ 
   }
 }
 
-int grid_for(long long items) {
-  return (int)((items + kInThreads - 1) / kInThreads < 132 * 16 ? (items + kInThreads - 1) / kInThreads : 132 * 16);
-}
-
 }  // namespace
 }  // namespace saicv
 
@@ -230,15 +226,15 @@ extern "C" int saicv_u8_mix_erase_norm(const void* in, float* out, int n, int h,
   const long long hw = (long long)h * w, pairs = n / 2;
   if (hw % 4 == 0 && ((uintptr_t)in & 3) == 0 && ((uintptr_t)out & 15) == 0) {
     const long long groups = pairs * (hw / 4);
-    u8_mix_erase_norm_vec_kernel<<<grid_for(groups), kInThreads, 0, st>>>(reinterpret_cast<const uint32_t*>(in), out, groups, n,
+    u8_mix_erase_norm_vec_kernel<<<grid_1d(groups, kInThreads), kInThreads, 0, st>>>(reinterpret_cast<const uint32_t*>(in), out, groups, n,
                                                                           (int)(hw / 4), w, a, er);
     if (check_launch("u8_mix_erase_norm_vec_kernel")) return 1;
   } else {
-    u8_mix_erase_norm_kernel<<<grid_for(pairs * hw), kInThreads, 0, st>>>(reinterpret_cast<const uint8_t*>(in), out, pairs * hw, n,
+    u8_mix_erase_norm_kernel<<<grid_1d(pairs * hw, kInThreads), kInThreads, 0, st>>>(reinterpret_cast<const uint8_t*>(in), out, pairs * hw, n,
                                                                          hw, w, a, er);
     if (check_launch("u8_mix_erase_norm_kernel")) return 1;
   }
-  mix_soft_label_kernel<<<grid_for((long long)n * num_classes), kInThreads, 0, st>>>(labels, soft, n, num_classes, on_value,
+  mix_soft_label_kernel<<<grid_1d((long long)n * num_classes, kInThreads), kInThreads, 0, st>>>(labels, soft, n, num_classes, on_value,
                                                                                      off_value, a.lam, a.lam1);
   return check_launch("mix_soft_label_kernel");
 }
@@ -255,11 +251,9 @@ extern "C" int saicv_u8_nhwc_to_nchw_norm(const void* in, float* out, int n, int
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (hw % 4 == 0 && ((uintptr_t)in & 3) == 0 && ((uintptr_t)out & 15) == 0) {
     const long long groups = pixels / 4;
-    const int blocks = (int)((groups + kInThreads - 1) / kInThreads < 132 * 16 ? (groups + kInThreads - 1) / kInThreads : 132 * 16);
-    u8_nhwc_to_nchw_norm_vec_kernel<<<blocks, kInThreads, 0, st>>>(reinterpret_cast<const uint32_t*>(in), out, groups, (int)(hw / 4), nm);
+    u8_nhwc_to_nchw_norm_vec_kernel<<<grid_1d(groups, kInThreads), kInThreads, 0, st>>>(reinterpret_cast<const uint32_t*>(in), out, groups, (int)(hw / 4), nm);
     return check_launch("u8_nhwc_to_nchw_norm_vec_kernel");
   }
-  const int blocks = (int)((pixels + kInThreads - 1) / kInThreads < 132 * 16 ? (pixels + kInThreads - 1) / kInThreads : 132 * 16);
-  u8_nhwc_to_nchw_norm_kernel<<<blocks, kInThreads, 0, st>>>(reinterpret_cast<const uint8_t*>(in), out, pixels, hw, nm);
+  u8_nhwc_to_nchw_norm_kernel<<<grid_1d(pixels, kInThreads), kInThreads, 0, st>>>(reinterpret_cast<const uint8_t*>(in), out, pixels, hw, nm);
   return check_launch("u8_nhwc_to_nchw_norm_kernel");
 }

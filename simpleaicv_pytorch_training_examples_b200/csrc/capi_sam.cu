@@ -17,14 +17,6 @@
 namespace saicv {
 namespace {
 
-
-int grid1d(long long items, int per_block = 256, int cap = 132 * 16) {
-  long long b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > cap) b = cap;
-  return (int)b;
-}
-
 // windows[(b*nwy+wy)*nwx+wx][iy*ws+ix][c] = x[b][wy*ws+iy][wx*ws+ix][c]  (0 outside H x W)
 __global__ void window_partition_kernel(const V8* __restrict__ x, V8* __restrict__ win, int B, int H, int W, int C, int ws, int nwy,
                                         int nwx) {
@@ -242,7 +234,7 @@ extern "C" {
 int saicv_window_partition(const void* x, void* windows, int b, int h, int w, int c, int ws, void* stream) {
   if (c % 8 || ws < 1) return set_error("saicv_window_partition: C %% 8 != 0 or bad window size");
   const int nwy = (h + ws - 1) / ws, nwx = (w + ws - 1) / ws;
-  window_partition_kernel<<<grid1d((long long)b * nwy * nwx * ws * ws * (c / 8)), 256, 0, ST>>>(
+  window_partition_kernel<<<grid_1d((long long)b * nwy * nwx * ws * ws * (c / 8)), 256, 0, ST>>>(
       reinterpret_cast<const V8*>(x), reinterpret_cast<V8*>(windows), b, h, w, c, ws, nwy, nwx);
   return check_launch("window_partition_kernel");
 }
@@ -250,14 +242,14 @@ int saicv_window_partition(const void* x, void* windows, int b, int h, int w, in
 int saicv_window_unpartition(const void* windows, void* x, int b, int h, int w, int c, int ws, void* stream) {
   if (c % 8 || ws < 1) return set_error("saicv_window_unpartition: C %% 8 != 0 or bad window size");
   const int nwy = (h + ws - 1) / ws, nwx = (w + ws - 1) / ws;
-  window_unpartition_kernel<<<grid1d((long long)b * h * w * (c / 8)), 256, 0, ST>>>(
+  window_unpartition_kernel<<<grid_1d((long long)b * h * w * (c / 8)), 256, 0, ST>>>(
       reinterpret_cast<const V8*>(windows), reinterpret_cast<V8*>(x), b, h, w, c, ws, nwy, nwx);
   return check_launch("window_unpartition_kernel");
 }
 
 int saicv_add_pos_embed(float* x, const float* pos, int b, long long per_batch, void* stream) {
   if (per_batch % 4) return set_error("saicv_add_pos_embed: per-batch size %% 4 != 0");
-  add_pos_kernel<<<grid1d((long long)b * per_batch / 4), 256, 0, ST>>>(reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(pos),
+  add_pos_kernel<<<grid_1d((long long)b * per_batch / 4), 256, 0, ST>>>(reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(pos),
                                                                       per_batch / 4, (long long)b * per_batch / 4);
   return check_launch("add_pos_kernel");
 }
@@ -270,14 +262,14 @@ static int relpos_check(const char* who, int hd, int sh, int sw, int dqk, int ni
 
 int saicv_relpos_pack_q(const void* qkv, void* qc, int bw, int heads, int hd, int l, void* stream) {
   if (hd % 8) return set_error("saicv_relpos_pack_q: hd %% 8 != 0");
-  relpos_packq_kernel<<<grid1d((long long)bw * heads * l * (hd / 8)), 256, 0, ST>>>(
+  relpos_packq_kernel<<<grid_1d((long long)bw * heads * l * (hd / 8)), 256, 0, ST>>>(
       reinterpret_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<__nv_bfloat16*>(qc), bw, heads, l, hd);
   return check_launch("relpos_packq_kernel");
 }
 
 int saicv_relpos_table(const float* rel_pos_h, const float* rel_pos_w, void* rtab, int sh, int sw, int nip, int hd, void* stream) {
   if (nip < 2 * sh - 1 + 2 * sw - 1) return set_error("saicv_relpos_table: nip too small");
-  relpos_table_kernel<<<grid1d((long long)nip * hd), 256, 0, ST>>>(rel_pos_h, rel_pos_w, reinterpret_cast<__nv_bfloat16*>(rtab), 2 * sh - 1,
+  relpos_table_kernel<<<grid_1d((long long)nip * hd), 256, 0, ST>>>(rel_pos_h, rel_pos_w, reinterpret_cast<__nv_bfloat16*>(rtab), 2 * sh - 1,
                                                                  2 * sw - 1, nip, hd);
   return check_launch("relpos_table_kernel");
 }
@@ -285,7 +277,7 @@ int saicv_relpos_table(const float* rel_pos_h, const float* rel_pos_w, void* rta
 int saicv_relpos_gather(const void* qkv, const void* t, void* qe, void* ke, int bw, int heads, int hd, int sh, int sw, int dqk, int nip,
                         float scale, void* stream) {
   if (int e = relpos_check("saicv_relpos_gather", hd, sh, sw, dqk, nip)) return e;
-  relpos_gather_kernel<<<grid1d((long long)bw * heads * sh * sw * (dqk / 8)), 256, 0, ST>>>(
+  relpos_gather_kernel<<<grid_1d((long long)bw * heads * sh * sw * (dqk / 8)), 256, 0, ST>>>(
       reinterpret_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<const __nv_bfloat16*>(t), reinterpret_cast<__nv_bfloat16*>(qe),
       reinterpret_cast<__nv_bfloat16*>(ke), bw, heads, sh, sw, hd, dqk, nip, scale);
   return check_launch("relpos_gather_kernel");
@@ -293,7 +285,7 @@ int saicv_relpos_gather(const void* qkv, const void* t, void* qe, void* ke, int 
 
 int saicv_relpos_shift(const void* dqe, void* ef, int bw, int heads, int hd, int sh, int sw, int dqk, int nip, void* stream) {
   if (int e = relpos_check("saicv_relpos_shift", hd, sh, sw, dqk, nip)) return e;
-  relpos_shift_kernel<<<grid1d((long long)bw * heads * sh * sw * (nip / 8)), 256, 0, ST>>>(
+  relpos_shift_kernel<<<grid_1d((long long)bw * heads * sh * sw * (nip / 8)), 256, 0, ST>>>(
       reinterpret_cast<const __nv_bfloat16*>(dqe), reinterpret_cast<__nv_bfloat16*>(ef), bw, heads, sh, sw, hd, dqk, nip);
   return check_launch("relpos_shift_kernel");
 }
@@ -301,7 +293,7 @@ int saicv_relpos_shift(const void* dqe, void* ef, int bw, int heads, int hd, int
 int saicv_relpos_dq_combine(const void* dqe, const float* dqx, void* dqkv, int bw, int heads, int hd, int l, int dqk, float scale,
                             void* stream) {
   if (hd % 8 || dqk % 8) return set_error("saicv_relpos_dq_combine: hd, dqk must be multiples of 8");
-  relpos_dq_combine_kernel<<<grid1d((long long)bw * heads * l * (hd / 8)), 256, 0, ST>>>(
+  relpos_dq_combine_kernel<<<grid_1d((long long)bw * heads * l * (hd / 8)), 256, 0, ST>>>(
       reinterpret_cast<const __nv_bfloat16*>(dqe), dqx, reinterpret_cast<__nv_bfloat16*>(dqkv), bw, heads, l, hd, dqk, scale);
   return check_launch("relpos_dq_combine_kernel");
 }

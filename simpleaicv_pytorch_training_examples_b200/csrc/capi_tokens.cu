@@ -87,11 +87,6 @@ token_fill_grad_kernel(const float* __restrict__ dout, const int* __restrict__ i
   }
 }
 
-int blocks_for(long long items) {
-  long long b = (items + kTokThreads - 1) / kTokThreads;
-  return (int)(b < 1 ? 1 : b > 132 * 16 ? 132 * 16 : b);
-}
-
 }  // namespace
 }  // namespace saicv
 
@@ -104,7 +99,7 @@ int saicv_token_gather_fwd(const float* src, long long src_rows, const int* idx,
                            const int* pos_idx, float* out, int b, int r, int c, void* stream) {
   if (c % 4) return set_error("saicv_token_gather_fwd: C %% 4 != 0");
   const long long rows = (long long)b * r;
-  token_gather_fwd_kernel<<<blocks_for(rows * (c / 4)), kTokThreads, 0, ST>>>(
+  token_gather_fwd_kernel<<<grid_1d(rows * (c / 4), kTokThreads), kTokThreads, 0, ST>>>(
       reinterpret_cast<const float4*>(src), src_rows, idx, reinterpret_cast<const float4*>(fill), reinterpret_cast<const float4*>(pos),
       pos_idx, reinterpret_cast<float4*>(out), rows, r, c / 4);
   return check_launch("token_gather_fwd_kernel");
@@ -121,10 +116,10 @@ int saicv_token_gather_bwd(const float* dout, const int* idx, void* dsrc, int ds
   const long long rows = (long long)b * r;
   if (dsrc != nullptr) {
     if (dsrc_bf16)
-      token_gather_bwd_kernel<true><<<blocks_for(rows * (c / 4)), kTokThreads, 0, ST>>>(reinterpret_cast<const float4*>(dout), idx, dsrc,
+      token_gather_bwd_kernel<true><<<grid_1d(rows * (c / 4), kTokThreads), kTokThreads, 0, ST>>>(reinterpret_cast<const float4*>(dout), idx, dsrc,
                                                                                          src_rows, rows, r, c / 4);
     else
-      token_gather_bwd_kernel<false><<<blocks_for(rows * (c / 4)), kTokThreads, 0, ST>>>(reinterpret_cast<const float4*>(dout), idx, dsrc,
+      token_gather_bwd_kernel<false><<<grid_1d(rows * (c / 4), kTokThreads), kTokThreads, 0, ST>>>(reinterpret_cast<const float4*>(dout), idx, dsrc,
                                                                                           src_rows, rows, r, c / 4);
     if (check_launch("token_gather_bwd_kernel")) return 1;
   }

@@ -417,13 +417,6 @@ __global__ void bn_bwd_apply_generic_kernel(const void* __restrict__ x, int x_f3
     store8(dx, i * 8, dx_f32 != 0, o);
   }
 }
-__global__ void bn_param_grad_generic_kernel(const float* __restrict__ sums, float* __restrict__ dgamma, float* __restrict__ dbeta,
-                                             int C, int accumulate) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  dbeta[c] = accumulate ? dbeta[c] + sums[c] : sums[c];
-  dgamma[c] = accumulate ? dgamma[c] + sums[C + c] : sums[C + c];
-}
 
 // ----------------------------------------------------------------------------- NHWC im2col / col2im
 // cols[(n*P+p)*Q+q][(r*S+s)*C + c] = x[n][p*stride-pad+r][q*stride-pad+s][c]   (0 outside)
@@ -480,17 +473,6 @@ __global__ void col2im_nhwc_kernel(const __nv_bfloat16* __restrict__ dcols, __nv
   }
 }
 
-int grid1d(long long items, int per_block = 256, int cap = 132 * 16) {
-  long long b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > cap) b = cap;
-  return (int)b;
-}
-int pow2_ge(int v) {
-  int p = 1;
-  while (p < v) p <<= 1;
-  return p;
-}
 // slab geometry of the column reductions: tx_count threads across 8-column vectors, rows split over <= 264 blocks
 void slab(long long rows, int C, int* tx_count, long long* rows_per_block, int* nblk) {
   const int vpr = C / 8;
@@ -519,7 +501,7 @@ int saicv_dwconv_fwd(const void* x, const float* w, const float* bias, void* y, 
                      int relu, int flip, void* stream) {
   if (c % 8) return set_error("saicv_dwconv_fwd: C %% 8 != 0");
   const long long npix = (long long)n * h * wd;
-  dim3 grid((unsigned)grid1d(npix, 32, 132 * 8), (unsigned)((c + 63) / 64));
+  dim3 grid((unsigned)grid_1d(npix, 32, 132 * 8), (unsigned)((c + 63) / 64));
   const __nv_bfloat16* xx = reinterpret_cast<const __nv_bfloat16*>(x);
   __nv_bfloat16* yy = reinterpret_cast<__nv_bfloat16*>(y);
   switch (k) {
@@ -537,7 +519,7 @@ int saicv_dwconv_dgrad_masked(const void* dy, const float* w, const void* mask, 
   if (!mask) return set_error("saicv_dwconv_dgrad_masked: mask is NULL");
   if (k != 7) return set_error("saicv_dwconv_dgrad_masked: kernel size %d (7)", k);
   const long long npix = (long long)n * h * wd;
-  dim3 grid((unsigned)grid1d(npix, 32, 132 * 8), (unsigned)((c + 63) / 64));
+  dim3 grid((unsigned)grid_1d(npix, 32, 132 * 8), (unsigned)((c + 63) / 64));
   dwconv_kernel<7, true><<<grid, 256, 0, ST>>>(reinterpret_cast<const __nv_bfloat16*>(dy), w, nullptr,
                                                reinterpret_cast<__nv_bfloat16*>(dx), n, h, wd, c, 1, 0, 1,
                                                reinterpret_cast<const __nv_bfloat16*>(mask));
@@ -546,23 +528,19 @@ int saicv_dwconv_dgrad_masked(const void* dy, const float* w, const void* mask, 
 
 int saicv_avgpool_stream_fwd(const void* x, int x_f32, void* y, int n, int hw, int c, void* stream) {
   if (c % 8) return set_error("saicv_avgpool_stream_fwd: C %% 8 != 0");
-  avgpool_stream_fwd_kernel<<<grid1d((long long)n * (c / 8), 128), 128, 0, ST>>>(x, x_f32, reinterpret_cast<__nv_bfloat16*>(y), n,
+  avgpool_stream_fwd_kernel<<<grid_1d((long long)n * (c / 8), 128), 128, 0, ST>>>(x, x_f32, reinterpret_cast<__nv_bfloat16*>(y), n,
                                                                                  hw, c);
   return check_launch("avgpool_stream_fwd_kernel");
 }
 
 int saicv_avgpool_stream_bwd(const void* dy, void* dx, int dx_f32, int n, int hw, int c, void* stream) {
   if (c % 8) return set_error("saicv_avgpool_stream_bwd: C %% 8 != 0");
-  avgpool_stream_bwd_kernel<<<grid1d((long long)n * hw * (c / 8)), 256, 0, ST>>>(reinterpret_cast<const __nv_bfloat16*>(dy), dx,
+  avgpool_stream_bwd_kernel<<<grid_1d((long long)n * hw * (c / 8)), 256, 0, ST>>>(reinterpret_cast<const __nv_bfloat16*>(dy), dx,
                                                                                  dx_f32, n, hw, c);
   return check_launch("avgpool_stream_bwd_kernel");
 }
 
-int saicv_dwconv_wgrad_blocks(long long npix) {
-  long long b = (npix + 255) / 256;
-  if (b > 132) b = 132;
-  return (int)(b < 1 ? 1 : b);
-}
+int saicv_dwconv_wgrad_blocks(long long npix) { return grid_1d(npix, 256, 132); }
 
 int saicv_dwconv_wgrad(const void* dy, const void* x, float* partial, float* dw, int n, int h, int wd, int c, int k, int dil,
                        int accumulate, void* stream) {
@@ -586,13 +564,13 @@ int saicv_dwconv_wgrad(const void* dy, const void* x, float* partial, float* dw,
 
 int saicv_mul_bf16(const void* a, const void* b, void* out, long long n, void* stream) {
   if (n % 8) return set_error("saicv_mul_bf16: n %% 8 != 0");
-  mul_kernel<<<grid1d(n / 8), 256, 0, ST>>>(reinterpret_cast<const V8*>(a), reinterpret_cast<const V8*>(b), reinterpret_cast<V8*>(out), n / 8);
+  mul_kernel<<<grid_1d(n / 8), 256, 0, ST>>>(reinterpret_cast<const V8*>(a), reinterpret_cast<const V8*>(b), reinterpret_cast<V8*>(out), n / 8);
   return check_launch("mul_kernel");
 }
 
 int saicv_gate_bwd(const void* dg, const void* c1, const void* dlk, const void* p1, void* out, long long n, void* stream) {
   if (n % 8) return set_error("saicv_gate_bwd: n %% 8 != 0");
-  gate_bwd_kernel<<<grid1d(n / 8), 256, 0, ST>>>(reinterpret_cast<const V8*>(dg), reinterpret_cast<const V8*>(c1),
+  gate_bwd_kernel<<<grid_1d(n / 8), 256, 0, ST>>>(reinterpret_cast<const V8*>(dg), reinterpret_cast<const V8*>(c1),
                                                  reinterpret_cast<const V8*>(dlk), reinterpret_cast<const V8*>(p1),
                                                  reinterpret_cast<V8*>(out), n / 8);
   return check_launch("gate_bwd_kernel");
@@ -602,7 +580,7 @@ int saicv_ls_residual_fwd(const void* x, int x_f32, const void* branch, const vo
                           int rows_per_scale, float* out, long long rows, int c, void* stream) {
   if (c % 8) return set_error("saicv_ls_residual_fwd: C %% 8 != 0");
   if (row_scale && rows_per_scale <= 0) return set_error("saicv_ls_residual_fwd: rows_per_scale must be > 0");
-  ls_residual_fwd_kernel<<<grid1d(rows * (c / 8)), 256, 0, ST>>>(x, x_f32, reinterpret_cast<const __nv_bfloat16*>(branch),
+  ls_residual_fwd_kernel<<<grid_1d(rows * (c / 8)), 256, 0, ST>>>(x, x_f32, reinterpret_cast<const __nv_bfloat16*>(branch),
                                                                  reinterpret_cast<const __nv_bfloat16*>(shortcut), ls, row_scale,
                                                                  rows_per_scale, out, rows, c);
   return check_launch("ls_residual_fwd_kernel");
@@ -641,7 +619,7 @@ int saicv_bn_generic_partial_rows(long long rows, int c) {
 int saicv_bn_apply_generic(const void* x, int x_f32, const float* scale_shift, void* out, int out_f32, long long rows, int c,
                            void* stream) {
   if (c % 8) return set_error("saicv_bn_apply_generic: C %% 8 != 0");
-  bn_apply_generic_kernel<<<grid1d(rows * (c / 8)), 256, 0, ST>>>(x, x_f32, scale_shift, out, out_f32, rows, c);
+  bn_apply_generic_kernel<<<grid_1d(rows * (c / 8)), 256, 0, ST>>>(x, x_f32, scale_shift, out, out_f32, rows, c);
   return check_launch("bn_apply_generic_kernel");
 }
 
@@ -655,17 +633,16 @@ int saicv_bn_bwd_generic(const void* x, int x_f32, const void* g, int g_f32, con
   bn_colreduce_generic_kernel<1><<<nblk, 256, 0, ST>>>(x, x_f32, g, g_f32, saved, partial, rows, c, tx, rpb);
   if (int e = check_launch("bn_colreduce_generic_kernel")) return e;
   if (int e = saicv_reduce_partials(partial, sums, nblk, 2LL * c, 0, stream)) return e;
-  bn_bwd_apply_generic_kernel<<<grid1d(rows * (c / 8)), 256, 0, ST>>>(x, x_f32, g, g_f32, saved, gamma, sums, dres, dx, dx_f32,
+  bn_bwd_apply_generic_kernel<<<grid_1d(rows * (c / 8)), 256, 0, ST>>>(x, x_f32, g, g_f32, saved, gamma, sums, dres, dx, dx_f32,
                                                                       rows, c, 1.0f / (float)rows);
   if (int e = check_launch("bn_bwd_apply_generic_kernel")) return e;
-  bn_param_grad_generic_kernel<<<(c + 127) / 128, 128, 0, ST>>>(sums, dgamma, dbeta, c, accumulate);
-  return check_launch("bn_param_grad_generic_kernel");
+  return bn_param_grad(sums, dgamma, dbeta, c, accumulate, ST);
 }
 
 int saicv_im2col_nhwc(const void* x, void* cols, int n, int h, int w, int c, int k, int stride, int pad, void* stream) {
   if (c % 8) return set_error("saicv_im2col_nhwc: C %% 8 != 0");
   const int P = (h + 2 * pad - k) / stride + 1, Q = (w + 2 * pad - k) / stride + 1;
-  im2col_nhwc_kernel<<<grid1d((long long)n * P * Q * k * k * (c / 8)), 256, 0, ST>>>(
+  im2col_nhwc_kernel<<<grid_1d((long long)n * P * Q * k * k * (c / 8)), 256, 0, ST>>>(
       reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<__nv_bfloat16*>(cols), n, h, w, c, k, stride, pad, P, Q);
   return check_launch("im2col_nhwc_kernel");
 }
@@ -673,7 +650,7 @@ int saicv_im2col_nhwc(const void* x, void* cols, int n, int h, int w, int c, int
 int saicv_col2im_nhwc(const void* dcols, void* dx, int n, int h, int w, int c, int k, int stride, int pad, void* stream) {
   if (c % 8) return set_error("saicv_col2im_nhwc: C %% 8 != 0");
   const int P = (h + 2 * pad - k) / stride + 1, Q = (w + 2 * pad - k) / stride + 1;
-  col2im_nhwc_kernel<<<grid1d((long long)n * h * w * (c / 8)), 256, 0, ST>>>(
+  col2im_nhwc_kernel<<<grid_1d((long long)n * h * w * (c / 8)), 256, 0, ST>>>(
       reinterpret_cast<const __nv_bfloat16*>(dcols), reinterpret_cast<__nv_bfloat16*>(dx), n, h, w, c, k, stride, pad, P, Q);
   return check_launch("col2im_nhwc_kernel");
 }

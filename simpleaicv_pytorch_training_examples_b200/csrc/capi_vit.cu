@@ -74,7 +74,7 @@ ln_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamma, cons
 
 // dx = dres + rstd*(dxhat - mean(dxhat) - xhat*mean(dxhat*xhat)), dxhat = dy*gamma; dgamma/dbeta
 // accumulated per warp in registers, folded through shared memory in a fixed order into one
-// partial row per block ([gridDim.x][2][C]); ln_fold_kernel sums the rows, again in a fixed order,
+// partial row per block ([gridDim.x][2][C]); fold_partials sums the rows, again in a fixed order,
 // so the parameter gradients are bit-reproducible (no atomics).
 template <int NCH>
 __global__ void __launch_bounds__(256)
@@ -139,26 +139,6 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restrict__ x,
       partials[((long long)blockIdx.x * 2 + pass) * C + c] = s;
     }
   }
-}
-
-// dgamma / dbeta (+)= sum over the per-block partial rows, fixed order: 8 columns x 32 row groups per block (the <= 264
-// partial rows are spread over 32 threads per column so the fold is a handful of loads deep instead of a 264-long chain)
-__global__ void ln_fold_kernel(const float* __restrict__ partials, float* __restrict__ dgamma, float* __restrict__ dbeta,
-                               int nblk, int C, int accumulate) {
-  __shared__ float sm[32][9];
-  const int cl = threadIdx.x & 7, grp = threadIdx.x >> 3;
-  const int j = blockIdx.x * 8 + cl;  // 0 .. 2C-1
-  float s = 0.f;
-  if (j < 2 * C)
-    for (int b = grp; b < nblk; b += 32) s += partials[(long long)b * 2 * C + j];
-  sm[grp][cl] = s;
-  __syncthreads();
-  if (grp != 0 || j >= 2 * C) return;
-  float t = 0.f;
-#pragma unroll
-  for (int g = 0; g < 32; ++g) t += sm[g][cl];
-  float* dst = j < C ? dgamma + j : dbeta + (j - C);
-  *dst = accumulate ? *dst + t : t;
 }
 
 // ----------------------------------------------------------------------------- GELU (exact, erf)
@@ -260,13 +240,6 @@ __global__ void token_pool_bwd_kernel(const float* __restrict__ dpooled, float* 
   }
 }
 
-int grid_1d(long long items, int per_block = 256, int cap = 132 * 16) {
-  long long b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > cap) b = cap;
-  return (int)b;
-}
-
 }  // namespace
 }  // namespace saicv
 
@@ -311,8 +284,7 @@ int saicv_layernorm_bwd(const void* dy, const float* x, const float* gamma, cons
     default: return set_error("saicv_layernorm_bwd: unsupported width %d", c);
   }
   if (int e = check_launch("ln_bwd_kernel")) return e;
-  ln_fold_kernel<<<(2 * c + 7) / 8, 256, 0, ST>>>(partials, dgamma, dbeta, grid, c, accumulate);
-  return check_launch("ln_fold_kernel");
+  return fold_partials(partials, grid, 2 * c, dgamma, dbeta, c, accumulate, ST);
 }
 
 int saicv_gelu_fwd(const void* u, void* h, long long n, void* stream) {

@@ -97,7 +97,9 @@ class _Block:
         t['ln1'], t['st1'] = ops.layernorm_fwd(x, blk.norm1.weight.detach(), blk.norm1.bias.detach(), blk.norm1.eps)
         qkv = t['qkv'] = self.qkv.fwd(t['ln1'])
         ops.rope_qk(qkv, rope[0], rope[1], b, l, self.heads, d)
-        t['att'], t['lse'] = ops.attention_fwd(qkv, b, l, self.heads, d, self.scale)
+        t['att'] = torch.empty(b * l, c, device=x.device, dtype=torch.bfloat16)
+        (out,) = ops.head_views(t['att'], b, l, self.heads, d)
+        _, t['lse'] = ops.attn_fwd(*ops.head_views(qkv, b, l, self.heads, d), self.scale, out=out)
         t['pa'] = self.proj.fwd(t['att'])
         x = t['x_mid'] = ops.ls_residual_fwd(x, t['pa'], None, blk.ls1.gamma.detach())
         ln2, t['st2'] = ops.layernorm_fwd(x, blk.norm2.weight.detach(), blk.norm2.bias.detach(), blk.norm2.eps)
@@ -137,7 +139,10 @@ class _Block:
         with sink.grad(ls1) as (acc, buf):
             dpa = ops.ls_residual_bwd(dx, t['pa'], None, ls1.detach(), buf, accumulate=acc)
         datt = self.proj.bwd(dpa, t['att'], sink)
-        dqkv = ops.attention_bwd(t['qkv'], t['att'], datt, t['lse'], b, l, self.heads, d, self.scale)
+        dqkv = torch.empty_like(t['qkv'])
+        q, k, v, out, dout, dq, dk, dv = (view for buf in (t['qkv'], t['att'], datt, dqkv)
+                                          for view in ops.head_views(buf, b, l, self.heads, d))
+        ops.attn_bwd(q, k, v, out, t['lse'], dout, self.scale, dq, dk, dv)
         ops.rope_qk(dqkv, rope[0], rope[1], b, l, self.heads, d, backward=True)
         dln1 = self.qkv.bwd(dqkv, t['ln1'], sink)
         return layernorm_bwd(blk.norm1, dln1, t['x_in'], t['st1'], sink, dres=dx, want_bf16=want_bf16)

@@ -63,13 +63,10 @@ class _Block:
         t['x_in'], t['p'], t['seeds'], t['sb'] = x, p, seeds, sb
         t['ln1'], t['st1'] = ops.layernorm_fwd(x, blk.norm1.weight.detach(), blk.norm1.bias.detach(), blk.norm1.eps)
         t['qkv'] = self.qkv.fwd(t['ln1'])
-        if p > 0.:
-            q, k, v = (t['qkv'].view(b, l, 3, self.heads, d)[:, :, i].permute(0, 2, 1, 3) for i in range(3))
-            t['att'] = torch.empty(b * l, c, device=x.device, dtype=torch.bfloat16)
-            _, t['lse'] = ops.attn_fwd(q, k, v, self.scale, out=t['att'].view(b, l, self.heads, d).permute(0, 2, 1, 3),
-                                       dropout_p=p, dropout_seed=seeds[0], dropout_seed_base=sb)
-        else:
-            t['att'], t['lse'] = ops.attention_fwd(t['qkv'], b, l, self.heads, d, self.scale)
+        t['att'] = torch.empty(b * l, c, device=x.device, dtype=torch.bfloat16)
+        (out,) = ops.head_views(t['att'], b, l, self.heads, d)
+        _, t['lse'] = ops.attn_fwd(*ops.head_views(t['qkv'], b, l, self.heads, d), self.scale, out=out, dropout_p=p,
+                                   dropout_seed=seeds[0] if p > 0. else 0, dropout_seed_base=sb)
         s1 = t['s1'] = scales[0] if scales is not None else drop_path_scale(self.drop_path, b, training, x.device)
         if p > 0.:
             x = ops.dropout(self.proj.fwd(t['att']), p, seeds[1], resid=x, row_scale=s1, elems_per_scale=l * c, seed_base=sb)
@@ -104,15 +101,11 @@ class _Block:
         # ---- attention branch
         g = ops.dropout(dxb, p, seeds[1], seed_base=sb) if p > 0. else dxb
         datt = self.proj.bwd(g, t['att'], sink)
-        if p > 0.:
-            c = dx.shape[1]
-            qv, kv, vv = (t['qkv'].view(b, l, 3, self.heads, d)[:, :, i].permute(0, 2, 1, 3) for i in range(3))
-            dqkv = torch.empty_like(t['qkv'])
-            dq, dk, dv = (dqkv.view(b, l, 3, self.heads, d)[:, :, i].permute(0, 2, 1, 3) for i in range(3))
-            ops.attn_bwd(qv, kv, vv, t['att'].view(b, l, self.heads, d).permute(0, 2, 1, 3), t['lse'],
-                         datt.view(b, l, self.heads, d).permute(0, 2, 1, 3), self.scale, dq, dk, dv, dropout_p=p, dropout_seed=seeds[0], dropout_seed_base=sb)
-        else:
-            dqkv = ops.attention_bwd(t['qkv'], t['att'], datt, t['lse'], b, l, self.heads, d, self.scale)
+        dqkv = torch.empty_like(t['qkv'])
+        q, k, v, out, dout, dq, dk, dv = (view for buf in (t['qkv'], t['att'], datt, dqkv)
+                                          for view in ops.head_views(buf, b, l, self.heads, d))
+        ops.attn_bwd(q, k, v, out, t['lse'], dout, self.scale, dq, dk, dv, dropout_p=p,
+                     dropout_seed=seeds[0] if p > 0. else 0, dropout_seed_base=sb)
         dln1 = self.qkv.bwd(dqkv, t['ln1'], sink)
         return layernorm_bwd(blk.norm1, dln1, t['x_in'], t['st1'], sink, dres=dx, scale=next_scale, rows_per_scale=l)
 

@@ -497,22 +497,11 @@ def token_pool_bwd(dpooled, l, mean_pool, dx=None, dx_bf16=None, bf16_row_scale=
     return dx
 
 
-def attention_fwd(qkv, b, l, h, d, scale, out=None, lse=None):
-    """Packed-qkv attention of the ViT blocks: qkv bf16 [b*l, 3*h*d] ([b][l][3][h][d]) -> out bf16 [b*l, h*d]."""
-    if out is None:
-        out = torch.empty(b * l, h * d, device=qkv.device, dtype=torch.bfloat16)
-    if lse is None:
-        lse = torch.empty(b, h, l, device=qkv.device, dtype=torch.float32)
-    _lib.call('saicv_attention_fwd', _p(qkv), _p(out), _p(lse), b, l, h, d, scale, _stream())
-    return out, lse
-
-
-def attention_bwd(qkv, out, dout, lse, b, l, h, d, scale, dqkv=None):
-    if dqkv is None:
-        dqkv = torch.empty_like(qkv)
-    delta = torch.empty(b, h, l, device=qkv.device, dtype=torch.float32)
-    _lib.call('saicv_attention_bwd', _p(qkv), _p(out), _p(dout), _p(lse), _p(delta), _p(dqkv), b, l, h, d, scale, _stream())
-    return dqkv
+def head_views(x, b, l, h, d):
+    """[b, h, l, d] views of the heads packed in the rows of x [b*l, n*h*d] ([b][l][n][h][d]), as attn_fwd / attn_bwd
+    take them: q, k, v of a qkv buffer (n = 3), or the one view of an attention output or its gradient (n = 1)."""
+    x = x.view(b, l, -1, h, d)
+    return tuple(x[:, :, i].permute(0, 2, 1, 3) for i in range(x.shape[2]))
 
 
 def _bhl_strides(t):

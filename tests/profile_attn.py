@@ -16,20 +16,22 @@ ap.add_argument('--d', type=int, default=64)
 ap.add_argument('--iters', type=int, default=3)
 a = ap.parse_args()
 g = torch.Generator(device='cuda').manual_seed(0)
-qkv = torch.randn(a.b, a.l, 3, a.h, a.d, device='cuda', generator=g).to(torch.bfloat16)
+qkv = torch.randn(a.b * a.l, 3 * a.h * a.d, device='cuda', generator=g).to(torch.bfloat16)
 dout = torch.randn(a.b * a.l, a.h * a.d, device='cuda', generator=g).to(torch.bfloat16)
+out, dqkv = torch.empty_like(dout), torch.empty_like(qkv)
+q, k, v, o, do, dq, dk, dv = (view for x in (qkv, out, dout, dqkv) for view in ops.head_views(x, a.b, a.l, a.h, a.d))
 scale = a.d ** -0.5
 for _ in range(2):
-    out, lse = ops.attention_fwd(qkv, a.b, a.l, a.h, a.d, scale)
-    ops.attention_bwd(qkv, out, dout, lse, a.b, a.l, a.h, a.d, scale)
+    _, lse = ops.attn_fwd(q, k, v, scale, out=o)
+    ops.attn_bwd(q, k, v, o, lse, do, scale, dq, dk, dv)
 torch.cuda.synchronize()
 ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
 ev[0].record()
 for _ in range(a.iters):
-    out, lse = ops.attention_fwd(qkv, a.b, a.l, a.h, a.d, scale)
+    _, lse = ops.attn_fwd(q, k, v, scale, out=o)
 ev[1].record()
 for _ in range(a.iters):
-    ops.attention_bwd(qkv, out, dout, lse, a.b, a.l, a.h, a.d, scale)
+    ops.attn_bwd(q, k, v, o, lse, do, scale, dq, dk, dv)
 ev[2].record()
 torch.cuda.synchronize()
 print(f'attention B{a.b} L{a.l} H{a.h} D{a.d}: fwd {ev[0].elapsed_time(ev[1]) / a.iters * 1e3:.1f} us, '

@@ -76,32 +76,32 @@ def test_attn_fwd_bwd_matches_torch(B, H, Lq, Lk, dqk, dv, masked):
         assert dvv[mask[:, None, :, None].expand_as(dvv)].abs().max().item() == 0
 
 
-def test_attn_partial_dk_columns_and_strided_views():
-    """dk_cols < dqk (bias columns of k carry no gradient) and packed [B, L, 3, H, D] views."""
+def test_attn_partial_dk_columns_on_packed_views():
+    """dk_cols < dqk (bias columns of k carry no gradient) on packed [B, L, 3, H, D] views."""
     ops = _ops()
     B, H, L, D = 2, 3, 150, 64
     g = torch.Generator(device='cuda').manual_seed(5)
     qkv = torch.randn(B, L, 3, H, D, device='cuda', generator=g).to(torch.bfloat16)
     q, k, v = (qkv[:, :, i].permute(0, 2, 1, 3) for i in range(3))
     out, lse = ops.attn_fwd(q, k, v, D ** -0.5)
-    out2, lse2 = ops.attention_fwd(qkv, B, L, H, D, D ** -0.5)
-    assert torch.equal(out.permute(0, 2, 1, 3).reshape(B * L, H * D), out2) and torch.equal(lse, lse2)
     dout = torch.randn(B, L, H, D, device='cuda', generator=g).to(torch.bfloat16).permute(0, 2, 1, 3)
-    dqkv = torch.zeros_like(qkv)
-    dq, dk, dv = (dqkv[:, :, i].permute(0, 2, 1, 3) for i in range(3))
-    ops.attn_bwd(q, k, v, out, lse, dout, D ** -0.5, dq, dk, dv, dk_cols=32)
-    full = ops.attention_bwd(qkv, out2, dout.permute(0, 2, 1, 3).reshape(B * L, H * D).contiguous(), lse2, B, L, H, D, D ** -0.5)
+    dqkv, full = torch.zeros_like(qkv), torch.empty_like(qkv)
+    ops.attn_bwd(q, k, v, out, lse, dout, D ** -0.5, *(dqkv[:, :, i].permute(0, 2, 1, 3) for i in range(3)), dk_cols=32)
+    ops.attn_bwd(q, k, v, out, lse, dout, D ** -0.5, *(full[:, :, i].permute(0, 2, 1, 3) for i in range(3)))
     assert torch.equal(dqkv[:, :, 0], full[:, :, 0]) and torch.equal(dqkv[:, :, 2], full[:, :, 2])
     assert torch.equal(dqkv[:, :, 1, :, :32], full[:, :, 1, :, :32]) and dqkv[:, :, 1, :, 32:].abs().max().item() == 0
 
 
-def test_attn_is_bit_reproducible():
+def test_attn_on_packed_views_is_bit_reproducible():
     ops = _ops()
     g = torch.Generator(device='cuda').manual_seed(3)
-    qkv = torch.randn(4, 197, 3, 12, 64, device='cuda', generator=g).to(torch.bfloat16)
+    qkv = torch.randn(4 * 197, 3 * 12 * 64, device='cuda', generator=g).to(torch.bfloat16)
     dout = torch.randn(4 * 197, 12 * 64, device='cuda', generator=g).to(torch.bfloat16)
     runs = []
     for _ in range(2):
-        out, lse = ops.attention_fwd(qkv, 4, 197, 12, 64, 0.125)
-        runs.append((out.clone(), lse.clone(), ops.attention_bwd(qkv, out, dout, lse, 4, 197, 12, 64, 0.125).clone()))
+        att, dqkv = torch.empty_like(dout), torch.empty_like(qkv)
+        q, k, v, o, do, dq, dk, dv = (view for x in (qkv, att, dout, dqkv) for view in ops.head_views(x, 4, 197, 12, 64))
+        _, lse = ops.attn_fwd(q, k, v, 0.125, out=o)
+        ops.attn_bwd(q, k, v, o, lse, do, 0.125, dq, dk, dv)
+        runs.append((att, lse, dqkv))
     assert all(torch.equal(a, b) for a, b in zip(*runs))

@@ -47,7 +47,7 @@ gamma(m) = m u / (1 - m u) bounds m chained roundings.
 Each check prints the largest fraction of its allowance an element used; at the end of the module the largest share
 per family is printed (run with -s), with the families that are checked bit for bit.
 
-Launch geometry.  Python mirrors of grid1d (capi_van.cu), grid_1d (capi_dinov3.cu), saicv_dwconv_wgrad_blocks and
+Launch geometry.  Python mirrors of grid_1d (host_util.cu), saicv_dwconv_wgrad_blocks and
 ppb; every shape list asserts that it runs a grid-stride loop more than once, and the weight-gradient list that it
 has nblk = 132 with a ragged last block.
 
@@ -124,14 +124,9 @@ def _zero_bits(what, out, dead):
 
 
 # ------------------------------------------------------------------ launch geometry mirrors
-def _grid1d(items, per_block=256, cap=132 * 16):
-    """capi_van.cu grid1d."""
+def _grid_1d(items, per_block=256, cap=132 * 16):
+    """host_util.cu grid_1d."""
     return max(1, min(-(-items // per_block), cap))
-
-
-def _grid_1d(items):
-    """capi_dinov3.cu grid_1d."""
-    return max(1, min(-(-items // 256), 132 * 16))
 
 
 def _loops(items, per_block, blocks):
@@ -150,7 +145,7 @@ def _ppb(npix):
 
 def _dw_loops(n, h, w):
     npix = n * h * w
-    return _loops(npix, 32, _grid1d(npix, 32, 132 * 8))
+    return _loops(npix, 32, _grid_1d(npix, 32, 132 * 8))
 
 
 # ------------------------------------------------------------------ shape lists
@@ -184,13 +179,13 @@ assert any(_wgrad_blocks(n * h * w) == 132 and not _ragged(n * h * w) for n, h, 
 assert any(h != w for _, h, w, *_ in DW_WGRAD)
 
 GATE = [(1, 8), (294, 96), (4 * 3136, 64), (64 * 3136, 256)]      # the last: VAN-B0 stage-1 gating at batch 64
-assert any(_loops(r * c // 8, 256, _grid1d(r * c // 8)) > 1 for r, c in GATE)
+assert any(_loops(r * c // 8, 256, _grid_1d(r * c // 8)) > 1 for r, c in GATE)
 
 # (rows, C, rows per drop-path scale): a single row, ViT-style token rows, VAN stage-1 at batch 64, and slab
 # reductions that use all 264 partial rows (40000 x 384 with a short last block, 8448 x 1536 with a full one)
 LS = [(1, 8, 1), (147, 1536, 49), (1570, 384, 785), (50176, 8, 3136), (40000, 384, 800), (2113, 1536, 197),
       (8448, 1536, 264), (64 * 3136, 32, 3136)]
-assert any(_loops(r * c // 8, 256, _grid1d(r * c // 8)) > 1 for r, c, _ in LS)
+assert any(_loops(r * c // 8, 256, _grid_1d(r * c // 8)) > 1 for r, c, _ in LS)
 assert any(_van_slab(r, c)[2] == 264 for r, c, _ in LS)
 
 SWIGLU_N = [8, 4104, 6291456]
@@ -207,9 +202,9 @@ def _out_size(h, k, s, p):
 
 
 assert any(_loops(n * _out_size(h, k, s, p) * _out_size(w, k, s, p) * k * k * c // 8, 256,
-                  _grid1d(n * _out_size(h, k, s, p) * _out_size(w, k, s, p) * k * k * c // 8)) > 1
+                  _grid_1d(n * _out_size(h, k, s, p) * _out_size(w, k, s, p) * k * k * c // 8)) > 1
            for n, h, w, c, k, s, p in IM2COL)
-assert any(_loops(n * h * w * c // 8, 256, _grid1d(n * h * w * c // 8)) > 1 for n, h, w, c, *_ in IM2COL)
+assert any(_loops(n * h * w * c // 8, 256, _grid_1d(n * h * w * c // 8)) > 1 for n, h, w, c, *_ in IM2COL)
 assert any((h + 2 * p - k) % s for _, h, _, _, k, s, p in IM2COL)
 
 

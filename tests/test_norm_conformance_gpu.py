@@ -179,7 +179,7 @@ def _van_slab(rows, c):
 
 
 def _ln_bwd_depth(rows, accumulate=False):
-    """ln_bwd_kernel / postln_bwd_kernel (grid_1d(rows, 64, 264) blocks of 8 warps) + ln_fold_kernel."""
+    """ln_bwd_kernel / postln_bwd_kernel (grid_1d(rows, 64, 264) blocks of 8 warps) + fold_partials_kernel."""
     grid = max(1, min(-(-rows // 64), 264))
     return -(-rows // (grid * 8)) + 8 + -(-grid // 32) + 32 + int(accumulate)
 

@@ -83,7 +83,7 @@ gpu = pytest.mark.gpu
 
 U = 2.0 ** -24          # one fp32 rounding, relative
 M32 = 0xFFFFFFFF
-CAP = 132 * 16 * 256    # items one sweep of grid_1d / grid1d / blocks_for covers (132 * 16 blocks of 256 threads)
+CAP = 132 * 16 * 256    # items one sweep of grid_1d covers (132 * 16 blocks of 256 threads)
 FILL_SLAB_ROWS, FILL_MAX_SLABS = 512, 128
 BF16, F32 = torch.bfloat16, torch.float32
 

@@ -76,13 +76,16 @@ def test_gelu_and_tokens_and_pool():
 
 
 @pytest.mark.parametrize('B,L,H', [(2, 197, 12), (3, 64, 4), (1, 256, 2), (2, 50, 3), (1, 17, 1)])
-def test_attention_fwd_bwd(B, L, H):
+def test_attn_on_packed_qkv_views(B, L, H):
     ops = _ops()
     D = 64
     g = torch.Generator(device='cuda').manual_seed(2)
     qkv = torch.randn(B, L, 3, H, D, device='cuda', generator=g).to(torch.bfloat16)
     scale = D ** -0.5
-    out, lse = ops.attention_fwd(qkv, B, L, H, D, scale)
+    out = torch.empty(B * L, H * D, device='cuda', dtype=torch.bfloat16)
+    heads = ops.head_views(qkv.view(B * L, -1), B, L, H, D)   # the ViT runtime's packed-qkv views
+    (o,) = ops.head_views(out, B, L, H, D)
+    _, lse = ops.attn_fwd(*heads, scale, out=o)
     qr = qkv.float().requires_grad_(True)
     q, k, v = qr.permute(2, 0, 3, 1, 4).unbind(0)  # [B, H, L, D] as in vit.py:66-69
     attn = ((q @ k.transpose(-2, -1)) * scale).softmax(-1)
@@ -92,7 +95,9 @@ def test_attention_fwd_bwd(B, L, H):
     assert (lse - ref_lse).abs().max().item() <= 1e-2
     dout = torch.randn(B * L, H * D, device='cuda', generator=g).to(torch.bfloat16)
     ref.backward(dout.float())
-    dqkv = ops.attention_bwd(qkv, out, dout, lse, B, L, H, D, scale)
+    dqkv = torch.empty_like(qkv)
+    (do,) = ops.head_views(dout, B, L, H, D)
+    ops.attn_bwd(*heads, o, lse, do, scale, *ops.head_views(dqkv.view(B * L, -1), B, L, H, D))
     for i, name in enumerate('qkv'):
         r = _rel(dqkv[:, :, i], qr.grad[:, :, i])
         assert r <= 2e-2, f'd{name} rel L2 {r}'
