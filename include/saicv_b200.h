@@ -507,6 +507,20 @@ int saicv_u8_mix_erase_norm(const void* in, float* out, int n, int h, int w, con
                             const int* box4, double lam, const long long* labels, float* soft, int num_classes,
                             float on_value, float off_value, void* stream);
 
+/* RandAugment(integer=True) of the same recipes (classification/auto_rand_augment.py:646-690) on the uint8 images, in
+ * place, from the draws the host made (classification.common.Uint8RandAugment): per image b and layer l, record
+ * r = b * layers + l holds ops[r] = (op, resample, iparam, 0), factors[r] and affine[r][6]:
+ *   op -1: skipped; 0 AutoContrast, 1 Equalize, 2 Invert, 4 Posterize (iparam bits 0..8), 5 Solarize (iparam threshold
+ *   0..256), 6 SolarizeAdd (iparam addend 0..255): per-channel LUTs; 7 Color, 8 Contrast, 9 Brightness, 10 Sharpness:
+ *   Image.blend(degenerate, image, factor) in float32; 3 Rotate, 11 ShearX, 12 ShearY, 13 TranslateXRel, 14 TranslateYRel:
+ *   Image.transform(AFFINE, affine[r], resample 2 BILINEAR / 3 BICUBIC, fill3) in float64.
+ * Bit-identical to Pillow.  ops_host / factors_host / affine_host: HOST copies (validated before any launch); ops /
+ * factors / affine: the same on the device.  img, scratch: device uint8 [n][h][w][3]; layers ping-pong img -> scratch ->
+ * img (an odd count ends with a copy back).  stats: device uint32 [n][770] workspace.  1 <= n <= 1024, layers <= 16. */
+int saicv_u8_rand_augment(void* img, void* scratch, int n, int h, int w, int layers, const int* ops_host,
+                          const float* factors_host, const double* affine_host, const int* ops, const float* factors,
+                          const double* affine, const int* fill3, unsigned int* stats, void* stream);
+
 /* ---- token gather / scatter for masked-token models (SURVEY.md 8 f4; csrc/capi_tokens.cu) -----------------------------
  * out fp32 [b][r][c] = (idx[b][r] >= 0 ? src[b][idx[b][r]][:] : fill[:]) + (pos ? pos[pos_idx ? pos_idx[b][r] : r][:] : 0);
  * src fp32 [b][src_rows][c].  One call is the torch.gather + cat(cls / mask token) + position-encoding add of

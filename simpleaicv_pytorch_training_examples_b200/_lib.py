@@ -107,6 +107,8 @@ SIGNATURES = {
     'saicv_u8_mix_erase_norm': [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.POINTER(c_float), ctypes.POINTER(c_float),
                                 c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p, ctypes.c_double, c_void_p, c_void_p,
                                 c_int, c_float, c_float, c_void_p],
+    'saicv_u8_rand_augment': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     'saicv_token_gather_fwd': [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     'saicv_token_fill_slabs': [c_ll],
     'saicv_token_gather_bwd': [c_void_p, c_void_p, c_void_p, c_int, c_ll, c_void_p, c_int, c_int, c_int, c_void_p],

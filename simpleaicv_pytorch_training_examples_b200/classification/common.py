@@ -3,8 +3,10 @@
 input-pipeline edge of SURVEY.md 8 f3: ``Uint8ClassificationCollater`` + ``DeviceNormalize`` move the batch over PCIe as
 uint8 pixels and normalise on the device; ``Uint8RandomErasing`` + ``Uint8MixupCutmixClassificationCollater`` do the same for
 the recipes that end in RandomErasing and Mixup / CutMix, with the random draws on the host and the pixel and label
-arithmetic on the device.  The per-sample transforms / datasets stay CPU data code (SURVEY.md section 2)."""
+arithmetic on the device; ``Uint8RandAugment`` makes RandAugment's draws on the host and leaves its pixel arithmetic to the
+same device edge.  The other per-sample transforms / datasets stay CPU data code (SURVEY.md section 2)."""
 import math
+import random
 
 import numpy as np
 import torch
@@ -35,6 +37,9 @@ class Uint8ClassificationCollater:
         self.pin_memory = pin_memory
 
     def __call__(self, data):
+        if any('randaug_ops' in s for s in data):
+            raise ValueError('samples carry a Uint8RandAugment record, which only Uint8MixupCutmixClassificationCollater '
+                             'passes on to the device: this collater would drop it')
         images = np.stack([np.ascontiguousarray(s['image']) for s in data])
         assert images.dtype == np.uint8 and images.ndim == 4 and images.shape[3] == 3, 'expects uint8 [H, W, 3] images'
         labels = torch.from_numpy(np.array([s['label'] for s in data]).astype(np.float32)).long()
@@ -54,17 +59,140 @@ class MixupEraseRecord:
     rects int32 [B, 4]: (top, left, h, w) of image b's erase rectangle, h = w = 0 when it was not erased;
     offsets int64 [B]: where image b's fp32 [h, w, 3] noise starts in ``noise`` (fp32, the rectangles' noise concatenated);
     mode: MIX_NONE / MIX_MIXUP / MIX_CUTMIX; box: the CutMix box (y0, y1, x0, x1); lam: the (corrected) float64 lambda;
-    on_value / off_value: the smoothed one-hot values, computed in float64 as the reference does."""
+    on_value / off_value: the smoothed one-hot values, computed in float64 as the reference does.
 
-    def __init__(self, rects, offsets, noise, mode, box, lam, num_classes, on_value, off_value):
+    When the samples came through ``Uint8RandAugment``, its per-sample records are stacked here and applied to the uint8
+    images first (ops.u8_rand_augment): randaug_ops int32 [B, L, 4], randaug_f float32 [B, L], randaug_affine float64
+    [B, L, 6] and randaug_fill, the (R, G, B) fill colour of the geometric ops; all four are None otherwise."""
+
+    def __init__(self, rects, offsets, noise, mode, box, lam, num_classes, on_value, off_value,
+                 randaug_ops=None, randaug_f=None, randaug_affine=None, randaug_fill=None):
         self.rects, self.offsets, self.noise = rects, offsets, noise
         self.mode, self.box, self.lam = mode, box, lam
         self.num_classes, self.on_value, self.off_value = num_classes, on_value, off_value
+        self.randaug_ops, self.randaug_f, self.randaug_affine = randaug_ops, randaug_f, randaug_affine
+        self.randaug_fill = randaug_fill
 
     def pin_memory(self):
-        """Called by DataLoader(pin_memory=True): only the noise is copied to the device, the rest is read on the host."""
+        """Called by DataLoader(pin_memory=True): the noise and the RandAugment record are copied to the device, the rest
+        is read on the host."""
         self.noise = self.noise.pin_memory()
+        if self.randaug_ops is not None:
+            self.randaug_ops = self.randaug_ops.pin_memory()
+            self.randaug_f = self.randaug_f.pin_memory()
+            self.randaug_affine = self.randaug_affine.pin_memory()
         return self
+
+
+# RandAugment(integer=True)'s op set in the reference's order (SimpleAICV/classification/auto_rand_augment.py:588-605):
+# the op codes of a Uint8RandAugment record, csrc/capi_input.cu's and oracle/randaugment.py's
+RANDAUG_OPS = ('AutoContrast', 'Equalize', 'Invert', 'Rotate', 'PosterizeIncreasing', 'SolarizeIncreasing', 'SolarizeAdd',
+               'ColorIncreasing', 'ContrastIncreasing', 'BrightnessIncreasing', 'SharpnessIncreasing', 'ShearX', 'ShearY',
+               'TranslateXRel', 'TranslateYRel')
+RANDAUG_SKIP = -1
+RESAMPLE_BILINEAR, RESAMPLE_BICUBIC = 2, 3   # PIL.Image.Resampling.BILINEAR / BICUBIC, the values random.choice returns
+
+
+def _randomly_negate(v):
+    return -v if random.random() > 0.5 else v
+
+
+def _rotate_coeffs(degrees, w, h):
+    """Image.rotate(degrees) as the AFFINE coefficients Image.transform receives (centre (w / 2, h / 2), no expand);
+    a whole turn is the identity, which Pillow returns as a copy."""
+    angle = degrees % 360.0
+    if angle == 0:
+        return (1.0, 0.0, 0.0, 0.0, 1.0, 0.0)
+    cx, cy = w / 2, h / 2
+    angle = -math.radians(angle)
+    m = [round(math.cos(angle), 15), round(math.sin(angle), 15), 0.0,
+         round(-math.sin(angle), 15), round(math.cos(angle), 15), 0.0]
+    a, b, c, d, e, f = m
+    m[2], m[5] = a * -cx + b * -cy + c, d * -cx + e * -cy + f
+    m[2] += cx
+    m[5] += cy
+    return tuple(m)
+
+
+class Uint8RandAugment:
+    """Takes the place of ``RandAugment(...)`` (SimpleAICV/classification/auto_rand_augment.py:646-690) in a transform
+    list whose batch is collated by ``Uint8MixupCutmixClassificationCollater``: the image stays uint8 [H, W, 3] and the
+    draws go into the sample as a record ('randaug_ops', 'randaug_f', 'randaug_affine', 'randaug_fill'); the device
+    applies them (ops.u8_rand_augment), bit-identical to the reference's PIL ops.
+
+    The draws are the reference's, in its order: np.random.choice over the 15 ops (with replacement); then per chosen op
+    random.random() against prob 0.5, random.gauss(magnitude, magnitude_std) clamped to [0, 10], the level function's
+    negate draw (random.random() > 0.5) and, for the five geometric ops, random.choice((BILINEAR, BICUBIC)).  None depends
+    on pixel values.  Per layer the record holds int32 (op, resample, iparam, 0) with op = -1 when the prob draw skipped
+    it and iparam the Posterize bits, Solarize threshold or SolarizeAdd addend; the float32 enhance factor; and the
+    float64 AFFINE coefficients, Rotate's computed as Image.rotate computes them.  Only the shipped setting (integer=True,
+    uniform choice, finite magnitude_std, no magnitude_max) is implemented."""
+
+    def __init__(self, magnitude=9, num_layers=2, resize=224, mean=(0.485, 0.456, 0.406), integer=True, weight_idx=None,
+                 magnitude_std=0.5, magnitude_max=None):
+        if not integer:
+            raise NotImplementedError('Uint8RandAugment integer=False: only the increasing op set (the shipped configs\' '
+                                      'integer=True) is implemented')
+        if weight_idx is not None:
+            raise NotImplementedError('Uint8RandAugment weight_idx: only the uniform op choice (the shipped configs\' '
+                                      'weight_idx=None) is implemented')
+        if magnitude_std == float('inf'):
+            raise NotImplementedError('Uint8RandAugment magnitude_std=inf: only a normal magnitude draw (the shipped '
+                                      'configs\' magnitude_std=0.5) is implemented')
+        if magnitude_max:
+            raise NotImplementedError('Uint8RandAugment magnitude_max: only the default bound of 10 (the shipped configs\' '
+                                      'magnitude_max=None) is implemented')
+        self.magnitude = magnitude
+        self.num_layers = num_layers
+        self.magnitude_std = float(magnitude_std) if magnitude_std else 0.
+        self.fill = tuple(min(255, round(255 * x)) for x in mean)
+
+    def _layer(self, op, w, h):
+        """One AugmentOp call's draws (auto_rand_augment.py:338-355) -> (op, resample, iparam, factor, coefficients)."""
+        if random.random() > 0.5:
+            return RANDAUG_SKIP, 0, 0, 0., (0.,) * 6
+        magnitude = self.magnitude
+        if self.magnitude_std > 0:
+            magnitude = random.gauss(magnitude, self.magnitude_std)
+        magnitude = max(0., min(magnitude, 10.))
+        name, iparam, factor, coeffs = RANDAUG_OPS[op], 0, 0., (0.,) * 6
+        if name == 'Rotate':
+            degrees = _randomly_negate((magnitude / 10.) * 30.)
+        elif name == 'PosterizeIncreasing':
+            iparam = 4 - int((magnitude / 10.) * 4)
+        elif name == 'SolarizeIncreasing':
+            iparam = 256 - int((magnitude / 10.) * 256)
+        elif name == 'SolarizeAdd':
+            iparam = int((magnitude / 10.) * 110)
+        elif name.endswith('Increasing'):
+            factor = max(0.1, 1.0 + _randomly_negate((magnitude / 10.) * .9))
+        elif name in ('ShearX', 'ShearY'):
+            shear = _randomly_negate((magnitude / 10.) * 0.3)
+            coeffs = (1, shear, 0, 0, 1, 0) if name == 'ShearX' else (1, 0, 0, shear, 1, 0)
+        elif name in ('TranslateXRel', 'TranslateYRel'):
+            pct = _randomly_negate((magnitude / 10.) * 0.45)
+            coeffs = (1, 0, pct * w, 0, 1, 0) if name == 'TranslateXRel' else (1, 0, 0, 0, 1, pct * h)
+        resample = 0
+        if name in ('Rotate', 'ShearX', 'ShearY', 'TranslateXRel', 'TranslateYRel'):
+            resample = random.choice((RESAMPLE_BILINEAR, RESAMPLE_BICUBIC))
+            if name == 'Rotate':
+                coeffs = _rotate_coeffs(degrees, w, h)
+        return op, resample, iparam, factor, coeffs
+
+    def __call__(self, sample):
+        image = np.asarray(sample['image'])
+        if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+            raise ValueError(f'Uint8RandAugment expects a PIL RGB image or a uint8 [H, W, 3] array, got {image.dtype} {image.shape}')
+        h, w = image.shape[:2]
+        chosen = np.random.choice(len(RANDAUG_OPS), self.num_layers, replace=True)
+        ops = np.zeros((self.num_layers, 4), dtype=np.int32)
+        factors = np.zeros(self.num_layers, dtype=np.float32)
+        coeffs = np.zeros((self.num_layers, 6), dtype=np.float64)
+        for i, op in enumerate(chosen):
+            ops[i, 0], ops[i, 1], ops[i, 2], factors[i], coeffs[i] = self._layer(int(op), w, h)
+        sample['image'], sample['randaug_ops'], sample['randaug_f'] = image, ops, factors
+        sample['randaug_affine'], sample['randaug_fill'] = coeffs, self.fill
+        return sample
 
 
 class Uint8RandomErasing:
@@ -182,6 +310,18 @@ class Uint8MixupCutmixClassificationCollater:
         offsets = np.zeros(b, dtype=np.int64)
         offsets[1:] = np.cumsum([len(n) for n in noises])[:-1]
 
+        randaug = [s.get('randaug_ops') is not None for s in data]
+        if any(randaug) and not all(randaug):
+            raise ValueError('some samples carry a Uint8RandAugment record and some do not')
+        ra = {}
+        if all(randaug):
+            if len({tuple(s['randaug_fill']) for s in data}) != 1 or len({np.shape(s['randaug_ops']) for s in data}) != 1:
+                raise ValueError('the samples\' Uint8RandAugment records differ in layer count or fill colour')
+            ra = dict(randaug_ops=torch.from_numpy(np.stack([s['randaug_ops'] for s in data]).astype(np.int32)),
+                      randaug_f=torch.from_numpy(np.stack([s['randaug_f'] for s in data]).astype(np.float32)),
+                      randaug_affine=torch.from_numpy(np.stack([s['randaug_affine'] for s in data]).astype(np.float64)),
+                      randaug_fill=tuple(int(v) for v in data[0]['randaug_fill']))
+
         lam, use_cutmix = self._params_per_batch()
         mode, box = MIX_NONE, (0, 0, 0, 0)
         if lam != 1.:
@@ -200,7 +340,7 @@ class Uint8MixupCutmixClassificationCollater:
         off_value = self.label_smoothing / self.num_classes
         record = MixupEraseRecord(torch.from_numpy(rects), torch.from_numpy(offsets),
                                   torch.from_numpy(np.concatenate(noises)),
-                                  mode, box, lam, self.num_classes, 1. - self.label_smoothing + off_value, off_value)
+                                  mode, box, lam, self.num_classes, 1. - self.label_smoothing + off_value, off_value, **ra)
         images, labels = torch.from_numpy(images), torch.from_numpy(labels)
         if self.pin_memory and torch.cuda.is_available():
             images, labels, record = images.pin_memory(), labels.pin_memory(), record.pin_memory()

@@ -174,6 +174,275 @@ mix_soft_label_kernel(const long long* __restrict__ labels, float* __restrict__ 
   }
 }
 
+// ---- RandAugment(integer=True) on the uint8 edge -----------------------------------------------------------------------
+// The reference's RandAugment (classification/auto_rand_augment.py:646-690) runs two of 15 PIL ops per image.  The host
+// made every draw (classification.common.Uint8RandAugment); per image and layer the record holds (op, resample, iparam),
+// the enhance factor and the AFFINE coefficients.  Per layer a stats pass takes the histograms / luma sum the op needs,
+// then one pass writes every output pixel with Pillow's arithmetic: integer LUTs, float32 blends, float64 affine gathers.
+// Every float operation is an explicit _rn intrinsic so that nothing contracts into an FMA Pillow does not execute.
+constexpr int kRAMaxImages = 1024;   // per launch: the stats list travels in the kernel's parameter space
+constexpr int kRAMaxLayers = 16;
+constexpr int kRAStatsWords = 770;   // per image: 3 x 256 histogram bins, then the 64-bit luma sum
+constexpr int kRAPixelsPerThread = 8;
+
+enum RAOp {
+  kRASkip = -1, kAutoContrast, kEqualize, kInvert, kRotate, kPosterize, kSolarize, kSolarizeAdd, kColor, kContrast,
+  kBrightness, kSharpness, kShearX, kShearY, kTranslateX, kTranslateY, kRANumOps
+};
+constexpr int kBilinear = 2, kBicubic = 3;   // PIL.Image.Resampling values
+
+__host__ __device__ __forceinline__ bool ra_geometric(int op) {
+  return op == kRotate || op == kShearX || op == kShearY || op == kTranslateX || op == kTranslateY;
+}
+__host__ __device__ __forceinline__ bool ra_enhance(int op) { return op >= kColor && op <= kSharpness; }
+__host__ __device__ __forceinline__ bool ra_lut(int op) { return op >= kAutoContrast && op <= kSolarizeAdd && op != kRotate; }
+__host__ __device__ __forceinline__ bool ra_needs_stats(int op) {
+  return op == kAutoContrast || op == kEqualize || op == kContrast;
+}
+
+struct RAStatsList {
+  int count;
+  unsigned short img[kRAMaxImages];
+};
+
+// Pillow's RGB -> L (Convert.c rgb2l)
+__device__ __forceinline__ uint32_t ra_luma(uint32_t r, uint32_t g, uint32_t b) {
+  return (r * 19595u + g * 38470u + b * 7471u + 0x8000u) >> 16;
+}
+
+// per listed image: 3 x 256 channel histograms (AutoContrast, Equalize) or the sum of L (Contrast), with integer atomics
+__global__ void __launch_bounds__(kInThreads)
+ra_stats_kernel(const uint8_t* __restrict__ in, unsigned int* __restrict__ stats, const int4* __restrict__ ops, int layers,
+                int layer, long long hw, const __grid_constant__ RAStatsList list) {
+  __shared__ unsigned int hist[768];
+  __shared__ unsigned long long lsum;
+  const int b = list.img[blockIdx.y];
+  const bool histo = __ldg(&ops[(long long)b * layers + layer].x) != kContrast;
+  for (int i = threadIdx.x; i < 768; i += blockDim.x) hist[i] = 0;
+  if (threadIdx.x == 0) lsum = 0;
+  __syncthreads();
+  const uint8_t* p = in + (long long)b * hw * 3;
+  unsigned long long s = 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < hw; i += (long long)gridDim.x * blockDim.x) {
+    const uint32_t r = __ldg(p + i * 3), g = __ldg(p + i * 3 + 1), bl = __ldg(p + i * 3 + 2);
+    if (histo) {
+      atomicAdd(&hist[r], 1u);
+      atomicAdd(&hist[256 + g], 1u);
+      atomicAdd(&hist[512 + bl], 1u);
+    } else {
+      s += ra_luma(r, g, bl);
+    }
+  }
+  if (!histo) atomicAdd(&lsum, s);
+  __syncthreads();
+  unsigned int* st = stats + (long long)b * kRAStatsWords;
+  if (histo) {
+    for (int i = threadIdx.x; i < 768; i += blockDim.x)
+      if (hist[i]) atomicAdd(st + i, hist[i]);
+  } else if (threadIdx.x == 0) {
+    atomicAdd(reinterpret_cast<unsigned long long*>(st + 768), lsum);
+  }
+}
+
+// ImageOps' LUTs for image b (blockDim.x == 256: thread t owns entry t of each channel)
+__device__ void ra_build_lut(int op, int iparam, const unsigned int* __restrict__ st, long long hw, uint8_t (*lut)[256]) {
+  __shared__ unsigned int cum[3][256];
+  __shared__ int lo[3], hi[3], nz[3];
+  const int t = threadIdx.x;
+  if (op == kInvert || op == kPosterize || op == kSolarize || op == kSolarizeAdd) {
+    int v;
+    if (op == kInvert) v = 255 - t;
+    else if (op == kPosterize) v = t & ~((1 << (8 - iparam)) - 1) & 255;
+    else if (op == kSolarize) v = t < iparam ? t : 255 - t;
+    else v = t < 128 ? min(255, t + iparam) : t;
+    lut[0][t] = lut[1][t] = lut[2][t] = (uint8_t)v;
+    return;
+  }
+  if (t < 3) {
+    lo[t] = 256;
+    hi[t] = -1;
+    nz[t] = 0;
+  }
+  unsigned int h[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) h[c] = st[c * 256 + t];
+  __syncthreads();
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    cum[c][t] = h[c];
+    if (h[c]) {
+      atomicMin(&lo[c], t);
+      atomicMax(&hi[c], t);
+      atomicAdd(&nz[c], 1);
+    }
+  }
+  __syncthreads();
+  if (op == kAutoContrast) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      int v = t;
+      if (hi[c] > lo[c]) {   // ImageOps.autocontrast(cutoff=0): int(ix * scale + offset) in float64, clipped
+        const double scale = __ddiv_rn(255.0, (double)(hi[c] - lo[c]));
+        const double offset = __dmul_rn((double)-lo[c], scale);
+        v = (int)__dadd_rn(__dmul_rn((double)t, scale), offset);
+        v = v < 0 ? 0 : (v > 255 ? 255 : v);
+      }
+      lut[c][t] = (uint8_t)v;
+    }
+    return;
+  }
+  // Equalize: n // step with n = step // 2 + the count below bin t, step = (pixels - count of the last used bin) // 255
+  for (int off = 1; off < 256; off <<= 1) {
+    unsigned int v[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = t >= off ? cum[c][t - off] : 0u;
+    __syncthreads();
+#pragma unroll
+    for (int c = 0; c < 3; ++c) cum[c][t] += v[c];
+    __syncthreads();
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    long long v = t;
+    if (nz[c] > 1) {
+      const long long step = (hw - (long long)st[c * 256 + hi[c]]) / 255;
+      if (step) {
+        v = (step / 2 + (long long)(cum[c][t] - h[c])) / step;
+        v = v > 255 ? 255 : v;
+      }
+    }
+    lut[c][t] = (uint8_t)v;
+  }
+}
+
+// Image.blend(degenerate, image, f): float32 deg + f * (img - deg), clipped, truncated (Pillow's Blend.c)
+__device__ __forceinline__ uint8_t ra_blend(int deg, int v, float f) {
+  const float r = __fadd_rn((float)deg, __fmul_rn(f, (float)(v - deg)));
+  return r <= 0.f ? 0 : (r >= 255.f ? 255 : (uint8_t)(int)r);
+}
+
+// ImageFilter.SMOOTH at an interior pixel: rows y+1, y, y-1 of (1 1 1 / 1 5 1 / 1 1 1) / 13 in float32, rounded
+__device__ __forceinline__ int ra_smooth(const uint8_t* __restrict__ p, int y, int x, int w, int c) {
+  const float k1 = 1.0f / 13.0f, k5 = 5.0f / 13.0f;
+  float ss = 0.f;
+#pragma unroll
+  for (int dy = 1; dy >= -1; --dy) {
+    const uint8_t* r = p + ((long long)(y + dy) * w + x) * 3 + c;
+    const float kc = dy == 0 ? k5 : k1;
+    ss = __fadd_rn(ss, __fadd_rn(__fadd_rn(__fmul_rn((float)__ldg(r - 3), k1), __fmul_rn((float)__ldg(r), kc)),
+                                 __fmul_rn((float)__ldg(r + 3), k1)));
+  }
+  return ss <= 0.f ? 0 : (ss >= 255.f ? 255 : (int)__dadd_rn((double)ss, 0.5));
+}
+
+// Pillow's bicubic kernel (Geometry.c BICUBIC) in float64
+__device__ __forceinline__ double ra_cubic(double v1, double v2, double v3, double v4, double d) {
+  const double p2 = __dadd_rn(-v1, v3);
+  const double p3 = __dsub_rn(__dadd_rn(__dmul_rn(2.0, __dsub_rn(v1, v2)), v3), v4);
+  const double p4 = __dadd_rn(__dsub_rn(__dadd_rn(-v1, v2), v3), v4);
+  return __dadd_rn(v2, __dmul_rn(d, __dadd_rn(p2, __dmul_rn(d, __dadd_rn(p3, __dmul_rn(d, p4))))));
+}
+
+// Image.transform(size, AFFINE, a, resample, fillcolor) at output pixel (x, y): Geometry.c affine_transform + the
+// bilinear / bicubic filters, neighbours clamped to the edge
+__device__ __forceinline__ void ra_affine(const uint8_t* __restrict__ p, int y, int x, int h, int w, const double* a,
+                                          int resample, const int* fill, uint8_t* o) {
+  const double xo = x + 0.5, yo = y + 0.5;
+  double xin = __dadd_rn(__dadd_rn(__dmul_rn(a[0], xo), __dmul_rn(a[1], yo)), a[2]);
+  double yin = __dadd_rn(__dadd_rn(__dmul_rn(a[3], xo), __dmul_rn(a[4], yo)), a[5]);
+  if (!(xin >= 0.0 && xin < (double)w && yin >= 0.0 && yin < (double)h)) {
+    o[0] = (uint8_t)fill[0], o[1] = (uint8_t)fill[1], o[2] = (uint8_t)fill[2];
+    return;
+  }
+  xin = __dsub_rn(xin, 0.5);
+  yin = __dsub_rn(yin, 0.5);
+  const int x0 = (int)floor(xin), y0 = (int)floor(yin);
+  const double dx = __dsub_rn(xin, (double)x0), dy = __dsub_rn(yin, (double)y0);
+  auto at = [&](int yy, int xx, int c) -> int {
+    yy = yy < 0 ? 0 : (yy >= h ? h - 1 : yy);
+    xx = xx < 0 ? 0 : (xx >= w ? w - 1 : xx);
+    return __ldg(p + ((long long)yy * w + xx) * 3 + c);
+  };
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    double v;
+    if (resample == kBilinear) {
+      const int p00 = at(y0, x0, c), p01 = at(y0, x0 + 1, c), p10 = at(y0 + 1, x0, c), p11 = at(y0 + 1, x0 + 1, c);
+      const double v1 = __dadd_rn((double)p00, __dmul_rn((double)(p01 - p00), dx));
+      const double v2 = __dadd_rn((double)p10, __dmul_rn((double)(p11 - p10), dx));
+      v = __dadd_rn(v1, __dmul_rn(__dsub_rn(v2, v1), dy));
+    } else {
+      double r[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        r[j] = ra_cubic(at(y0 + j - 1, x0 - 1, c), at(y0 + j - 1, x0, c), at(y0 + j - 1, x0 + 1, c), at(y0 + j - 1, x0 + 2, c), dx);
+      v = ra_cubic(r[0], r[1], r[2], r[3], dy);
+    }
+    o[c] = v <= 0.0 ? 0 : (v >= 255.0 ? 255 : (uint8_t)(int)v);
+  }
+}
+
+struct RAFill {
+  int rgb[3];
+};
+
+// one layer for image blockIdx.y: in -> out (both uint8 [n][h][w][3]); the op is uniform over the block
+__global__ void __launch_bounds__(kInThreads)
+ra_apply_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, const unsigned int* __restrict__ stats,
+                const int4* __restrict__ ops, const float* __restrict__ factors, const double* __restrict__ affine,
+                int layers, int layer, int h, int w, RAFill fill) {
+  __shared__ uint8_t lut[3][256];
+  __shared__ int contrast_deg;
+  const int b = blockIdx.y;
+  const long long rec = (long long)b * layers + layer, hw = (long long)h * w;
+  const int4 o = ops[rec];
+  const int op = o.x;
+  const uint8_t* src = in + (long long)b * hw * 3;
+  uint8_t* dst = out + (long long)b * hw * 3;
+  const long long first = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
+  if (ra_lut(op)) {
+    ra_build_lut(op, o.z, stats + (long long)b * kRAStatsWords, hw, lut);
+    __syncthreads();
+    for (long long i = first; i < hw; i += stride)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) dst[i * 3 + c] = lut[c][__ldg(src + i * 3 + c)];
+  } else if (ra_enhance(op)) {
+    const float f = factors[rec];
+    if (op == kContrast) {
+      if (threadIdx.x == 0) {   // ImageEnhance.Contrast: int(mean(L) + 0.5), the mean in float64
+        const unsigned long long s = *reinterpret_cast<const unsigned long long*>(stats + (long long)b * kRAStatsWords + 768);
+        contrast_deg = (int)__dadd_rn(__ddiv_rn((double)s, (double)hw), 0.5);
+      }
+      __syncthreads();
+    }
+    for (long long i = first; i < hw; i += stride) {
+      const int y = (int)(i / w), x = (int)(i - (long long)y * w);
+      const int r = __ldg(src + i * 3), g = __ldg(src + i * 3 + 1), bl = __ldg(src + i * 3 + 2);
+      const int px[3] = {r, g, bl};
+      const bool interior = y > 0 && y < h - 1 && x > 0 && x < w - 1;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        int deg;
+        if (op == kBrightness) deg = 0;
+        else if (op == kContrast) deg = contrast_deg;
+        else if (op == kColor) deg = (int)ra_luma(r, g, bl);
+        else deg = interior ? ra_smooth(src, y, x, w, c) : px[c];   // SMOOTH copies the border
+        dst[i * 3 + c] = ra_blend(deg, px[c], f);
+      }
+    }
+  } else if (ra_geometric(op)) {
+    double a[6];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) a[k] = affine[rec * 6 + k];
+    for (long long i = first; i < hw; i += stride) {
+      const int y = (int)(i / w), x = (int)(i - (long long)y * w);
+      ra_affine(src, y, x, h, w, a, o.y, fill.rgb, dst + i * 3);
+    }
+  } else {
+    for (long long i = first; i < hw * 3; i += stride) dst[i] = __ldg(src + i);
+  }
+}
+
 }  // namespace
 }  // namespace saicv
 
@@ -256,4 +525,63 @@ extern "C" int saicv_u8_nhwc_to_nchw_norm(const void* in, float* out, int n, int
   }
   u8_nhwc_to_nchw_norm_kernel<<<grid_1d(pixels, kInThreads), kInThreads, 0, st>>>(reinterpret_cast<const uint8_t*>(in), out, pixels, hw, nm);
   return check_launch("u8_nhwc_to_nchw_norm_kernel");
+}
+
+extern "C" int saicv_u8_rand_augment(void* img, void* scratch, int n, int h, int w, int layers, const int* ops_host,
+                                     const float* factors_host, const double* affine_host, const int* ops,
+                                     const float* factors, const double* affine, const int* fill3, unsigned int* stats,
+                                     void* stream) {
+  const char* fn = "saicv_u8_rand_augment";
+  if (!img || !scratch || !ops_host || !factors_host || !affine_host || !ops || !factors || !affine || !fill3 || !stats)
+    return set_error("%s: null pointer", fn);
+  if (img == scratch) return set_error("%s: the scratch buffer must not be the image buffer", fn);
+  if (n < 1 || n > kRAMaxImages) return set_error("%s: 1 <= n <= %d (n=%d)", fn, kRAMaxImages, n);
+  if (h < 1 || w < 1 || (long long)h * w >= (1ll << 31)) return set_error("%s: image %d x %d is empty or too large", fn, h, w);
+  if (layers < 0 || layers > kRAMaxLayers) return set_error("%s: 0 <= layers <= %d (layers=%d)", fn, kRAMaxLayers, layers);
+  RAFill fill;
+  for (int c = 0; c < 3; ++c) {
+    if (fill3[c] < 0 || fill3[c] > 255) return set_error("%s: fill colour component %d is %d, not in [0, 255]", fn, c, fill3[c]);
+    fill.rgb[c] = fill3[c];
+  }
+  for (long long r = 0; r < (long long)n * layers; ++r) {
+    const int b = (int)(r / layers), l = (int)(r % layers);
+    const int op = ops_host[4 * r], resample = ops_host[4 * r + 1], ip = ops_host[4 * r + 2];
+    if (op < kRASkip || op >= kRANumOps) return set_error("%s: image %d layer %d: op %d is not in [-1, %d]", fn, b, l, op, kRANumOps - 1);
+    if (ra_geometric(op)) {
+      if (resample != kBilinear && resample != kBicubic)
+        return set_error("%s: image %d layer %d: resample %d is not BILINEAR (2) or BICUBIC (3)", fn, b, l, resample);
+      for (int k = 0; k < 6; ++k)
+        if (!isfinite(affine_host[6 * r + k])) return set_error("%s: image %d layer %d: affine coefficient %d is not finite", fn, b, l, k);
+    }
+    if (ra_enhance(op) && !isfinite(factors_host[r])) return set_error("%s: image %d layer %d: enhance factor is not finite", fn, b, l);
+    const int ip_max = op == kPosterize ? 8 : op == kSolarize ? 256 : op == kSolarizeAdd ? 255 : 0;
+    if ((op == kPosterize || op == kSolarize || op == kSolarizeAdd) && (ip < 0 || ip > ip_max))
+      return set_error("%s: image %d layer %d: iparam %d of op %d is not in [0, %d]", fn, b, l, ip, op, ip_max);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const long long hw = (long long)h * w;
+  const int gx = grid_1d((hw + kRAPixelsPerThread - 1) / kRAPixelsPerThread, kInThreads, 65535);
+  uint8_t* buf[2] = {reinterpret_cast<uint8_t*>(img), reinterpret_cast<uint8_t*>(scratch)};
+  static thread_local RAStatsList list;
+  for (int l = 0; l < layers; ++l) {
+    const uint8_t* in = buf[l & 1];
+    uint8_t* out = buf[(l + 1) & 1];
+    list.count = 0;
+    for (int b = 0; b < n; ++b)
+      if (ra_needs_stats(ops_host[4 * ((long long)b * layers + l)])) list.img[list.count++] = (unsigned short)b;
+    if (list.count) {
+      if (cudaMemsetAsync(stats, 0, sizeof(unsigned int) * kRAStatsWords * (size_t)n, st) != cudaSuccess)
+        return set_error("%s: cudaMemsetAsync of the statistics failed", fn);
+      ra_stats_kernel<<<dim3(gx, list.count), kInThreads, 0, st>>>(in, stats, reinterpret_cast<const int4*>(ops), layers, l, hw, list);
+      if (check_launch("ra_stats_kernel")) return 1;
+    }
+    ra_apply_kernel<<<dim3(gx, n), kInThreads, 0, st>>>(in, out, stats, reinterpret_cast<const int4*>(ops), factors, affine,
+                                                         layers, l, h, w, fill);
+    if (check_launch("ra_apply_kernel")) return 1;
+  }
+  if (layers & 1) {   // the last layer wrote the scratch buffer
+    if (cudaMemcpyAsync(img, scratch, (size_t)n * hw * 3, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+      return set_error("%s: copy back from the scratch buffer failed", fn);
+  }
+  return 0;
 }

@@ -215,6 +215,32 @@ def u8_mix_erase_normalize(images, labels, mean, std, record, noise, out=None, s
     return out, soft
 
 
+def u8_rand_augment(images, record, scratch=None, stats=None):
+    """RandAugment(integer=True) applied in place to images uint8 [N, H, W, 3] (device) from the draws the host made:
+    record is the batch's classification.common.MixupEraseRecord with its randaug_* fields set (read on the host, and
+    copied to the device here).  Bit-identical to the reference's PIL ops.  scratch: device uint8 like images; stats:
+    device int32 [N, 770] workspace."""
+    assert images.is_cuda and images.dtype == torch.uint8 and images.dim() == 4 and images.shape[3] == 3 and images.is_contiguous()
+    n, h, w, _ = images.shape
+    ra_ops, ra_f, ra_aff = record.randaug_ops, record.randaug_f, record.randaug_affine
+    layers = ra_ops.shape[1]
+    assert ra_ops.dtype == torch.int32 and tuple(ra_ops.shape) == (n, layers, 4) and not ra_ops.is_cuda and ra_ops.is_contiguous()
+    assert ra_f.dtype == torch.float32 and tuple(ra_f.shape) == (n, layers) and not ra_f.is_cuda and ra_f.is_contiguous()
+    assert ra_aff.dtype == torch.float64 and tuple(ra_aff.shape) == (n, layers, 6) and not ra_aff.is_cuda and ra_aff.is_contiguous()
+    if scratch is None:
+        scratch = torch.empty_like(images)
+    assert scratch.dtype == torch.uint8 and scratch.shape == images.shape
+    if stats is None:
+        stats = torch.empty(n, 770, device=images.device, dtype=torch.int32)
+    assert stats.dtype == torch.int32 and stats.numel() >= n * 770
+    d_ops, d_f, d_aff = (t.to(images.device, non_blocking=True) for t in (ra_ops, ra_f, ra_aff))
+    fill = (ctypes.c_int * 3)(*[int(v) for v in record.randaug_fill])
+    _lib.call('saicv_u8_rand_augment', _p(images), _p(scratch), n, h, w, layers, ctypes.c_void_p(ra_ops.data_ptr()),
+              ctypes.c_void_p(ra_f.data_ptr()), ctypes.c_void_p(ra_aff.data_ptr()), _p(d_ops), _p(d_f), _p(d_aff), fill,
+              _p(stats), _stream())
+    return images
+
+
 def nchw_to_nhwc_bf16(x, out=None):
     n, c, h, w = x.shape
     if out is None:

@@ -245,7 +245,8 @@ class CudaPrefetcher:
         normalised batch on the device, on the copy stream (SURVEY.md 8 f3; csrc/capi_input.cu).  Batches that also carry a
         'mixup' record (classification.common.Uint8MixupCutmixClassificationCollater) get the reference's RandomErasing and
         Mixup / CutMix applied by the same pass and are yielded as {'image': fp32 [B, 3, H, W], 'label': fp32 [B, classes]};
-        such a batch without ``normalize`` raises.
+        such a batch without ``normalize`` raises.  When that record also holds RandAugment draws (classification.common.
+        Uint8RandAugment), RandAugment is applied to the uint8 copy first, on the same stream.
         copy_streams > 1: tensors of 32 MB and more are copied in that many chunks on separate streams, so that the copy of
         the next batch keeps its bandwidth while the current step's kernels run (tests/profile_h2d.py measures it)."""
         self.loader = loader
@@ -311,6 +312,12 @@ class CudaPrefetcher:
 
     def _mix(self, slot, img, labels, rec, out):
         from .. import ops
+        if rec.randaug_ops is not None:
+            scratch = slot.get('randaug_scratch')
+            if scratch is None or scratch.shape != img.shape:
+                scratch = slot['randaug_scratch'] = torch.empty_like(img)
+                slot['randaug_stats'] = torch.empty(img.shape[0], 770, dtype=torch.int32, device=self.device)
+            ops.u8_rand_augment(img, rec, scratch=scratch, stats=slot['randaug_stats'])
         used = rec.noise.numel()
         noise = slot.get('mixup_noise')
         if noise is None or noise.numel() < used:
