@@ -21,8 +21,6 @@ extern "C" {
 /* epilogue flags for the GEMM family */
 #define SAICV_EPI_BIAS 1
 #define SAICV_EPI_RELU 2
-#define SAICV_EPI_GELU 4
-#define SAICV_EPI_DIRECT 8 /* debugging: registers -> global without the TMA store path */
 #define SAICV_EPI_RESID 16 /* += fp32 residual[M, N] */
 #define SAICV_EPI_ADD_BF16 32   /* saicv_linear_dgrad: the aux bf16 operand is ADDED to dx */
 #define SAICV_EPI_MUL_DRELU 512 /* saicv_linear_dgrad: the aux bf16 operand is a ReLU output; dx *= (aux > 0) */
@@ -37,18 +35,20 @@ long long saicv_launch_count(void);
 /* ---- dense layers: nn.Linear (vit.py:57-58,87-89; resnet.py:204) ------------------------ */
 /* y[M,N] = resid + row_scale[row / rows_per_scale] * act(x[M,K] w[N,K]^T + bias); x,w bf16; y bf16
  * or fp32 (out_f32); bias [N] fp32, resid [M,N] fp32 and row_scale (drop-path, vit.py:118-135) may
- * be NULL. */
+ * be NULL.  flags: SAICV_EPI_RELU (act); any other bit is refused. */
 int saicv_linear_fwd(const void* x, const void* w, const float* bias, const float* resid,
                      const float* row_scale, int rows_per_scale, float* stats_partial, void* y,
                      int M, int N, int K, int flags, int out_f32, void* stream);
 /* Forward GEMMs (saicv_linear_fwd / saicv_conv_fprop) can accumulate the BatchNorm statistics of
- * their own (bf16) output in the epilogue: pass stats_partial (saicv_gemm_stats_rows(M, N) * 2 * N
- * floats, <= SAICV_BN_PARTIAL_ROWS rows) and hand it to saicv_bn_finalize with that row count. */
+ * their own (bf16) output in the epilogue, with no bias, residual or row scale: pass stats_partial
+ * (saicv_gemm_stats_rows(M, N) * 2 * N floats, <= SAICV_BN_PARTIAL_ROWS rows) and hand it to saicv_bn_finalize with
+ * that row count. */
 int saicv_gemm_stats_rows(long long out_rows, int out_cols);
 /* dx[M,K] = (dy[M,N] w[N,K]) (* gelu'(gelu_pre[M,K])) (+ resid[M,K]); dy,w,gelu_pre bf16; dx bf16
  * or fp32; gelu_pre (the pre-activation saved by the forward, vit.py:87-89) and resid may be NULL.
  * With SAICV_EPI_MUL_DRELU / SAICV_EPI_ADD_BF16 in flags the bf16 operand passed as gelu_pre is instead a
- * ReLU output used as a mask (van.py:46-51: fc2 <- relu) / a second bf16 gradient added to dx. */
+ * ReLU output used as a mask (van.py:46-51: fc2 <- relu) / a second bf16 gradient added to dx.  Any other flag
+ * bit is refused. */
 int saicv_linear_dgrad(const void* dy, const void* w, const float* resid, const void* gelu_pre,
                        void* dx, int M, int N, int K, int flags, int out_f32, void* stream);
 /* dw_partial[splits][N][K] (fp32) = dy[M,N]^T x[M,K], reduction over M split `splits` ways.
@@ -75,7 +75,7 @@ typedef struct {
   int stride, pad;
 } saicv_conv_shape;
 /* y[n,p,q,k] bf16; requires c % 64 == 0 (the 3-channel stem goes through saicv_stem_im2col +
- * saicv_linear_fwd). */
+ * saicv_linear_fwd).  flags: SAICV_EPI_RELU; any other bit is refused. */
 int saicv_conv_fprop(const void* x, const void* w, float* stats_partial, void* y,
                      const saicv_conv_shape* cs, int flags, void* stream);
 /* dx[n,h,w,c] = sum dy[n, h+pad-r, w+pad-s, k] w[k,r,s,c] (+ add[n,h,w,c]) (* mask): stride-1 data
@@ -111,14 +111,11 @@ int saicv_finish_conv_wgrad(const float* partial, float* grad, int splits, int k
 int saicv_reduce_partials(const float* partial, float* out, int splits, long long n,
                           int accumulate, void* stream);
 int saicv_cast_bf16(const float* src, void* dst, long long n, void* stream);
-/* NCHW fp32 image batch -> NHWC bf16 */
-int saicv_nchw_to_nhwc_bf16(const float* x, void* y, int n, int c, int h, int w, void* stream);
 /* NCHW fp32 image batch -> im2col matrix [n*p*q][kpad] bf16 for the 3-channel stem conv
  * (resnet.py:173-180 7x7/2, resnetforcifar.py:38-45 3x3/1; vit.py:31-37 16x16/16 patches);
  * column (ch*R+r)*S8 + s with S8 = S rounded up to a multiple of 8 (every filter row is a whole number of 16-byte
- * vectors; padding columns are zero).  kpad = saicv_stem_kpad(c, r, s) = c*r*S8 rounded up to 64; the weight operand
+ * vectors; padding columns are zero).  kpad = c*r*S8 rounded up to a multiple of 64; the weight operand
  * uses the same column order (saicv_prep_conv_weight / saicv_finish_conv_wgrad with order 1). */
-int saicv_stem_kpad(int c, int r, int s);
 int saicv_stem_im2col(const float* x, void* cols, int n, int c, int h, int w, int r, int s,
                       int stride, int pad, int kpad, void* stream);
 /* u[n, 2p, 2q, c] = dy[n,p,q,c], zero elsewhere; u is [n,h,w,c]. */
@@ -213,9 +210,9 @@ int saicv_layernorm_bwd(const void* dy, const float* x, const float* gamma, cons
                         const float* dres, float* dx, void* dx_bf16, const float* bf16_row_scale,
                         int rows_per_scale, float* partials /* [SAICV_BN_PARTIAL_ROWS][2*c] workspace */,
                         float* dgamma, float* dbeta, long long rows, int c, int accumulate, void* stream);
-/* nn.GELU() exact erf (vit.py:87-89): h = gelu(u); du = dh * gelu'(u); bf16, n % 8 == 0. */
+/* nn.GELU() exact erf (vit.py:87-89): h = gelu(u); bf16, n % 8 == 0.  The backward, dh * gelu'(u), runs in the
+ * epilogue of saicv_linear_dgrad (gelu_pre). */
 int saicv_gelu_fwd(const void* u, void* h, long long n, void* stream);
-int saicv_gelu_bwd(const void* dh, const void* u, void* du, long long n, void* stream);
 /* x[b,0] = cls + pos[0]; x[b,1+i] = patch[b*np+i] + pos[1+i] (vit.py:242-243); all fp32. */
 int saicv_vit_assemble_tokens(const float* patch, const float* cls, const float* pos, float* x,
                               int b, int np, int c, void* stream);

@@ -59,8 +59,6 @@ SIGNATURES = {
     'saicv_finish_conv_wgrad': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_reduce_partials': [c_void_p, c_void_p, c_int, c_ll, c_int, c_void_p],
     'saicv_cast_bf16': [c_void_p, c_void_p, c_ll, c_void_p],
-    'saicv_nchw_to_nhwc_bf16': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
-    'saicv_stem_kpad': [c_int, c_int, c_int],
     'saicv_stem_im2col': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_zero_upsample2': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_add_strided2': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
@@ -82,7 +80,6 @@ SIGNATURES = {
     'saicv_layernorm_fwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_float, c_void_p],
     'saicv_layernorm_bwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
     'saicv_gelu_fwd': [c_void_p, c_void_p, c_ll, c_void_p],
-    'saicv_gelu_bwd': [c_void_p, c_void_p, c_void_p, c_ll, c_void_p],
     'saicv_vit_assemble_tokens': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     'saicv_vit_assemble_tokens_bwd': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_token_pool_fwd': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],

@@ -677,17 +677,6 @@ __global__ void finish_conv_wgrad_kernel(const float* __restrict__ partial, floa
   }
 }
 
-__global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int C, int H,
-                                    int W) {
-  const long long total = (long long)N * H * W;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const long long hw = i % ((long long)H * W);
-    const long long n = i / ((long long)H * W);
-    for (int c = 0; c < C; ++c) y[i * C + c] = __float2bfloat16_rn(x[(n * C + c) * (long long)H * W + hw]);
-  }
-}
-
 // Explicit im2col for 3-channel inputs (ResNet stems, ViT / SAM / VAN patch embeddings).  One block owns T consecutive
 // output pixels of one output row: the (C, R, (T-1)*stride+S) input patch is staged in shared memory with coalesced
 // loads; every thread then produces whole 16-byte vectors of one (pixel, channel, filter row): column
@@ -1128,18 +1117,10 @@ int saicv_finish_conv_wgrad(const float* partial, float* grad, int splits, int k
   return check_launch("finish_conv_wgrad_kernel");
 }
 
-int saicv_nchw_to_nhwc_bf16(const float* x, void* y, int n, int c, int h, int w, void* stream) {
-  nchw_to_nhwc_kernel<<<grid_1d((long long)n * h * w), kThreads, 0, ST>>>(x, reinterpret_cast<__nv_bfloat16*>(y),
-                                                                           n, c, h, w);
-  return check_launch("nchw_to_nhwc_kernel");
-}
-
-int saicv_stem_kpad(int c, int r, int s) { return (c * r * ((s + 7) / 8 * 8) + 63) / 64 * 64; }
-
 int saicv_stem_im2col(const float* x, void* cols, int n, int c, int h, int w, int r, int s, int stride, int pad,
                       int kpad, void* stream) {
   if (kpad % 8 || kpad < r * c * ((s + 7) / 8 * 8))
-    return set_error("saicv_stem_im2col: kpad %d must be a multiple of 8 >= c*r*roundup(s, 8) = %d (saicv_stem_kpad)", kpad, r * c * ((s + 7) / 8 * 8));
+    return set_error("saicv_stem_im2col: kpad %d must be a multiple of 8 >= c*r*roundup(s, 8) = %d", kpad, r * c * ((s + 7) / 8 * 8));
   const int P = (h + 2 * pad - r) / stride + 1, Q = (w + 2 * pad - s) / stride + 1;
   int T = 32;  // output pixels per block; shrink until the staged patch fits in 40 KB
   while (T > 1 && ((size_t)c * r * ((T - 1) * stride + s) * 4) > 40 * 1024) T >>= 1;

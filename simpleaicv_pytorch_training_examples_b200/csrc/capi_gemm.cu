@@ -151,7 +151,7 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, con
   const long long total = (long long)num_m * num_n * p.splits * p.phases * (GemmVariant<VAR>::kBatch ? p.batch : 1);
   const int sms = device()->sms;
   const int grid = (int)(total < sms ? total : sms);
-  const int stat_bytes = (p.epi_flags & EPI_STATS) ? ((8 * p.N + 15) & ~15) : 0;
+  const int stat_bytes = GemmVariant<VAR>::kStatsWarps ? ((8 * p.N + 15) & ~15) : 0;
   int stages = 0, nb = 1;
   pick_smem_split<BN>(p, stat_bytes, &stages, &nb);
   if (stages < 2) return set_error("gemm_sm90_kernel<%d>: %d bytes of statistics do not fit in shared memory", BN, stat_bytes);
@@ -188,12 +188,13 @@ int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorM
   if (p.tile_rows == 0) p.tile_rows = BM;
   if (p.phases == 0) p.phases = 1;
   const bool both = (p.epi_flags & EPI_RESID) && (p.epi_flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU));
-  if (aux && !both && !(p.epi_flags & EPI_DIRECT) && p.splits == 1 && aux_f32 == (p.out_f32 != 0) && aligned16(aux) &&
+  if (aux && !both && p.splits == 1 && aux_f32 == (p.out_f32 != 0) && aligned16(aux) &&
       !getenv("SAICV_GEMM_NO_AUX_TMA")) {
     if (!encode_out(&r, aux, aux_f32, p.N, p.M, p.ldd, 1, 0)) return 2;
     p.aux_tma = 1;
   }
-  // compile-time epilogue variant (gemm_sm90.cuh GemmVariant); SAICV_GEMM_FULL_VARIANT=1 forces the run-time one
+  // compile-time epilogue variant (gemm_sm90.cuh GemmVariant); SAICV_GEMM_FULL_VARIANT=1 forces the run-time one, except
+  // for the phase data gradient and the statistics, which only their own variants compute
   int var = VAR_FULL;
   if (p.a_mode == A_IM2COL_MN && (p.epi_flags || !p.out_f32 || getenv("SAICV_GEMM_FULL_VARIANT")))
     return set_error("the transposed conv weight gradient runs on the plain fp32 epilogue (VAR_PLAIN_F32) only");
@@ -201,10 +202,11 @@ int dispatch(int bn, const CUtensorMap& a, const CUtensorMap& b, const CUtensorM
     if (p.epi_flags || p.aux_tma || p.out_f32 || p.splits != 1)
       return set_error("the phase data gradient has a plain bf16 epilogue: no epilogue flags, aux operand or split-K");
     var = VAR_PHASE_BF16;
+  } else if (p.epi_flags & EPI_STATS) {
+    var = VAR_STATS_BF16;   // the launchers admit statistics only with a plain bf16 output (ReLU at most)
   } else if (!getenv("SAICV_GEMM_FULL_VARIANT")) {
     if (p.aux_tma && !(p.epi_flags & ~GemmVariant<VAR_AUX>::kMask)) var = VAR_AUX;
-    else if (!p.aux_tma && !p.out_f32 && !(p.epi_flags & ~GemmVariant<VAR_PLAIN_BF16>::kMask))
-      var = ((p.epi_flags & EPI_STATS) && !getenv("SAICV_GEMM_INLINE_STATS")) ? VAR_STATS_BF16 : VAR_PLAIN_BF16;
+    else if (!p.aux_tma && !p.out_f32 && !(p.epi_flags & ~GemmVariant<VAR_PLAIN_BF16>::kMask)) var = VAR_PLAIN_BF16;
     else if (!p.aux_tma && p.out_f32 && !(p.epi_flags & ~GemmVariant<VAR_PLAIN_F32>::kMask)) var = VAR_PLAIN_F32;
   }
   if ((p.epi_flags & EPI_MASK_BITS) && var != VAR_AUX)
@@ -248,7 +250,7 @@ int conv_dgrad_phases(const void* dy, const void* w, const void* add, const uint
   p.a_mode = A_IM2COL; p.b_mode = B_MN2D; p.b_cin = cs->c;
   p.g.P = P; p.g.Q = Q; p.g.stride = 1; p.g.lc_h = 0; p.g.lc_w = 0;
   p.g.R = 3; p.g.S = 3; p.g.cchunks = cs->k / 64; p.g.n_img = cs->n;
-  p.epi_flags = 0; p.out_f32 = 0; p.out = dx; p.ldd = cs->c;
+  p.epi_flags = 0; p.out_f32 = 0; p.ldd = cs->c;
   p.tile_rows = rows * Q;
   p.phases = 4;
   // (weight tap, dy offset) of each output parity along one dimension
@@ -326,6 +328,7 @@ int saicv_linear_fwd(const void* x, const void* w, const float* bias, const floa
   if (!device()) return 1;
   if (!aligned16(x) || !aligned16(w) || !aligned16(y) || (K % 8) || (N % (out_f32 ? 4 : 8)))
     return set_error("saicv_linear_fwd: unaligned operand (M=%d N=%d K=%d)", M, N, K);
+  if (flags & ~EPI_RELU) return set_error("saicv_linear_fwd: unknown flags %d", flags);
   const int bn = pick_bn(N);
   CUtensorMap ta, tb, td;
   if (!encode_2d(&ta, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, M, K, 64, 128)) return 2;
@@ -335,16 +338,16 @@ int saicv_linear_fwd(const void* x, const void* w, const float* bias, const floa
   p.M = M; p.N = N; p.num_kb = (K + BK - 1) / BK; p.kb_per_split = p.num_kb; p.splits = 1;
   p.a_mode = A_K2D; p.b_mode = B_K2D;
   p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
-  p.epi_flags = (flags & (EPI_RELU | EPI_GELU | EPI_DIRECT)) | (bias ? EPI_BIAS : 0) | (resid ? EPI_RESID : 0) |
+  p.epi_flags = flags | (bias ? EPI_BIAS : 0) | (resid ? EPI_RESID : 0) |
                 (row_scale ? EPI_ROW_SCALE : 0);
   if (row_scale && rows_per_scale <= 0) return set_error("saicv_linear_fwd: rows_per_scale must be > 0");
   p.row_scale = row_scale; p.rows_per_scale = rows_per_scale;
   if (stats_partial) {
-    if (bias || resid || out_f32 || (flags & EPI_DIRECT))
-      return set_error("saicv_linear_fwd: stats_partial needs a plain bf16 output through the TMA-store epilogue (no bias / residual)");
+    if (bias || resid || row_scale || out_f32)
+      return set_error("saicv_linear_fwd: stats_partial needs a plain bf16 output (no bias / residual / row scale)");
     p.epi_flags |= EPI_STATS; p.stats_partial = stats_partial;
   }
-  p.out_f32 = out_f32; p.bias = bias; p.resid = resid; p.out = y; p.ldd = N; p.split_stride = 0;
+  p.out_f32 = out_f32; p.bias = bias; p.resid = resid; p.ldd = N;
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream, resid, true);
 }
 
@@ -353,6 +356,7 @@ int saicv_linear_dgrad(const void* dy, const void* w, const float* resid, const 
   if (!device()) return 1;
   if (!aligned16(dy) || !aligned16(w) || !aligned16(dx) || (K % 8) || (N % 8))
     return set_error("saicv_linear_dgrad: unaligned operand (M=%d N=%d K=%d)", M, N, K);
+  if (flags & ~(EPI_MUL_DRELU | EPI_RESID_BF16)) return set_error("saicv_linear_dgrad: unknown flags %d", flags);
   // GEMM: D[M, K] = dy[M, N] * W[N, K]; reduction over N; B = W stored [N(red)][K(out)] -> MN-major
   const int bn = pick_bn(K);
   CUtensorMap ta, tb, td;
@@ -365,9 +369,9 @@ int saicv_linear_dgrad(const void* dy, const void* w, const float* resid, const 
   p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
   // aux bf16 operand [M, K]: SAICV_EPI_MUL_DRELU -> ReLU output (mask), SAICV_EPI_ADD_BF16 -> added, default -> dGELU pre-activation
   const int aux_mode = !gelu_pre ? 0 : (flags & EPI_MUL_DRELU) ? EPI_MUL_DRELU : (flags & EPI_RESID_BF16) ? EPI_RESID_BF16 : EPI_MUL_DGELU;
-  p.epi_flags = (flags & EPI_DIRECT) | (resid ? EPI_RESID : 0) | aux_mode;
+  p.epi_flags = (resid ? EPI_RESID : 0) | aux_mode;
   if (gelu_pre && !aligned16(gelu_pre)) return set_error("saicv_linear_dgrad: unaligned aux operand");
-  p.out_f32 = out_f32; p.resid = resid; p.resid_bf16 = gelu_pre; p.out = dx; p.ldd = K;
+  p.out_f32 = out_f32; p.resid = resid; p.resid_bf16 = gelu_pre; p.ldd = K;
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream, resid ? (const void*)resid : gelu_pre, resid != nullptr);
 }
 
@@ -389,7 +393,7 @@ int saicv_linear_wgrad(const void* dy, const void* x, float* dw_partial, int M, 
   if (p.splits != splits) return set_error("saicv_linear_wgrad: splits=%d leaves an empty split (use saicv_wgrad_splits)", splits);
   p.a_mode = A_MN2D; p.b_mode = B_MN2D;
   p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
-  p.epi_flags = 0; p.out_f32 = 1; p.out = dw_partial; p.ldd = K; p.split_stride = (long long)N * K;
+  p.epi_flags = 0; p.out_f32 = 1; p.ldd = K;
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream);
 }
 
@@ -400,6 +404,7 @@ int saicv_conv_fprop(const void* x, const void* w, float* stats_partial, void* y
   if (!device()) return 1;
   if (cs->c % 64 || cs->k % 8 || !aligned16(x) || !aligned16(w) || !aligned16(y))
     return set_error("saicv_conv_fprop: needs c%%64==0, k%%8==0 and 16B-aligned pointers (c=%d k=%d)", cs->c, cs->k);
+  if (flags & ~EPI_RELU) return set_error("saicv_conv_fprop: unknown flags %d", flags);
   const int P = conv_out(cs->h, cs->pad, cs->r, cs->stride), Q = conv_out(cs->w, cs->pad, cs->s, cs->stride);
   const long long M = (long long)cs->n * P * Q;
   const int Kred = cs->r * cs->s * cs->c;
@@ -415,9 +420,8 @@ int saicv_conv_fprop(const void* x, const void* w, float* stats_partial, void* y
   p.a_mode = A_IM2COL; p.b_mode = B_K2D; p.b_cin = cs->c;
   p.g.P = P; p.g.Q = Q; p.g.stride = cs->stride; p.g.lc_h = -cs->pad; p.g.lc_w = -cs->pad;
   p.g.R = cs->r; p.g.S = cs->s; p.g.cchunks = cs->c / 64; p.g.n_img = cs->n;
-  p.epi_flags = flags & (EPI_RELU | EPI_DIRECT); p.out_f32 = 0; p.out = y; p.ldd = cs->k;
+  p.epi_flags = flags; p.out_f32 = 0; p.ldd = cs->k;
   if (stats_partial) {
-    if (flags & EPI_DIRECT) return set_error("saicv_conv_fprop: stats_partial is not available with SAICV_EPI_DIRECT");
     p.epi_flags |= EPI_STATS; p.stats_partial = stats_partial;
   }
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream);
@@ -446,7 +450,7 @@ int saicv_conv_dgrad(const void* dy, const void* w, const void* add, const uint3
   p.g.P = cs->h; p.g.Q = cs->w; p.g.stride = 1; p.g.lc_h = lc_h; p.g.lc_w = lc_w;
   p.g.R = cs->r; p.g.S = cs->s; p.g.cchunks = cs->k / 64; p.g.n_img = cs->n;
   p.epi_flags = (add ? EPI_RESID_BF16 : 0) | (mask_bits ? EPI_MASK_BITS : 0);
-  p.resid_bf16 = add; p.mask_bits = mask_bits; p.out_f32 = 0; p.out = dx; p.ldd = cs->c;
+  p.resid_bf16 = add; p.mask_bits = mask_bits; p.out_f32 = 0; p.ldd = cs->c;
   if (add && !aligned16(add)) return set_error("saicv_conv_dgrad: unaligned `add`");
   if (mask_bits && !add) return set_error("saicv_conv_dgrad: mask_bits is applied in the epilogue of the fused `add` only");
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream, add, false);
@@ -481,7 +485,7 @@ int saicv_conv_wgrad(const void* dy, const void* x, float* dw_partial, const sai
   p.a_mode = tr ? A_IM2COL_MN : A_MN2D; p.b_mode = tr ? B_MN2D : B_IM2COL;
   p.g.P = P; p.g.Q = Q; p.g.stride = cs->stride; p.g.lc_h = -cs->pad; p.g.lc_w = -cs->pad;
   p.g.R = cs->r; p.g.S = cs->s; p.g.cchunks = cs->c / 64; p.g.n_img = cs->n;
-  p.epi_flags = 0; p.out_f32 = 1; p.out = dw_partial; p.ldd = p.N; p.split_stride = (long long)cs->k * Ncols;
+  p.epi_flags = 0; p.out_f32 = 1; p.ldd = p.N;
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream);
 }
 
@@ -514,7 +518,7 @@ int saicv_ns_gemm(int mode, const void* x, const void* y, void* out, int batch, 
   p.M = m; p.N = out_cols; p.num_kb = (red + BK - 1) / BK; p.kb_per_split = p.num_kb; p.splits = 1;
   p.a_mode = A_K2D; p.b_mode = mode == 0 ? B_K2D : B_MN2D;
   p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
-  p.out_f32 = 0; p.out = out; p.ldd = out_cols; p.tile_rows = BM; p.phases = 1;
+  p.out_f32 = 0; p.ldd = out_cols; p.tile_rows = BM; p.phases = 1;
   p.batch = batch; p.alpha = alpha; p.beta = beta;
   if (mode != 0) {
     const void* aux = mode == 1 ? x : y;

@@ -143,7 +143,7 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restrict__ x,
 
 // ----------------------------------------------------------------------------- GELU (exact, erf)
 // gelu_terms (gelu_math.cuh): A&S 7.1.26 erf with one ex2 and one rcp MUFU per element; libdevice erff costs ~40
-// instructions per element, which made these streaming kernels compute bound.
+// instructions per element, which made this streaming kernel compute bound.
 __device__ __forceinline__ float gelu_val(float x) { return gelu_erf(x); }
 __global__ void gelu_fwd_kernel(const uint4* __restrict__ u, uint4* __restrict__ h, long long nvec) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
@@ -155,22 +155,6 @@ __global__ void gelu_fwd_kernel(const uint4* __restrict__ u, uint4* __restrict__
       w[k] = pack2(gelu_val(f.x), gelu_val(f.y));
     }
     h[i] = make_uint4(w[0], w[1], w[2], w[3]);
-  }
-}
-__device__ __forceinline__ float gelu_grad(float x) { return gelu_erf_grad(x); }
-// du = dh * gelu'(u)
-__global__ void gelu_bwd_kernel(const uint4* __restrict__ dh, const uint4* __restrict__ u, uint4* __restrict__ du,
-                                long long nvec) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
-    const uint4 a = dh[i], b = u[i];
-    const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
-    uint32_t o[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float2 d = unpack2(aw[k]), x = unpack2(bw[k]);
-      o[k] = pack2(d.x * gelu_grad(x.x), d.y * gelu_grad(x.y));
-    }
-    du[i] = make_uint4(o[0], o[1], o[2], o[3]);
   }
 }
 
@@ -291,13 +275,6 @@ int saicv_gelu_fwd(const void* u, void* h, long long n, void* stream) {
   if (n % 8) return set_error("saicv_gelu_fwd: n %% 8 != 0");
   gelu_fwd_kernel<<<grid_1d(n / 8), 256, 0, ST>>>(reinterpret_cast<const uint4*>(u), reinterpret_cast<uint4*>(h), n / 8);
   return check_launch("gelu_fwd_kernel");
-}
-
-int saicv_gelu_bwd(const void* dh, const void* u, void* du, long long n, void* stream) {
-  if (n % 8) return set_error("saicv_gelu_bwd: n %% 8 != 0");
-  gelu_bwd_kernel<<<grid_1d(n / 8), 256, 0, ST>>>(reinterpret_cast<const uint4*>(dh), reinterpret_cast<const uint4*>(u),
-                                                  reinterpret_cast<uint4*>(du), n / 8);
-  return check_launch("gelu_bwd_kernel");
 }
 
 int saicv_vit_assemble_tokens(const float* patch, const float* cls, const float* pos, float* x, int b, int np, int c,

@@ -28,7 +28,7 @@ namespace saicv {
 
 enum : int { A_K2D = 0, A_IM2COL = 1, A_MN2D = 2, A_IM2COL_MN = 3 };
 enum : int { B_K2D = 0, B_MN2D = 2, B_IM2COL = 3 };
-enum : int { EPI_BIAS = 1, EPI_RELU = 2, EPI_GELU = 4, EPI_DIRECT = 8, EPI_RESID = 16, EPI_RESID_BF16 = 32,
+enum : int { EPI_BIAS = 1, EPI_RELU = 2, EPI_RESID = 16, EPI_RESID_BF16 = 32,
               EPI_MUL_DGELU = 64, EPI_ROW_SCALE = 128, EPI_STATS = 256, EPI_MUL_DRELU = 512, EPI_MASK_BITS = 1024,
               EPI_AXPBY = 2048 };
 
@@ -83,9 +83,7 @@ struct GemmParams {
   const void* resid_bf16;  // bf16 [M, ldd]: added (EPI_RESID_BF16); as pre-activation u, D *= gelu'(u) (EPI_MUL_DGELU); as ReLU output, D *= (r > 0) (EPI_MUL_DRELU)
   const float* row_scale;  // EPI_ROW_SCALE: D = resid + row_scale[row / rows_per_scale] * (acc + bias) (drop-path)
   int rows_per_scale;
-  void* out;           // direct-store path
-  long long ldd;       // leading dimension of D in elements
-  long long split_stride;  // elements between split-K partial outputs
+  long long ldd;       // leading dimension of D (and of the aux operand) in elements
   int num_stages;      // smem ring depth actually used (<= GemmCfg::kStages)
   int store_bufs;      // 1..kMaxStoreBufs: the epilogue rotates through 2 * store_bufs staging slices
   int aux_tma;         // 1: the aux operand of the epilogue (resid when out_f32, resid_bf16 otherwise) has the
@@ -112,8 +110,8 @@ struct GemmParams {
 // instruction stream (with every feature a run-time branch, branch resolution and instruction fetch take a large share of
 // the issue slots of the short-reduction launches, whose pace the epilogue sets).  No variant spills (ptxas -v); VAR_FULL
 // and VAR_AUX at BN = 128 sit at the 168-register cap of 384 threads.
-//   VAR_FULL        every flag but EPI_MASK_BITS / output type at run time (GELU forward, EPI_DIRECT, per-thread aux loads)
-//   VAR_PLAIN_BF16  bf16 output, optional bias / ReLU / BatchNorm statistics       (conv fprop, plain dgrad, Linear)
+//   VAR_FULL        every flag but EPI_MASK_BITS / EPI_STATS / output type at run time (per-thread aux loads)
+//   VAR_PLAIN_BF16  bf16 output, optional bias / ReLU                                (conv fprop, plain dgrad, Linear)
 //   VAR_PLAIN_F32   fp32 output, optional bias                                       (split-K weight gradients, fp32 Linear)
 //   VAR_AUX         aux operand by TMA (fp32 residual, bf16 addend / ReLU mask / GELU pre-activation), bias, row scale,
 //                   1-bit ReLU mask (conv dgrad + shortcut gradient, masked by the previous residual block's output ReLU)
@@ -128,8 +126,9 @@ struct GemmParams {
 enum : int { VAR_FULL = 0, VAR_PLAIN_BF16 = 1, VAR_PLAIN_F32 = 2, VAR_AUX = 3, VAR_STATS_BF16 = 4, VAR_PHASE_BF16 = 5, VAR_NS = 6 };
 template <int VAR>
 struct GemmVariant {
-  static constexpr int kMask = VAR == VAR_FULL ? (0x7fffffff & ~EPI_MASK_BITS)
-                               : (VAR == VAR_PLAIN_BF16 || VAR == VAR_STATS_BF16) ? (EPI_BIAS | EPI_RELU | EPI_STATS)
+  static constexpr int kMask = VAR == VAR_FULL ? (0x7fffffff & ~(EPI_MASK_BITS | EPI_STATS))
+                               : VAR == VAR_PLAIN_BF16 ? (EPI_BIAS | EPI_RELU)
+                               : VAR == VAR_STATS_BF16 ? (EPI_BIAS | EPI_RELU | EPI_STATS)
                                : VAR == VAR_PLAIN_F32 ? EPI_BIAS
                                : VAR == VAR_PHASE_BF16 ? 0
                                : VAR == VAR_NS ? EPI_AXPBY
@@ -231,13 +230,12 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int flags = p.epi_flags & V::kMask;          // bits outside the variant's mask are known zeros
   const bool out_f32 = V::kOut == 0 ? (p.out_f32 != 0) : (V::kOut == 2);
   const int nstages = p.num_stages;
-  const bool do_stats = (flags & EPI_STATS) != 0;
   uint8_t* sA = smem;
   uint8_t* sB = smem + nstages * kABytes;
   uint8_t* sD = smem + nstages * Cfg::kStageBytes;
   const int NB = p.store_bufs;
-  float* sStat = reinterpret_cast<float*>(sD + 2 * NB * kStoreBufBytes);  // [2][N] when EPI_STATS
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sD + 2 * NB * kStoreBufBytes + (do_stats ? ((8 * p.N + 15) & ~15) : 0));
+  float* sStat = reinterpret_cast<float*>(sD + 2 * NB * kStoreBufBytes);  // [2][N] in VAR_STATS_BF16
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sD + 2 * NB * kStoreBufBytes + (V::kStatsWarps ? ((8 * p.N + 15) & ~15) : 0));
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* aux_bar = empty_bar + kStages;   // [2 * kMaxStoreBufs]: aux slice landed in staging slice b
   uint64_t* staged_bar = aux_bar + 2 * kMaxStoreBufs;    // [2 * kMaxStoreBufs] VAR_STATS_BF16: staging slice b is staged
@@ -404,7 +402,6 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const uint32_t bar_id = 1;
     const int NBT = 2 * NB;                           // staging slices of the tile
     float* const xp = sXpose + e * 32 * kXposeStride;
-    const bool direct = (flags & EPI_DIRECT) != 0;
     const bool aux_tma = V::kAux == 0 ? (p.aux_tma != 0) : (V::kAux == 2);
     constexpr int NCH = BN / 32;                      // 32-column chunks of a tile
     const bool a_mn = VAR == VAR_PLAIN_F32 ? (p.a_mode == A_MN2D || p.a_mode == A_IM2COL_MN) : (p.a_mode == A_MN2D);
@@ -432,11 +429,10 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (aux_tma && leader) {
       for (int i = 0; i < NBT - 1; ++i) request_aux();
     }
-    constexpr int kStatBarThreads = V::kStatsWarps ? 384 : 256;
     uint32_t sd_phase = 0;     // VAR_STATS_BF16: bit b = parity of the stats-done barrier of staging slice b
-    if (do_stats) {
+    if (V::kStatsWarps) {
       for (int j = threadIdx.x - 128; j < 2 * p.N; j += 256) sStat[j] = 0.f;
-      named_bar_sync(3, kStatBarThreads);
+      named_bar_sync(3, 384);   // with the four stats warps
     }
     for (int w = blockIdx.x; w < total; w += gridDim.x) {
       const int ph = (V::kPhases || V::kBatch) ? w / per_phase : 0;
@@ -505,11 +501,11 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
         __syncwarp();
         if (aux_tma && s_begin) mbar_wait(&aux_bar[bufi], (aux_phase >> bufi) & 1u);   // the aux slice has landed in this staging slice
-        if (!direct && s_begin && !aux_tma) {
+        if (s_begin && !aux_tma) {
           // the store that last read this staging slice (2*NB slices ago) must have drained it (and the stats warps too)
           if (leader) {
             tma_store_wait_read_n(NBT - 1);
-            if (V::kStatsWarps && do_stats) {
+            if (V::kStatsWarps) {
               mbar_wait(&sdone_bar[bufi], ((sd_phase >> bufi) & 1u) ^ 1u);
               sd_phase ^= (1u << bufi);
             }
@@ -534,10 +530,6 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (flags & EPI_BIAS) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) f[j] += __shfl_sync(0xffffffffu, bv, hh * 16 + g * 8 + j);
-          }
-          if (flags & EPI_GELU) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] = gelu_erf(f[j]);
           }
           if (flags & EPI_RELU) {
 #pragma unroll
@@ -589,20 +581,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
             for (int j = 0; j < 8; ++j) f[j] *= ((mbits >> (g * 8 + j)) & 1u) ? 1.f : 0.f;
           }
-          if (direct) {
-            if (row < p.M && tcol + g * 8 < p.N) {
-              if (out_f32) {
-                float* o = reinterpret_cast<float*>(p.out) + split * p.split_stride + row * p.ldd + tcol + g * 8;
-                *reinterpret_cast<float4*>(o) = make_float4(f[0], f[1], f[2], f[3]);
-                if (tcol + g * 8 + 4 < p.N) *reinterpret_cast<float4*>(o + 4) = make_float4(f[4], f[5], f[6], f[7]);
-              } else {
-                __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + split * p.split_stride +
-                                   row * p.ldd + tcol + g * 8;
-                *reinterpret_cast<uint4*>(o) = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]),
-                                                          pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
-              }
-            }
-          } else if (out_f32) {
+          if (out_f32) {
             // one 128 B (32 x fp32) slice per TMA store
 #pragma unroll
             for (int j = 0; j < 2; ++j)
@@ -615,147 +594,100 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                            pack_bf16x2(f[6], f[7]));
           }
         }
-        if (!direct) {
-          if (s_end) {
-            fence_proxy_async_smem();
-            named_bar_sync(bar_id, 256);
-            const int scol = out_f32 ? col0 : col0 - 32;
-            if (leader) {
-              if (scol < p.N && phases > 1) {
-                const int ab = p.ph_out[ph];
-                asm volatile(
-                    "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(
-                        reinterpret_cast<uint64_t>(&tmD)),
-                    "r"(smem_u32(sbuf)), "r"(scol), "r"(ab & 1), "r"(0), "r"(ab >> 1), "r"(m0 / p.g.Q)
-                    : "memory");
-              } else if (scol < p.N) {
-                asm volatile(
-                    "cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                        reinterpret_cast<uint64_t>(&tmD)),
-                    "r"(smem_u32(sbuf)), "r"(scol), "r"(m0), "r"(V::kBatch ? ph : split)
-                    : "memory");
-              }
-              tma_store_commit();
-              if (aux_tma) {
-                // the slice that store s-1 read becomes the landing buffer of aux slice s + LA
-                tma_store_wait_read_n(1);
-                request_aux();
-              }
+        if (s_end) {
+          fence_proxy_async_smem();
+          named_bar_sync(bar_id, 256);
+          const int scol = out_f32 ? col0 : col0 - 32;
+          if (leader) {
+            if (scol < p.N && phases > 1) {
+              const int ab = p.ph_out[ph];
+              asm volatile(
+                  "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(
+                      reinterpret_cast<uint64_t>(&tmD)),
+                  "r"(smem_u32(sbuf)), "r"(scol), "r"(ab & 1), "r"(0), "r"(ab >> 1), "r"(m0 / p.g.Q)
+                  : "memory");
+            } else if (scol < p.N) {
+              asm volatile(
+                  "cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                      reinterpret_cast<uint64_t>(&tmD)),
+                  "r"(smem_u32(sbuf)), "r"(scol), "r"(m0), "r"(V::kBatch ? ph : split)
+                  : "memory");
             }
-            if (V::kStatsWarps && do_stats) {
-              if (leader) mbar_arrive(&staged_bar[bufi]);   // hand the slice to the stats warps
-            } else if (do_stats && half == (bufi & 1)) {   // 2*NB slices in rotation: the slice count's parity
-              // BatchNorm statistics of the slice just staged (the bf16 values as stored), read back
-              // from the swizzled buffer (conflict free: a warp reads the 128 contiguous bytes of one
-              // row) concurrently with the TMA store of the same buffer.  Rows >= M / cols >= N are zero.
-              // Fixed summation order (bit-reproducible, no atomics): the warpgroups take alternate slices;
-              // warp wq of the one whose turn it is owns columns wq*16..+15 of the slice for all 128 rows.
-              // Lane l reads 8 bytes (4 columns) of row
-              // i*8 + l/4: the 8 rows of one load hit 8 distinct swizzled 16-byte chunks, so the
-              // 256-byte request is conflict free.  The 8 row-lanes are then folded by shuffles and
-              // lanes 0..3 add to the accumulators they alone own.
-              const int wq = q;
-              const int piece = lane & 3;
-              const int chunk = wq * 2 + (piece >> 1);
-              const int r0 = lane >> 2;        // row of load i is i*8 + r0: its swizzle phase (row & 7) is r0 for every i
-              const uint8_t* const sp = sbuf + r0 * 128 + ((chunk ^ r0) << 4) + (piece & 1) * 8;
-              float sx[4] = {0.f, 0.f, 0.f, 0.f}, sq[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const uint2 w2 = *reinterpret_cast<const uint2*>(sp + i * 1024);
-                const float a0 = __uint_as_float(w2.x << 16), a1 = __uint_as_float(w2.x & 0xffff0000u);
-                const float b0 = __uint_as_float(w2.y << 16), b1 = __uint_as_float(w2.y & 0xffff0000u);
-                sx[0] += a0; sq[0] = fmaf(a0, a0, sq[0]);
-                sx[1] += a1; sq[1] = fmaf(a1, a1, sq[1]);
-                sx[2] += b0; sq[2] = fmaf(b0, b0, sq[2]);
-                sx[3] += b1; sq[3] = fmaf(b1, b1, sq[3]);
-              }
-#pragma unroll
-              for (int o = 4; o < 32; o <<= 1) {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  sx[j] += __shfl_xor_sync(0xffffffffu, sx[j], o);
-                  sq[j] += __shfl_xor_sync(0xffffffffu, sq[j], o);
-                }
-              }
-              const int gcol = scol + wq * 16 + piece * 4;
-              if (lane < 4 && gcol < p.N) {  // N % 8 == 0: the 4 columns are valid together
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  sStat[gcol + j] += sx[j];
-                  sStat[p.N + gcol + j] += sq[j];
-                }
-              }
+            tma_store_commit();
+            if (aux_tma) {
+              // the slice that store s-1 read becomes the landing buffer of aux slice s + LA
+              tma_store_wait_read_n(1);
+              request_aux();
             }
-            aux_phase ^= (1u << bufi);
-            if (++bufi == NBT) bufi = 0;
           }
+          if (V::kStatsWarps && leader) mbar_arrive(&staged_bar[bufi]);   // hand the slice to the stats warps
+          aux_phase ^= (1u << bufi);
+          if (++bufi == NBT) bufi = 0;
         }
       }
     }
     if (leader) tma_store_wait<0>();
-    if (do_stats) {
-      named_bar_sync(3, kStatBarThreads);
+    if (V::kStatsWarps) {
+      named_bar_sync(3, 384);
       float* dst = p.stats_partial + (long long)blockIdx.x * 2 * p.N;
       for (int j = threadIdx.x - 128; j < 2 * p.N; j += 256) dst[j] = sStat[j];
     }
   } else if (V::kStatsWarps && warp >= 12) {
     // ================================================================ statistics warps (VAR_STATS_BF16)
     // Warp wq owns columns wq*16 .. +15 of every staged 64-column slice for all 128 rows (fixed
-    // ownership and summation order: bit-reproducible, no atomics).  Lane l reads 8 bytes (4 columns) of row i*8 + l/4;
-    // the 8 row-lanes are folded by shuffles and lanes 0..3 add to the shared-memory accumulators they alone own.
-    if (do_stats) {
-      const int wq = warp - 12;
-      const int piece = lane & 3;
-      const int chunk = wq * 2 + (piece >> 1);
-      const int r0 = lane >> 2;
-      const int soff = r0 * 128 + ((chunk ^ r0) << 4) + (piece & 1) * 8;
-      const int NBT = 2 * NB;
-      int b = 0;                         // staging slice of the next output slice (the epilogue's rotation)
-      uint32_t st_phase = 0u;
-      named_bar_sync(3, 384);            // accumulators zeroed by the epilogue warps
-      for (int w = blockIdx.x; w < total; w += gridDim.x) {
-        const int n0 = (w % num_n) * BN;
+    // ownership and summation order: bit-reproducible, no atomics).  Lane l reads 8 bytes (4 columns) of row i*8 + l/4:
+    // the 8 rows of one load hit 8 distinct swizzled 16-byte chunks, so the 256-byte request is conflict free.  The 8
+    // row-lanes are folded by shuffles and lanes 0..3 add to the shared-memory accumulators they alone own.
+    const int wq = warp - 12;
+    const int piece = lane & 3;
+    const int chunk = wq * 2 + (piece >> 1);
+    const int r0 = lane >> 2;
+    const int soff = r0 * 128 + ((chunk ^ r0) << 4) + (piece & 1) * 8;
+    const int NBT = 2 * NB;
+    int b = 0;                         // staging slice of the next output slice (the epilogue's rotation)
+    uint32_t st_phase = 0u;
+    named_bar_sync(3, 384);            // accumulators zeroed by the epilogue warps
+    for (int w = blockIdx.x; w < total; w += gridDim.x) {
+      const int n0 = (w % num_n) * BN;
 #pragma unroll 1
-        for (int j = 0; j < BN / 64; ++j) {
-          mbar_wait(&staged_bar[b], (st_phase >> b) & 1u);
-          const uint8_t* const sp = sD + b * kStoreBufBytes + soff;
-          float sx[4] = {0.f, 0.f, 0.f, 0.f}, sq[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int j = 0; j < BN / 64; ++j) {
+        mbar_wait(&staged_bar[b], (st_phase >> b) & 1u);
+        const uint8_t* const sp = sD + b * kStoreBufBytes + soff;
+        float sx[4] = {0.f, 0.f, 0.f, 0.f}, sq[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const uint2 w2 = *reinterpret_cast<const uint2*>(sp + i * 1024);
-            const float a0 = __uint_as_float(w2.x << 16), a1 = __uint_as_float(w2.x & 0xffff0000u);
-            const float b0 = __uint_as_float(w2.y << 16), b1 = __uint_as_float(w2.y & 0xffff0000u);
-            sx[0] += a0; sq[0] = fmaf(a0, a0, sq[0]);
-            sx[1] += a1; sq[1] = fmaf(a1, a1, sq[1]);
-            sx[2] += b0; sq[2] = fmaf(b0, b0, sq[2]);
-            sx[3] += b1; sq[3] = fmaf(b1, b1, sq[3]);
-          }
-          // the slice is read: the epilogue may reuse it (after its TMA store has drained it too)
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&sdone_bar[b]);
-#pragma unroll
-          for (int o = 4; o < 32; o <<= 1) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              sx[k] += __shfl_xor_sync(0xffffffffu, sx[k], o);
-              sq[k] += __shfl_xor_sync(0xffffffffu, sq[k], o);
-            }
-          }
-          const int gcol = n0 + j * 64 + wq * 16 + piece * 4;
-          if (lane < 4 && gcol < p.N) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              sStat[gcol + k] += sx[k];
-              sStat[p.N + gcol + k] += sq[k];
-            }
-          }
-          st_phase ^= (1u << b);
-          b = (b + 1 == NBT) ? 0 : b + 1;
+        for (int i = 0; i < 16; ++i) {
+          const uint2 w2 = *reinterpret_cast<const uint2*>(sp + i * 1024);
+          const float a0 = __uint_as_float(w2.x << 16), a1 = __uint_as_float(w2.x & 0xffff0000u);
+          const float b0 = __uint_as_float(w2.y << 16), b1 = __uint_as_float(w2.y & 0xffff0000u);
+          sx[0] += a0; sq[0] = fmaf(a0, a0, sq[0]);
+          sx[1] += a1; sq[1] = fmaf(a1, a1, sq[1]);
+          sx[2] += b0; sq[2] = fmaf(b0, b0, sq[2]);
+          sx[3] += b1; sq[3] = fmaf(b1, b1, sq[3]);
         }
+        // the slice is read: the epilogue may reuse it (after its TMA store has drained it too)
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&sdone_bar[b]);
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            sx[k] += __shfl_xor_sync(0xffffffffu, sx[k], o);
+            sq[k] += __shfl_xor_sync(0xffffffffu, sq[k], o);
+          }
+        }
+        const int gcol = n0 + j * 64 + wq * 16 + piece * 4;
+        if (lane < 4 && gcol < p.N) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            sStat[gcol + k] += sx[k];
+            sStat[p.N + gcol + k] += sq[k];
+          }
+        }
+        st_phase ^= (1u << b);
+        b = (b + 1 == NBT) ? 0 : b + 1;
       }
-      named_bar_sync(3, 384);            // all slices accumulated: the epilogue warps write the partial row
     }
+    named_bar_sync(3, 384);            // all slices accumulated: the epilogue warps write the partial row
   }
 }
 

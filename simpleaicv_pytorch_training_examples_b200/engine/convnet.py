@@ -24,8 +24,6 @@ from .operands import CONV, STEM, Linear, Operand, rows_wgrad
 from .runtime import Runtime
 
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SILU = 0, 1, 2, 3
-# BatchNorm batch statistics are accumulated by the conv GEMM's epilogue instead of a separate pass over y
-FUSE_BN_STATS = True
 
 
 def _round_up(v, m):
@@ -171,7 +169,7 @@ class ConvBN:
         """conv -> BN -> (+res) -> act (or act then +res when res_after_act).  res_ss: BN scale/shift
         applied to `res` on the fly (downsample branch).  want_mask: also keep the ReLU mask of the
         output, packed to one bit per element, as tape['bits']."""
-        y = self.conv_fwd(a_in, tape, want_stats=training and FUSE_BN_STATS)
+        y = self.conv_fwd(a_in, tape, want_stats=training)
         self.bn_prepare(y, training, tape)
         out = torch.empty_like(y)
         act = self.act | (8 if (self.res_after_act and res is not None) else 0)
@@ -271,7 +269,7 @@ class ResidualBlockRT:
         # the ReLU mask of the block output, one bit per element: the backward applies it instead of reading `out`
         if self.down is not None:
             td = tape.setdefault('d', dict())
-            yd = self.down.conv_fwd(a_in, td, want_stats=training and FUSE_BN_STATS)
+            yd = self.down.conv_fwd(a_in, td, want_stats=training)
             self.down.bn_prepare(yd, training, td)
             out = last.forward(x, tl, training, res=yd, res_ss=td['ss'], want_mask=training)
         else:

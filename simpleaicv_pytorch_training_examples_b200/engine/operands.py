@@ -90,7 +90,7 @@ class Linear:
                               row_scale=row_scale, rows_per_scale=rows_per_scale)
 
     def fwd_flags(self, x, flags):
-        """Forward with an activation fused in the epilogue (ops.EPI_RELU / ops.EPI_GELU)."""
+        """Forward with ReLU fused in the epilogue (flags = ops.EPI_RELU)."""
         return ops.linear_fwd(x, self.op.w, bias=self.b_pad, flags=flags)
 
     def bwd(self, dy, x, sink, need_dx=True, gelu_pre=None, relu_out=None, add=None):

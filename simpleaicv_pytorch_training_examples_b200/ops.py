@@ -11,7 +11,7 @@ import torch
 from . import _lib
 from ._lib import ConvShape
 
-EPI_BIAS, EPI_RELU, EPI_GELU, EPI_DIRECT, EPI_RESID, EPI_ADD_BF16, EPI_MUL_DRELU = 1, 2, 4, 8, 16, 32, 512
+EPI_BIAS, EPI_RELU, EPI_RESID, EPI_ADD_BF16, EPI_MUL_DRELU = 1, 2, 16, 32, 512
 
 
 def _p(t):
@@ -239,14 +239,6 @@ def u8_rand_augment(images, record, scratch=None, stats=None):
               ctypes.c_void_p(ra_f.data_ptr()), ctypes.c_void_p(ra_aff.data_ptr()), _p(d_ops), _p(d_f), _p(d_aff), fill,
               _p(stats), _stream())
     return images
-
-
-def nchw_to_nhwc_bf16(x, out=None):
-    n, c, h, w = x.shape
-    if out is None:
-        out = torch.empty(n, h, w, c, device=x.device, dtype=torch.bfloat16)
-    _lib.call('saicv_nchw_to_nhwc_bf16', _p(x), _p(out), n, c, h, w, _stream())
-    return out
 
 
 def stem_kpad(c, r, s):
@@ -482,13 +474,6 @@ def gelu_fwd(u, out=None):
     if out is None:
         out = torch.empty_like(u)
     _lib.call('saicv_gelu_fwd', _p(u), _p(out), u.numel(), _stream())
-    return out
-
-
-def gelu_bwd(dh, u, out=None):
-    if out is None:
-        out = torch.empty_like(u)
-    _lib.call('saicv_gelu_bwd', _p(dh), _p(u), _p(out), u.numel(), _stream())
     return out
 
 

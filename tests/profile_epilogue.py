@@ -1,5 +1,5 @@
 """Cost of the GEMM epilogue variants at the ViT-B fc2 data-gradient shape (M 50432, reduction 768, output 3072) and
-the SAM-H one (M 32768, 1280 -> 5120): plain, + dGELU(aux), * (aux > 0), + aux; and the unfused alternative."""
+the SAM-H one (M 32768, 1280 -> 5120): plain, + dGELU(aux), * (aux > 0), + aux."""
 import sys
 
 import torch
@@ -26,14 +26,12 @@ for M, N, K in ((50432, 768, 3072), (32768, 1280, 5120)):
     w = torch.randn(N, K, device='cuda').bfloat16()
     aux = torch.randn(M, K, device='cuda').bfloat16()
     out = torch.empty(M, K, device='cuda', dtype=torch.bfloat16)
-    tmp = torch.empty_like(out)
     fl = 2.0 * M * N * K
     res = {
         'plain': timeit(lambda: ops.linear_dgrad(dy, w, out=out)),
         'dgelu epilogue': timeit(lambda: ops.linear_dgrad(dy, w, out=out, gelu_pre=aux)),
         'drelu epilogue': timeit(lambda: ops.linear_dgrad(dy, w, out=out, relu_out=aux)),
         'add epilogue': timeit(lambda: ops.linear_dgrad(dy, w, out=out, add=aux)),
-        'plain + gelu_bwd kernel': timeit(lambda: (ops.linear_dgrad(dy, w, out=tmp), ops.gelu_bwd(tmp, aux, out))),
     }
     for k, us in res.items():
         print(f'dgrad M{M} N{N} K{K} {k:26s} {us:8.1f} us  {fl / us / 1e6:7.0f} TFLOP/s')

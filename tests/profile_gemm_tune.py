@@ -72,8 +72,6 @@ if which in ('all', 'vit'):
     w1 = (torch.randn(3072, 768, device='cuda') * 768 ** -0.5).bfloat16()
     b1 = torch.randn(3072, device='cuda')
     sweep('linear_fwd M50432 N3072 K768 bias -> bf16', lambda: ops.linear_fwd(dy, w1, bias=b1, out=out), fl, by, ['default', '256:4:1', '256:3:2', '192:4:2'])
-    sweep('linear_fwd M50432 N3072 K768 bias+GELU -> bf16', lambda: ops.linear_fwd(dy, w1, bias=b1, out=out, flags=ops.EPI_GELU), fl, by,
-          ['default', '256:4:1', '256:3:2', '192:4:2'])
 
 if which in ('all', 'conv'):
     NB_ = 256

@@ -33,29 +33,43 @@ def _close(got, ref, rtol, atol, what, max_bad_frac=0.0):
 
 
 # ------------------------------------------------------------------ dense layers
-@pytest.mark.parametrize('direct', [True, False])
 @pytest.mark.parametrize('M,N,K', [(256, 128, 64), (300, 1000, 2048), (1024, 768, 768), (4096, 64, 192)])
-def test_linear_fwd(M, N, K, direct):
+def test_linear_fwd(M, N, K):
     ops = _ops()
     x, w = _bf(M, K, seed=1), _bf(N, K, scale=K ** -0.5, seed=2)
     bias = torch.randn(N, device='cuda')
-    y = ops.linear_fwd(x, w, bias=bias, flags=ops.EPI_DIRECT if direct else 0)
+    y = ops.linear_fwd(x, w, bias=bias)
     ref = x.float() @ w.float().t() + bias
-    _close(y, ref, 1e-2, 1e-2, f'linear_fwd bf16 direct={direct}')
-    y32 = ops.linear_fwd(x, w, bias=bias, flags=ops.EPI_DIRECT if direct else 0, out_f32=True)
-    _close(y32, ref, 1e-4, 1e-4, f'linear_fwd f32 direct={direct}')
+    _close(y, ref, 1e-2, 1e-2, 'linear_fwd bf16')
+    y32 = ops.linear_fwd(x, w, bias=bias, out_f32=True)
+    _close(y32, ref, 1e-4, 1e-4, 'linear_fwd f32')
 
 
-def test_linear_fwd_gelu_resid():
+def test_linear_fwd_resid():
     ops = _ops()
     M, N, K = 512, 256, 128
     x, w = _bf(M, K, seed=1), _bf(N, K, scale=K ** -0.5, seed=2)
     bias = torch.randn(N, device='cuda')
     resid = torch.randn(M, N, device='cuda')
-    y = ops.linear_fwd(x, w, bias=bias, flags=ops.EPI_GELU)
-    _close(y, F.gelu(x.float() @ w.float().t() + bias), 1e-2, 1e-2, 'gelu epilogue')
     y = ops.linear_fwd(x, w, bias=bias, resid=resid, out_f32=True)
     _close(y, x.float() @ w.float().t() + bias + resid, 1e-4, 1e-4, 'residual epilogue')
+
+
+def test_gemm_entries_refuse_unknown_flags():
+    """linear_fwd / linear_dgrad / conv_fprop refuse a flag bit they do not implement (4, 8, ...) before launching
+    anything, instead of computing a plain result."""
+    from simpleaicv_pytorch_training_examples_b200 import _lib
+    ops = _ops()
+    x, w = _bf(256, 128, seed=1), _bf(128, 128, seed=2)
+    xc, wc = _bf(2, 8, 8, 64, seed=3), _bf(64, 9 * 64, seed=4)
+    cs = ops.make_conv_shape(2, 8, 8, 64, 64, 3, 3, 1, 1)
+    for flags in (4, 8, 1 << 20):
+        n0 = _lib.launch_count()
+        for call in (lambda: ops.linear_fwd(x, w, flags=flags), lambda: ops.linear_dgrad(x, w, flags=flags),
+                     lambda: ops.conv_fprop(xc, wc, cs, flags=flags)):
+            with pytest.raises(RuntimeError, match='unknown flags'):
+                call()
+        assert _lib.launch_count() == n0
 
 
 def test_linear_epilogue_rowscale_and_dgelu():

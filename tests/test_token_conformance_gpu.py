@@ -32,8 +32,9 @@ read.  Allowances are derived from the operation, never fitted to measured error
     seed_base and in place (out is x), as engine/vit.py calls it.
   * GELU on every finite bf16 input (non-finite inputs are out of scope: torch's own fp32 and fp64 GELU disagree at
     +-inf): the bf16 output lies in [rne(g - a), rne(g + a)] with a = GELU_ABS + 2u|g| (the A&S 7.1.26 erf, then
-    1 - h and x * cdf round).  The backward with dh = 1 is rne(gelu_erf_grad(u)) within GELU_GRAD_ABS + u|g'|; with
-    random bf16 dh the allowance is |dh| GELU_GRAD_ABS + u|dh g'|.  GELU_ABS and GELU_GRAD_ABS are the GEMM module's.
+    1 - h and x * cdf round).  GELU_ABS bounds |gelu_erf - gelu|: gelu_math.cuh gives <= 2.2e-7 in float64 for
+    |x| <= 12, 4e-7 here.  It is an absolute allowance: below x ~ -6, |gelu| < 1e-8 and a relative bound would be
+    meaningless.  The backward, gelu_erf_grad, runs in the GEMM epilogue (test_gemm_conformance_gpu.py).
 Every element must conform; no fraction may miss.  Outputs a wrapper would allocate with torch.empty are allocated
 here, filled with NaN, and passed to the C entry through _lib.call, so an element that is never written fails.
 
@@ -74,7 +75,6 @@ _gemm = _load('gemm_conformance', 'test_gemm_conformance_gpu.py')
 _attn = _load('attn_conformance', 'test_attn_conformance_gpu.py')
 _norm = _load('norm_conformance', 'test_norm_conformance_gpu.py')
 _rne_bf16 = _gemm._rne_bf16
-GELU_ABS, GELU_GRAD_ABS, _gelu64, _gelu_grad64 = _gemm.GELU_ABS, _gemm.GELU_GRAD_ABS, _gemm._gelu64, _gemm._gelu_grad64
 _keep, _drop_scale = _attn._keep, _attn._drop_scale       # _keep: the counter hash against _threshold(p)
 _every_bf16, _check, _same, _nan, _randn, _rand = _norm._every_bf16, _norm._check, _norm._same, _norm._nan, _norm._randn, _norm._rand
 USED = _norm.USED       # this module's own copy of the norm module: only the checks below record into it
@@ -82,6 +82,7 @@ USED = _norm.USED       # this module's own copy of the norm module: only the ch
 gpu = pytest.mark.gpu
 
 U = 2.0 ** -24          # one fp32 rounding, relative
+GELU_ABS = 4e-7         # |gelu_erf - gelu| of the A&S 7.1.26 formula, plus margin
 M32 = 0xFFFFFFFF
 CAP = 132 * 16 * 256    # items one sweep of grid_1d covers (132 * 16 blocks of 256 threads)
 FILL_SLAB_ROWS, FILL_MAX_SLABS = 512, 128
@@ -182,7 +183,7 @@ def _wrap_items():
     nip = lambda s: ops.relpos_nip(s[0], s[1])                 # noqa: E731
     nw = lambda h, w, ws: -(-h // ws) * -(-w // ws)            # noqa: E731
     return {
-        'gelu_fwd / gelu_bwd': max(n // 8 for n in GELU_N),
+        'gelu_fwd': max(n // 8 for n in GELU_N),
         'dropout': max(n // 4 for _, n, *_ in DROP),
         'assemble_tokens': max(b * (np_ + 1) * c // 4 for b, np_, c in VIT),
         'assemble_tokens_bwd': max((np_ + 1) * c for _, np_, c in VIT),
@@ -216,26 +217,24 @@ def test_cases_wrap_every_grid_cpu():
 
 
 # ------------------------------------------------------------------ GELU
+def _gelu64(x):
+    return x * 0.5 * (1.0 + torch.erf(x * 0.5 ** 0.5))
+
+
 @gpu
 def test_gelu_on_every_bf16_input():
-    """gelu_erf (forward) and gelu_erf_grad (backward, dh = 1 and random dh) on every finite bf16 value."""
+    """gelu_erf (forward) on every finite bf16 value."""
     u = _every_bf16(256)
     n = u.numel()
-    g, gp = _gelu64(u.double()), _gelu_grad64(u.double())
-    dh = _randb(*u.shape, seed=1, scale=2.0)
+    g = _gelu64(u.double())
 
     def run():
-        o = {'h': _nanb(*u.shape), 'du1': _nanb(*u.shape), 'du': _nanb(*u.shape)}
+        o = {'h': _nanb(*u.shape)}
         _c('saicv_gelu_fwd', u, o['h'], n)
-        _c('saicv_gelu_bwd', torch.ones_like(u), u, o['du1'], n)
-        _c('saicv_gelu_bwd', dh, u, o['du'], n)
         return o
 
     o = run()
     _check('gelu', 'gelu forward on every bf16 input', o['h'], g, GELU_ABS + 2 * U * g.abs())
-    _check('gelu', "gelu' (dh = 1) on every bf16 input", o['du1'], gp, GELU_GRAD_ABS + U * gp.abs())
-    v = dh.double() * gp
-    _check('gelu', "dh * gelu' on every bf16 input", o['du'], v, dh.double().abs() * GELU_GRAD_ABS + U * v.abs())
     for k, t in run().items():
         _same(f'gelu {k} on a second launch', t, o[k])
 
@@ -245,15 +244,10 @@ def test_gelu_on_every_bf16_input():
 def test_gelu_streams_conform(n):
     """The MLP hidden activation of ViT-B/16 at batch 64: the grid-stride loop wraps nine times."""
     u = _randb(n, seed=2, scale=2.0)
-    dh = _randb(n, seed=3)
-    h, du = _nanb(n), _nanb(n)
+    h = _nanb(n)
     _c('saicv_gelu_fwd', u, h, n)
-    _c('saicv_gelu_bwd', dh, u, du, n)
     g = _gelu64(u.double())
     _check('gelu', f'gelu forward n {n}', h, g, GELU_ABS + 2 * U * g.abs())
-    del g
-    v = dh.double() * _gelu_grad64(u.double())
-    _check('gelu', f'gelu backward n {n}', du, v, dh.double().abs() * GELU_GRAD_ABS + U * v.abs())
 
 
 # ------------------------------------------------------------------ dropout
@@ -668,7 +662,6 @@ def _refusals(f, i):
         ('saicv_token_gather_fwd', (f, 4, i, f, f, None, f, 2, 3, 6), 'C % 4'),
         ('saicv_token_gather_bwd', (f, i, f, 0, 4, f, 2, 3, 6), 'C % 4'),
         ('saicv_gelu_fwd', (f, f, 12), 'n % 8'),
-        ('saicv_gelu_bwd', (f, f, f, 12), 'n % 8'),
         ('saicv_dropout', (f, 1, None, f, 0, f, 1, 16, 0.1, 0, None), 'elems_per_scale'),
         ('saicv_dropout', (f, 1, None, f, 6, f, 1, 16, 0.1, 0, None), 'elems_per_scale'),
         ('saicv_dropout', (f, 1, None, None, 0, f, 1, 18, 0.1, 0, None), 'n % 4'),

@@ -47,10 +47,6 @@ def test_gelu_and_tokens_and_pool():
     u = (torch.randn(512, 3072, device='cuda', generator=g) * 2).to(torch.bfloat16)
     h = ops.gelu_fwd(u)
     assert (h.float() - F.gelu(u.float())).abs().max().item() <= 2e-2
-    dh = torch.randn(512, 3072, device='cuda', generator=g).to(torch.bfloat16)
-    ur = u.float().requires_grad_(True)
-    F.gelu(ur).backward(dh.float())
-    assert _rel(ops.gelu_bwd(dh, u), ur.grad) <= 5e-3
     B, NP, C = 5, 196, 768
     patch = torch.randn(B * NP, C, device='cuda', generator=g)
     cls, pos = torch.randn(C, device='cuda', generator=g), torch.randn(NP + 1, C, device='cuda', generator=g)
