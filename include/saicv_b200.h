@@ -518,6 +518,18 @@ int saicv_u8_rand_augment(void* img, void* scratch, int n, int h, int w, int lay
                           const float* factors_host, const double* affine_host, const int* ops, const float* factors,
                           const double* affine, const int* fill3, unsigned int* stats, void* stream);
 
+/* RandomResizedCrop / Resize + CenterCrop + RandomHorizontalFlip of the ImageNet recipes (torchvision's PIL path:
+ * Image.resize(BILINEAR), Pillow's ImagingResample for 8-bit images, 22-bit fixed point, horizontal pass rounded to
+ * uint8 before the vertical one) from the crops the host made (classification.common.Uint8RandomResizedCrop /
+ * Uint8Resize).  src: device uint8, the images' [h][w][3] pixels packed into src_len bytes.  Per image b, HOST
+ * offsets[b] (int64) and geom[b] (int32 x 9: src_h, src_w, full_h, full_w, top, left, out_h, out_w, flip): the source
+ * is resized to full_h x full_w and the oh x ow window at (top, left) is written to out uint8 [n][oh][ow][3], mirrored
+ * when flip is 1.  Bit-identical to Pillow.  Pixels past src_len, empty sizes, a window outside the resized image or one
+ * of another size than the output, and a downscale whose coefficient tables do not fit in shared memory are rejected
+ * before any launch. */
+int saicv_u8_resample(const void* src, long long src_len, const long long* offsets, const int* geom, int n, void* out,
+                      int oh, int ow, void* stream);
+
 /* ---- token gather / scatter for masked-token models (SURVEY.md 8 f4; csrc/capi_tokens.cu) -----------------------------
  * out fp32 [b][r][c] = (idx[b][r] >= 0 ? src[b][idx[b][r]][:] : fill[:]) + (pos ? pos[pos_idx ? pos_idx[b][r] : r][:] : 0);
  * src fp32 [b][src_rows][c].  One call is the torch.gather + cat(cls / mask token) + position-encoding add of

@@ -4,7 +4,9 @@ input-pipeline edge of SURVEY.md 8 f3: ``Uint8ClassificationCollater`` + ``Devic
 uint8 pixels and normalise on the device; ``Uint8RandomErasing`` + ``Uint8MixupCutmixClassificationCollater`` do the same for
 the recipes that end in RandomErasing and Mixup / CutMix, with the random draws on the host and the pixel and label
 arithmetic on the device; ``Uint8RandAugment`` makes RandAugment's draws on the host and leaves its pixel arithmetic to the
-same device edge.  The other per-sample transforms / datasets stay CPU data code (SURVEY.md section 2)."""
+same device edge; ``Uint8RandomResizedCrop`` / ``Uint8RandomHorizontalFlip`` and ``Uint8Resize`` / ``Uint8CenterCrop``
+make torchvision's crop and flip draws on the host and leave the Pillow resize to the device.  The other per-sample
+transforms / datasets stay CPU data code (SURVEY.md section 2)."""
 import math
 import random
 
@@ -40,13 +42,213 @@ class Uint8ClassificationCollater:
         if any('randaug_ops' in s for s in data):
             raise ValueError('samples carry a Uint8RandAugment record, which only Uint8MixupCutmixClassificationCollater '
                              'passes on to the device: this collater would drop it')
+        labels = torch.from_numpy(np.array([s['label'] for s in data]).astype(np.float32)).long()
+        pin = self.pin_memory and torch.cuda.is_available()
+        resample = pack_resample(data, pin)
+        if resample is not None:
+            return {'label': labels.pin_memory() if pin else labels, 'resample': resample}
         images = np.stack([np.ascontiguousarray(s['image']) for s in data])
         assert images.dtype == np.uint8 and images.ndim == 4 and images.shape[3] == 3, 'expects uint8 [H, W, 3] images'
-        labels = torch.from_numpy(np.array([s['label'] for s in data]).astype(np.float32)).long()
         images = torch.from_numpy(images)
-        if self.pin_memory and torch.cuda.is_available():
+        if pin:
             images, labels = images.pin_memory(), labels.pin_memory()
         return {'image': images, 'label': labels}
+
+
+# the int32 geometry record of a Uint8RandomResizedCrop / Uint8Resize sample ('resample_geom') and the rows of
+# ResampleBatch.geom: csrc/capi_input.cu's and oracle/resample.py's layout
+GEOM_SRC_H, GEOM_SRC_W, GEOM_FULL_H, GEOM_FULL_W, GEOM_TOP, GEOM_LEFT, GEOM_OUT_H, GEOM_OUT_W, GEOM_FLIP = range(9)
+
+
+class ResampleBatch:
+    """The ragged uint8 crops of one batch and their geometry, for the device resize (ops.u8_resample).
+
+    data uint8 [total]: every sample's [src_h, src_w, 3] crop, concatenated (pinned when the collater pins);
+    offsets int64 [B]: where image b starts in ``data``; geom int32 [B, 9]: the samples' 'resample_geom' records.  Image b
+    is resized to (full_h, full_w) with Pillow's bilinear filter, and the (out_h, out_w) window at (top, left) is kept,
+    mirrored when flip is 1."""
+
+    def __init__(self, data, offsets, geom):
+        self.data, self.offsets, self.geom = data, offsets, geom
+
+    @property
+    def out_hw(self):
+        return int(self.geom[0, GEOM_OUT_H]), int(self.geom[0, GEOM_OUT_W])
+
+    def pin_memory(self):
+        """Called by DataLoader(pin_memory=True): only the pixels are copied to the device; offsets and geometry are read
+        on the host."""
+        self.data = self.data.pin_memory()
+        return self
+
+
+def pack_resample(data, pin=False):
+    """The samples' crops packed into one ResampleBatch (into pinned memory when ``pin``), or None when no sample carries
+    a geometry record.  Raises when only some do, when the output sizes differ or when a crop does not match its record."""
+    has = [s.get('resample_geom') is not None for s in data]
+    if not any(has):
+        return None
+    if not all(has):
+        raise ValueError('some samples carry a Uint8RandomResizedCrop / Uint8Resize geometry record and some do not')
+    geom = np.stack([np.asarray(s['resample_geom'], dtype=np.int32) for s in data])
+    if geom.shape[1] != 9 or len({(int(g[GEOM_OUT_H]), int(g[GEOM_OUT_W])) for g in geom}) != 1:
+        raise ValueError(f'the samples\' geometry records differ in output size: {sorted({tuple(g[6:8]) for g in geom})}')
+    sizes = []
+    for s, g in zip(data, geom):
+        image = s['image']
+        if not isinstance(image, np.ndarray) or image.dtype != np.uint8 or image.shape != (g[GEOM_SRC_H], g[GEOM_SRC_W], 3):
+            raise ValueError(f'a crop of {np.shape(image)} does not match its record\'s source size {tuple(g[:2])}')
+        sizes.append(image.size)
+    offsets = np.zeros(len(data), dtype=np.int64)
+    offsets[1:] = np.cumsum(sizes)[:-1]
+    packed = torch.empty(int(sum(sizes)), dtype=torch.uint8, pin_memory=pin)
+    flat = packed.numpy()
+    for s, off, size in zip(data, offsets, sizes):
+        flat[off:off + size] = s['image'].reshape(-1)
+    return ResampleBatch(packed, torch.from_numpy(offsets), torch.from_numpy(geom))
+
+
+def _interpolation_is_bilinear(interpolation):
+    return str(getattr(interpolation, 'value', interpolation)).lower() == 'bilinear'
+
+
+def _source_image(sample, who):
+    image = np.asarray(sample['image'])
+    if image.ndim != 3 or image.shape[2] != 3 or image.shape[0] < 1 or image.shape[1] < 1:
+        raise ValueError(f'{who} expects the decoded [H, W, 3] image, got {image.dtype} {image.shape}')
+    if sample.get('resample_geom') is not None:
+        raise ValueError(f'{who} starts the transform list: the sample already carries a geometry record')
+    return image
+
+
+def random_resized_crop_params(height, width, scale, ratio):
+    """torchvision.transforms.RandomResizedCrop.get_params: the same torch draws from the global generator, in its
+    order, -> (top, left, h, w)."""
+    area = height * width
+    log_ratio = torch.log(torch.tensor(ratio))
+    for _ in range(10):
+        target_area = area * torch.empty(1).uniform_(scale[0], scale[1]).item()
+        aspect_ratio = torch.exp(torch.empty(1).uniform_(log_ratio[0], log_ratio[1])).item()
+        w = int(round(math.sqrt(target_area * aspect_ratio)))
+        h = int(round(math.sqrt(target_area / aspect_ratio)))
+        if 0 < w <= width and 0 < h <= height:
+            i = torch.randint(0, height - h + 1, size=(1,)).item()
+            j = torch.randint(0, width - w + 1, size=(1,)).item()
+            return i, j, h, w
+    in_ratio = float(width) / float(height)
+    if in_ratio < min(ratio):
+        w = width
+        h = int(round(w / min(ratio)))
+    elif in_ratio > max(ratio):
+        h = height
+        w = int(round(h * max(ratio)))
+    else:
+        w = width
+        h = height
+    return (height - h) // 2, (width - w) // 2, h, w
+
+
+class Uint8RandomResizedCrop:
+    """Takes the place of ``Opencv2PIL(), TorchRandomResizedCrop(resize, scale)`` (SimpleAICV/classification/common.py:
+    22-75) in a transform list collated by ``Uint8ClassificationCollater`` or ``Uint8MixupCutmixClassificationCollater``:
+    it makes torchvision's crop draws (random_resized_crop_params) and keeps only the crop, as uint8 (np.uint8 of the
+    dataset's integer-valued float32 or uint8 image).  The resize to resize x resize is left to the device
+    (ops.u8_resample, Pillow's bilinear arithmetic); the sample's 'resample_geom' record holds the crop size, the output
+    size, the output window (0, 0, resize, resize) and the flip flag.  Only the shipped setting (bilinear, the default
+    ratio) is implemented."""
+
+    def __init__(self, resize=224, scale=(0.08, 1.0), ratio=(3. / 4., 4. / 3.), interpolation='bilinear'):
+        if not isinstance(resize, (int, np.integer)):
+            raise NotImplementedError(f'Uint8RandomResizedCrop resize={resize!r}: only a square int size (the shipped '
+                                      'configs\') is implemented')
+        if tuple(ratio) != (3. / 4., 4. / 3.):
+            raise NotImplementedError(f'Uint8RandomResizedCrop ratio={ratio!r}: only the default (3/4, 4/3) (the shipped '
+                                      'configs\') is implemented')
+        if not _interpolation_is_bilinear(interpolation):
+            raise NotImplementedError(f'Uint8RandomResizedCrop interpolation={interpolation!r}: only bilinear (the shipped '
+                                      'configs\') is implemented')
+        self.size, self.scale, self.ratio = int(resize), tuple(scale), tuple(ratio)
+
+    def __call__(self, sample):
+        image = _source_image(sample, 'Uint8RandomResizedCrop')
+        top, left, h, w = random_resized_crop_params(image.shape[0], image.shape[1], self.scale, self.ratio)
+        sample['image'] = image[top:top + h, left:left + w].astype(np.uint8)
+        sample['resample_geom'] = np.array([h, w, self.size, self.size, 0, 0, self.size, self.size, 0], dtype=np.int32)
+        return sample
+
+
+class Uint8RandomHorizontalFlip:
+    """Takes the place of ``TorchRandomHorizontalFlip(prob)`` after ``Uint8RandomResizedCrop``: torchvision's
+    torch.rand(1) < prob draw toggles the record's flip flag; the device mirrors the output."""
+
+    def __init__(self, prob=0.5):
+        self.prob = prob
+
+    def __call__(self, sample):
+        if sample.get('resample_geom') is None:
+            raise ValueError('Uint8RandomHorizontalFlip follows Uint8RandomResizedCrop or Uint8Resize: the sample has no '
+                             'geometry record')
+        if torch.rand(1) < self.prob:
+            sample['resample_geom'][GEOM_FLIP] ^= 1
+        return sample
+
+
+class Uint8Resize:
+    """Takes the place of ``Opencv2PIL(), TorchResize(resize)`` (SimpleAICV/classification/common.py:22-37,154-169) in an
+    evaluation list: the whole image is kept as uint8 and the record holds torchvision's output size for an int size
+    (the short side becomes ``resize``, the long one int(resize * long / short)), which the device resizes to with
+    Pillow's bilinear arithmetic.  Only the shipped setting (int size, no max_size, bilinear) is implemented."""
+
+    def __init__(self, resize=256, max_size=None, interpolation='bilinear'):
+        if not isinstance(resize, (int, np.integer)):
+            raise NotImplementedError(f'Uint8Resize resize={resize!r}: only an int size (the shipped configs\') is '
+                                      'implemented')
+        if max_size is not None:
+            raise NotImplementedError('Uint8Resize max_size: only max_size=None (the shipped configs\') is implemented')
+        if not _interpolation_is_bilinear(interpolation):
+            raise NotImplementedError(f'Uint8Resize interpolation={interpolation!r}: only bilinear (the shipped '
+                                      'configs\') is implemented')
+        self.size = int(resize)
+
+    def __call__(self, sample):
+        image = _source_image(sample, 'Uint8Resize')
+        h, w = image.shape[:2]
+        short, long = (w, h) if w <= h else (h, w)
+        new_short, new_long = self.size, int(self.size * long / short)
+        new_w, new_h = (new_short, new_long) if w <= h else (new_long, new_short)
+        sample['image'] = np.ascontiguousarray(image, dtype=np.uint8)
+        sample['resample_geom'] = np.array([h, w, new_h, new_w, 0, 0, new_h, new_w, 0], dtype=np.int32)
+        return sample
+
+
+class Uint8CenterCrop:
+    """Takes the place of ``TorchCenterCrop(resize)`` after ``Uint8Resize``: the record's output window becomes the
+    centred resize x resize square, at torchvision's int(round((H - resize) / 2.0)) / int(round((W - resize) / 2.0)).
+    A crop larger than the resized image, which torchvision pads, is refused."""
+
+    def __init__(self, resize=224):
+        if not isinstance(resize, (int, np.integer)):
+            raise NotImplementedError(f'Uint8CenterCrop resize={resize!r}: only a square int size (the shipped configs\') '
+                                      'is implemented')
+        self.size = int(resize)
+
+    def __call__(self, sample):
+        g = sample.get('resample_geom')
+        if g is None:
+            raise ValueError('Uint8CenterCrop follows Uint8Resize: the sample has no geometry record')
+        h, w = int(g[GEOM_OUT_H]), int(g[GEOM_OUT_W])
+        if self.size > h or self.size > w:
+            raise ValueError(f'Uint8CenterCrop({self.size}) of a {h} x {w} image would pad, which is not implemented')
+        g[GEOM_TOP] += int(round((h - self.size) / 2.0))
+        g[GEOM_LEFT] += int(round((w - self.size) / 2.0))
+        g[GEOM_OUT_H] = g[GEOM_OUT_W] = self.size
+        return sample
+
+
+def _logical_hw(sample, image):
+    """(h, w) of the image a transform sees: the output window of a geometry record, else the array's."""
+    g = sample.get('resample_geom')
+    return (int(g[GEOM_OUT_H]), int(g[GEOM_OUT_W])) if g is not None else image.shape[:2]
 
 
 MIX_NONE, MIX_MIXUP, MIX_CUTMIX = 0, 1, 2
@@ -183,7 +385,7 @@ class Uint8RandAugment:
         image = np.asarray(sample['image'])
         if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
             raise ValueError(f'Uint8RandAugment expects a PIL RGB image or a uint8 [H, W, 3] array, got {image.dtype} {image.shape}')
-        h, w = image.shape[:2]
+        h, w = _logical_hw(sample, image)
         chosen = np.random.choice(len(RANDAUG_OPS), self.num_layers, replace=True)
         ops = np.zeros((self.num_layers, 4), dtype=np.int32)
         factors = np.zeros(self.num_layers, dtype=np.float32)
@@ -224,7 +426,7 @@ class Uint8RandomErasing:
         image = np.asarray(sample['image'])
         if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
             raise ValueError(f'Uint8RandomErasing expects a PIL RGB image or a uint8 [H, W, 3] array, got {image.dtype} {image.shape}')
-        image_h, image_w = image.shape[:2]
+        image_h, image_w = _logical_hw(sample, image)
         rect, noise = np.zeros(4, dtype=np.int32), np.zeros(0, dtype=np.float32)
         if np.random.uniform(0, 1) < self.prob:
             area = image_h * image_w
@@ -253,7 +455,10 @@ class Uint8MixupCutmixClassificationCollater:
     The batch-mode draws are the reference's, in its order: rand() against mixup_cutmix_prob; with both alphas > 0, rand()
     against switch_to_cutmix_prob; beta(alpha, alpha); for CutMix randint(0, H) for the box centre row and randint(0, W)
     for its column.  The corrected lambda is 1 - box area / (H * W) in float64; when lambda is 1 nothing is mixed.
-    Only the shipped setting (use_mixup=True, mode='batch', cutmix_minmax=None) is implemented."""
+    Only the shipped setting (use_mixup=True, mode='batch', cutmix_minmax=None) is implemented.
+
+    Samples from ``Uint8RandomResizedCrop`` carry ragged crops: they are packed into a ResampleBatch under 'resample'
+    instead of stacked under 'image', and H x W is the records' output size."""
 
     def __init__(self, use_mixup=True, mixup_alpha=0.8, cutmix_alpha=1.0, cutmix_minmax=None, mixup_cutmix_prob=1.0,
                  switch_to_cutmix_prob=0.5, mode='batch', correct_lam=True, label_smoothing=0.1, num_classes=1000,
@@ -292,19 +497,24 @@ class Uint8MixupCutmixClassificationCollater:
         return lam, use_cutmix
 
     def __call__(self, data):
-        shape = np.shape(data[0]['image'])
-        for s in data:
-            img = s['image']
-            if np.shape(img) != shape or len(shape) != 3 or shape[2] != 3 or np.asarray(img).dtype != np.uint8:
-                raise ValueError(f'expects uint8 [H, W, 3] images of one shape, got {np.asarray(img).dtype} {np.shape(img)} '
-                                 f'next to {shape}')
-        b, (h, w) = len(data), shape[:2]
+        pin = self.pin_memory and torch.cuda.is_available()
+        resample = pack_resample(data, pin)
+        if resample is None:
+            shape = np.shape(data[0]['image'])
+            for s in data:
+                img = s['image']
+                if np.shape(img) != shape or len(shape) != 3 or shape[2] != 3 or np.asarray(img).dtype != np.uint8:
+                    raise ValueError(f'expects uint8 [H, W, 3] images of one shape, got {np.asarray(img).dtype} '
+                                     f'{np.shape(img)} next to {shape}')
+            h, w = shape[:2]
+        else:
+            h, w = resample.out_hw
+        b = len(data)
         if b % 2 != 0:
             raise ValueError(f'Mixup / CutMix pairs image b with image B-1-b: the batch size must be even (got {b})')
         labels = np.array([s['label'] for s in data]).astype(np.float32).astype(np.int64)
         if labels.min() < 0 or labels.max() >= self.num_classes:
             raise ValueError(f'labels must lie in [0, {self.num_classes}), got {labels.min()}..{labels.max()}')
-        images = np.stack([np.ascontiguousarray(s['image']) for s in data])
         rects = np.stack([s.get('erase_rect', np.zeros(4, np.int32)) for s in data]).astype(np.int32)
         noises = [np.asarray(s.get('erase_noise', np.zeros(0, np.float32)), dtype=np.float32).reshape(-1) for s in data]
         offsets = np.zeros(b, dtype=np.int64)
@@ -341,10 +551,13 @@ class Uint8MixupCutmixClassificationCollater:
         record = MixupEraseRecord(torch.from_numpy(rects), torch.from_numpy(offsets),
                                   torch.from_numpy(np.concatenate(noises)),
                                   mode, box, lam, self.num_classes, 1. - self.label_smoothing + off_value, off_value, **ra)
-        images, labels = torch.from_numpy(images), torch.from_numpy(labels)
-        if self.pin_memory and torch.cuda.is_available():
-            images, labels, record = images.pin_memory(), labels.pin_memory(), record.pin_memory()
-        return {'image': images, 'label': labels, 'mixup': record}
+        labels = torch.from_numpy(labels)
+        if pin:
+            labels, record = labels.pin_memory(), record.pin_memory()
+        if resample is not None:
+            return {'label': labels, 'mixup': record, 'resample': resample}
+        images = torch.from_numpy(np.stack([np.ascontiguousarray(s['image']) for s in data]))
+        return {'image': images.pin_memory() if pin else images, 'label': labels, 'mixup': record}
 
 
 class DeviceNormalize:

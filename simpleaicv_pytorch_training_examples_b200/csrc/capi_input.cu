@@ -12,6 +12,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 #include "../../include/saicv_b200.h"
 #include "host_util.h"
 
@@ -443,6 +445,139 @@ ra_apply_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, const
   }
 }
 
+// ---- RandomResizedCrop / Resize + CenterCrop + horizontal flip on the uint8 edge --------------------------------------
+// torchvision's PIL path resizes with Image.resize(BILINEAR), i.e. Pillow's ImagingResample for 8-bit images: per axis a
+// float64 triangle-filter table normalised and rounded to 22-bit fixed point, a horizontal pass whose results are
+// rounded and kept as uint8, then a vertical pass over those with the same rounding.  The host made the crop and the
+// draws (classification.common.Uint8RandomResizedCrop / Uint8Resize); per image the kernel reads the source (h, w), the
+// full resized size (fh, fw), the window (top, left) of the oh x ow output inside it and the flip flag.  Each output
+// pixel depends only on its own taps, so only the window is computed.  A CTA owns a kRsRows x kRsCols tile: it builds
+// the tile's coefficients in shared memory, filters the source rows its vertical taps need horizontally in chunks of
+// kRsChunk rows and accumulates the vertical pass in registers, so any downscale factor runs in bounded shared memory
+// except for the coefficient tables, whose size the host checks.  Every float64 operation is an explicit _rn intrinsic.
+constexpr int kRsMaxImages = 512;   // per launch: the geometry travels in the kernel's parameter space
+constexpr int kRsRows = 16, kRsCols = 32, kRsChunk = 32;
+constexpr int kRsPixelsPerThread = kRsRows * kRsCols / kInThreads;
+constexpr int kRsPrecision = 22;    // Pillow's PRECISION_BITS
+constexpr int kRsGeomFields = 9;    // src_h, src_w, full_h, full_w, top, left, out_h, out_w, flip
+
+struct RsImage {
+  long long off;                    // first byte of the image's [h][w][3] pixels in the packed source
+  int h, w, fh, fw, top, left, flip, pad;
+};
+struct RsBatch {
+  RsImage img[kRsMaxImages];
+};
+
+__device__ __forceinline__ uint8_t rs_clip8(int v) {
+  return v >= (1 << kRsPrecision << 8) ? 255 : (v <= 0 ? 0 : (uint8_t)(v >> kRsPrecision));
+}
+
+__device__ __forceinline__ double rs_triangle(double x) {
+  if (x < 0.0) x = -x;
+  return x < 1.0 ? __dsub_rn(1.0, x) : 0.0;
+}
+
+// Resample.c precompute_coeffs + normalize_coeffs_8bpc (bilinear, box = the whole input) for output index xx:
+// first tap xmin, n taps, fixed-point weights k[0..n)
+__device__ void rs_coeffs(int in_size, int out_size, int xx, int* k, int* xmin_out, int* n_out) {
+  const double scale = __ddiv_rn((double)in_size, (double)out_size);
+  const double support = scale < 1.0 ? 1.0 : scale;
+  const double ss = __ddiv_rn(1.0, support);
+  const double center = __dmul_rn(__dadd_rn((double)xx, 0.5), scale);
+  int xmin = (int)__dadd_rn(__dsub_rn(center, support), 0.5);
+  xmin = xmin < 0 ? 0 : xmin;
+  int xmax = (int)__dadd_rn(__dadd_rn(center, support), 0.5);
+  xmax = xmax > in_size ? in_size : xmax;
+  const int n = xmax - xmin;
+  double ww = 0.0;
+  for (int x = 0; x < n; ++x) ww = __dadd_rn(ww, rs_triangle(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss)));
+  for (int x = 0; x < n; ++x) {
+    double w = rs_triangle(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss));
+    if (ww != 0.0) w = __ddiv_rn(w, ww);
+    const double s = __dmul_rn(w, (double)(1 << kRsPrecision));
+    k[x] = (int)(w < 0.0 ? __dadd_rn(-0.5, s) : __dadd_rn(0.5, s));
+  }
+  *xmin_out = xmin;
+  *n_out = n;
+}
+
+// one tile of image blockIdx.z; dynamic shared memory: kh [kRsCols][kx], kv [kRsRows][ky] int32, then the uint8 chunk
+__global__ void __launch_bounds__(kInThreads)
+u8_resample_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ out, int oh, int ow, int kx, int ky,
+                   const __grid_constant__ RsBatch g) {
+  extern __shared__ int rs_smem[];
+  __shared__ int hx0[kRsCols], hn[kRsCols], vy0[kRsRows], vn[kRsRows];
+  int* kh = rs_smem;
+  int* kv = kh + kRsCols * kx;
+  uint8_t* chunk = reinterpret_cast<uint8_t*>(kv + kRsRows * ky);   // [kRsChunk][kRsCols][3] horizontal-pass results
+  const RsImage im = g.img[blockIdx.z];
+  const int x0 = blockIdx.x * kRsCols, y0 = blockIdx.y * kRsRows;
+  const int cols = min(kRsCols, ow - x0), rows = min(kRsRows, oh - y0);
+  const int t = threadIdx.x;
+  if (t < cols) rs_coeffs(im.w, im.fw, im.left + x0 + t, kh + t * kx, &hx0[t], &hn[t]);
+  else if (t >= kRsCols && t < kRsCols + rows) rs_coeffs(im.h, im.fh, im.top + y0 + t - kRsCols, kv + (t - kRsCols) * ky,
+                                                         &vy0[t - kRsCols], &vn[t - kRsCols]);
+  __syncthreads();
+  int ys = vy0[0], ye = 0;
+  for (int r = 0; r < rows; ++r) {
+    ys = min(ys, vy0[r]);
+    ye = max(ye, vy0[r] + vn[r]);
+  }
+  int acc[kRsPixelsPerThread][3];
+#pragma unroll
+  for (int i = 0; i < kRsPixelsPerThread; ++i) acc[i][0] = acc[i][1] = acc[i][2] = 1 << (kRsPrecision - 1);
+  const uint8_t* s = src + im.off;
+  for (int c0 = ys; c0 < ye; c0 += kRsChunk) {
+    const int cn = min(kRsChunk, ye - c0);
+    for (int i = t; i < cn * kRsCols; i += kInThreads) {
+      const int r = i / kRsCols, c = i - r * kRsCols;
+      if (c >= cols) continue;
+      const uint8_t* p = s + ((long long)(c0 + r) * im.w + hx0[c]) * 3;
+      const int* k = kh + c * kx;
+      int a0 = 1 << (kRsPrecision - 1), a1 = a0, a2 = a0;
+      for (int j = 0; j < hn[c]; ++j) {
+        const int kj = k[j];
+        a0 += (int)__ldg(p + 3 * j) * kj;
+        a1 += (int)__ldg(p + 3 * j + 1) * kj;
+        a2 += (int)__ldg(p + 3 * j + 2) * kj;
+      }
+      uint8_t* q = chunk + (r * kRsCols + c) * 3;
+      q[0] = rs_clip8(a0), q[1] = rs_clip8(a1), q[2] = rs_clip8(a2);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < kRsPixelsPerThread; ++i) {
+      const int px = t + i * kInThreads, r = px / kRsCols, c = px - r * kRsCols;
+      if (r >= rows || c >= cols) continue;
+      const int lo = max(c0, vy0[r]), hi = min(c0 + cn, vy0[r] + vn[r]);
+      const int* k = kv + r * ky;
+      for (int y = lo; y < hi; ++y) {
+        const uint8_t* q = chunk + ((y - c0) * kRsCols + c) * 3;
+        const int kj = k[y - vy0[r]];
+        acc[i][0] += (int)q[0] * kj;
+        acc[i][1] += (int)q[1] * kj;
+        acc[i][2] += (int)q[2] * kj;
+      }
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < kRsPixelsPerThread; ++i) {
+    const int px = t + i * kInThreads, r = px / kRsCols, c = px - r * kRsCols;
+    if (r >= rows || c >= cols) continue;
+    const int x = im.flip ? ow - 1 - (x0 + c) : x0 + c;
+    uint8_t* o = out + (((long long)blockIdx.z * oh + y0 + r) * ow + x) * 3;
+    o[0] = rs_clip8(acc[i][0]), o[1] = rs_clip8(acc[i][1]), o[2] = rs_clip8(acc[i][2]);
+  }
+}
+
+// taps of Pillow's bilinear table for an in_size -> out_size axis: 2 * ceil(support) + 1
+int rs_ksize(int in_size, int out_size) {
+  const double scale = (double)in_size / (double)out_size;
+  return (int)ceil(scale < 1.0 ? 1.0 : scale) * 2 + 1;
+}
+
 }  // namespace
 }  // namespace saicv
 
@@ -582,6 +717,57 @@ extern "C" int saicv_u8_rand_augment(void* img, void* scratch, int n, int h, int
   if (layers & 1) {   // the last layer wrote the scratch buffer
     if (cudaMemcpyAsync(img, scratch, (size_t)n * hw * 3, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
       return set_error("%s: copy back from the scratch buffer failed", fn);
+  }
+  return 0;
+}
+
+extern "C" int saicv_u8_resample(const void* src, long long src_len, const long long* offsets, const int* geom, int n,
+                                 void* out, int oh, int ow, void* stream) {
+  const char* fn = "saicv_u8_resample";
+  if (!src || !offsets || !geom || !out) return set_error("%s: null pointer", fn);
+  if (n < 1 || oh < 1 || ow < 1 || src_len < 0) return set_error("%s: empty batch or output (n=%d, %d x %d)", fn, n, oh, ow);
+  if ((long long)oh * ow >= (1ll << 31)) return set_error("%s: output %d x %d is too large", fn, oh, ow);
+  int kx = 1, ky = 1;
+  for (int b = 0; b < n; ++b) {
+    const int* gm = geom + (long long)b * kRsGeomFields;
+    const int h = gm[0], w = gm[1], fh = gm[2], fw = gm[3], top = gm[4], left = gm[5], flip = gm[8];
+    const long long off = offsets[b];
+    if (h < 1 || w < 1 || fh < 1 || fw < 1)
+      return set_error("%s: image %d has an empty source (%d x %d) or resized size (%d x %d)", fn, b, h, w, fh, fw);
+    if (off < 0 || off > src_len || (long long)h * w > (src_len - off) / 3)
+      return set_error("%s: image %d's %d x %d pixels at offset %lld are past the packed buffer of %lld bytes", fn, b, h, w,
+                       off, src_len);
+    if (gm[6] != oh || gm[7] != ow)
+      return set_error("%s: image %d's window is %d x %d, the output is %d x %d", fn, b, gm[6], gm[7], oh, ow);
+    if (top < 0 || left < 0 || (long long)top + oh > fh || (long long)left + ow > fw)
+      return set_error("%s: image %d's window (top %d, left %d, %d x %d) leaves the %d x %d resized image", fn, b, top, left, oh,
+                       ow, fh, fw);
+    if (flip != 0 && flip != 1) return set_error("%s: image %d's flip flag is %d, not 0 or 1", fn, b, flip);
+    kx = std::max(kx, rs_ksize(w, fw));
+    ky = std::max(ky, rs_ksize(h, fh));
+  }
+  const size_t smem = sizeof(int) * ((size_t)kRsCols * kx + (size_t)kRsRows * ky) + kRsChunk * kRsCols * 3;
+  constexpr size_t kSmemCap = 227 * 1024 - 4 * sizeof(int) * (kRsCols + kRsRows);
+  if (smem > kSmemCap)
+    return set_error("%s: a downscale by more than %d x %d taps needs %zu bytes of coefficients, over %zu", fn, kx, ky, smem,
+                     kSmemCap);
+  if (smem > 48 * 1024) {
+    const cudaError_t e = cudaFuncSetAttribute(u8_resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return set_error("%s: %s", fn, cudaGetErrorString(e));
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  static thread_local RsBatch batch;
+  for (int b0 = 0; b0 < n; b0 += kRsMaxImages) {
+    const int count = std::min(kRsMaxImages, n - b0);
+    for (int i = 0; i < count; ++i) {
+      const int* gm = geom + (long long)(b0 + i) * kRsGeomFields;
+      batch.img[i] = RsImage{offsets[b0 + i], gm[0], gm[1], gm[2], gm[3], gm[4], gm[5], gm[8], 0};
+    }
+    const dim3 grid((ow + kRsCols - 1) / kRsCols, (oh + kRsRows - 1) / kRsRows, count);
+    u8_resample_kernel<<<grid, kInThreads, smem, st>>>(reinterpret_cast<const uint8_t*>(src),
+                                                       reinterpret_cast<uint8_t*>(out) + (long long)b0 * oh * ow * 3, oh, ow,
+                                                       kx, ky, batch);
+    if (check_launch("u8_resample_kernel")) return 1;
   }
   return 0;
 }

@@ -241,6 +241,24 @@ def u8_rand_augment(images, record, scratch=None, stats=None):
     return images
 
 
+def u8_resample(src, offsets, geom, out=None):
+    """RandomResizedCrop / Resize + CenterCrop + horizontal flip of torchvision's PIL path on the device, bit-identical:
+    src: device uint8 holding the packed [h, w, 3] crops; offsets: host int64 [N] (where image b starts in src); geom: host
+    int32 [N, 9] (src_h, src_w, full_h, full_w, top, left, out_h, out_w, flip), the rows of
+    classification.common.ResampleBatch.  Returns out uint8 [N, out_h, out_w, 3] (device)."""
+    assert src.is_cuda and src.dtype == torch.uint8 and src.is_contiguous()
+    n = geom.shape[0]
+    assert geom.dtype == torch.int32 and tuple(geom.shape) == (n, 9) and not geom.is_cuda and geom.is_contiguous()
+    assert offsets.dtype == torch.int64 and tuple(offsets.shape) == (n,) and not offsets.is_cuda and offsets.is_contiguous()
+    oh, ow = (int(v) for v in geom[0, 6:8]) if n else (0, 0)
+    if out is None:
+        out = torch.empty(n, oh, ow, 3, device=src.device, dtype=torch.uint8)
+    assert out.dtype == torch.uint8 and tuple(out.shape) == (n, oh, ow, 3)
+    _lib.call('saicv_u8_resample', _p(src), src.numel(), ctypes.c_void_p(offsets.data_ptr()),
+              ctypes.c_void_p(geom.data_ptr()), n, _p(out), oh, ow, _stream())
+    return out
+
+
 def stem_kpad(c, r, s):
     """Columns of the explicit-im2col matrix / weight operand of a c-channel r x s stem conv (filter rows padded to 8,
     total rounded up to the 64-wide reduction block)."""

@@ -229,6 +229,16 @@ def train_detection(train_loader, model, criterion, optimizer, scheduler, epoch,
     return train_epoch_with_loss_terms(train_loader, model, criterion, optimizer, scheduler, epoch, logger, config, compute)
 
 
+def _eval_batches(test_loader, config):
+    """config.device_normalize = (mean, std): the batches go through CudaPrefetcher, so uint8 ones (Uint8Resize +
+    Uint8CenterCrop + Uint8ClassificationCollater) are resized and normalised on the device; fp32 ones pass unchanged."""
+    normalize = getattr(config, 'device_normalize', None)
+    if normalize is None:
+        return test_loader
+    from .utils import CudaPrefetcher
+    return CudaPrefetcher(test_loader, normalize=normalize)
+
+
 @torch.no_grad()
 def test_classification(test_loader, model, criterion, config):
     """Returns (acc1 %, acc5 %, loss); top-k indices come from torch.topk like the reference
@@ -237,7 +247,7 @@ def test_classification(test_loader, model, criterion, config):
     group = getattr(config, 'group', None)
     meter = AccMeter()
     loss_sum = 0.
-    for data in test_loader:
+    for data in _eval_batches(test_loader, config):
         images, labels = data['image'].cuda(non_blocking=True), data['label'].cuda(non_blocking=True)
         outputs = model(images)
         loss = criterion(outputs, labels)
@@ -262,7 +272,7 @@ def test_imagenet21k_classification(test_loader, model, criterion, config):
     group = getattr(config, 'group', None)
     accs = SemanticSoftmaxMeter()
     loss_sum, samples = 0., 0
-    for data in test_loader:
+    for data in _eval_batches(test_loader, config):
         images, labels = data['image'].cuda(non_blocking=True), data['label'].cuda(non_blocking=True)
         outputs = tree.convert_outputs_to_semantic_outputs(model(images))
         labels = tree.convert_single_labels_to_semantic_labels(labels)

@@ -246,7 +246,9 @@ class CudaPrefetcher:
         'mixup' record (classification.common.Uint8MixupCutmixClassificationCollater) get the reference's RandomErasing and
         Mixup / CutMix applied by the same pass and are yielded as {'image': fp32 [B, 3, H, W], 'label': fp32 [B, classes]};
         such a batch without ``normalize`` raises.  When that record also holds RandAugment draws (classification.common.
-        Uint8RandAugment), RandAugment is applied to the uint8 copy first, on the same stream.
+        Uint8RandAugment), RandAugment is applied to the uint8 copy first, on the same stream.  Batches that carry a 'resample'
+        ResampleBatch (samples from classification.common.Uint8RandomResizedCrop or Uint8Resize) copy the packed crops into
+        a device buffer that only grows and resize them into the uint8 image first (ops.u8_resample), on the same stream.
         copy_streams > 1: tensors of 32 MB and more are copied in that many chunks on separate streams, so that the copy of
         the next batch keeps its bandwidth while the current step's kernels run (tests/profile_h2d.py measures it)."""
         self.loader = loader
@@ -274,7 +276,7 @@ class CudaPrefetcher:
                 self.stream.wait_event(self._free[k & 1])
             out = {}
             for name, v in batch.items():
-                if name == 'mixup':
+                if name in ('mixup', 'resample'):
                     continue
                 if not torch.is_tensor(v):
                     out[name] = v
@@ -282,20 +284,28 @@ class CudaPrefetcher:
                 buf = slot.get(name)
                 if buf is None or buf.shape != v.shape or buf.dtype != v.dtype:
                     buf = slot[name] = torch.empty(v.shape, dtype=v.dtype, device=self.device)
-                if self._extra and v.dim() > 0 and v.numel() * v.element_size() >= (32 << 20) and v.shape[0] >= len(self._extra) + 1:
-                    parts = len(self._extra) + 1
-                    step = (v.shape[0] + parts - 1) // parts
-                    buf[:step].copy_(v[:step], non_blocking=True)
-                    for j, st in enumerate(self._extra):
-                        st.wait_stream(self.stream)            # inherits the slot-free dependency
-                        with torch.cuda.stream(st):
-                            lo = (j + 1) * step
-                            buf[lo:lo + step].copy_(v[lo:lo + step], non_blocking=True)
-                else:
-                    buf.copy_(v, non_blocking=True)
+                self._copy(buf, v)
                 out[name] = buf
+            rs = batch.get('resample')
+            packed = None
+            if rs is not None:
+                used = rs.data.numel()
+                packed = slot.get('resample_src')
+                if packed is None or packed.numel() < used:
+                    # the packed length changes every batch: the buffer only grows, to powers of two
+                    packed = slot['resample_src'] = torch.empty(1 << max(used - 1, 0).bit_length(), dtype=torch.uint8,
+                                                                device=self.device)
+                packed = packed[:used]
+                self._copy(packed, rs.data)
             for st in self._extra:
                 self.stream.wait_stream(st)
+            if rs is not None:
+                from .. import ops
+                shape = (rs.geom.shape[0],) + rs.out_hw + (3,)
+                img = slot.get('resample_image')
+                if img is None or tuple(img.shape) != shape:
+                    img = slot['resample_image'] = torch.empty(shape, dtype=torch.uint8, device=self.device)
+                out['image'] = ops.u8_resample(packed, rs.offsets, rs.geom, out=img)
             img = out.get('image')
             if self.normalize is not None and torch.is_tensor(img) and img.dtype == torch.uint8:
                 from .. import ops
@@ -309,6 +319,20 @@ class CudaPrefetcher:
             ev = torch.cuda.Event()
             ev.record(self.stream)
         return out, ev
+
+    def _copy(self, buf, v):
+        """buf.copy_(v) on the copy stream; 32 MB and more are split over the extra streams."""
+        if self._extra and v.dim() > 0 and v.numel() * v.element_size() >= (32 << 20) and v.shape[0] >= len(self._extra) + 1:
+            parts = len(self._extra) + 1
+            step = (v.shape[0] + parts - 1) // parts
+            buf[:step].copy_(v[:step], non_blocking=True)
+            for j, st in enumerate(self._extra):
+                st.wait_stream(self.stream)            # inherits the slot-free dependency
+                with torch.cuda.stream(st):
+                    lo = (j + 1) * step
+                    buf[lo:lo + step].copy_(v[lo:lo + step], non_blocking=True)
+        else:
+            buf.copy_(v, non_blocking=True)
 
     def _mix(self, slot, img, labels, rec, out):
         from .. import ops
