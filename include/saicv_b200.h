@@ -429,7 +429,10 @@ int saicv_semantic_accuracy(const void* logits, int logits_bf16, const long long
  * hyper: device fp32 [SAICV_OPT_RING][n_groups][8]; the update reads table (*step %% SAICV_OPT_RING) and a one-thread
  * kernel then advances *step (device int).  Rows:
  *   SGD   {lr, weight_decay, momentum, nesterov, 0...}       (dampening 0; buf = momentum buf + (g + wd p); p -= lr buf)
- *   AdamW {lr, weight_decay, beta1, beta2, eps, 1 - beta1^t, sqrt(1 - beta2^t), 0}   (torch.optim.AdamW's update)
+ *   AdamW {lr, weight_decay, beta1, beta2, eps, 0...}   (torch.optim.AdamW's update; the bias corrections 1 - beta1^t and
+ *         sqrt(1 - beta2^t) are computed in double from the parameter's own count t = steps[step_idx] + 1, and a one-thread-
+ *         per-row kernel then advances steps[step_idx] of every row: a parameter without a gradient is not in the table and
+ *         keeps its count, as torch skips it)
  * clip: device fp32 [2] = {gradient scale, global norm} written by saicv_multi_tensor_clip_coef, or NULL.  All launch
  * arguments are step-invariant: a captured step replays with new learning rates once the host has rewritten slot
  * t %% SAICV_OPT_RING of the (pinned) table the captured copy brings in. */
@@ -446,14 +449,16 @@ typedef struct {
   int rs;              /* shadow layout: 0 = same linear index ([N][K] Linear weights); > 0 = conv weight [K][C][rs taps]
                           -> [K][kpad] with column tap * cp + c (saicv_prep_conv_weight order 0) */
   int c, cp, kpad;
-  int pad_;
+  int step_idx;        /* AdamW: index of the parameter's step count in `steps` (unused by SGD) */
 } saicv_opt_tensor;
 int saicv_opt_chunk(void);
 int saicv_multi_tensor_sgd(const void* tensors, const int* chunk_tensor, const int* chunk_index, int n_chunks,
                            const float* hyper, int n_groups, int* step, const float* clip, void* stream);
-int saicv_multi_tensor_adamw(const void* tensors, const int* chunk_tensor, const int* chunk_index, int n_chunks,
-                             const float* hyper, int n_groups, int* step, const float* clip, void* stream);
-/* partial: fp32 [n_chunks] workspace; clip = {min(1, max_norm / (norm + 1e-6)), norm}; fixed summation order. */
+/* n_tensors: rows of `tensors`; steps: device int32 per-parameter step counts, indexed by step_idx. */
+int saicv_multi_tensor_adamw(const void* tensors, const int* chunk_tensor, const int* chunk_index, int n_chunks, int n_tensors,
+                             const float* hyper, int n_groups, int* step, const float* clip, int* steps, void* stream);
+/* partial: fp32 [n_chunks] workspace; clip = {min(1, max_norm / (norm + 1e-6)), norm}; fixed summation order.  A NaN norm
+ * gives a NaN coefficient (torch.clamp keeps NaN), an infinite one 0. */
 int saicv_multi_tensor_clip_coef(const void* tensors, const int* chunk_tensor, const int* chunk_index, int n_chunks,
                                  float max_norm, float* partial, float* clip, void* stream);
 /* Muon (the reference's tools/muon_optimizer.py): one saicv_muon_tensor per saicv_opt_tensor row.  Muon rows (slot >= 0):

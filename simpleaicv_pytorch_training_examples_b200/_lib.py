@@ -112,7 +112,7 @@ SIGNATURES = {
     'saicv_token_gather_bwd': [c_void_p, c_void_p, c_void_p, c_int, c_ll, c_void_p, c_int, c_int, c_int, c_void_p],
     'saicv_opt_chunk': [],
     'saicv_multi_tensor_sgd': [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p],
-    'saicv_multi_tensor_adamw': [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p],
+    'saicv_multi_tensor_adamw': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     'saicv_multi_tensor_clip_coef': [c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p],
     'saicv_muon_prep': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     'saicv_muon_apply': [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],

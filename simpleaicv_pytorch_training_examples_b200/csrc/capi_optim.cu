@@ -34,7 +34,7 @@ struct OptTensor {
   int group;         // row of the hyper-parameter table
   int rs;            // shadow layout: 0 = same linear index; > 0 = conv weight [K][C][rs taps] -> [K][kpad], column tap*cp + c
   int c, cp, kpad;
-  int pad_;
+  int step_idx;      // AdamW: index of the parameter's step count
 };
 static_assert(sizeof(OptTensor) == sizeof(saicv_opt_tensor) && sizeof(OptTensor) == 72, "saicv_opt_tensor layout");
 
@@ -105,25 +105,30 @@ multi_sgd_kernel(const OptTensor* __restrict__ tensors, const int* __restrict__ 
   else sgd_chunk<false>(t, base, n, lr, wd, mom, nesterov, gs);
 }
 
-// AdamW exactly as torch.optim.AdamW (decoupled decay first, bias corrections from the host):
-// hyper[group] = {lr, weight_decay, beta1, beta2, eps, 1 - beta1^t, sqrt(1 - beta2^t), -}
+// AdamW exactly as torch.optim.AdamW (decoupled decay first): hyper[group] = {lr, weight_decay, beta1, beta2, eps, -, -, -}.
+// The bias corrections come from the parameter's own step count t = steps[step_idx] + 1, which advances only in the steps
+// that have its gradient (torch skips a parameter whose .grad is None), and are computed in double as torch does on the host.
 __device__ __forceinline__ void adamw_elem(float& p, float g, float& m, float& v, float lr, float wd, float b1, float b2, float eps,
-                                           float bc1, float bc2s) {
+                                           float step_size, float bc2s) {
   p *= 1.f - lr * wd;
   m = m + (g - m) * (1.f - b1);                 // torch: exp_avg.lerp_(grad, 1 - beta1)
   v = b2 * v + (1.f - b2) * g * g;
   const float denom = sqrtf(v) / bc2s + eps;
-  p -= (lr / bc1) * (m / denom);
+  p -= step_size * (m / denom);
 }
 
 __global__ void __launch_bounds__(kOptThreads)
 multi_adamw_kernel(const OptTensor* __restrict__ tensors, const int* __restrict__ chunk_tensor, const int* __restrict__ chunk_index,
-                   const float* __restrict__ hyper, int n_groups, const int* __restrict__ step, const float* __restrict__ clip) {
+                   const float* __restrict__ hyper, int n_groups, const int* __restrict__ step, const float* __restrict__ clip,
+                   const int* __restrict__ steps) {
   const OptTensor t = tensors[chunk_tensor[blockIdx.x]];
   const long long base = (long long)chunk_index[blockIdx.x] * kChunk;
   const int n = (int)min((long long)kChunk, t.numel - base);
   const float* h = hyper + ((long long)(*step % SAICV_OPT_RING) * n_groups + t.group) * 8;
-  const float lr = h[0], wd = h[1], b1 = h[2], b2 = h[3], eps = h[4], bc1 = h[5], bc2s = h[6];
+  const float lr = h[0], wd = h[1], b1 = h[2], b2 = h[3], eps = h[4];
+  const int st = steps[t.step_idx] + 1;
+  const float step_size = (float)((double)lr / (1.0 - pow((double)b1, st)));   // torch: lr / (1 - beta1^t)
+  const float bc2s = (float)sqrt(1.0 - pow((double)b2, st));                   // torch: (1 - beta2^t) ** 0.5
   const float gs = clip ? clip[0] : 1.f;
   const bool vec = ((reinterpret_cast<uintptr_t>(t.p + base) | reinterpret_cast<uintptr_t>(t.g + base) |
                      reinterpret_cast<uintptr_t>(t.s1 + base) | reinterpret_cast<uintptr_t>(t.s2 + base)) & 15) == 0 && (n & 3) == 0;
@@ -135,10 +140,10 @@ multi_adamw_kernel(const OptTensor* __restrict__ tensors, const int* __restrict_
     for (int i = threadIdx.x; i < n / 4; i += kOptThreads) {
       float4 p = p4[i], m = m4[i], v = v4[i];
       const float4 g = g4[i];
-      adamw_elem(p.x, g.x * gs, m.x, v.x, lr, wd, b1, b2, eps, bc1, bc2s);
-      adamw_elem(p.y, g.y * gs, m.y, v.y, lr, wd, b1, b2, eps, bc1, bc2s);
-      adamw_elem(p.z, g.z * gs, m.z, v.z, lr, wd, b1, b2, eps, bc1, bc2s);
-      adamw_elem(p.w, g.w * gs, m.w, v.w, lr, wd, b1, b2, eps, bc1, bc2s);
+      adamw_elem(p.x, g.x * gs, m.x, v.x, lr, wd, b1, b2, eps, step_size, bc2s);
+      adamw_elem(p.y, g.y * gs, m.y, v.y, lr, wd, b1, b2, eps, step_size, bc2s);
+      adamw_elem(p.z, g.z * gs, m.z, v.z, lr, wd, b1, b2, eps, step_size, bc2s);
+      adamw_elem(p.w, g.w * gs, m.w, v.w, lr, wd, b1, b2, eps, step_size, bc2s);
       p4[i] = p; m4[i] = m; v4[i] = v;
       if (t.shadow) {
         const float pv[4] = {p.x, p.y, p.z, p.w};
@@ -149,15 +154,23 @@ multi_adamw_kernel(const OptTensor* __restrict__ tensors, const int* __restrict_
   } else {
     for (int i = threadIdx.x; i < n; i += kOptThreads) {
       float p = t.p[base + i], m = t.s1[base + i], v = t.s2[base + i];
-      adamw_elem(p, t.g[base + i] * gs, m, v, lr, wd, b1, b2, eps, bc1, bc2s);
+      adamw_elem(p, t.g[base + i] * gs, m, v, lr, wd, b1, b2, eps, step_size, bc2s);
       t.p[base + i] = p; t.s1[base + i] = m; t.s2[base + i] = v;
       if (t.shadow) write_shadow(t, base + i, p);
     }
   }
 }
 
+// Advances the step count of every parameter of the table (those with a gradient) and the ring step.
+__global__ void adamw_advance_kernel(const OptTensor* __restrict__ tensors, int n_tensors, int* __restrict__ steps,
+                                     int* __restrict__ step) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_tensors) steps[tensors[i].step_idx] += 1;
+  if (i == 0) *step += 1;
+}
+
 // Global gradient norm, deterministic: per-chunk sums of squares, then one block folds them in chunk order and writes
-// clip = {min(1, max_norm / (norm + 1e-6)), norm}   (torch.nn.utils.clip_grad_norm_'s coefficient).
+// clip = {min(1, max_norm / (norm + 1e-6)), norm}   (torch.nn.utils.clip_grad_norm_'s coefficient, NaN when the norm is).
 __global__ void __launch_bounds__(kOptThreads)
 multi_sqnorm_kernel(const OptTensor* __restrict__ tensors, const int* __restrict__ chunk_tensor, const int* __restrict__ chunk_index,
                     float* __restrict__ partial) {
@@ -194,7 +207,8 @@ clip_coef_kernel(const float* __restrict__ partial, int n, float max_norm, float
   }
   if (threadIdx.x == 0) {
     const float norm = (float)sqrt(red[0]);
-    clip[0] = fminf(1.f, max_norm / (norm + 1e-6f));
+    const float c = max_norm / (norm + 1e-6f);
+    clip[0] = isnan(c) ? c : fminf(1.f, c);   // a NaN norm scales every gradient to NaN, as torch.clamp keeps it
     clip[1] = norm;
   }
 }
@@ -361,14 +375,14 @@ int saicv_multi_tensor_sgd(const void* tensors, const int* chunk_tensor, const i
   return check_launch("opt_advance_kernel");
 }
 
-int saicv_multi_tensor_adamw(const void* tensors, const int* chunk_tensor, const int* chunk_index, int n_chunks,
-                             const float* hyper, int n_groups, int* step, const float* clip, void* stream) {
+int saicv_multi_tensor_adamw(const void* tensors, const int* chunk_tensor, const int* chunk_index, int n_chunks, int n_tensors,
+                             const float* hyper, int n_groups, int* step, const float* clip, int* steps, void* stream) {
   if (n_chunks <= 0) return 0;
-  multi_adamw_kernel<<<n_chunks, kOptThreads, 0, ST>>>(reinterpret_cast<const OptTensor*>(tensors), chunk_tensor, chunk_index, hyper,
-                                                       n_groups, step, clip);
+  const OptTensor* t = reinterpret_cast<const OptTensor*>(tensors);
+  multi_adamw_kernel<<<n_chunks, kOptThreads, 0, ST>>>(t, chunk_tensor, chunk_index, hyper, n_groups, step, clip, steps);
   if (check_launch("multi_adamw_kernel")) return 1;
-  opt_advance_kernel<<<1, 1, 0, ST>>>(step);
-  return check_launch("opt_advance_kernel");
+  adamw_advance_kernel<<<(n_tensors + 255) / 256, 256, 0, ST>>>(t, n_tensors, steps, step);
+  return check_launch("adamw_advance_kernel");
 }
 
 int saicv_multi_tensor_clip_coef(const void* tensors, const int* chunk_tensor, const int* chunk_index, int n_chunks,

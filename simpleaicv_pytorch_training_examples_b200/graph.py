@@ -48,7 +48,7 @@ class GraphedTrainStep:
 
     def _replay(self):
         # fused optimizers (optim.py) read their hyper-parameters from a pinned table through a copy node of the graph:
-        # per-iteration learning rates / AdamW bias corrections are a host write before the launch
+        # per-iteration learning rates are a host write before the launch
         sync = getattr(self.optimizer, 'sync_hyper', None)
         if sync is not None:
             sync()

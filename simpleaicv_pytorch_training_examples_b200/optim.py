@@ -26,7 +26,7 @@ from . import _lib
 RING = 8   # SAICV_OPT_RING
 
 _TENSOR_DTYPE = np.dtype([('p', '<u8'), ('g', '<u8'), ('s1', '<u8'), ('s2', '<u8'), ('shadow', '<u8'), ('numel', '<i8'),
-                          ('group', '<i4'), ('rs', '<i4'), ('c', '<i4'), ('cp', '<i4'), ('kpad', '<i4'), ('pad_', '<i4')])
+                          ('group', '<i4'), ('rs', '<i4'), ('c', '<i4'), ('cp', '<i4'), ('kpad', '<i4'), ('step_idx', '<i4')])
 assert _TENSOR_DTYPE.itemsize == 72   # saicv_opt_tensor (include/saicv_b200.h)
 
 # a registered copy that is one fixed tensor; an engine.operands.Operand has the same two fields
@@ -54,7 +54,7 @@ class _FusedBase(torch.optim.Optimizer):
         self._shadows = {}        # id(param) -> copy refreshed by the step: _Fixed or engine.operands.Operand (.w, .conv)
         self._key = None          # identity of the table (pointers of p / grad / operand copy)
         self._tab = None
-        self._t = 0               # optimizer steps taken (AdamW bias correction)
+        self._t = 0               # optimizer steps taken (selects the ring slot)
         self._clip = None
         self._use_clip = False
         self._hyper_host = None   # pinned [RING][groups][8]; slot t % RING holds the table of step t
@@ -101,6 +101,9 @@ class _FusedBase(torch.optim.Optimizer):
     def _state_tensors(self, p):
         raise NotImplementedError
 
+    def _step_index(self, p):
+        return 0
+
     def _build(self, plist):
         dev = plist[0][1].device
         chunk = _lib.load().saicv_opt_chunk()
@@ -114,6 +117,7 @@ class _FusedBase(torch.optim.Optimizer):
             r['p'], r['g'], r['s1'] = p.data_ptr(), p.grad.data_ptr(), st[0].data_ptr()
             r['s2'] = st[1].data_ptr() if len(st) > 1 else 0
             r['numel'], r['group'] = p.numel(), gi
+            r['step_idx'] = self._step_index(p)
             op = self._shadows.get(id(p))
             if op is not None and op.w is not None:
                 r['shadow'] = op.w.data_ptr()
@@ -128,7 +132,7 @@ class _FusedBase(torch.optim.Optimizer):
         tab = {
             'tensors': torch.from_numpy(rows.view(np.uint8).copy()).to(dev),
             'ct': torch.tensor(ct, dtype=torch.int32).to(dev), 'ci': torch.tensor(ci, dtype=torch.int32).to(dev),
-            'n': len(ct), 'partial': torch.empty(len(ct), device=dev), 'dev': dev,
+            'n': len(ct), 'n_tensors': len(plist), 'partial': torch.empty(len(ct), device=dev), 'dev': dev,
         }
         if self._hyper_host is None or self._hyper_host.shape[1] != len(self.param_groups):
             self._hyper_host = torch.zeros(RING, len(self.param_groups), 8).pin_memory()
@@ -149,17 +153,17 @@ class _FusedBase(torch.optim.Optimizer):
         return self._tab
 
     # ---- hyper-parameters
-    def _hyper_row(self, g, t):
+    def _hyper_row(self, g):
         raise NotImplementedError
 
     def _publish(self):
         """Host side of step number self._t (0-based): waits until the step that last used its ring slot has been
-        launched RING steps ago AND executed, writes the table (AdamW bias corrections are those of update t + 1)."""
+        launched RING steps ago AND executed, writes the table."""
         slot = self._t % RING
         if self._events[slot] is not None and not torch.cuda.is_current_stream_capturing():
             self._events[slot].synchronize()
         for gi, g in enumerate(self.param_groups):
-            row = self._hyper_row(g, self._t + 1)
+            row = self._hyper_row(g)
             self._hyper_np[slot, gi, :len(row)] = row
         self._t += 1
         return slot
@@ -236,16 +240,21 @@ class FusedSGD(_FusedBase):
             st['momentum_buffer'] = torch.zeros_like(p, memory_format=torch.preserve_format)   # first step: buf = g
         return (st['momentum_buffer'],)
 
-    def _hyper_row(self, g, t):
+    def _hyper_row(self, g):
         return (g['lr'], g['weight_decay'], g['momentum'], 1. if g['nesterov'] else 0.)
 
 
 class FusedAdamW(_FusedBase):
-    """torch.optim.AdamW(params, lr, betas, eps, weight_decay) (amsgrad / maximize off; tools/utils.py:591-600)."""
+    """torch.optim.AdamW(params, lr, betas, eps, weight_decay) (amsgrad / maximize off; tools/utils.py:591-600).  Like
+    torch, every parameter has its own step count, advanced only by the steps that have its gradient: a parameter whose
+    .grad is None (zero_grad(), an unused branch) keeps its bias corrections.  The counts live on the device
+    (int32, indexed by the parameter's position in param_groups), so nothing per parameter is written by the host in a step."""
     _entry = 'saicv_multi_tensor_adamw'
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
+        self._index = {}          # id(param) -> its row of self._steps
+        self._steps = None        # device int32 [parameters]: step counts
 
     def _state_tensors(self, p):
         st = self.state[p]
@@ -255,24 +264,54 @@ class FusedAdamW(_FusedBase):
             st['exp_avg_sq'] = torch.zeros_like(p, memory_format=torch.preserve_format)
         return st['exp_avg'], st['exp_avg_sq']
 
-    def _hyper_row(self, g, t):
+    def _step_index(self, p):
+        return self._index[id(p)]
+
+    def _hyper_row(self, g):
         b1, b2 = g['betas']
-        t = max(t, 1)
-        return (g['lr'], g['weight_decay'], b1, b2, g['eps'], 1. - b1 ** t, math.sqrt(1. - b2 ** t))
+        return (g['lr'], g['weight_decay'], b1, b2, g['eps'])
+
+    def _build(self, plist):
+        order = [p for g in self.param_groups for p in g['params']]
+        if self._steps is None or self._steps.numel() != len(order):   # first step, or add_param_group()
+            self._save_steps()
+            self._index = {id(p): i for i, p in enumerate(order)}
+            self._steps = torch.zeros(len(order), dtype=torch.int32, device=plist[0][1].device)
+            self._load_steps()
+        return super()._build(plist)
+
+    def _launch(self, tab, clip):
+        _lib.call(self._entry, _p(tab['tensors']), _p(tab['ct']), _p(tab['ci']), tab['n'], tab['n_tensors'],
+                  _p(self._hyper_dev), len(self.param_groups), _p(self._step_dev), clip, _p(self._steps), _stream())
+
+    def _save_steps(self):
+        """device step counts -> state['step']"""
+        if self._steps is None:
+            return
+        host = self._steps.cpu()
+        for p in (p for g in self.param_groups for p in g['params']):
+            i = self._index.get(id(p))
+            if i is not None and 'step' in self.state[p]:
+                self.state[p]['step'] = torch.tensor(float(host[i]))
+
+    def _load_steps(self):
+        """state['step'] -> device step counts"""
+        if self._steps is None:
+            return
+        host = torch.zeros(self._steps.numel(), dtype=torch.int32)
+        for p in (p for g in self.param_groups for p in g['params']):
+            i = self._index.get(id(p))
+            if i is not None and 'step' in self.state[p]:
+                host[i] = int(self.state[p]['step'])
+        self._steps.copy_(host)
 
     def state_dict(self):
-        for st in self.state.values():
-            if 'step' in st:
-                st['step'] = torch.tensor(float(self._t))
+        self._save_steps()
         return super().state_dict()
 
     def load_state_dict(self, state_dict):
         super().load_state_dict(state_dict)
-        steps = [float(st['step']) for st in self.state.values() if 'step' in st]
-        self._t = int(max(steps)) if steps else 0
-        self._key = None
-        if self._hyper_host is not None:
-            self._step_dev.fill_(self._t)
+        self._load_steps()
 
 
 _MUON_DTYPE = np.dtype([('slot', '<i8'), ('rows', '<i4'), ('cols', '<i4'), ('ld', '<i4'), ('transposed', '<i4'),
@@ -363,7 +402,7 @@ class FusedMuon(_FusedBase):
             st['moment2'] = torch.zeros_like(p)
         return st['moment1'], st['moment2']
 
-    def _hyper_row(self, g, t):
+    def _hyper_row(self, g):
         b1, b2 = g['adamw_betas']
         return (g['lr'], g['wd'], g['momentum'], 1. if g['nesterov'] else 0., b1, b2, g['adamw_eps'])
 
@@ -385,7 +424,6 @@ class FusedMuon(_FusedBase):
             else:
                 r['slot'], r['step_idx'] = -1, self._adam_index[id(p)]
         tab['muon'] = torch.from_numpy(rows.view(np.uint8).copy()).to(dev)
-        tab['n_tensors'] = len(plist)
         if self._ns is None:
             big_x = max((b * mp * np_ for _, b, mp, np_ in self._classes), default=0)
             big_a = max((b * mp * mp for _, b, mp, _ in self._classes), default=0)
