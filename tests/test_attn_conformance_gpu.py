@@ -50,64 +50,26 @@ Invariants (compared as raw bits):
   * owned writes: output storage with slack rows and columns is filled with a NaN sentinel; after the launches
     everything outside the O, dQ, dK and dV views, and dK's columns from dk_cols on, still holds it.
 """
-import importlib.util
 import math
-import os
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-_spec = importlib.util.spec_from_file_location('gemm_conformance', os.path.join(HERE, 'test_gemm_conformance_gpu.py'))
-_gemm = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(_gemm)
-_rne_bf16, _conform, _same = _gemm._rne_bf16, _gemm._conform, _gemm._same
+from conformance import M32, U, check, drop_scale, dropout_hash, dropout_keep, dropout_threshold, rne_bf16, same
 
-U = 2.0 ** -24          # one fp32 rounding, relative
+from simpleaicv_pytorch_training_examples_b200 import _lib, ops
+
 APPROX = 2.0 ** -21     # ex2.approx, __fdividef, relative
 ACC = 2.0 ** -16        # wgmma fp32 accumulation, relative to the absolute product sum
 TINY = 2.0 ** -125      # below this an ex2.approx.ftz result may be flushed to zero
-M32 = 0xFFFFFFFF
 WIDTHS = [(32, 32), (48, 32), (64, 64), (80, 80), (96, 64), (112, 64), (112, 80), (128, 80), (192, 64), (208, 80)]
 DROP_WIDTHS = [(32, 32), (48, 32), (64, 64)]
 SENTINEL = 0x7FA5       # a bf16 NaN the kernels never produce
 
 
-def _ops():
-    from simpleaicv_pytorch_training_examples_b200 import ops
-    return ops
-
-
-# ------------------------------------------------------------------ the counter hash and its threshold, as the C ABI sees them
-def _hash(seed, a, b):
-    """csrc/dropout_hash.cuh on int64 tensors a, b (32-bit values): int64 products wrap, the low 32 bits are exact."""
-    lo, hi = seed & M32, (seed >> 32) & M32
-    x = ((a + lo) & M32) * 0x9E3779B1 & M32
-    x = x ^ (((b + hi) & M32) * 0x85EBCA77 & M32)
-    x = x ^ (x >> 16)
-    x = x * 0x7FEB352D & M32
-    x = x ^ (x >> 15)
-    x = x * 0x846CA68B & M32
-    return x ^ (x >> 16)
-
-
-def _threshold(p):
-    """dropout_threshold((float)p): the entries take p as a C float."""
-    t = float(np.float32(p)) * 4294967296.0
-    return M32 if t >= 4294967295.0 else int(t)
-
-
-def _keep(seed, a, b, p):
-    return _hash(seed, a, b) >= _threshold(p)
-
-
-def _drop_scale(p):
-    """AttnDrop.scale = 1.f / (1.f - p) in fp32."""
-    return float(np.float32(1.0) / (np.float32(1.0) - np.float32(p)))
-
-
+# ------------------------------------------------------------------ the counter hash copy (conformance.py) against the C ABI
 def _seed_hashing_element0_to(h):
     """A seed (high word 0) whose hash of element (0, 0) is h: the finaliser is a bijection, invert it."""
     x = h ^ (h >> 16)
@@ -138,13 +100,15 @@ def test_dropout_hash_copy_and_threshold_cpu():
     a = torch.randint(0, 1 << 32, (2000,), generator=g, dtype=torch.int64)
     b = torch.randint(0, 1 << 32, (2000,), generator=g, dtype=torch.int64)
     for seed in (0, 0x0123456789ABCDEF, 0xFFFFFFFFFFFFFF00):
-        got = _hash(seed, a, b).tolist()
+        got = dropout_hash(seed, a, b).tolist()
         assert got == [ref(seed, x, y) for x, y in zip(a.tolist(), b.tolist())]
-    assert _threshold(0.1) - int(0.1 * 4294967296.0) == 7 and _threshold(0.2) - int(0.2 * 4294967296.0) == 13
-    assert _threshold(0.5) == 1 << 31 and _threshold(0.0) == 0
-    assert _hash(SEED_BETWEEN, torch.zeros(1, dtype=torch.int64), torch.zeros(1, dtype=torch.int64)).item() == int(0.1 * 2 ** 32)
-    assert not _keep(SEED_BETWEEN, torch.zeros(1, dtype=torch.int64), torch.zeros(1, dtype=torch.int64), 0.1).item()
-    assert _drop_scale(0.1) == float(np.float32(1) / np.float32(0.9))
+    assert dropout_threshold(0.1) - int(0.1 * 4294967296.0) == 7
+    assert dropout_threshold(0.2) - int(0.2 * 4294967296.0) == 13
+    assert dropout_threshold(0.5) == 1 << 31 and dropout_threshold(0.0) == 0
+    zero = torch.zeros(1, dtype=torch.int64)
+    assert dropout_hash(SEED_BETWEEN, zero, zero).item() == int(0.1 * 2 ** 32)
+    assert not dropout_keep(SEED_BETWEEN, zero, zero, 0.1).item()
+    assert drop_scale(0.1) == float(np.float32(1) / np.float32(0.9))
 
 
 @pytest.mark.gpu
@@ -152,11 +116,10 @@ def test_dropout_hash_copy_and_threshold_cpu():
 def test_dropout_hash_copy_matches_device(p, seed):
     """ops.dropout on ones keeps exactly the hash(seed, i mod 2^32, i >> 32) mask (capi_detr.cu's indexing), which pins
     the torch copy the attention references use."""
-    ops = _ops()
     n = 1 << 16
     got = ops.dropout(torch.ones(n, device='cuda', dtype=torch.bfloat16), p, seed) != 0
     i = torch.arange(n, device='cuda', dtype=torch.int64)
-    want = _keep(seed, i & M32, i >> 32, p)
+    want = dropout_keep(seed, i & M32, i >> 32, p)
     assert torch.equal(got, want), f'{int((got != want).sum())} of {n} keep decisions differ'
 
 
@@ -233,14 +196,14 @@ def _mask(kind, B, Lk, seed=0):
     words = (Lk + 127) // 128 * 4 + (4 if kind == 'wide' else 0)
     full = torch.ones(B, words * 32, dtype=torch.bool, device='cuda')
     full[:, :Lk] = dead
-    return dead, _ops().pack_key_mask(full, words * 32)
+    return dead, ops.pack_key_mask(full, words * 32)
 
 
 def _keep_mask(B, H, Lq, Lk, p, seed):
     """keep [B, H, Lq, Lk] of the attention kernels: hash row (b H + h) Lq + q, column key."""
     rows = torch.arange(B * H * Lq, device='cuda', dtype=torch.int64).view(B, H, Lq, 1)
     cols = torch.arange(Lk, device='cuda', dtype=torch.int64).view(1, 1, 1, Lk)
-    return _keep(seed, rows, cols, p)
+    return dropout_keep(seed, rows, cols, p)
 
 
 def _live(dead, shape):
@@ -285,7 +248,7 @@ def _fwd_ref(q, k, v, sigma, dead, keep, dscale):
     if keep is not None:
         plo = torch.where(keep, plo * dscale * (1 - U), 0.0)
         phi = torch.where(keep, phi * dscale * (1 + U) + 2.0 ** -149, 0.0)
-    wlo, whi = _rne_bf16(plo), _rne_bf16(phi)
+    wlo, whi = rne_bf16(plo), rne_bf16(phi)
     del plo, phi
     vd = v.double()
     num = ((wlo + whi) / 2 * pi) @ vd
@@ -346,8 +309,8 @@ def _bwd_ref(q, k, v, o, lse, do, sigma, dead, keep, dscale):
     rds = torch.maximum(phi - pc, pc - plo) * (yc.abs() + ry) + pc * ry
     rds = rds + U * (ds.abs() + rds) + 2.0 ** -149
     del yc, ry
-    dslo = torch.where(live, _rne_bf16(ds - rds), 0.0)
-    dshi = torch.where(live, _rne_bf16(ds + rds), 0.0)
+    dslo = torch.where(live, rne_bf16(ds - rds), 0.0)
+    dshi = torch.where(live, rne_bf16(ds + rds), 0.0)
     del ds, rds
     dq = _mm_interval(dslo, dshi, k, sg)
     dk = _mm_interval(dslo.transpose(-1, -2), dshi.transpose(-1, -2), q, sg)
@@ -355,8 +318,8 @@ def _bwd_ref(q, k, v, o, lse, do, sigma, dead, keep, dscale):
     if keep is not None:
         plo = torch.where(keep, plo * dscale * (1 - U), 0.0)
         phi = torch.where(keep, phi * dscale * (1 + U) + 2.0 ** -149, 0.0)
-    ptlo = torch.where(live, _rne_bf16(plo), 0.0).transpose(-1, -2)
-    pthi = torch.where(live, _rne_bf16(phi), 0.0).transpose(-1, -2)
+    ptlo = torch.where(live, rne_bf16(plo), 0.0).transpose(-1, -2)
+    pthi = torch.where(live, rne_bf16(phi), 0.0).transpose(-1, -2)
     del plo, phi, pc
     return dq, dk, _mm_interval(ptlo, pthi, do)
 
@@ -367,18 +330,17 @@ def _dk_cols(dqk, dv):
 
 
 def _run(B, H, Lq, Lk, dqk, dv, regime='random', mask=None, p=0.0, seed=0xFFFFFFFFFFFFFF00, tag=''):
-    ops = _ops()
     q, k, v, sigma = _operands(B, H, Lq, Lk, dqk, dv, regime, seed=B * 7 + Lq + 3 * Lk + dqk)
     dead, bits = _mask(mask, B, Lk, seed=Lq + Lk)
     keep = _keep_mask(B, H, Lq, Lk, p, seed) if p > 0 else None
-    dscale = _drop_scale(p) if p > 0 else 1.0
+    dscale = drop_scale(p) if p > 0 else 1.0
     what = f'{tag}B{B} H{H} Lq{Lq} Lk{Lk} ({dqk},{dv}) {regime} mask={mask} p={p}'
     out, lse = ops.attn_fwd(q, k, v, sigma, mask_bits=bits, dropout_p=p, dropout_seed=seed)
     oc, oa, os_, lc, la, rowlive = _fwd_ref(q, k, v, sigma, dead, keep, dscale)
-    _conform(f'O {what}', out, oc, oa, os_)
+    check(None, f'O {what}', out, oc, oa, os_)
     assert torch.equal(lse[~rowlive], torch.full_like(lse[~rowlive], float('-inf'))), f'lse {what}: rows without keys'
     if rowlive.any():
-        _conform(f'lse {what}', lse[rowlive], lc[rowlive], la[rowlive], torch.ones_like(la[rowlive]))
+        check(None, f'lse {what}', lse[rowlive], lc[rowlive], la[rowlive], torch.ones_like(la[rowlive]))
     del oc, oa, os_, lc, la
     g = torch.Generator(device='cuda').manual_seed(Lq * 31 + Lk)
     do = torch.randn(B, Lq, H, dv, device='cuda', generator=g).bfloat16().permute(0, 2, 1, 3)   # the layout of out
@@ -386,9 +348,9 @@ def _run(B, H, Lq, Lk, dqk, dv, regime='random', mask=None, p=0.0, seed=0xFFFFFF
     dkc = _dk_cols(dqk, dv)
     ops.attn_bwd(q, k, v, out, lse, do, sigma, dq, dk, dvv, dk_cols=dkc, mask_bits=bits, dropout_p=p, dropout_seed=seed)
     (qc, qa, qs), (kc, ka, ks), (vc, va, vs) = _bwd_ref(q, k, v, out, lse, do, sigma, dead, keep, dscale)
-    _conform(f'dQ {what}', dq, qc, qa, qs)
-    _conform(f'dK {what}', dk[..., :dkc], kc[..., :dkc], ka[..., :dkc], ks[..., :dkc])
-    _conform(f'dV {what}', dvv, vc, va, vs)
+    check(None, f'dQ {what}', dq, qc, qa, qs)
+    check(None, f'dK {what}', dk[..., :dkc], kc[..., :dkc], ka[..., :dkc], ks[..., :dkc])
+    check(None, f'dV {what}', dvv, vc, va, vs)
 
 
 CASES = []
@@ -432,7 +394,6 @@ def test_attn_lengths_conform(dqk, dv):
 @pytest.mark.parametrize('B,H,L,dqk,dv', [(6, 16, 150, 64, 64), (4, 12, 150, 208, 80)])
 def test_attn_items_are_independent(B, H, L, dqk, dv):
     """Each (b, h) of a launch with more items than resident CTAs equals the same (b, h) launched alone."""
-    ops = _ops()
     q, k, v, sigma = _operands(B, H, L, L, dqk, dv, seed=5)
     _, bits = _mask('holes', B, L, seed=5)
     do = torch.randn(B, L, H, dv, device='cuda', generator=torch.Generator(device='cuda').manual_seed(6)).bfloat16().permute(0, 2, 1, 3)
@@ -448,12 +409,12 @@ def test_attn_items_are_independent(B, H, L, dqk, dv):
             _, lse1[i] = ops.attn_fwd(q[i], k[i], v[i], sigma, out=out1[i], mask_bits=bits[b:b + 1])
             ops.attn_bwd(q[i], k[i], v[i], out[i], lse[i], do[i], sigma, *(t[i] for t in grads1), dk_cols=dkc,
                          mask_bits=bits[b:b + 1])
-    _same('O alone vs in a multi-item launch', out1, out)
-    _same('lse alone vs in a multi-item launch', lse1, lse)
+    same('O alone vs in a multi-item launch', out1, out)
+    same('lse alone vs in a multi-item launch', lse1, lse)
     for name, a, b_ in zip(('dQ', 'dK', 'dV'), grads1, grads):
         if name == 'dK':
             a, b_ = a[..., :dkc], b_[..., :dkc]
-        _same(f'{name} alone vs in a multi-item launch', a, b_)
+        same(f'{name} alone vs in a multi-item launch', a, b_)
 
 
 def _sentinel(*shape):
@@ -465,7 +426,6 @@ def _sentinel(*shape):
 def test_attn_layouts_and_owned_writes(dqk, dv, dk_cols):
     """The same data as contiguous [B, H, L, D], packed [B, L, 3, H, D] views (dqk == dv) and views with slack between
     rows give the same bits; outputs written into sentinel-filled storage with slack leave everything else untouched."""
-    ops = _ops()
     B, H, L = 2, 3, 150
     q, k, v, sigma = _operands(B, H, L, L, dqk, dv, seed=9)
     _, bits = _mask('holes', B, L, seed=9)
@@ -498,7 +458,7 @@ def test_attn_layouts_and_owned_writes(dqk, dv, dk_cols):
     gst = [slack(t) for t in (q, k, v)]
     got = run(qs, ks, vs, ov, dov, [g[1] for g in gst])
     for n, a, b in zip(names, got, base):
-        _same(f'{n} with slack between rows vs contiguous', a, b)
+        same(f'{n} with slack between rows vs contiguous', a, b)
     owned = [(ost, dv), (gst[0][0], dqk), (gst[1][0], dk_cols), (gst[2][0], dv)]
     for n, (st, cols) in zip(('O', 'dQ', 'dK', 'dV'), owned):
         region = torch.zeros(st.shape, dtype=torch.bool, device='cuda')
@@ -515,7 +475,7 @@ def test_attn_layouts_and_owned_writes(dqk, dv, dk_cols):
         dqkv = torch.empty_like(qkv)
         got = run(qp, kp, vp, op, dop, [dqkv[:, :, i].permute(0, 2, 1, 3) for i in range(3)])
         for n, a, b in zip(names, got, base):
-            _same(f'{n} packed [B, L, 3, H, D] vs contiguous', a, b)
+            same(f'{n} packed [B, L, 3, H, D] vs contiguous', a, b)
         assert (dqkv[:, :, 1, :, dk_cols:].contiguous().view(torch.int16) == SENTINEL).all(), 'dK columns >= dk_cols written'
 
 
@@ -524,7 +484,6 @@ def test_attn_layouts_and_owned_writes(dqk, dv, dk_cols):
 def test_attn_dropout_seed_base_carries(dqk, dv):
     """A device seed base whose addition carries from the low seed word into the high one gives the same masks as the
     equivalent constant seed, forward and backward."""
-    ops = _ops()
     B, H, L, p = 2, 4, 150, 0.5
     q, k, v, sigma = _operands(B, H, L, L, dqk, dv, seed=12)
     _, bits = _mask('holes', B, L, seed=12)
@@ -540,15 +499,13 @@ def test_attn_dropout_seed_base_carries(dqk, dv):
         grads[1] = grads[1][..., :_dk_cols(dqk, dv)]
         runs.append([out, lse, *grads])
     for n, a, b in zip(('O', 'lse', 'dQ', 'dK', 'dV'), *runs):
-        _same(f'{n}: seed base carrying into the high word vs the constant seed', a, b)
+        same(f'{n}: seed base carrying into the high word vs the constant seed', a, b)
 
 
 # ------------------------------------------------------------------ refusals
 @pytest.mark.gpu
 def test_attn_refusals_launch_nothing():
     """Malformed arguments raise through _lib.call before either entry launches a kernel."""
-    from simpleaicv_pytorch_training_examples_b200 import _lib
-    ops = _ops()
     B, H, L = 1, 2, 200
 
     def operands(dqk, dv):

@@ -40,12 +40,9 @@ gamma(m) = m u / (1 - m u) bounds m chained roundings.
     are products of two bf16 values (b or dh times the stored bf16 silu), so given the stored silu they are bit-exact.
   * im2col_nhwc is bit-exact against a float64 unfold, including its zero padding.  col2im_nhwc adds at most
     ceil(k / s)^2 bf16 terms in (r, s) order from 0: fp32 within gamma(ceil(k / s)^2) sum |terms|, then bf16.
-  * Outputs: a bf16 output must lie in [rne(v - B), rne(v + B)], an fp32 output within B of v.  Every element must
-    conform; no fraction may miss.  A bf16 output shows its fp32 error only where the exact value lies within B of
-    a bf16 rounding boundary, so families whose fp32 value is exact or a few roundings from it (gate_bwd, col2im,
-    silu) can report a share of 0.
-Each check prints the largest fraction of its allowance an element used; at the end of the module the largest share
-per family is printed (run with -s), with the families that are checked bit for bit.
+  * A bf16 output shows its fp32 error only where the exact value lies within B of a bf16 rounding boundary, so
+    families whose fp32 value is exact or a few roundings from it (gate_bwd, col2im, silu) can report a share of 0,
+    as the bit-exact ones do.
 
 Launch geometry.  Python mirrors of grid_1d (host_util.cu), saicv_dwconv_wgrad_blocks and
 ppb; every shape list asserts that it runs a grid-stride loop more than once, and the weight-gradient list that it
@@ -54,67 +51,28 @@ has nblk = 132 with a ragged last block.
 Invariants (raw bits): outputs and partial workspaces are filled with NaN before each launch, so an unwritten
 element or a folded stale partial fails, and two consecutive launches give identical outputs.
 """
-import importlib.util
 import math
-import os
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-_spec = importlib.util.spec_from_file_location('norm_conformance', os.path.join(HERE, 'test_norm_conformance_gpu.py'))
-_norm = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(_norm)
-_check, _same, _rnd, _van_slab, _rne_bf16 = _norm._check, _norm._same, _norm._rnd, _norm._van_slab, _norm._rne_bf16
-_randn, _rand, _nan, _every_bf16 = _norm._randn, _norm._rand, _norm._nan, _norm._every_bf16
+from conformance import NAN, U, call, check, every_bf16, exact, nan, rand, randn, rne_bf16, rnd, same, van_slab
+from conformance import report  # noqa: F401  (autouse: this module's allowance report)
+
+from simpleaicv_pytorch_training_examples_b200 import _lib, ops
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -24              # one fp32 rounding, relative
 ETA = 2.0 ** -150           # one fp32 rounding in the subnormal range, absolute
 EXP_REL = 4 * U             # expf: 2 ulp
 EXP_ABS = 2.0 ** -148       # expf: 2 ulp of a subnormal result
 FP32_OVF = 2.0 ** 128 * (1 - 2.0 ** -25)    # an fp32 rounding of a value at or above this gives +inf
-NAN = float('nan')
 BF16 = torch.bfloat16
-EXACT = set()
-
-
-def _lib():
-    from simpleaicv_pytorch_training_examples_b200 import _lib
-    return _lib
-
-
-def _ops():
-    from simpleaicv_pytorch_training_examples_b200 import ops
-    return ops
-
-
-def _call(name, *args):
-    ops = _ops()
-    _lib().call(name, *[ops._p(a) if isinstance(a, torch.Tensor) else a for a in args], ops._stream())
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _report():
-    yield
-    if _norm.USED:
-        print('\nlargest share of the allowance used, by family:')
-        for k in sorted(_norm.USED):
-            print(f'  {k:28s} {_norm.USED[k]:.3g}')
-    if EXACT:
-        print('bit-exact: ' + ', '.join(sorted(EXACT)))
 
 
 def _gamma(m):
     return m * U / (1 - m * U)
-
-
-def _exact(family, what, out, want):
-    _same(what, out, want)
-    EXACT.add(family)
-    print(f'{what}: bit-exact')
 
 
 def _zero_bits(what, out, dead):
@@ -186,7 +144,7 @@ assert any(_loops(r * c // 8, 256, _grid_1d(r * c // 8)) > 1 for r, c in GATE)
 LS = [(1, 8, 1), (147, 1536, 49), (1570, 384, 785), (50176, 8, 3136), (40000, 384, 800), (2113, 1536, 197),
       (8448, 1536, 264), (64 * 3136, 32, 3136)]
 assert any(_loops(r * c // 8, 256, _grid_1d(r * c // 8)) > 1 for r, c, _ in LS)
-assert any(_van_slab(r, c)[2] == 264 for r, c, _ in LS)
+assert any(van_slab(r, c)[2] == 264 for r, c, _ in LS)
 
 SWIGLU_N = [8, 4104, 6291456]
 assert any(_loops(n // 8, 256, _grid_1d(n // 8)) > 1 for n in SWIGLU_N)
@@ -211,11 +169,11 @@ assert any((h + 2 * p - k) % s for _, h, _, _, k, s, p in IM2COL)
 def test_launch_geometry_mirrors_match_the_library():
     """The mirrors against the host functions the library exports: saicv_dwconv_wgrad_blocks, and the block count of
     capi_van.cu slab (saicv_bn_generic_partial_rows), which ls_residual_bwd shares."""
-    lib = _lib().load()
+    lib = _lib.load()
     for npix in [1, 255, 256, 257, 33535, 33536, 33537, 200704, 100352]:
         assert lib.saicv_dwconv_wgrad_blocks(npix) == _wgrad_blocks(npix), npix
     for rows, c, _ in LS:
-        assert lib.saicv_bn_generic_partial_rows(rows, c) == _van_slab(rows, c)[2], (rows, c)
+        assert lib.saicv_bn_generic_partial_rows(rows, c) == van_slab(rows, c)[2], (rows, c)
 
 
 # ------------------------------------------------------------------ depthwise references
@@ -257,9 +215,9 @@ def _dw_wgrad_ref(dy, x, k, dil):
 def test_dwconv_reference_matches_torch():
     """The tap-by-tap references above against torch's float64 conv2d, its input gradient and its weight gradient."""
     for n, h, w, c, k, dil in [(2, 5, 9, 8, 7, 3), (1, 6, 4, 16, 5, 1), (2, 3, 2, 8, 3, 1)]:
-        x = _randn(n, c, h, w, seed=1).double().requires_grad_(True)
-        wt = _randn(c, 1, k, k, seed=2).double().requires_grad_(True)
-        dy = _randn(n, c, h, w, seed=3).double()
+        x = randn(n, c, h, w, seed=1).double().requires_grad_(True)
+        wt = randn(c, 1, k, k, seed=2).double().requires_grad_(True)
+        dy = randn(n, c, h, w, seed=3).double()
         y = F.conv2d(x, wt, None, 1, dil * (k - 1) // 2, dil, c)
         y.backward(dy)
         nhwc = lambda t: t.detach().permute(0, 2, 3, 1).contiguous()
@@ -273,14 +231,14 @@ def test_dwconv_reference_matches_torch():
 def _dwconv(x, w, bias, k, dil, relu, flip):
     n, h, wd, c = x.shape
     y = torch.full_like(x, NAN)
-    _call('saicv_dwconv_fwd', x, w, bias, y, n, h, wd, c, k, dil, int(relu), int(flip))
+    call('saicv_dwconv_fwd', x, w, bias, y, n, h, wd, c, k, dil, int(relu), int(flip))
     return y
 
 
 def _dw_case(n, h, w, c, k, seed):
-    x = _randn(n, h, w, c, seed=seed).to(BF16)
-    wt = _randn(c, 1, k, k, seed=seed + 1) / k
-    bias = _randn(c, seed=seed + 2) * 0.5
+    x = randn(n, h, w, c, seed=seed).to(BF16)
+    wt = randn(c, 1, k, k, seed=seed + 1) / k
+    bias = randn(c, seed=seed + 2) * 0.5
     return x, wt, bias
 
 
@@ -299,21 +257,21 @@ def test_dwconv_fwd_conforms(n, h, w, c, k, dil):
         for relu in (False, True):
             y = _dwconv(x, wt, bias if use_bias else None, k, dil, relu, False)
             tag = f'{what}{" bias" if use_bias else ""}{" relu" if relu else ""}'
-            _check('dwconv fwd', tag, y, vb.clamp_min(0) if relu else vb, ab)
-            _same(f'{tag} on a second launch', y, _dwconv(x, wt, bias if use_bias else None, k, dil, relu, False))
+            check('dwconv fwd', tag, y, vb.clamp_min(0) if relu else vb, ab)
+            same(f'{tag} on a second launch', y, _dwconv(x, wt, bias if use_bias else None, k, dil, relu, False))
         del vb, ab
     del v, a
-    dy = _randn(n, h, w, c, seed=seed + 3).to(BF16)
+    dy = randn(n, h, w, c, seed=seed + 3).to(BF16)
     v, a = _dw_ref(dy, wt, k, dil, flip=True)
     dx = _dwconv(dy, wt, None, k, dil, False, True)
-    _check('dwconv fwd flip (dgrad)', f'{what} flip', dx, v, g * a)
-    _same(f'{what} flip on a second launch', dx, _dwconv(dy, wt, None, k, dil, False, True))
+    check('dwconv fwd flip (dgrad)', f'{what} flip', dx, v, g * a)
+    same(f'{what} flip on a second launch', dx, _dwconv(dy, wt, None, k, dil, False, True))
 
 
 def _dgrad_masked(dy, w, mask):
     n, h, wd, c = dy.shape
     dx = torch.full_like(dy, NAN)
-    _call('saicv_dwconv_dgrad_masked', dy, w, mask, dx, n, h, wd, c, 7)
+    call('saicv_dwconv_dgrad_masked', dy, w, mask, dx, n, h, wd, c, 7)
     return dx
 
 
@@ -324,30 +282,30 @@ def test_dwconv_dgrad_masked_conforms(n, h, w, c):
     and a few negative values."""
     seed = 2000 + 7 * n + 131 * h + 17 * w + c
     dy, wt, _ = _dw_case(n, h, w, c, 7, seed)
-    m = _randn(n, h, w, c, seed=seed + 5).clamp_min(0)
+    m = randn(n, h, w, c, seed=seed + 5).clamp_min(0)
     m[:, (h + 1) // 2:] = 0
     m[..., ::3] = 0
     checker = ((torch.arange(h, device='cuda')[:, None] + torch.arange(w, device='cuda')[None, :]) % 2 == 0)
     m = torch.where((m == 0) & checker[None, :, :, None], torch.tensor(-0.0, device='cuda'), m)
-    m[..., 1::7] = -_rand(n, h, w, len(range(1, c, 7)), seed=seed + 6)
+    m[..., 1::7] = -rand(n, h, w, len(range(1, c, 7)), seed=seed + 6)
     mask = m.to(BF16)
     live = mask.double() > 0
     assert live.any() and (~live).any() and bool((mask.view(torch.int16) == -32768).any())   # -0.0 present
     what = f'dwconv dgrad masked {n}x{h}x{w}x{c}'
     v, a = _dw_ref(dy, wt, 7, 1, flip=True)
     dx = _dgrad_masked(dy, wt, mask)
-    _check('dwconv dgrad masked', what, dx[live], v[live], _gamma(49) * a[live])
+    check('dwconv dgrad masked', what, dx[live], v[live], _gamma(49) * a[live])
     _zero_bits(what, dx, ~live)
-    _same(f'{what} on a second launch', dx, _dgrad_masked(dy, wt, mask))
+    same(f'{what} on a second launch', dx, _dgrad_masked(dy, wt, mask))
 
 
 def _wgrad(dy, x, k, dil, dw, accumulate):
     n, h, wd, c = x.shape
     npix = n * h * wd
-    nblk = _lib().load().saicv_dwconv_wgrad_blocks(npix)
+    nblk = _lib.load().saicv_dwconv_wgrad_blocks(npix)
     assert nblk == _wgrad_blocks(npix)
-    partial = _nan(nblk * k * k * c)
-    _call('saicv_dwconv_wgrad', dy, x, partial, dw, n, h, wd, c, k, dil, int(accumulate))
+    partial = nan(nblk * k * k * c)
+    call('saicv_dwconv_wgrad', dy, x, partial, dw, n, h, wd, c, k, dil, int(accumulate))
     return dw
 
 
@@ -356,33 +314,33 @@ def test_dwconv_wgrad_conforms(n, h, w, c, k, dil):
     """saicv_dwconv_wgrad into a NaN-filled dw and accumulated onto a previous dw, with a NaN-filled partial buffer of
     nblk k^2 C floats."""
     seed = 3000 + 7 * n + 131 * h + 17 * w + c + 1000 * k + dil
-    x = _randn(n, h, w, c, seed=seed).to(BF16)
-    dy = _randn(n, h, w, c, seed=seed + 1).to(BF16)
+    x = randn(n, h, w, c, seed=seed).to(BF16)
+    dy = randn(n, h, w, c, seed=seed + 1).to(BF16)
     npix = n * h * w
     nblk, ppb = _wgrad_blocks(npix), _ppb(npix)
     d = -(-ppb // 32) + 32 + nblk
     what = f'dwconv wgrad {n}x{h}x{w}x{c} k{k} d{dil} (nblk {nblk}, ppb {ppb})'
     v, a = _dw_wgrad_ref(dy, x, k, dil)
-    dw = _wgrad(dy, x, k, dil, _nan(c, 1, k, k), False)
-    _check('dwconv wgrad', what, dw, v, (d + 1) * U * a)
-    _same(f'{what} on a second launch', dw, _wgrad(dy, x, k, dil, _nan(c, 1, k, k), False))
-    prev = _randn(c, 1, k, k, seed=seed + 2) * a.mean().float().sqrt()
+    dw = _wgrad(dy, x, k, dil, nan(c, 1, k, k), False)
+    check('dwconv wgrad', what, dw, v, (d + 1) * U * a)
+    same(f'{what} on a second launch', dw, _wgrad(dy, x, k, dil, nan(c, 1, k, k), False))
+    prev = randn(c, 1, k, k, seed=seed + 2) * a.mean().float().sqrt()
     dw2 = _wgrad(dy, x, k, dil, prev.clone(), True)
     v2 = v + prev.double()
-    _check('dwconv wgrad', f'{what} accumulate', dw2, v2, (d + 2) * U * (a + prev.double().abs()))
-    _same(f'{what} accumulate on a second launch', dw2, _wgrad(dy, x, k, dil, prev.clone(), True))
+    check('dwconv wgrad', f'{what} accumulate', dw2, v2, (d + 2) * U * (a + prev.double().abs()))
+    same(f'{what} accumulate on a second launch', dw2, _wgrad(dy, x, k, dil, prev.clone(), True))
 
 
 # ------------------------------------------------------------------ gating
 def _mul(a, b):
     out = torch.full_like(a, NAN)
-    _call('saicv_mul_bf16', a, b, out, a.numel())
+    call('saicv_mul_bf16', a, b, out, a.numel())
     return out
 
 
 def _gate_bwd(dg, c1, dlk, p1):
     out = torch.full_like(dg, NAN)
-    _call('saicv_gate_bwd', dg, c1, dlk, p1, out, dg.numel())
+    call('saicv_gate_bwd', dg, c1, dlk, p1, out, dg.numel())
     return out
 
 
@@ -391,39 +349,39 @@ def test_mul_and_gate_bwd_conform(rows, c):
     """saicv_mul_bf16 bit for bit against rne_bf16(a b); saicv_gate_bwd against dg c1 + dlk where p1 > 0 and +0 where
     p1 <= 0 (p1 a ReLU output with -0.0 on every fifth zero)."""
     seed = 4000 + rows + c
-    a, b, dlk = (_randn(rows, c, seed=seed + i).to(BF16) for i in range(3))
-    p = _randn(rows, c, seed=seed + 3).clamp_min(0)
+    a, b, dlk = (randn(rows, c, seed=seed + i).to(BF16) for i in range(3))
+    p = randn(rows, c, seed=seed + 3).clamp_min(0)
     p.view(-1)[::5] = torch.where(p.view(-1)[::5] == 0, torch.tensor(-0.0, device='cuda'), p.view(-1)[::5])
     p1 = p.to(BF16)
     del p
     what = f'gating {rows}x{c}'
     out = _mul(a, b)
-    _exact('mul_bf16', f'{what} mul_bf16', out, _rne_bf16(a.double() * b.double()).to(BF16))
-    _same(f'{what} mul_bf16 on a second launch', out, _mul(a, b))
+    exact('mul_bf16', f'{what} mul_bf16', out, rne_bf16(a.double() * b.double()).to(BF16))
+    same(f'{what} mul_bf16 on a second launch', out, _mul(a, b))
     del out
     live = p1.double() > 0
     out = _gate_bwd(a, b, dlk, p1)
     v = a.double()[live] * b.double()[live] + dlk.double()[live]
-    _check('gate_bwd', f'{what} gate_bwd', out[live], v, U * v.abs())
+    check('gate_bwd', f'{what} gate_bwd', out[live], v, U * v.abs())
     del v
     _zero_bits(f'{what} gate_bwd', out, ~live)
-    _same(f'{what} gate_bwd on a second launch', out, _gate_bwd(a, b, dlk, p1))
+    same(f'{what} gate_bwd on a second launch', out, _gate_bwd(a, b, dlk, p1))
 
 
 # ------------------------------------------------------------------ layer-scale residual
 def _ls_fwd(x, br, sc, ls, rs, rps):
     rows, c = br.shape
-    out = _nan(rows, c)
-    _call('saicv_ls_residual_fwd', x, int(x.dtype == torch.float32), br, sc, ls, rs, rps, out, rows, c)
+    out = nan(rows, c)
+    call('saicv_ls_residual_fwd', x, int(x.dtype == torch.float32), br, sc, ls, rs, rps, out, rows, c)
     return out
 
 
 def _ls_bwd(dxn, br, sc, ls, rs, rps, dls, accumulate):
     rows, c = br.shape
     dy = torch.full((rows, c), NAN, device='cuda', dtype=BF16)
-    ws = _ops().partial_ws(dxn.device, 2 * c)
+    ws = ops.partial_ws(dxn.device, 2 * c)
     ws.fill_(NAN)
-    _call('saicv_ls_residual_bwd', dxn, br, sc, ls, rs, rps, dy, ws, dls, rows, c, int(accumulate))
+    call('saicv_ls_residual_bwd', dxn, br, sc, ls, rs, rps, dy, ws, dls, rows, c, int(accumulate))
     return dy
 
 
@@ -435,16 +393,16 @@ def test_ls_residual_conforms(rows, c, rps, shortcut):
     i = LS.index((rows, c, rps)) * 2 + int(shortcut)
     seed = 5000 + 10 * i
     x_f32 = i % 2 == 0
-    x = _randn(rows, c, seed=seed) * 2
+    x = randn(rows, c, seed=seed) * 2
     x = x if x_f32 else x.to(BF16)
-    br = _randn(rows, c, seed=seed + 1).to(BF16)
-    sc = _randn(rows, c, seed=seed + 2).to(BF16) if shortcut else None
-    ls = (_rand(c, seed=seed + 3) * 2 - 1) * 0.5
+    br = randn(rows, c, seed=seed + 1).to(BF16)
+    sc = randn(rows, c, seed=seed + 2).to(BF16) if shortcut else None
+    ls = (rand(c, seed=seed + 3) * 2 - 1) * 0.5
     nsc = -(-rows // rps)
-    keep = _rand(nsc, seed=seed + 4) > 0.3
+    keep = rand(nsc, seed=seed + 4) > 0.3
     keep[0] = True
     rs = None if i % 3 == 2 else torch.where(keep, torch.tensor(1 / 0.9, device='cuda'), torch.tensor(0.0, device='cuda'))
-    dxn = _randn(rows, c, seed=seed + 5)
+    dxn = randn(rows, c, seed=seed + 5)
     what = f'ls_residual rows {rows} c {c} x {"f32" if x_f32 else "bf16"}{" shortcut" if shortcut else ""}' \
            f'{"" if rs is None else f" drop-path/{rps}"}'
     s = rs.double().repeat_interleave(rps)[:rows, None] if rs is not None else 1.0
@@ -454,32 +412,32 @@ def test_ls_residual_conforms(rows, c, rps, shortcut):
     P = s * ls.double() * b
     v = x.double() + P
     out = _ls_fwd(x, br, sc, ls, rs, rps)
-    _check('ls_residual fwd', what, out, v, _rnd(v, _gamma(k) * P.abs()))
-    _same(f'{what} fwd on a second launch', out, _ls_fwd(x, br, sc, ls, rs, rps))
+    check('ls_residual fwd', what, out, v, rnd(v, _gamma(k) * P.abs()))
+    same(f'{what} fwd on a second launch', out, _ls_fwd(x, br, sc, ls, rs, rps))
     del P, v, out
     # backward
     g = dxn.double()
     vd = s * ls.double() * g
-    dls = _nan(c)
+    dls = nan(c)
     dy = _ls_bwd(dxn, br, sc, ls, rs, rps, dls, False)
-    _check('ls_residual bwd dy', f'{what} dy', dy, vd, _gamma(2) * vd.abs())
+    check('ls_residual bwd dy', f'{what} dy', dy, vd, _gamma(2) * vd.abs())
     del vd
     t = s * g * b
     st, sa = t.sum(0), t.abs().sum(0)
     del t
-    ty, rpb, nblk = _van_slab(rows, c)
+    ty, rpb, nblk = van_slab(rows, c)
     d = -(-rpb // ty) + ty + nblk
-    _check('ls_residual bwd dls', f'{what} dls (slab {nblk} x {rpb} rows)', dls, st, (d + 1 + k) * U * sa)
-    prev = _randn(c, seed=seed + 6) * sa.float().mean()
+    check('ls_residual bwd dls', f'{what} dls (slab {nblk} x {rpb} rows)', dls, st, (d + 1 + k) * U * sa)
+    prev = randn(c, seed=seed + 6) * sa.float().mean()
     dls2 = prev.clone()
     dy2 = _ls_bwd(dxn, br, sc, ls, rs, rps, dls2, True)
-    _same(f'{what} dy (accumulate call)', dy2, dy)
+    same(f'{what} dy (accumulate call)', dy2, dy)
     v2 = prev.double() + st
-    _check('ls_residual bwd dls', f'{what} dls accumulate', dls2, v2,
-           (d + 2 + k) * U * sa + (d + 2) * U * prev.double().abs())
-    dls3 = _nan(c)
-    _same(f'{what} dy on a second launch', _ls_bwd(dxn, br, sc, ls, rs, rps, dls3, False), dy)
-    _same(f'{what} dls on a second launch', dls3, dls)
+    check('ls_residual bwd dls', f'{what} dls accumulate', dls2, v2,
+          (d + 2 + k) * U * sa + (d + 2) * U * prev.double().abs())
+    dls3 = nan(c)
+    same(f'{what} dy on a second launch', _ls_bwd(dxn, br, sc, ls, rs, rps, dls3, False), dy)
+    same(f'{what} dls on a second launch', dls3, dls)
 
 
 # ------------------------------------------------------------------ SwiGLU
@@ -525,13 +483,13 @@ def _overflow(a64):
 
 def _swiglu_fwd(a, b):
     out = torch.full_like(a, NAN)
-    _call('saicv_swiglu_fwd', a, b, out, a.numel())
+    call('saicv_swiglu_fwd', a, b, out, a.numel())
     return out
 
 
 def _swiglu_bwd(dh, a, b):
     da, db = torch.full_like(a, NAN), torch.full_like(a, NAN)
-    _call('saicv_swiglu_bwd', dh, a, b, da, db, a.numel())
+    call('saicv_swiglu_bwd', dh, a, b, da, db, a.numel())
     return da, db
 
 
@@ -541,45 +499,45 @@ def _check_swiglu(what, a, h, da, ds):
     inf, fin = _overflow(a64)
     silu, a_silu, g, a_g = _swiglu_ref(a64[fin], ds[fin])
     if h is not None:
-        _check('swiglu silu', f'{what} silu', h[fin], silu, a_silu)
+        check('swiglu silu', f'{what} silu', h[fin], silu, a_silu)
         assert bool((h[inf].double() == 0).all()), f'{what}: silu is not 0 where expf(-a) overflows'
-    _check('swiglu da', f'{what} da', da[fin], g, a_g)
+    check('swiglu da', f'{what} da', da[fin], g, a_g)
     assert bool((da[inf].double() == 0).all()), f'{what}: da is not 0 where expf(-a) overflows'
 
 
 def test_swiglu_on_every_bf16_input():
     """Every finite bf16 a with b = 1 and dh = 1: h is the stored bf16(silu(a)), db equals it, and da = silu'(a)."""
-    a = _every_bf16(256).view(-1)
+    a = every_bf16(256).view(-1)
     one = torch.ones_like(a)
     h = _swiglu_fwd(a, one)
     da, db = _swiglu_bwd(one, a, one)
     what = 'swiglu on every bf16 a'
     _check_swiglu(what, a, h, da, torch.ones_like(a, dtype=torch.float64))
-    _exact('swiglu db', f'{what} db (dh = 1)', db, h)
-    _same(f'{what} h on a second launch', h, _swiglu_fwd(a, one))
+    exact('swiglu db', f'{what} db (dh = 1)', db, h)
+    same(f'{what} h on a second launch', h, _swiglu_fwd(a, one))
     da2, db2 = _swiglu_bwd(one, a, one)
-    _same(f'{what} da on a second launch', da2, da)
-    _same(f'{what} db on a second launch', db2, db)
+    same(f'{what} da on a second launch', da2, da)
+    same(f'{what} db on a second launch', db2, db)
 
 
 @pytest.mark.parametrize('n', SWIGLU_N)
 def test_swiglu_random_b_dh_conforms(n):
     """Random a (4 randn), b and dh: h = rne(silu_b b) and db = rne(dh silu_b) bit for bit given the stored bf16
     silu_b = swiglu_fwd(a, 1), and da against ds silu'(a) with ds = rne_bf16(dh b)."""
-    a = (_randn(n, seed=6000 + n) * 4).to(BF16)
-    b = _randn(n, seed=6001 + n).to(BF16)
-    dh = _randn(n, seed=6002 + n).to(BF16)
+    a = (randn(n, seed=6000 + n) * 4).to(BF16)
+    b = randn(n, seed=6001 + n).to(BF16)
+    dh = randn(n, seed=6002 + n).to(BF16)
     what = f'swiglu n {n}'
     s = _swiglu_fwd(a, torch.ones_like(a)).double()
     h = _swiglu_fwd(a, b)
-    _exact('swiglu h', f'{what} h', h, _rne_bf16(s * b.double()).to(BF16))
+    exact('swiglu h', f'{what} h', h, rne_bf16(s * b.double()).to(BF16))
     da, db = _swiglu_bwd(dh, a, b)
-    _exact('swiglu db', f'{what} db', db, _rne_bf16(dh.double() * s).to(BF16))
-    _check_swiglu(what, a, None, da, _rne_bf16(dh.double() * b.double()))
-    _same(f'{what} h on a second launch', h, _swiglu_fwd(a, b))
+    exact('swiglu db', f'{what} db', db, rne_bf16(dh.double() * s).to(BF16))
+    _check_swiglu(what, a, None, da, rne_bf16(dh.double() * b.double()))
+    same(f'{what} h on a second launch', h, _swiglu_fwd(a, b))
     da2, db2 = _swiglu_bwd(dh, a, b)
-    _same(f'{what} da on a second launch', da2, da)
-    _same(f'{what} db on a second launch', db2, db)
+    same(f'{what} da on a second launch', da2, da)
+    same(f'{what} db on a second launch', db2, db)
 
 
 # ------------------------------------------------------------------ NHWC im2col / col2im
@@ -587,13 +545,13 @@ def _im2col(x, k, st, pad):
     n, h, w, c = x.shape
     P, Q = _out_size(h, k, st, pad), _out_size(w, k, st, pad)
     cols = torch.full((n * P * Q, k * k * c), NAN, device='cuda', dtype=BF16)
-    _call('saicv_im2col_nhwc', x, cols, n, h, w, c, k, st, pad)
+    call('saicv_im2col_nhwc', x, cols, n, h, w, c, k, st, pad)
     return cols
 
 
 def _col2im(dcols, n, h, w, c, k, st, pad):
     dx = torch.full((n, h, w, c), NAN, device='cuda', dtype=BF16)
-    _call('saicv_col2im_nhwc', dcols, dx, n, h, w, c, k, st, pad)
+    call('saicv_col2im_nhwc', dcols, dx, n, h, w, c, k, st, pad)
     return dx
 
 
@@ -603,15 +561,15 @@ def test_im2col_col2im_nhwc_conform(n, h, w, c, k, st, pad):
     saicv_col2im_nhwc against F.fold in float64."""
     seed = 7000 + n + h + 3 * w + c + k
     P, Q = _out_size(h, k, st, pad), _out_size(w, k, st, pad)
-    x = _randn(n, h, w, c, seed=seed).to(BF16)
+    x = randn(n, h, w, c, seed=seed).to(BF16)
     what = f'im2col {n}x{h}x{w}x{c} k{k} s{st} p{pad}'
     ref = F.unfold(x.double().permute(0, 3, 1, 2), k, padding=pad, stride=st)          # [n, c k^2, P Q]
     ref = ref.view(n, c, k * k, P * Q).permute(0, 3, 2, 1).reshape(n * P * Q, k * k * c)
     cols = _im2col(x, k, st, pad)
-    _exact('im2col_nhwc', what, cols, ref.to(BF16))
-    _same(f'{what} on a second launch', cols, _im2col(x, k, st, pad))
+    exact('im2col_nhwc', what, cols, ref.to(BF16))
+    same(f'{what} on a second launch', cols, _im2col(x, k, st, pad))
     del ref, cols
-    dcols = _randn(n * P * Q, k * k * c, seed=seed + 1).to(BF16)
+    dcols = randn(n * P * Q, k * k * c, seed=seed + 1).to(BF16)
 
     def fold(t):
         t = t.view(n, P * Q, k * k, c).permute(0, 3, 2, 1).reshape(n, c * k * k, P * Q)
@@ -620,5 +578,5 @@ def test_im2col_col2im_nhwc_conform(n, h, w, c, k, st, pad):
     v, a = fold(dcols.double()), fold(dcols.double().abs())
     dx = _col2im(dcols, n, h, w, c, k, st, pad)
     what = f'col2im {n}x{h}x{w}x{c} k{k} s{st} p{pad}'
-    _check('col2im_nhwc', what, dx, v, _gamma(math.ceil(k / st) ** 2) * a)
-    _same(f'{what} on a second launch', dx, _col2im(dcols, n, h, w, c, k, st, pad))
+    check('col2im_nhwc', what, dx, v, _gamma(math.ceil(k / st) ** 2) * a)
+    same(f'{what} on a second launch', dx, _col2im(dcols, n, h, w, c, k, st, pad))

@@ -29,133 +29,46 @@ Allowances are derived from the operation, never fitted to measured errors (u = 
     |silu'| <= 1.1 and |silu''| <= 0.5 plus SILU_ABS for the fast-math __expf / __fdividef, which is checked on every
     finite bf16 input by test_silu_fast_math_on_every_bf16_input.  A recomputed ReLU mask whose pre-activation lies
     within its rounding allowance of 0 may go either way, so that element's gradient allowance is |g|.
-  * Outputs: a bf16 output must lie in [rne(v - B'), rne(v + B')] (a correctly rounded bf16 of some value within the
-    allowance of the exact v), an fp32 output within B' of v.  Every element must conform; no fraction may miss.
   * Running statistics follow torch's documented update: r = (1 - m) r + m x with the unbiased variance
     var * rows / (rows - 1).
   * Max-pool: the forward value and argmax are bit-exact against a float64 reference that applies torch's rule (the
     first maximum in (r, s) scan order wins; -inf padding never wins, a zero-padded tap carries code 255).  The
     backward adds at most ceil(k / stride)^2 bf16 gradients, so it gets that many roundings.
-Each check prints the largest fraction of its allowance an element used; at the end of the module the largest share
-per family is printed (run with -s).
 
 Invariants (raw bits): two consecutive launches of every kernel give identical outputs, and bn_finalize with
 partial_rows = 0 equals the call given the partial-row count of the Python mirror of slab_geom (a disagreement
 between partial_rows() and the stats launch would drop or double a block).  Partial workspaces and outputs are
 filled with NaN before each launch, so an unwritten element or a folded stale row fails.
 """
-import importlib.util
 import math
-import os
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-_spec = importlib.util.spec_from_file_location('gemm_conformance', os.path.join(HERE, 'test_gemm_conformance_gpu.py'))
-_gemm = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(_gemm)
-_quantum_bf16, _rne_bf16 = _gemm._quantum_bf16, _gemm._rne_bf16
+from conformance import (NAN, PARTIAL_ROWS, U, check, every_bf16, gen, nan, next_pow2, quantum_bf16, rand, randn, rnd,
+                         rne_bf16, same, van_slab)
+from conformance import report  # noqa: F401  (autouse: this module's allowance report)
+
+from simpleaicv_pytorch_training_examples_b200 import ops
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -24          # one fp32 rounding, relative
 RSQRT = 2.0 ** -22      # rsqrtf: 2 ulp, relative
 SILU_ABS = 4e-6         # |fast-math silu - silu| and |fast-math silu' - silu'| beyond their final roundings
 LEAKY = 0.1
-PARTIAL_ROWS = 264      # SAICV_BN_PARTIAL_ROWS
-NAN = float('nan')
-USED = {}
-
-
-def _ops():
-    from simpleaicv_pytorch_training_examples_b200 import ops
-    return ops
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _report():
-    yield
-    if USED:
-        print('\nlargest share of the allowance used, by family:')
-        for k in sorted(USED):
-            print(f'  {k:28s} {USED[k]:.3g}')
-
-
-def _gen(seed):
-    return torch.Generator(device='cuda').manual_seed(seed)
-
-
-def _randn(*shape, seed=0):
-    return torch.randn(*shape, device='cuda', generator=_gen(seed))
-
-
-def _rand(*shape, seed=0):
-    return torch.rand(*shape, device='cuda', generator=_gen(seed))
-
-
-def _nan(*shape, dtype=torch.float32):
-    return torch.full(shape, NAN, device='cuda', dtype=dtype)
-
-
-def _rnd(v, a):
-    """Allowance after one fp32 rounding of a value within a of v."""
-    return a + U * (v.abs() + a)
-
-
-def _check(family, what, out, v, allow):
-    """out: kernel output; v: exact float64 value; allow: its allowance B' (broadcastable to v)."""
-    v = v.expand(out.shape) if v.shape != out.shape else v
-    allow = torch.as_tensor(allow, dtype=torch.float64, device=v.device).expand(v.shape)
-    o = out.double()
-    if out.dtype == torch.bfloat16:
-        lo, hi = _rne_bf16(v - allow), _rne_bf16(v + allow)
-        bad = (o < lo) | (o > hi)
-        dist = ((o - v).abs() - _quantum_bf16(o) / 2).clamp_min(0)
-    else:
-        bad = (o - v).abs() > allow
-        dist = (o - v).abs()
-    bad |= ~torch.isfinite(o)
-    used = (dist / allow.clamp_min(1e-300)).max().item() if o.numel() else 0.0
-    if math.isfinite(used):
-        USED[family] = max(USED.get(family, 0.0), used)
-    print(f'{what}: allowance used {used:.3g}')
-    n_bad = int(bad.sum())
-    if n_bad:
-        i = int(bad.flatten().nonzero()[0])
-        raise AssertionError(
-            f'{what}: {n_bad}/{out.numel()} elements outside the allowance; first at flat index {i}: '
-            f'out {o.flatten()[i].item():.9g}, exact {v.flatten()[i].item():.9g}, allowance {allow.flatten()[i].item():.3g}')
-
-
-def _same(what, a, b):
-    """Raw-bit equality (floats as their bit patterns, so signed zeros and NaN payloads count too)."""
-    assert a.shape == b.shape and a.dtype == b.dtype, f'{what}: {tuple(a.shape)} {a.dtype} vs {tuple(b.shape)} {b.dtype}'
-    bits = {torch.bfloat16: torch.int16, torch.float32: torch.int32}
-    if a.dtype in bits:
-        a, b = a.view(bits[a.dtype]), b.view(bits[b.dtype])
-    n_bad = int((a != b).sum())
-    assert n_bad == 0, f'{what}: {n_bad}/{a.numel()} elements differ'
 
 
 def _same_all(what, a, b):
     for k in a:
         if a[k] is not None:
-            _same(f'{what}: {k} on a second launch', a[k], b[k])
+            same(f'{what}: {k} on a second launch', a[k], b[k])
 
 
 # ------------------------------------------------------------------ launch geometry mirrors
-def _next_pow2(v):
-    p = 1
-    while p < v:
-        p <<= 1
-    return p
-
-
 def _slab(rows, c, unroll, max_blocks=PARTIAL_ROWS):
     """capi_elementwise.cu slab_geom: (ty_count, rows_per_block, blocks)."""
-    tx = min(_next_pow2(c // 8), 256)
+    tx = min(next_pow2(c // 8), 256)
     ty = 256 // tx
     b = max(1, min(-(-rows // (ty * unroll)), max_blocks))
     q = ty * unroll
@@ -167,15 +80,6 @@ def _slab_depth(rows, c, unroll, accumulate=False):
     """Depth of a slab column reduction (colreduce_kernel / colreduce2_kernel) folded by fold_partials / bn_finalize."""
     ty, rpb, nblk = _slab(rows, c, unroll)
     return -(-rpb // ty) + int(math.log2(ty)) + -(-nblk // 32) + 32 + int(accumulate)
-
-
-def _van_slab(rows, c):
-    """capi_van.cu slab: (ty_count, rows_per_block, blocks)."""
-    tx = min(_next_pow2(c // 8), 256)
-    ty = 256 // tx
-    b = max(1, min(-(-rows // (ty * 8)), PARTIAL_ROWS))
-    rpb = -(-(-(-rows // b)) // ty) * ty
-    return ty, rpb, -(-rows // rpb)
 
 
 def _ln_bwd_depth(rows, accumulate=False):
@@ -263,15 +167,15 @@ def _check_finalize(fam, what, x, gamma, beta, eps, mom, rm0, rv0, o, depth):
     mean, var, a_m, a_v = _stats_allow(x.double(), depth)
     r, a_r = _rstd_interval(var, a_v, eps)
     g, b = gamma.double(), beta.double()
-    _check(fam, f'{what} mean', o['saved'][0], mean, a_m)
-    _check(fam, f'{what} rstd', o['saved'][1], r, a_r)
+    check(fam, f'{what} mean', o['saved'][0], mean, a_m)
+    check(fam, f'{what} rstd', o['saved'][1], r, a_r)
     sc = g * r
     a_sc = g.abs() * a_r + U * g.abs() * (r + a_r)
     sh = b - mean * sc
     # mean * scale and beta - that: two roundings of values within (a_m, a_sc) of the exact factors
     a_sh = mean.abs() * a_sc + (sc.abs() + a_sc) * a_m + 2 * U * ((mean.abs() + a_m) * (sc.abs() + a_sc) + b.abs())
-    _check(fam, f'{what} scale', o['ss'][0], sc, a_sc)
-    _check(fam, f'{what} shift', o['ss'][1], sh, a_sh)
+    check(fam, f'{what} scale', o['ss'][0], sc, a_sc)
+    check(fam, f'{what} shift', o['ss'][1], sh, a_sh)
     if rm0 is not None:
         # (1 - m) r + m x in fp32: 1 - m, two products and the sum round (4u), and 0.1f differs from 0.1 by 1.5e-8
         # relative (under u); the unbiased factor rows / (rows - 1) and its product add two more
@@ -280,18 +184,17 @@ def _check_finalize(fam, what, x, gamma, beta, eps, mom, rm0, rv0, o, depth):
         unb = n / (n - 1) if n > 1 else 1.0
         rv = (1 - mom) * rv0.double() + mom * unb * var
         a_rv = mom * unb * a_v + 7 * U * ((1 - mom) * rv0.double().abs() + mom * unb * (var + a_v))
-        _check(fam, f'{what} running_mean', o['rm'], rm, a_rm)
-        _check(fam, f'{what} running_var', o['rv'], rv, a_rv)
+        check(fam, f'{what} running_mean', o['rm'], rm, a_rm)
+        check(fam, f'{what} running_var', o['rv'], rv, a_rv)
     return r, a_r
 
 
 def _bn_forward(y, gamma, beta, eps, mom, rm0, rv0, partial_rows=0):
-    ops = _ops()
     c = y.shape[1]
     ws = ops.partial_ws(y.device, 2 * c)
     ws.fill_(NAN)
     ops.bn_stats(y, ws)
-    o = {'ss': _nan(2, c), 'saved': _nan(2, c),
+    o = {'ss': nan(2, c), 'saved': nan(2, c),
          'rm': rm0.clone() if rm0 is not None else None, 'rv': rv0.clone() if rv0 is not None else None}
     ops.bn_finalize(ws, gamma, beta, o['rm'], o['rv'], o['ss'], o['saved'], y.shape[0], eps, mom, partial_rows=partial_rows)
     return o
@@ -314,11 +217,11 @@ def _apply_ref(y, ss, act, res, rss):
         a = _act_allow(v, a, act & 7)
         if res is not None:
             f = f + r
-            a = _rnd(f, a + a_r)
+            a = rnd(f, a + a_r)
         return f, a
     if res is not None:
         v = v + r
-        a = _rnd(v, a + a_r)
+        a = rnd(v, a + a_r)
     return _act64(v, act), _act_allow(v, a, act)
 
 
@@ -336,32 +239,31 @@ def _check_bwd(fam, what, dout, y, saved, gamma, f, a_f, o, depth, prev=None):
     s0, s1 = ge.sum(0), t1.sum(0)
     a0 = (depth + 1) * U * ge.abs().sum(0) + a_ge.sum(0)
     a1 = (depth + 1) * U * t1.abs().sum(0) + (a_ge * xh.abs() + 3 * U * t1.abs()).sum(0)
-    _check(fam, f'{what} sum g', o['sums'][0], s0, a0)
-    _check(fam, f'{what} sum g*xhat', o['sums'][1], s1, a1)
+    check(fam, f'{what} sum g', o['sums'][0], s0, a0)
+    check(fam, f'{what} sum g*xhat', o['sums'][1], s1, a1)
     if prev is None:
-        _check(fam, f'{what} dbeta', o['dbeta'], s0, a0)
-        _check(fam, f'{what} dgamma', o['dgamma'], s1, a1)
+        check(fam, f'{what} dbeta', o['dbeta'], s0, a0)
+        check(fam, f'{what} dgamma', o['dgamma'], s1, a1)
     else:
         v0, v1 = prev[1].double() + s0, prev[0].double() + s1
-        _check(fam, f'{what} dbeta (accumulate)', o['dbeta'], v0, _rnd(v0, a0))
-        _check(fam, f'{what} dgamma (accumulate)', o['dgamma'], v1, _rnd(v1, a1))
+        check(fam, f'{what} dbeta (accumulate)', o['dbeta'], v0, rnd(v0, a0))
+        check(fam, f'{what} dgamma (accumulate)', o['dgamma'], v1, rnd(v1, a1))
     del t1
     if o.get('dres') is not None:
-        _check(fam, f'{what} dres', o['dres'], ge, a_ge)
+        check(fam, f'{what} dres', o['dres'], ge, a_ge)
     A = gamma.double() * rstd
     k2, k3 = o['sums'][0].double() / n, o['sums'][1].double() / n
     T1, T2, B = A * k2, A * k3 * rstd * mean, -A * k3 * rstd
     By = B * y64
     v = A * ge + By + (T2 - T1)
     a = A.abs() * a_ge + 10 * U * ((A * ge).abs() + By.abs() + T1.abs() + T2.abs())
-    _check(fam, f'{what} dy', o['dy'], v, a)
+    check(fam, f'{what} dy', o['dy'], v, a)
 
 
 def _bn_backward(dout, y, saved, gamma, ss, act, src, out, bits, want_dres, accumulate=False, prev=None):
-    ops = _ops()
     c = y.shape[1]
-    o = {'sums': _nan(2, c), 'dy': torch.full_like(y, NAN), 'dres': torch.full_like(y, NAN) if want_dres else None,
-         'dgamma': prev[0].clone() if accumulate else _nan(c), 'dbeta': prev[1].clone() if accumulate else _nan(c)}
+    o = {'sums': nan(2, c), 'dy': torch.full_like(y, NAN), 'dres': torch.full_like(y, NAN) if want_dres else None,
+         'dgamma': prev[0].clone() if accumulate else nan(c), 'dbeta': prev[1].clone() if accumulate else nan(c)}
     mo = out if src == 'out' else None
     mb = bits if src == 'bits' else None
     ms = ss if src == 'recompute' else None
@@ -373,22 +275,21 @@ def _bn_backward(dout, y, saved, gamma, ss, act, src, out, bits, want_dres, accu
 
 def _bn_case(rows, c, seed, offset=1.0):
     """y bf16 [rows, c] with per-channel |mean| / std up to `offset`, gamma (either sign), beta, running stats."""
-    std = _rand(c, seed=seed) * 1.5 + 0.5
-    mean = (_rand(c, seed=seed + 1) * 2 - 1) * offset * std
-    y = (_randn(rows, c, seed=seed + 2) * std + mean).to(torch.bfloat16)
-    gamma = _randn(c, seed=seed + 3) * 0.5 + 1.0
-    beta = _randn(c, seed=seed + 4) * 0.5
-    rm0, rv0 = _randn(c, seed=seed + 5) * 0.1, _rand(c, seed=seed + 6) + 0.5
+    std = rand(c, seed=seed) * 1.5 + 0.5
+    mean = (rand(c, seed=seed + 1) * 2 - 1) * offset * std
+    y = (randn(rows, c, seed=seed + 2) * std + mean).to(torch.bfloat16)
+    gamma = randn(c, seed=seed + 3) * 0.5 + 1.0
+    beta = randn(c, seed=seed + 4) * 0.5
+    rm0, rv0 = randn(c, seed=seed + 5) * 0.1, rand(c, seed=seed + 6) + 0.5
     return y, gamma, beta, rm0, rv0
 
 
 def _run_slab_bn(rows, c, act, res_kind, srcs, seed, accumulate=(False,), what=''):
     """Forward (stats, finalize, apply) and backward (reduce, apply) for each mask source; returns the raw outputs."""
-    ops = _ops()
     y, gamma, beta, rm0, rv0 = _bn_case(rows, c, seed)
-    res = _randn(rows, c, seed=seed + 7).to(torch.bfloat16) if res_kind != 'none' else None
-    rss = torch.stack([_rand(c, seed=seed + 8) + 0.5, _randn(c, seed=seed + 9) * 0.5]) if res_kind == 'bn' else None
-    dout = _randn(rows, c, seed=seed + 10).to(torch.bfloat16)
+    res = randn(rows, c, seed=seed + 7).to(torch.bfloat16) if res_kind != 'none' else None
+    rss = torch.stack([rand(c, seed=seed + 8) + 0.5, randn(c, seed=seed + 9) * 0.5]) if res_kind == 'bn' else None
+    dout = randn(rows, c, seed=seed + 10).to(torch.bfloat16)
     fo = _bn_forward(y, gamma, beta, 1e-5, 0.1, rm0, rv0)
     out = torch.full_like(y, NAN)
     bits = ops.mask_bits_like(y) if 'bits' in srcs else None
@@ -396,7 +297,7 @@ def _run_slab_bn(rows, c, act, res_kind, srcs, seed, accumulate=(False,), what='
     outs = {'fwd': fo, 'out': out, 'bits': bits, 'bwd': {}}
     for src in srcs:
         for acc in accumulate:
-            prev = (_randn(c, seed=seed + 11), _randn(c, seed=seed + 12)) if acc else None
+            prev = (randn(c, seed=seed + 11), randn(c, seed=seed + 12)) if acc else None
             outs['bwd'][(src, acc)] = (_bn_backward(dout, y, fo['saved'], gamma, fo['ss'], act & 7, src, out, bits,
                                                     want_dres=res_kind == 'plain' and not act & 8,
                                                     accumulate=acc, prev=prev), prev)
@@ -408,7 +309,7 @@ def _check_slab_bn(fam, what, inputs, outs, rows, c, act):
     fo = outs['fwd']
     _check_finalize(fam + ' stats', what, y, gamma, beta, 1e-5, 0.1, rm0, rv0, fo, _slab_depth(rows, c, 8))
     v, a = _apply_ref(y, fo['ss'], act, res, rss)
-    _check(fam + ' apply', f'{what} out', outs['out'], v, a)
+    check(fam + ' apply', f'{what} out', outs['out'], v, a)
     del v, a
     for (src, acc), (o, prev) in outs['bwd'].items():
         f, a_f = _grad_factor(act & 7, src, y, outs['out'], outs['bits'], fo['ss'])
@@ -426,45 +327,38 @@ def _flatten(outs):
 
 
 # ------------------------------------------------------------------ SiLU fast math, on every bf16 input
-def _every_bf16(width):
-    u = torch.arange(-2 ** 15, 2 ** 15, device='cuda', dtype=torch.int32).to(torch.int16).view(torch.bfloat16)
-    u = u[torch.isfinite(u.float())]
-    return torch.cat([u, u.new_zeros((-u.numel()) % width)]).view(-1, width).contiguous()
-
-
 def test_silu_fast_math_on_every_bf16_input():
     """SiLU forward (bn_apply act 3|8) and its gradient (the recompute mask of bn_bwd_reduce) on every finite bf16
     value, with scale 1 and shift 0 so the activation sees the bf16 value itself.
     Forward: the residual is -rne(silu(y)), so the bf16 output resolves the fp32 silu to about 2^-9 of its error.
     Gradient: one row per launch, so sum g = silu'(y) exactly as the kernel formed it (every other addend is 0)."""
-    ops = _ops()
     c = 256
-    y = _every_bf16(c)
+    y = every_bf16(c)
     rows = y.shape[0]
     ss = torch.stack([torch.ones(c, device='cuda'), torch.zeros(c, device='cuda')])
     f64 = _act64(y.double(), 3)
-    res = _rne_bf16(-f64).to(torch.bfloat16)
+    res = rne_bf16(-f64).to(torch.bfloat16)
     out = torch.full_like(y, NAN)
     ops.bn_apply(y, ss, out, 3 | 8, res=res)
     v, a = _apply_ref(y, ss, 3 | 8, res, None)
     o = out.double()
-    err = (((o - v).abs() - _quantum_bf16(o) / 2).clamp_min(0) - 2 * U * f64.abs()).max().item()
+    err = (((o - v).abs() - quantum_bf16(o) / 2).clamp_min(0) - 2 * U * f64.abs()).max().item()
     print(f'silu: max |fast-math silu - silu| beyond 2u|silu| <= {err:.3g} (SILU_ABS {SILU_ABS:.3g})')
-    _check('silu', 'silu forward on every bf16 input', out, v, a)
+    check('silu', 'silu forward on every bf16 input', out, v, a)
     c = 2048
-    yg = _every_bf16(c)
+    yg = every_bf16(c)
     saved = torch.stack([torch.zeros(c, device='cuda'), torch.ones(c, device='cuda')])
     ss = torch.stack([torch.ones(c, device='cuda'), torch.zeros(c, device='cuda')])
     one = torch.ones(1, c, device='cuda', dtype=torch.bfloat16)
     got = torch.empty(yg.shape, device='cuda')
     for i in range(yg.shape[0]):
-        sums = _nan(2, c)
+        sums = nan(2, c)
         ops.bn_bwd_reduce(one, None, yg[i:i + 1].contiguous(), saved, sums, 3, scale_shift=ss)
         got[i] = sums[0]
     f, a = _silu_grad64(yg.double())
     err = ((got.double() - f).abs() - 4 * U * torch.sigmoid(yg.double()) * (1 + yg.double().abs())).max().item()
     print(f"silu': max |fast-math silu' - silu'| beyond its roundings ~ {err:.3g} (SILU_ABS {SILU_ABS:.3g})")
-    _check('silu', "silu' on every bf16 input", got, f, a)
+    check('silu', "silu' on every bf16 input", got, f, a)
 
 
 # ------------------------------------------------------------------ slab BatchNorm: geometry
@@ -509,7 +403,7 @@ def test_slab_bn_geometry_conforms(c, rows):
         a, b = _flatten(outs), _flatten(again)
         for k in a:
             if a[k] is not None:
-                _same(f'{what} {k} on a second launch', a[k], b[k])
+                same(f'{what} {k} on a second launch', a[k], b[k])
 
 
 def _sources(act, c):
@@ -544,23 +438,22 @@ def test_two_bn_backward_conforms(rows, c, masked):
     their bit equality with two single calls is test_mask_bits_gpu.py's."""
     if masked and c % 32:
         pytest.skip('mask bits need c % 32 == 0')
-    ops = _ops()
     ya, ga, ba, _, _ = _bn_case(rows, c, 500)
     yb, gb, bb, _, _ = _bn_case(rows, c, 510)
     fa = _bn_forward(ya, ga, ba, 1e-5, 0.1, None, None)
     fb = _bn_forward(yb, gb, bb, 1e-5, 0.1, None, None)
     out, bits = torch.full_like(ya, NAN), (ops.mask_bits_like(ya) if masked else None)
     ops.bn_apply(ya, fa['ss'], out, 1, res=yb, res_scale_shift=fb['ss'], mask_bits=bits)
-    dout = _randn(rows, c, seed=520).to(torch.bfloat16)
-    prev = [(_randn(c, seed=530 + k), _randn(c, seed=540 + k)) for k in range(2)]
+    dout = randn(rows, c, seed=520).to(torch.bfloat16)
+    prev = [(randn(c, seed=530 + k), randn(c, seed=540 + k)) for k in range(2)]
 
     def run():
-        sums = _nan(4, c)
+        sums = nan(4, c)
         ws = ops.partial_ws(ya.device, 4 * c)
         ws.fill_(NAN)
         ops.bn_bwd_reduce2(dout, bits, ya, yb, fa['saved'], fb['saved'], sums)
         o = {'sums': sums, 'dya': torch.full_like(ya, NAN), 'dyb': torch.full_like(yb, NAN),
-             'dga': _nan(c), 'dba': _nan(c), 'dgb': prev[1][0].clone(), 'dbb': prev[1][1].clone()}
+             'dga': nan(c), 'dba': nan(c), 'dgb': prev[1][0].clone(), 'dbb': prev[1][1].clone()}
         ops.bn_bwd_apply2(dout, bits, ya, yb, fa['saved'], fb['saved'], ga, gb, sums, o['dya'], o['dyb'], o['dga'],
                           o['dba'], o['dgb'], o['dbb'], accumulate_a=False, accumulate_b=True)
         return o
@@ -594,7 +487,7 @@ def test_slab_bn_offset_statistics(offset):
     ours = ((fo['saved'][1].double() - r).abs() / r).max().item()
     theirs = ((_torch_rstd(y).double() - r).abs() / r).max().item()
     print(f'{what}: max relative rstd error {ours:.3g} (torch fp32 batch_norm: {theirs:.3g})')
-    dout = _randn(rows, c, seed=610).to(torch.bfloat16)
+    dout = randn(rows, c, seed=610).to(torch.bfloat16)
     o = _bn_backward(dout, y, fo['saved'], gamma, None, 0, 'none', None, None, want_dres=False)
     _check_bwd('slab bn offset', what + ' bwd', dout, y, fo['saved'], gamma, 1.0, 0.0, o, _slab_depth(rows, c, 4))
 
@@ -602,18 +495,17 @@ def test_slab_bn_offset_statistics(offset):
 @pytest.mark.parametrize('offset', [0, 64, 512])
 def test_generic_bn_offset_statistics(offset):
     """The generic BatchNorm's statistics of an fp32 stream (VAN) with |mean| / std up to `offset`."""
-    ops = _ops()
     rows, c = 6272, 96
-    std = _rand(c, seed=620) * 1.5 + 0.5
-    mean = (_rand(c, seed=621) * 2 - 1) * offset * std
-    x = _randn(rows, c, seed=622) * std + mean
-    gamma, beta = _randn(c, seed=623) * 0.5 + 1, _randn(c, seed=624) * 0.5
+    std = rand(c, seed=620) * 1.5 + 0.5
+    mean = (rand(c, seed=621) * 2 - 1) * offset * std
+    x = randn(rows, c, seed=622) * std + mean
+    gamma, beta = randn(c, seed=623) * 0.5 + 1, randn(c, seed=624) * 0.5
     ws = ops.partial_ws(x.device, 2 * c)
     ws.fill_(NAN)
     part, nrows = ops.bn_stats_generic(x)
-    fo = {'ss': _nan(2, c), 'saved': _nan(2, c)}
+    fo = {'ss': nan(2, c), 'saved': nan(2, c)}
     ops.bn_finalize(part, gamma, beta, None, None, fo['ss'], fo['saved'], rows, 1e-5, 0.1, partial_rows=nrows)
-    ty, rpb, nblk = _van_slab(rows, c)
+    ty, rpb, nblk = van_slab(rows, c)
     what = f'generic bn offset {offset}'
     r, _ = _check_finalize('generic bn offset', what, x, gamma, beta, 1e-5, 0.1, None, None, fo,
                            -(-rpb // ty) + ty + -(-nblk // 32) + 32)
@@ -628,16 +520,15 @@ def test_generic_bn_offset_statistics(offset):
 @pytest.mark.parametrize('with_dres', [False, True])
 def test_generic_bn_conforms(c, x_f32, g_f32, dx_f32, with_dres):
     """saicv_bn_*_generic over every dtype combination of x / g / dx; C = 3072 makes each thread loop over two vectors."""
-    ops = _ops()
     rows = 6272 if c < 3072 else 1000
     seed = 700 + c
-    x = _randn(rows, c, seed=seed) * 1.5 + 0.3
+    x = randn(rows, c, seed=seed) * 1.5 + 0.3
     x = x if x_f32 else x.to(torch.bfloat16)
-    g = _randn(rows, c, seed=seed + 1)
+    g = randn(rows, c, seed=seed + 1)
     g = g if g_f32 else g.to(torch.bfloat16)
-    dres = _randn(rows, c, seed=seed + 2) if with_dres else None
-    gamma, beta = _randn(c, seed=seed + 3) * 0.5 + 1, _randn(c, seed=seed + 4) * 0.5
-    ty, rpb, nblk = _van_slab(rows, c)
+    dres = randn(rows, c, seed=seed + 2) if with_dres else None
+    gamma, beta = randn(c, seed=seed + 3) * 0.5 + 1, randn(c, seed=seed + 4) * 0.5
+    ty, rpb, nblk = van_slab(rows, c)
     what = f'generic bn c {c} x {"f32" if x_f32 else "bf16"} g {"f32" if g_f32 else "bf16"} dx {"f32" if dx_f32 else "bf16"}'
 
     def run():
@@ -645,10 +536,10 @@ def test_generic_bn_conforms(c, x_f32, g_f32, dx_f32, with_dres):
         ws.fill_(NAN)
         part, nrows = ops.bn_stats_generic(x)
         assert nrows == nblk
-        o = {'ss': _nan(2, c), 'saved': _nan(2, c)}
+        o = {'ss': nan(2, c), 'saved': nan(2, c)}
         ops.bn_finalize(part, gamma, beta, None, None, o['ss'], o['saved'], rows, 1e-5, 0.1, partial_rows=nrows)
         o['out'] = ops.bn_apply_generic(x, o['ss'], dx_f32)
-        o['dgamma'], o['dbeta'] = _nan(c), _nan(c)
+        o['dgamma'], o['dbeta'] = nan(c), nan(c)
         ws.fill_(NAN)
         o['dx'] = ops.bn_bwd_generic(x, g, o['saved'], gamma, o['dgamma'], o['dbeta'], dres=dres, dx_f32=dx_f32)
         return o
@@ -656,7 +547,7 @@ def test_generic_bn_conforms(c, x_f32, g_f32, dx_f32, with_dres):
     o = run()
     _check_finalize('generic bn stats', what, x, gamma, beta, 1e-5, 0.1, None, None, o, -(-rpb // ty) + ty + -(-nblk // 32) + 32)
     v = x.double() * o['ss'][0].double() + o['ss'][1].double()
-    _check('generic bn apply', f'{what} apply', o['out'], v, U * v.abs())
+    check('generic bn apply', f'{what} apply', o['out'], v, U * v.abs())
     # backward: sums through reduce_partials (sequential over the partial rows)
     n = rows
     depth = -(-rpb // ty) + ty + nblk
@@ -666,8 +557,8 @@ def test_generic_bn_conforms(c, x_f32, g_f32, dx_f32, with_dres):
     t1 = g64 * xh
     a0 = (depth + 1) * U * g64.abs().sum(0)
     a1 = (depth + 1) * U * t1.abs().sum(0) + 2 * U * t1.abs().sum(0)
-    _check('generic bn backward', f'{what} dbeta', o['dbeta'], g64.sum(0), a0)
-    _check('generic bn backward', f'{what} dgamma', o['dgamma'], t1.sum(0), a1)
+    check('generic bn backward', f'{what} dbeta', o['dbeta'], g64.sum(0), a0)
+    check('generic bn backward', f'{what} dgamma', o['dgamma'], t1.sum(0), a1)
     k1 = gamma.double() * rstd
     m0, m1 = o['dbeta'].double() / n, o['dgamma'].double() / n
     inner = g64 - m0 - xh * m1
@@ -676,8 +567,8 @@ def test_generic_bn_conforms(c, x_f32, g_f32, dx_f32, with_dres):
     a = k1.abs() * 8 * U * (g64.abs() + m0.abs() + (xh * m1).abs()) + 2 * U * v.abs()
     if dres is not None:
         v = v + dres.double()
-        a = _rnd(v, a)
-    _check('generic bn backward', f'{what} dx', o['dx'], v, a)
+        a = rnd(v, a)
+    check('generic bn backward', f'{what} dx', o['dx'], v, a)
     _same_all(what, o, run())
 
 
@@ -728,8 +619,8 @@ def _check_param_grads(fam, what, dy64, xh, o, depth, prev=None):
         a = (depth + 1) * U * t.abs().sum(0) + (3 * U * t.abs().sum(0) if name == 'dgamma' else 0.0)
         if prev is not None:
             s = prev[k].double() + s
-            a = _rnd(s, a)
-        _check(fam, f'{what} {name}{" (accumulate)" if prev is not None else ""}', o[name], s, a)
+            a = rnd(s, a)
+        check(fam, f'{what} {name}{" (accumulate)" if prev is not None else ""}', o[name], s, a)
 
 
 LN_C = [128, 256, 384, 512, 768, 1024, 1280]
@@ -743,44 +634,43 @@ def test_layernorm_conforms(c, rows, eps):
     """saicv_layernorm_fwd / _bwd at every compiled width.  The backward runs twice: plain into fresh dgamma / dbeta,
     then with the residual-stream gradient dres, the bf16 copy scaled per 197 rows by a drop-path scale, accumulating
     onto the first call's parameter gradients."""
-    ops = _ops()
     seed = 800 + c + rows
-    x = _randn(rows, c, seed=seed) * 2 + (_randn(c, seed=seed + 1) * 0.5)
-    gamma, beta = _randn(c, seed=seed + 2) * 0.5 + 1, _randn(c, seed=seed + 3) * 0.5
-    dy = _randn(rows, c, seed=seed + 4).to(torch.bfloat16)
-    dres = _randn(rows, c, seed=seed + 5)
+    x = randn(rows, c, seed=seed) * 2 + (randn(c, seed=seed + 1) * 0.5)
+    gamma, beta = randn(c, seed=seed + 2) * 0.5 + 1, randn(c, seed=seed + 3) * 0.5
+    dy = randn(rows, c, seed=seed + 4).to(torch.bfloat16)
+    dres = randn(rows, c, seed=seed + 5)
     rps = 197
-    scale = (_rand(-(-rows // rps), seed=seed + 6) > 0.3).float() * 1.25
+    scale = (rand(-(-rows // rps), seed=seed + 6) > 0.3).float() * 1.25
     what = f'ln rows {rows} c {c} eps {eps:g}'
 
     def run():
-        o = {'y': torch.full((rows, c), NAN, device='cuda', dtype=torch.bfloat16), 'stats': _nan(2, rows)}
+        o = {'y': torch.full((rows, c), NAN, device='cuda', dtype=torch.bfloat16), 'stats': nan(2, rows)}
         ops.layernorm_fwd(x, gamma, beta, eps, out=o['y'], stats=o['stats'])
-        o['dgamma'], o['dbeta'] = _nan(c), _nan(c)
-        o['dx'] = ops.layernorm_bwd(dy, x, gamma, o['stats'], o['dgamma'], o['dbeta'], dx=_nan(rows, c))
+        o['dgamma'], o['dbeta'] = nan(c), nan(c)
+        o['dx'] = ops.layernorm_bwd(dy, x, gamma, o['stats'], o['dgamma'], o['dbeta'], dx=nan(rows, c))
         o['dgamma1'], o['dbeta1'] = o['dgamma'].clone(), o['dbeta'].clone()
         o['dxb'] = torch.full((rows, c), NAN, device='cuda', dtype=torch.bfloat16)
-        o['dx2'] = ops.layernorm_bwd(dy, x, gamma, o['stats'], o['dgamma1'], o['dbeta1'], dres=dres, dx=_nan(rows, c),
+        o['dx2'] = ops.layernorm_bwd(dy, x, gamma, o['stats'], o['dgamma1'], o['dbeta1'], dres=dres, dx=nan(rows, c),
                                      dx_bf16=o['dxb'], accumulate=True, bf16_row_scale=scale, rows_per_scale=rps)
         return o
 
     o = run()
     x64 = x.double()
     mean, a_m, r, a_r, y, a_y = _ln_fwd_ref(x64, gamma, beta, eps)
-    _check('layernorm fwd', f'{what} mean', o['stats'][0], mean, a_m)
-    _check('layernorm fwd', f'{what} rstd', o['stats'][1], r, a_r)
-    _check('layernorm fwd', f'{what} y', o['y'], y, a_y)
+    check('layernorm fwd', f'{what} mean', o['stats'][0], mean, a_m)
+    check('layernorm fwd', f'{what} rstd', o['stats'][1], r, a_r)
+    check('layernorm fwd', f'{what} y', o['y'], y, a_y)
     del y, a_y
     dy64 = dy.double()
     v, a, xh = _ln_bwd_ref(dy64, x64, gamma, o['stats'])
-    _check('layernorm bwd', f'{what} dx', o['dx'], v, a)
+    check('layernorm bwd', f'{what} dx', o['dx'], v, a)
     depth = _ln_bwd_depth(rows)
     _check_param_grads('layernorm bwd', what, dy64, xh, o, depth)
     v = v + dres.double()
-    a = _rnd(v, a)
-    _check('layernorm bwd', f'{what} dx + dres', o['dx2'], v, a)
+    a = rnd(v, a)
+    check('layernorm bwd', f'{what} dx + dres', o['dx2'], v, a)
     sc = scale.double().repeat_interleave(rps)[:rows, None]
-    _check('layernorm bwd', f'{what} bf16 dx * drop-path scale', o['dxb'], v * sc, a * sc + U * (v * sc).abs())
+    check('layernorm bwd', f'{what} bf16 dx * drop-path scale', o['dxb'], v * sc, a * sc + U * (v * sc).abs())
     _check_param_grads('layernorm bwd', what, dy64, xh, {'dgamma': o['dgamma1'], 'dbeta': o['dbeta1']},
                        _ln_bwd_depth(rows, True), prev=(o['dgamma'], o['dbeta']))
     del v, a, xh
@@ -794,14 +684,13 @@ POSTLN = [(c, rows, pr) for c in (128, 256, 384, 512) for rows, pr in ((2 * 850,
 def test_postln_conforms(c, rows, pos_rows):
     """saicv_postln_fwd / _bwd (DETR): y fp32, its bf16 copy, bf16(y + pos[row % pos_rows]) with pos_rows dividing rows
     or equal to it; the backward with dres and both outputs; add_pos_cast."""
-    ops = _ops()
     seed = 900 + c + rows
-    z = _randn(rows, c, seed=seed) * 3
-    gamma, beta = _randn(c, seed=seed + 1) * 0.5 + 1, _randn(c, seed=seed + 2) * 0.5
-    pos = _randn(pos_rows, c, seed=seed + 3)
-    dy = _randn(rows, c, seed=seed + 4)
-    dres = _randn(rows, c, seed=seed + 5)
-    prev = (_randn(c, seed=seed + 6), _randn(c, seed=seed + 7))
+    z = randn(rows, c, seed=seed) * 3
+    gamma, beta = randn(c, seed=seed + 1) * 0.5 + 1, randn(c, seed=seed + 2) * 0.5
+    pos = randn(pos_rows, c, seed=seed + 3)
+    dy = randn(rows, c, seed=seed + 4)
+    dres = randn(rows, c, seed=seed + 5)
+    prev = (randn(c, seed=seed + 6), randn(c, seed=seed + 7))
     what = f'postln rows {rows} c {c} pos_rows {pos_rows}'
 
     def run():
@@ -815,24 +704,24 @@ def test_postln_conforms(c, rows, pos_rows):
     o = run()
     z64 = z.double()
     mean, a_m, r, a_r, y, a_y = _ln_fwd_ref(z64, gamma, beta, 1e-5)
-    _check('postln fwd', f'{what} mean', o['stats'][0], mean, a_m)
-    _check('postln fwd', f'{what} rstd', o['stats'][1], r, a_r)
-    _check('postln fwd', f'{what} y', o['y'], y, a_y)
-    _check('postln fwd', f'{what} yb', o['yb'], y, a_y)
+    check('postln fwd', f'{what} mean', o['stats'][0], mean, a_m)
+    check('postln fwd', f'{what} rstd', o['stats'][1], r, a_r)
+    check('postln fwd', f'{what} y', o['y'], y, a_y)
+    check('postln fwd', f'{what} yb', o['yb'], y, a_y)
     p64 = pos.double().repeat(rows // pos_rows, 1)
     yp = y + p64
-    _check('postln fwd', f'{what} ypb', o['ypb'], yp, _rnd(yp, a_y))
+    check('postln fwd', f'{what} ypb', o['ypb'], yp, rnd(yp, a_y))
     del y, a_y, yp
     dy64 = dy.double()
     v, a, xh = _ln_bwd_ref(dy64, z64, gamma, o['stats'])
     v = v + dres.double()
-    a = _rnd(v, a)
-    _check('postln bwd', f'{what} dz', o['dz'], v, a)
-    _check('postln bwd', f'{what} dzb', o['dzb'], v, a)
+    a = rnd(v, a)
+    check('postln bwd', f'{what} dz', o['dz'], v, a)
+    check('postln bwd', f'{what} dzb', o['dzb'], v, a)
     _check_param_grads('postln bwd', what, dy64, xh, o, _ln_bwd_depth(rows, True), prev=prev)
-    _same('add_pos_cast xb', o['xb'], z.to(torch.bfloat16))
+    same('add_pos_cast xb', o['xb'], z.to(torch.bfloat16))
     zp = z64 + p64
-    _check('add_pos_cast', f'{what} add_pos_cast xpb', o['xpb'], zp, U * zp.abs())
+    check('add_pos_cast', f'{what} add_pos_cast xpb', o['xpb'], zp, U * zp.abs())
     _same_all(what, o, run())
 
 
@@ -840,34 +729,33 @@ def test_postln_conforms(c, rows, pos_rows):
 @pytest.mark.parametrize('want_dz,want_dzb', [(False, False), (False, True), (True, False), (True, True)])
 def test_postln_nullable_outputs(want_y, want_yb, want_ypb, want_dz, want_dzb):
     """Every nullable output combination writes what the full call writes, bit for bit (and add_pos_cast's)."""
-    ops = _ops()
     rows, c, pos_rows = 300, 256, 100
-    z = _randn(rows, c, seed=950) * 3
-    gamma, beta = _randn(c, seed=951) * 0.5 + 1, _randn(c, seed=952) * 0.5
-    pos = _randn(pos_rows, c, seed=953)
-    dy = _randn(rows, c, seed=954)
+    z = randn(rows, c, seed=950) * 3
+    gamma, beta = randn(c, seed=951) * 0.5 + 1, randn(c, seed=952) * 0.5
+    pos = randn(pos_rows, c, seed=953)
+    dy = randn(rows, c, seed=954)
     y0, yb0, ypb0, st0 = ops.postln_fwd(z, gamma, beta, 1e-5, pos=pos, want_y=True, want_yb=True, want_ypb=True)
     y, yb, ypb, st = ops.postln_fwd(z, gamma, beta, 1e-5, pos=pos, want_y=want_y, want_yb=want_yb, want_ypb=want_ypb)
-    _same('stats', st, st0)
+    same('stats', st, st0)
     for name, a, b in (('y', y, y0), ('yb', yb, yb0), ('ypb', ypb, ypb0)):
         assert (a is not None) == {'y': want_y, 'yb': want_yb, 'ypb': want_ypb}[name]
         if a is not None:
-            _same(name, a, b)
-    dg0, db0, dg, db = _nan(c), _nan(c), _nan(c), _nan(c)
+            same(name, a, b)
+    dg0, db0, dg, db = nan(c), nan(c), nan(c), nan(c)
     dz0, dzb0 = ops.postln_bwd(dy, z, gamma, st0, dg0, db0)
     dz, dzb = ops.postln_bwd(dy, z, gamma, st0, dg, db, want_dz=want_dz, want_dzb=want_dzb)
-    _same('dgamma', dg, dg0)
-    _same('dbeta', db, db0)
+    same('dgamma', dg, dg0)
+    same('dbeta', db, db0)
     if want_dz:
-        _same('dz', dz, dz0)
+        same('dz', dz, dz0)
     if want_dzb:
-        _same('dzb', dzb, dzb0)
+        same('dzb', dzb, dzb0)
     xb0, xpb0 = ops.add_pos_cast(z, pos)
     xb, xpb = ops.add_pos_cast(z, pos, want_xb=want_y, want_xpb=want_yb)
     if want_y:
-        _same('xb', xb, xb0)
+        same('xb', xb, xb0)
     if want_yb:
-        _same('xpb', xpb, xpb0)
+        same('xpb', xpb, xpb0)
 
 
 # ------------------------------------------------------------------ column sums
@@ -875,13 +763,12 @@ def test_postln_nullable_outputs(want_y, want_yb, want_ypb, want_dz, want_dzb):
 @pytest.mark.parametrize('accumulate', [False, True])
 def test_colsum_conforms(c, accumulate):
     """bf16 column sums in chunks of at most 2048 columns (2056 and 4104 leave an 8-column chunk)."""
-    ops = _ops()
     rows = 20000
-    x = _randn(rows, c, seed=1000 + c).to(torch.bfloat16)
-    prev = _randn(c, seed=1001)
+    x = randn(rows, c, seed=1000 + c).to(torch.bfloat16)
+    prev = randn(c, seed=1001)
 
     def run():
-        out = prev.clone() if accumulate else _nan(c)
+        out = prev.clone() if accumulate else nan(c)
         ops.partial_ws(x.device, c).fill_(NAN)
         return {'out': ops.colsum(x, out, accumulate=accumulate)}
 
@@ -893,20 +780,19 @@ def test_colsum_conforms(c, accumulate):
         a[c0:c0 + cw] = (_slab_depth(rows, cw, 8) + 1) * U * x64[:, c0:c0 + cw].abs().sum(0)
     if accumulate:
         s = prev.double() + s
-        a = _rnd(s, a)
-    _check('colsum', f'colsum c {c} rows {rows}{" accumulate" if accumulate else ""}', o['out'], s, a)
+        a = rnd(s, a)
+    check('colsum', f'colsum c {c} rows {rows}{" accumulate" if accumulate else ""}', o['out'], s, a)
     _same_all(f'colsum c {c}', o, run())
 
 
 @pytest.mark.parametrize('rows,c', [(256, 1000), (50, 4104)])
 @pytest.mark.parametrize('accumulate', [False, True])
 def test_colsum_f32_conforms(rows, c, accumulate):
-    ops = _ops()
-    x = _randn(rows, c, seed=1100 + c)
-    prev = _randn(c, seed=1101)
+    x = randn(rows, c, seed=1100 + c)
+    prev = randn(c, seed=1101)
 
     def run():
-        out = prev.clone() if accumulate else _nan(c)
+        out = prev.clone() if accumulate else nan(c)
         return {'out': ops.colsum(x, out, accumulate=accumulate)}
 
     o = run()
@@ -914,8 +800,8 @@ def test_colsum_f32_conforms(rows, c, accumulate):
     s, a = x64.sum(0), (rows + 1) * U * x64.abs().sum(0)
     if accumulate:
         s = prev.double() + s
-        a = _rnd(s, a)
-    _check('colsum f32', f'colsum f32 rows {rows} c {c}', o['out'], s, a)
+        a = rnd(s, a)
+    check('colsum f32', f'colsum f32 rows {rows} c {c}', o['out'], s, a)
     _same_all('colsum f32', o, run())
 
 
@@ -959,12 +845,11 @@ def _maxpool_bwd_ref(dy, code, h, w, k, stride, pad, pad_hi):
 def test_maxpool_conforms(n, h, w, c, k, stride, pad, pad_hi, oob_zero):
     """Inputs are ReLU outputs of a few bf16 values: most windows hold ties and some are all zero, so the tie rule
     decides the argmax, and with it which input receives the gradient."""
-    ops = _ops()
     vals = torch.tensor([-1.0, -0.5, 0.0, 0.5, 1.0, 0.5, 0.0], device='cuda')
-    idx = torch.randint(0, vals.numel(), (n, h, w, c), device='cuda', generator=_gen(1200 + k + h))
+    idx = torch.randint(0, vals.numel(), (n, h, w, c), device='cuda', generator=gen(1200 + k + h))
     x = vals[idx].clamp_min(0).to(torch.bfloat16)
     P, Q = (h + pad + pad_hi - k) // stride + 1, (w + pad + pad_hi - k) // stride + 1
-    dy = _randn(n, P, Q, c, seed=1201).to(torch.bfloat16)
+    dy = randn(n, P, Q, c, seed=1201).to(torch.bfloat16)
 
     def run():
         y, am = ops.maxpool_fwd(x, k, stride, pad, pad_hi, bool(oob_zero))
@@ -982,15 +867,14 @@ def test_maxpool_conforms(n, h, w, c, k, stride, pad, pad_hi, oob_zero):
     n_bad = int((o['argmax'].long() != code).sum())
     assert n_bad == 0, f'{what}: {n_bad} argmax codes differ from the first maximum in scan order'
     v, s = _maxpool_bwd_ref(dy, code, h, w, k, stride, pad, pad_hi)
-    _check('maxpool bwd', f'{what} dx', o['dx'], v, (-(-k // stride)) ** 2 * U * s)
+    check('maxpool bwd', f'{what} dx', o['dx'], v, (-(-k // stride)) ** 2 * U * s)
     _same_all(what, o, run())
 
 
 @pytest.mark.parametrize('n,h,w,c', [(8, 7, 7, 2048), (4, 14, 14, 512), (3, 1, 1, 64)])
 def test_avgpool_conforms(n, h, w, c):
-    ops = _ops()
-    x = (_randn(n, h, w, c, seed=1300) + 0.5).to(torch.bfloat16)
-    dy = _randn(n, c, seed=1301).to(torch.bfloat16)
+    x = (randn(n, h, w, c, seed=1300) + 0.5).to(torch.bfloat16)
+    dy = randn(n, c, seed=1301).to(torch.bfloat16)
 
     def run():
         return {'y': ops.avgpool_fwd(x), 'dx': ops.avgpool_bwd(dy, h, w)}
@@ -999,21 +883,20 @@ def test_avgpool_conforms(n, h, w, c):
     hw = h * w
     x64 = x.double().view(n, hw, c)
     v = x64.sum(1) / hw
-    a = _rnd(v, _rnd(v, hw * U * x64.abs().sum(1) / hw))      # hw - 1 adds, then 1 / hw and the product round
-    _check('avgpool', f'avgpool fwd {n}x{h}x{w}x{c}', o['y'], v, a)
+    a = rnd(v, rnd(v, hw * U * x64.abs().sum(1) / hw))      # hw - 1 adds, then 1 / hw and the product round
+    check('avgpool', f'avgpool fwd {n}x{h}x{w}x{c}', o['y'], v, a)
     vb = (dy.double() / hw)[:, None, None, :].expand(n, h, w, c)
-    _check('avgpool', f'avgpool bwd {n}x{h}x{w}x{c}', o['dx'], vb, 2 * U * vb.abs())
+    check('avgpool', f'avgpool bwd {n}x{h}x{w}x{c}', o['dx'], vb, 2 * U * vb.abs())
     _same_all('avgpool', o, run())
 
 
 @pytest.mark.parametrize('x_f32', [False, True])
 @pytest.mark.parametrize('dx_f32', [False, True])
 def test_avgpool_stream_conforms(x_f32, dx_f32):
-    ops = _ops()
     n, h, w, c = 4, 7, 7, 512
-    x = _randn(n, h, w, c, seed=1400) + 0.5
+    x = randn(n, h, w, c, seed=1400) + 0.5
     x = x if x_f32 else x.to(torch.bfloat16)
-    dy = _randn(n, c, seed=1401).to(torch.bfloat16)
+    dy = randn(n, c, seed=1401).to(torch.bfloat16)
 
     def run():
         return {'y': ops.avgpool_stream_fwd(x), 'dx': ops.avgpool_stream_bwd(dy, h, w, dx_f32=dx_f32)}
@@ -1022,9 +905,9 @@ def test_avgpool_stream_conforms(x_f32, dx_f32):
     hw = h * w
     x64 = x.double().view(n, hw, c)
     v = x64.sum(1) / hw
-    a = _rnd(v, _rnd(v, hw * U * x64.abs().sum(1) / hw))      # hw - 1 adds, then 1 / hw and the product round
+    a = rnd(v, rnd(v, hw * U * x64.abs().sum(1) / hw))      # hw - 1 adds, then 1 / hw and the product round
     what = f'avgpool_stream x {"f32" if x_f32 else "bf16"} dx {"f32" if dx_f32 else "bf16"}'
-    _check('avgpool stream', f'{what} fwd', o['y'], v, a)
+    check('avgpool stream', f'{what} fwd', o['y'], v, a)
     vb = (dy.double() / hw)[:, None, None, :].expand(n, h, w, c)
-    _check('avgpool stream', f'{what} bwd', o['dx'], vb, 2 * U * vb.abs())
+    check('avgpool stream', f'{what} bwd', o['dx'], vb, 2 * U * vb.abs())
     _same_all(what, o, run())

@@ -30,14 +30,11 @@ Allowances are derived from the operation, never fitted to measured errors (u = 
     partials; X = bf16(bf16(u) * (1 / (norm + 1e-7))).
   * Newton-Schulz GEMMs: the GEMM-conformance bound B = 2^-16 S + 2^-22 |ref| (S = sum |a b| over the reduction),
     carried through fmaf(beta, aux, alpha acc) as |alpha| B + 2u (|alpha| (|ref| + B) + |beta aux|).
-  * A bf16 output must lie in [rne(v - A), rne(v + A)]; an fp32 output within A of v.  The bf16 operand copies must
-    equal rne_bf16 of the stored fp32 p' bit for bit, and every element of a copy the layout does not map (extra rows,
-    channel and tap padding) keeps its sentinel.
-Every element must conform; no fraction of misses is allowed.  Each check prints the largest share of its allowance
-an element used, and the module prints the largest share per family at the end (run with -s).  Measured on an NVIDIA
-H100 80GB HBM3 at a 700 W power limit: SGD 99.7 % and the Muon prep 99.6 % (a correctly rounded final operation may use
-all of its rounding), the Muon apply 90 %, AdamW 83 %, the Newton-Schulz GEMMs 36 %, the clip norm 3.4 %; the operand
-copies are bit-exact.  The file runs in about 25 s.
+  * The bf16 operand copies must equal rne_bf16 of the stored fp32 p' bit for bit, and every element of a copy the
+    layout does not map (extra rows, channel and tap padding) keeps its sentinel.
+Largest shares of the allowance, measured on an NVIDIA H100 80GB HBM3 at a 700 W power limit: SGD 99.7 % and the Muon
+prep 99.6 % (a correctly rounded final operation may use all of its rounding), the Muon apply 90 %, AdamW 83 %, the
+Newton-Schulz GEMMs 36 %, the clip norm 3.4 %; the operand copies are bit-exact.  The file runs in about 25 s.
 
 Cases.  The SGD / AdamW tensors cover the chunk edges (numel 1, 3, 4, 7, 8191, 8192, 8193, 3 * 8192 + 5 and 2304 * 768),
 gradient views at float offsets 1, 2 and 3 (the scalar path), a tensor whose last chunk has n % 4 != 0 after float4
@@ -49,33 +46,17 @@ shape class, padded slots, a 1024 x 4096 matrix of 512 chunks, Nesterov on and o
 """
 import copy
 import ctypes
-import importlib.util
 import math
-import os
 
 import numpy as np
 import pytest
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _load(name, fname):
-    spec = importlib.util.spec_from_file_location(name, os.path.join(HERE, fname))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-_gemm = _load('gemm_conformance', 'test_gemm_conformance_gpu.py')
-_norm = _load('norm_conformance', 'test_norm_conformance_gpu.py')
-_rne_bf16, _quantum_bf16, _acc_allowance, _conform = _gemm._rne_bf16, _gemm._quantum_bf16, _gemm._acc_allowance, _gemm._conform
-_check, _same = _norm._check, _norm._same
-USED = _norm.USED       # this module's own copy of the norm module: only the checks below record into it
+from conformance import U, acc_allowance, call, check, exact, f32, gen, quantum_bf16, rne_bf16, same
+from conformance import report  # noqa: F401  (autouse: this module's allowance report)
 
 gpu = pytest.mark.gpu
 
-U = 2.0 ** -24          # one fp32 rounding, relative
 CHUNK = 8192            # SAICV_OPT_CHUNK
 THREADS = 256           # kOptThreads
 SUMSQ_DEPTH = 1 + CHUNK // THREADS + 5 + THREADS // 32   # g^2, the per-thread chain, the shuffles, the warp partials
@@ -94,23 +75,6 @@ STEPS = 10              # > SAICV_OPT_RING
 # Muon: matrices (three in one shape class, one of them transposed; padded slots; 512 chunks) and AdamW rows
 MUON_MATS = [(96, 200), (96, 200), (200, 96), (8, 5, 3, 3), (130, 70), (1024, 4096)]
 MUON_ADAMW = [(77,), (CHUNK + 1,), (3, 5)]
-
-
-def _f32(x):
-    return float(np.float32(x))
-
-
-def _gen(seed):
-    return torch.Generator(device='cuda').manual_seed(seed)
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _report():
-    yield
-    if USED:
-        print('\nlargest share of the allowance used, by family (0: bit-exact):')
-        for k in sorted(USED):
-            print(f'  {k:28s} {USED[k]:.3g}')
 
 
 # ------------------------------------------------------------------ interval arithmetic of the fp32 kernels
@@ -153,7 +117,7 @@ class _V:
 
 def _c(x):
     """An fp32 constant as the kernel reads it (exact)."""
-    return _V(_f32(float(x)))
+    return _V(f32(float(x)))
 
 
 def _dbl(x):
@@ -217,14 +181,14 @@ def test_cases_reach_every_chunk_path_cpu():
 
 # ------------------------------------------------------------------ SGD / AdamW over the chunk geometry
 def _geom_params(seed):
-    g = _gen(seed)
+    g = gen(seed)
     return [torch.randn(numel, device='cuda', generator=g).requires_grad_(True) for numel, _, _ in GEOM]
 
 
 def _geom_grads(ps, step, scale=1.0):
     """Gradient views at the cases' offsets into one flat buffer (the same storage every step)."""
     starts, total = _grad_starts(GEOM)
-    flat = torch.randn(total, device='cuda', generator=_gen(1000 + step)) * scale
+    flat = torch.randn(total, device='cuda', generator=gen(1000 + step)) * scale
     return flat, [flat[s:s + p.numel()] for s, p in zip(starts, ps)]
 
 
@@ -258,25 +222,25 @@ def _sgd_check(what, p0, g0, b0, p1, b1, gs, lr, wd, mom, nest):
     g = _V(g0) if gs is None else _V(g0) * _c(gs)
     d = g + _c(wd) * _V(p0)
     bn = _c(mom) * _V(b0) + d
-    _check('sgd', f'{what} momentum buffer', b1, bn.v, bn.a)
+    check('sgd', f'{what} momentum buffer', b1, bn.v, bn.a)
     upd = d + _c(mom) * _V(b1) if nest else _V(b1)
     pn = _V(p0) - _c(lr) * upd
-    _check('sgd', f'{what} parameter', p1, pn.v, pn.a)
+    check('sgd', f'{what} parameter', p1, pn.v, pn.a)
 
 
 def _adamw_check(what, p0, g0, m0, v0, p1, m1, v1, gs, lr, wd, t):
     """multi_adamw_kernel (torch.optim.AdamW): p *= 1 - lr wd; m' = m + (g - m)(1 - b1); v' = b2 v + (1 - b2) g g;
     p' = p - fp32(lr / (1 - b1^t)) m' / (sqrt(v') / fp32(sqrt(1 - b2^t)) + eps)."""
-    b1, b2 = _f32(BETAS[0]), _f32(BETAS[1])
+    b1, b2 = f32(BETAS[0]), f32(BETAS[1])
     g = _V(g0) if gs is None else _V(g0) * _c(gs)
     mn = _V(m0) + (g - _V(m0)) * (_c(1) - _c(b1))
     vn = _c(b2) * _V(v0) + (_c(1) - _c(b2)) * g * g
-    _check('adamw', f'{what} exp_avg', m1, mn.v, mn.a)
-    _check('adamw', f'{what} exp_avg_sq', v1, vn.v, vn.a)
-    step, bc2s = _dbl(_f32(lr) / (1.0 - b1 ** t)), _dbl(math.sqrt(1.0 - b2 ** t))
+    check('adamw', f'{what} exp_avg', m1, mn.v, mn.a)
+    check('adamw', f'{what} exp_avg_sq', v1, vn.v, vn.a)
+    step, bc2s = _dbl(f32(lr) / (1.0 - b1 ** t)), _dbl(math.sqrt(1.0 - b2 ** t))
     pd = _V(p0) * (_c(1) - _c(lr) * _c(wd))
     pn = pd - step * (_V(m1) / (_V(v1).sqrt() / bc2s + _c(EPS)))
-    _check('adamw', f'{what} parameter', p1, pn.v, pn.a)
+    check('adamw', f'{what} parameter', p1, pn.v, pn.a)
 
 
 def _set_lr(opt, step, base):
@@ -349,10 +313,10 @@ def test_adamw_with_intermittent_gradients_keeps_per_parameter_steps():
         torch.cuda.synchronize()
         for i, (p, q, (p0, g0, st0)) in enumerate(zip(ps, ref_ps, snap)):
             if g0 is None:
-                _same(f'adamw step {step} tensor {i} without a gradient', p.detach(), p0)
+                same(f'adamw step {step} tensor {i} without a gradient', p.detach(), p0)
                 for k, s0 in zip(['exp_avg', 'exp_avg_sq'], st0):
                     if k in opt.state[p]:
-                        _same(f'adamw step {step} tensor {i} {k} without a gradient', opt.state[p][k], s0)
+                        same(f'adamw step {step} tensor {i} {k} without a gradient', opt.state[p][k], s0)
                 continue
             t = int(ref.state[q]['step'])
             gi = GEOM[i][2]
@@ -378,7 +342,7 @@ def test_adamw_with_intermittent_gradients_keeps_per_parameter_steps():
         opt2.step()
     torch.cuda.synchronize()
     for i, (p, p2) in enumerate(zip(ps, ps2)):
-        _same(f'adamw tensor {i} after a state_dict round trip', p2.detach(), p.detach())
+        same(f'adamw tensor {i} after a state_dict round trip', p2.detach(), p.detach())
 
 
 # ------------------------------------------------------------------ the global-norm clip
@@ -391,11 +355,11 @@ def _clip_check(what, opt, grads, max_norm):
     sq = _V(torch.tensor(sumsq, dtype=torch.float64, device='cuda'), torch.tensor(_fold_allowance(sumsq, chunks),
                                                                                   dtype=torch.float64, device='cuda'))
     norm = sq.sqrt()
-    _check('clip', f'{what}: norm ({chunks} chunks)', clip[1:2], norm.v.view(1), norm.a.view(1))
-    c = torch.tensor(_f32(max_norm), device='cuda') / (clip[1] + torch.tensor(1e-6, device='cuda'))
+    check('clip', f'{what}: norm ({chunks} chunks)', clip[1:2], norm.v.view(1), norm.a.view(1))
+    c = torch.tensor(f32(max_norm), device='cuda') / (clip[1] + torch.tensor(1e-6, device='cuda'))
     want = c if bool(torch.isnan(c)) else torch.clamp(c, max=1.0)
-    _same(f'{what}: coefficient', clip[0:1], want.view(1))
-    if float(clip[1]) + _f32(1e-6) <= _f32(max_norm):
+    same(f'{what}: coefficient', clip[0:1], want.view(1))
+    if float(clip[1]) + f32(1e-6) <= f32(max_norm):
         assert float(clip[0]) == 1.0
     return clip[0]
 
@@ -436,8 +400,8 @@ def test_clip_conforms_and_scales_exactly_one_step():
     assert float(_clip_check('clip of zero gradients', opt, zeros, 1.0)) == 1.0 and float(opt._clip[1]) == 0.0
     # a single tensor (one chunk) whose norm is below max_norm
     from simpleaicv_pytorch_training_examples_b200 import optim
-    q = torch.randn(77, device='cuda', generator=_gen(4)).requires_grad_(True)
-    q.grad = torch.randn(77, device='cuda', generator=_gen(5)) * 0.01
+    q = torch.randn(77, device='cuda', generator=gen(4)).requires_grad_(True)
+    q.grad = torch.randn(77, device='cuda', generator=gen(5)) * 0.01
     one = optim.FusedSGD([q], lr=0.1, momentum=0.9)
     one.clip_grad_norm(1.0)
     torch.cuda.synchronize()
@@ -452,7 +416,7 @@ def test_clip_with_a_non_finite_gradient_follows_torch(bad):
     inf: the norm is inf, the coefficient 0, and only that element becomes NaN; the others take the step with g = 0."""
     from simpleaicv_pytorch_training_examples_b200 import optim
     shapes = [(1000, 64), (8193,), (5, 3, 3, 3)]
-    g = _gen(6)
+    g = gen(6)
     ps = [torch.randn(*s, device='cuda', generator=g).requires_grad_(True) for s in shapes]
     ref_ps = [p.detach().clone().requires_grad_(True) for p in ps]
     grads = [torch.randn(*s, device='cuda', generator=g) for s in shapes]
@@ -492,7 +456,7 @@ def _shadow_setup(opt_kind, offset, seed):
     """Parameters with operand copies (Linear [N + extra][K] and conv [K][kpad], tap-major with cp >= c), filled with the
     sentinel; gradients at a float offset (0: float4 path where numel % 4 == 0, 1: scalar path)."""
     from simpleaicv_pytorch_training_examples_b200 import optim
-    g = _gen(seed)
+    g = gen(seed)
     params, copies = [], []
     for n, k, extra in SHADOW_LIN:
         params.append(torch.randn(n, k, device='cuda', generator=g).requires_grad_(True))
@@ -549,10 +513,9 @@ def test_operand_copies_are_exact_and_padding_is_untouched(opt_kind, offset):
         for i, (p, (w, conv)) in enumerate(zip(params, copies)):
             want, mask = _mapped(p, w, conv)
             what = f'{opt_kind} offset {offset} step {step} copy {i} ({tuple(p.shape)})'
-            _same(f'{what} mapped elements', w[mask], want[mask])
+            exact('operand copies', f'{what} mapped elements', w[mask], want[mask])
             bits = w.view(torch.int16)[~mask]
             assert bool((bits == SENTINEL).all()), f'{what}: {int((bits != SENTINEL).sum())} unmapped elements written'
-            USED.setdefault('operand copies', 0.0)
 
 
 # ------------------------------------------------------------------ Newton-Schulz GEMMs
@@ -568,7 +531,7 @@ def _ns_operand(batch, rows, cols, seed):
     """bf16 [batch, rows, cols] whose neighbouring matrices differ in magnitude by 2^8 and 2^16: a tile that read or wrote
     rows of the next matrix would leave the bound."""
     scale = torch.tensor([2.0 ** (8 * (j % 3)) for j in range(batch)], device='cuda').view(batch, 1, 1)
-    return (torch.randn(batch, rows, cols, device='cuda', generator=_gen(seed)) * scale).to(torch.bfloat16)
+    return (torch.randn(batch, rows, cols, device='cuda', generator=gen(seed)) * scale).to(torch.bfloat16)
 
 
 @gpu
@@ -577,13 +540,11 @@ def test_ns_gemm_conforms(mode, m, n, batch):
     """saicv_ns_gemm, the batched VAR_NS GEMM over 3-D TMA maps: mode 0 X X^T, mode 1 alpha A A + beta A, mode 2
     alpha B X + beta X (aux by TMA), per element against float64 in every matrix of the batch; the output starts as NaN,
     so an element no tile wrote fails."""
-    from simpleaicv_pytorch_training_examples_b200 import _lib, ops
     alpha, beta = NS_ALPHA_BETA[mode]
     x = _ns_operand(batch, m, n if mode == 0 else m, 10 + mode)
     y = _ns_operand(batch, m, n, 20) if mode == 2 else None
     out = torch.full((batch, m, n if mode == 2 else m), float('nan'), device='cuda', dtype=torch.bfloat16)
-    _lib.call('saicv_ns_gemm', mode, ops._p(x), ops._p(y) if y is not None else None, ops._p(out), batch, m, n,
-              ctypes.c_float(alpha), ctypes.c_float(beta), ops._stream())
+    call('saicv_ns_gemm', mode, x, y, out, batch, m, n, ctypes.c_float(alpha), ctypes.c_float(beta))
     xd = x.double()
     if mode == 0:
         ref, s = xd @ xd.mT, xd.abs() @ xd.abs().mT
@@ -591,20 +552,20 @@ def test_ns_gemm_conforms(mode, m, n, batch):
         ref, s = xd @ xd, xd.abs() @ xd.abs()
     else:
         ref, s = xd @ y.double(), xd.abs() @ y.double().abs()
-    allow = _acc_allowance(ref, s)
+    allow = acc_allowance(ref, s)
     v = ref
     if mode:
-        a, b = _f32(alpha), _f32(beta)
+        a, b = f32(alpha), f32(beta)
         aux = (x if mode == 1 else y).double()
         v = a * ref + b * aux
         allow = abs(a) * allow + 2 * U * (abs(a) * (ref.abs() + allow) + (b * aux).abs())
-    _conform(f'ns_gemm mode {mode} {batch}x{m}x{n}', out, v, allow, s)
+    check(None, f'ns_gemm mode {mode} {batch}x{m}x{n}', out, v, allow, s)
 
 
 # ------------------------------------------------------------------ Muon prep and apply
 def _muon_setup(nesterov, seed):
     from simpleaicv_pytorch_training_examples_b200 import optim
-    g = _gen(seed)
+    g = gen(seed)
     mats = [(torch.randn(*s, device='cuda', generator=g) * 0.1).requires_grad_(True) for s in MUON_MATS]
     adams = [(torch.randn(*s, device='cuda', generator=g) * 0.1).requires_grad_(True) for s in MUON_ADAMW]
     opt = optim.FusedMuon(lr=0.02, wd=0.05, muon_params=mats, momentum=0.95, nesterov=nesterov, ns_steps=5,
@@ -653,12 +614,12 @@ def test_muon_prep_and_apply_conform(nesterov, clip, monkeypatch):
         return real_ns(x, *args)
 
     monkeypatch.setattr(optim, 'newton_schulz', spy)
-    b1, b2 = _f32(BETAS[0]), _f32(BETAS[1])
+    b1, b2 = f32(BETAS[0]), f32(BETAS[1])
     mom = 0.95
     for step in range(4):
         opt.param_groups[0]['lr'] = 0.02 * 0.9 ** step
         lr, wd = opt.param_groups[0]['lr'], opt.param_groups[0]['wd']
-        g = _gen(100 + step)
+        g = gen(100 + step)
         for i, p in enumerate(mats):
             p.grad = torch.randn(p.shape, device='cuda', generator=g) if _muon_has('mat', i, step) else None
         for i, p in enumerate(adams):
@@ -687,18 +648,18 @@ def test_muon_prep_and_apply_conform(nesterov, clip, monkeypatch):
             for name, sl in (('prep', slot0), ('apply', slot1)):
                 assert not sl[lo:].any() and not sl[:, hi:].any(), f'{what}: {name} slot padding is not zero'
             if g0 is None:
-                _same(f'{what} without a gradient', p.detach(), p0)
+                same(f'{what} without a gradient', p.detach(), p0)
                 continue
             r, c = b0.shape
             gm = _V(g0.reshape(r, c)) if gs is None else _V(g0.reshape(r, c)) * _c(gs)
             b1s = opt.state[p]['momentum_buffer']
             bn = _c(mom) * _V(b0) + gm
-            _check('muon prep', f'{what} momentum buffer', b1s, bn.v, bn.a)
+            check('muon prep', f'{what} momentum buffer', b1s, bn.v, bn.a)
             if nesterov:
                 u = gm + _c(mom) * _V(b1s)
-                ub = _V(u.v, u.a + _quantum_bf16(u.v.abs() + u.a) / 2)
+                ub = _V(u.v, u.a + quantum_bf16(u.v.abs() + u.a) / 2)
             else:
-                ub = _V(_rne_bf16(b1s.double()))
+                ub = _V(rne_bf16(b1s.double()))
             sumsq = float(ub.v.square().sum())
             unc = float((2 * ub.v.abs() * ub.a + ub.a.square()).sum())
             chunks = -(-p.numel() // CHUNK)
@@ -706,26 +667,26 @@ def test_muon_prep_and_apply_conform(nesterov, clip, monkeypatch):
                     torch.tensor(unc + _fold_allowance(sumsq + unc, chunks), dtype=torch.float64, device='cuda'))
             inv = _c(1) / (sq.sqrt() + _c(1e-7))
             x = ub * inv
-            _check('muon prep', f'{what} slot X ({"transposed" if p.shape[0] > c else "direct"})', x0, x.v, x.a)
+            check('muon prep', f'{what} slot X ({"transposed" if p.shape[0] > c else "direct"})', x0, x.v, x.a)
             row = table[id(p)]
             assert int(row['transposed']) == int(p.shape[0] > c)
             pn = _V(p0) * (_c(1) - _c(lr) * _c(wd)) - _c(lr) * _V(float(row['adj'])) * _V(u1.reshape(p.shape))
-            _check('muon apply', f'{what} parameter', p.detach(), pn.v, pn.a)
+            check('muon apply', f'{what} parameter', p.detach(), pn.v, pn.a)
         for i, (p, (p0, g0, st0)) in enumerate(zip(adams, snap_a)):
             what = f'muon step {step} AdamW row {i} {tuple(p.shape)}'
             if g0 is None:
-                _same(f'{what} without a gradient', p.detach(), p0)
+                same(f'{what} without a gradient', p.detach(), p0)
                 continue
             t = int(adam0[i]) + 1
             gv = _V(g0) if gs is None else _V(g0) * _c(gs)
             m1, v1 = opt.state[p]['moment1'], opt.state[p]['moment2']
             mn = _V(st0[0]) + (gv - _V(st0[0])) * (_c(1) - _c(b1))
             vn = _V(st0[1]) + (gv * gv - _V(st0[1])) * (_c(1) - _c(b2))
-            _check('muon apply', f'{what} moment1', m1, mn.v, mn.a)
-            _check('muon apply', f'{what} moment2', v1, vn.v, vn.a)
-            a = _dbl(_f32(lr) * math.sqrt(1.0 - b2 ** t) / (1.0 - b1 ** t))
+            check('muon apply', f'{what} moment1', m1, mn.v, mn.a)
+            check('muon apply', f'{what} moment2', v1, vn.v, vn.a)
+            a = _dbl(f32(lr) * math.sqrt(1.0 - b2 ** t) / (1.0 - b1 ** t))
             pn = _V(p0) * (_c(1) - _c(lr) * _c(wd)) - a * (_V(m1) / (_c(EPS) + _V(v1).sqrt()))
-            _check('muon apply', f'{what} parameter', p.detach(), pn.v, pn.a)
+            check('muon apply', f'{what} parameter', p.detach(), pn.v, pn.a)
         want = adam0 + torch.tensor([int(_muon_has('adam', i, step)) for i in range(len(adams))], dtype=torch.int32,
                                     device='cuda')
         assert torch.equal(opt._adam_steps, want), (step, opt._adam_steps.tolist(), want.tolist())

@@ -27,16 +27,16 @@ read.  Allowances are derived from the operation, never fitted to measured error
         slab count mirrored from saicv_token_fill_slabs.
   * Dropout is bit-exact against the kernel's formula evaluated in float64 with one fp32 rounding per operation:
     keep(i) ? x * rn(rn(1 / (1 - p)) * row_scale[i / elems_per_scale]) : +0, then rn(+ resid), then rne to bf16 for a
-    bf16 output.  keep is the counter hash of test_attn_conformance_gpu.py (_keep) on the element index, with the
-    device seed base added to the seed.  Every in / out dtype pair, with and without resid, with row_scale, with
-    seed_base and in place (out is x), as engine/vit.py calls it.
+    bf16 output.  keep is the counter hash (conformance.dropout_keep) on the element index, with the device seed base
+    added to the seed.  Every in / out dtype pair, with and without resid, with row_scale, with seed_base and in place
+    (out is x), as engine/vit.py calls it.
   * GELU on every finite bf16 input (non-finite inputs are out of scope: torch's own fp32 and fp64 GELU disagree at
     +-inf): the bf16 output lies in [rne(g - a), rne(g + a)] with a = GELU_ABS + 2u|g| (the A&S 7.1.26 erf, then
     1 - h and x * cdf round).  GELU_ABS bounds |gelu_erf - gelu|: gelu_math.cuh gives <= 2.2e-7 in float64 for
     |x| <= 12, 4e-7 here.  It is an absolute allowance: below x ~ -6, |gelu| < 1e-8 and a relative bound would be
     meaningless.  The backward, gelu_erf_grad, runs in the GEMM epilogue (test_gemm_conformance_gpu.py).
-Every element must conform; no fraction may miss.  Outputs a wrapper would allocate with torch.empty are allocated
-here, filled with NaN, and passed to the C entry through _lib.call, so an element that is never written fails.
+Outputs a wrapper would allocate with torch.empty are allocated here, filled with NaN, and passed to the C entry
+directly, so an element that is never written fails.
 
 Shapes are the runtime's (ViT-B/L/H at batch 256, the MAE encoder and decoder, SAM-B/H windows and rel-pos grids,
 DETR queries and a 25 x 34 feature map) plus ragged ones.  Every kernel has at least one case with more items than one
@@ -47,94 +47,41 @@ launch mirrors.
 Invariants (raw bits): two consecutive launches give identical outputs; with accumulate the output is a first call
 plus the second call's value (within the allowance); each C entry's documented refusals raise and launch nothing.
 
-Each check prints the largest fraction of its allowance an element used (0 for a bit-exact check); at the end of the
-module the largest share per family is printed (run with -s).  Measured on an NVIDIA H100 80GB HBM3 at a 700 W power
-limit: the rel-pos dq_combine uses 96 % of its allowance (a correctly rounded fmaf may use all of it), token_pool_bwd
-85 %, assemble_tokens_bwd 56 %, GELU 34 %, token_pool_fwd 16 %, the fill gradient 3 %.  The file runs in about 11 s.
+Largest shares of the allowance, measured on an NVIDIA H100 80GB HBM3 at a 700 W power limit: the rel-pos dq_combine
+uses 96 % of its allowance (a correctly rounded fmaf may use all of it), token_pool_bwd 85 %, assemble_tokens_bwd 56 %,
+GELU 34 %, token_pool_fwd 16 %, the fill gradient 3 %.  The file runs in about 11 s.
 """
-import importlib.util
-import os
 import re
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-HERE = os.path.dirname(os.path.abspath(__file__))
+from conformance import (M32, U, call, check, drop_scale, dropout_keep, every_bf16, exact, f32, nan, rand, randn, rnd,
+                         rne_bf16, same)
+from conformance import report  # noqa: F401  (autouse: this module's allowance report)
 
-
-def _load(name, fname):
-    spec = importlib.util.spec_from_file_location(name, os.path.join(HERE, fname))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-_gemm = _load('gemm_conformance', 'test_gemm_conformance_gpu.py')
-_attn = _load('attn_conformance', 'test_attn_conformance_gpu.py')
-_norm = _load('norm_conformance', 'test_norm_conformance_gpu.py')
-_rne_bf16 = _gemm._rne_bf16
-_keep, _drop_scale = _attn._keep, _attn._drop_scale       # _keep: the counter hash against _threshold(p)
-_every_bf16, _check, _same, _nan, _randn, _rand = _norm._every_bf16, _norm._check, _norm._same, _norm._nan, _norm._randn, _norm._rand
-USED = _norm.USED       # this module's own copy of the norm module: only the checks below record into it
+from simpleaicv_pytorch_training_examples_b200 import _lib, ops
 
 gpu = pytest.mark.gpu
 
-U = 2.0 ** -24          # one fp32 rounding, relative
 GELU_ABS = 4e-7         # |gelu_erf - gelu| of the A&S 7.1.26 formula, plus margin
-M32 = 0xFFFFFFFF
 CAP = 132 * 16 * 256    # items one sweep of grid_1d covers (132 * 16 blocks of 256 threads)
 FILL_SLAB_ROWS, FILL_MAX_SLABS = 512, 128
 BF16, F32 = torch.bfloat16, torch.float32
 
 
-def _ops():
-    from simpleaicv_pytorch_training_examples_b200 import ops
-    return ops
-
-
-def _libmod():
-    from simpleaicv_pytorch_training_examples_b200 import _lib
-    return _lib
-
-
-def _c(name, *args):
-    """Call C entry `name` on the current stream; tensors are passed as pointers, None as a null pointer."""
-    ops = _ops()
-    _libmod().call(name, *[ops._p(a) if isinstance(a, torch.Tensor) else a for a in args], ops._stream())
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _report():
-    yield
-    if USED:
-        print('\nlargest share of the allowance used, by family (0: bit-exact):')
-        for k in sorted(USED):
-            print(f'  {k:28s} {USED[k]:.3g}')
-
-
-def _exact(fam, what, out, ref):
-    _same(what, out, ref)
-    USED.setdefault(fam, 0.0)
-    print(f'{what}: bit-exact')
-
-
 def _bf(t):
     """rne_bf16 of an fp32 / float64 tensor, as bf16."""
-    return _rne_bf16(t.double()).to(BF16)
-
-
-def _f32(x):
-    return float(np.float32(x))
+    return rne_bf16(t.double()).to(BF16)
 
 
 def _nanb(*shape):
-    return _nan(*shape, dtype=BF16)
+    return nan(*shape, dtype=BF16)
 
 
 def _randb(*shape, seed=0, scale=1.0):
-    return (_randn(*shape, seed=seed) * scale).to(BF16)
+    return randn(*shape, scale=scale, seed=seed).to(BF16)
 
 
 # ------------------------------------------------------------------ launch mirrors
@@ -178,7 +125,6 @@ HEADS = [  # B, L, ld / C, col0 / C, extra from a tensor, scale
 
 def _wrap_items():
     """Items of each kernel's largest case, per the launches of its C entry."""
-    ops = _ops()
     dqk = lambda s: ops.relpos_dqk(s[2], s[0], s[1])           # noqa: E731
     nip = lambda s: ops.relpos_nip(s[0], s[1])                 # noqa: E731
     nw = lambda h, w, ws: -(-h // ws) * -(-w // ws)            # noqa: E731
@@ -211,7 +157,7 @@ def test_cases_wrap_every_grid_cpu():
     rows = max(b * 197 for b, _ in MAE_DEC)
     nslab = _fill_slabs(rows)
     assert nslab == FILL_MAX_SLABS and -(-rows // nslab) > FILL_SLAB_ROWS
-    lib = _libmod().load()
+    lib = _lib.load()
     for r in (1, 2, 511, 512, 513, 12800, 50432, 65535, 65536, 65537, 100864, 10 ** 7):
         assert lib.saicv_token_fill_slabs(r) == _fill_slabs(r), r
 
@@ -224,19 +170,19 @@ def _gelu64(x):
 @gpu
 def test_gelu_on_every_bf16_input():
     """gelu_erf (forward) on every finite bf16 value."""
-    u = _every_bf16(256)
+    u = every_bf16(256)
     n = u.numel()
     g = _gelu64(u.double())
 
     def run():
         o = {'h': _nanb(*u.shape)}
-        _c('saicv_gelu_fwd', u, o['h'], n)
+        call('saicv_gelu_fwd', u, o['h'], n)
         return o
 
     o = run()
-    _check('gelu', 'gelu forward on every bf16 input', o['h'], g, GELU_ABS + 2 * U * g.abs())
+    check('gelu', 'gelu forward on every bf16 input', o['h'], g, GELU_ABS + 2 * U * g.abs())
     for k, t in run().items():
-        _same(f'gelu {k} on a second launch', t, o[k])
+        same(f'gelu {k} on a second launch', t, o[k])
 
 
 @gpu
@@ -245,9 +191,9 @@ def test_gelu_streams_conform(n):
     """The MLP hidden activation of ViT-B/16 at batch 64: the grid-stride loop wraps nine times."""
     u = _randb(n, seed=2, scale=2.0)
     h = _nanb(n)
-    _c('saicv_gelu_fwd', u, h, n)
+    call('saicv_gelu_fwd', u, h, n)
     g = _gelu64(u.double())
-    _check('gelu', f'gelu forward n {n}', h, g, GELU_ABS + 2 * U * g.abs())
+    check('gelu', f'gelu forward n {n}', h, g, GELU_ABS + 2 * U * g.abs())
 
 
 # ------------------------------------------------------------------ dropout
@@ -255,8 +201,8 @@ def _dropout_ref(x, p, seed, resid, row_scale, eps, out_f32):
     """The kernel's formula with one fp32 rounding per operation (float64 products / sums of fp32 values, rounded)."""
     n = x.numel()
     j = torch.arange(n, device='cuda', dtype=torch.int64)
-    keep = _keep(seed, j & M32, j >> 32, p)
-    inv = _drop_scale(p)
+    keep = dropout_keep(seed, j & M32, j >> 32, p)
+    inv = drop_scale(p)
     if row_scale is not None:
         sc = (inv * row_scale.double()).float().double()[j // eps]
     else:
@@ -274,10 +220,10 @@ def _dropout_ref(x, p, seed, resid, row_scale, eps, out_f32):
 def test_dropout_values_conform(case):
     """saicv_dropout values and mask, bit for bit, over the four dtype variants, resid, row_scale, seed_base, in place."""
     name, n, in_f32, out_f32, with_resid, eps, inplace, p, seed, with_base = case
-    x = _randn(n, seed=10) * 3
+    x = randn(n, seed=10) * 3
     x = x if in_f32 else x.to(BF16)
-    resid = _randn(n, seed=11) if with_resid else None
-    rs = ((_rand(n // eps, seed=12) > 0.2).float() * (_rand(n // eps, seed=13) + 0.5)) if eps else None
+    resid = randn(n, seed=11) if with_resid else None
+    rs = ((rand(n // eps, seed=12) > 0.2).float() * (rand(n // eps, seed=13) + 0.5)) if eps else None
     base = torch.tensor([123456789012345], device='cuda', dtype=torch.int64) if with_base else None
     eff_seed = (seed + (int(base.item()) if with_base else 0)) & ((1 << 64) - 1)
     ref = _dropout_ref(x, p, eff_seed, resid, rs, eps, out_f32)
@@ -288,17 +234,17 @@ def test_dropout_values_conform(case):
             out = x.clone()
             src = out
         else:
-            out = _nan(n, dtype=F32 if out_f32 else BF16)
+            out = nan(n, dtype=F32 if out_f32 else BF16)
             src = x
-        _c('saicv_dropout', src, int(in_f32), resid, rs, eps, out, int(out_f32), n, p, seed, base)
+        call('saicv_dropout', src, int(in_f32), resid, rs, eps, out, int(out_f32), n, p, seed, base)
         return out
 
     out = run()
-    _exact('dropout', f'dropout {name} (n {n}, p {p})', out, ref)
+    exact('dropout', f'dropout {name} (n {n}, p {p})', out, ref)
     if p > 0 and resid is None and n > 10 ** 5:
         kept = (out != 0).double().mean().item()
         assert abs(kept - (1 - p)) < 0.01, f'{name}: kept fraction {kept}'
-    _same(f'dropout {name} on a second launch', run(), out)
+    same(f'dropout {name} on a second launch', run(), out)
 
 
 # ------------------------------------------------------------------ ViT token assembly
@@ -307,35 +253,35 @@ def test_dropout_values_conform(case):
 def test_assemble_tokens_conforms(b, np_, c):
     """saicv_vit_assemble_tokens (fp32 add, bit-exact) and its backward: dpatch = rne(dx), dpos / dcls sum over the batch,
     then a second backward accumulated onto the first (engine/vit.py passes accumulate when the sink holds a gradient)."""
-    patch, cls, pos = _randn(b * np_, c, seed=20), _randn(c, seed=21), _randn(np_ + 1, c, seed=22)
-    dx1 = _randn(b, np_ + 1, c, seed=23) * (_rand(1, np_ + 1, c, seed=24) * 4)
-    dx2 = _randn(b, np_ + 1, c, seed=25)
+    patch, cls, pos = randn(b * np_, c, seed=20), randn(c, seed=21), randn(np_ + 1, c, seed=22)
+    dx1 = randn(b, np_ + 1, c, seed=23) * (rand(1, np_ + 1, c, seed=24) * 4)
+    dx2 = randn(b, np_ + 1, c, seed=25)
     what = f'assemble B {b} NP {np_} C {c}'
 
     def run():
-        o = {'x': _nan(b, np_ + 1, c), 'dpos': _nan(np_ + 1, c), 'dcls': _nan(c), 'dpatch': _nanb(b * np_, c),
+        o = {'x': nan(b, np_ + 1, c), 'dpos': nan(np_ + 1, c), 'dcls': nan(c), 'dpatch': _nanb(b * np_, c),
              'dpatch2': _nanb(b * np_, c)}
-        _c('saicv_vit_assemble_tokens', patch, cls, pos, o['x'], b, np_, c)
-        _c('saicv_vit_assemble_tokens_bwd', dx1, o['dpos'], o['dcls'], o['dpatch'], b, np_, c, 0)
+        call('saicv_vit_assemble_tokens', patch, cls, pos, o['x'], b, np_, c)
+        call('saicv_vit_assemble_tokens_bwd', dx1, o['dpos'], o['dcls'], o['dpatch'], b, np_, c, 0)
         o['dpos1'], o['dcls1'] = o['dpos'].clone(), o['dcls'].clone()
-        _c('saicv_vit_assemble_tokens_bwd', dx2, o['dpos'], o['dcls'], o['dpatch2'], b, np_, c, 1)
+        call('saicv_vit_assemble_tokens_bwd', dx2, o['dpos'], o['dcls'], o['dpatch2'], b, np_, c, 1)
         return o
 
     o = run()
     src = torch.cat([cls.expand(b, 1, c), patch.view(b, np_, c)], 1)
-    _exact('assemble_tokens', f'{what} x', o['x'], (src.double() + pos.double()).float())
-    _exact('assemble_tokens_bwd', f'{what} dpatch', o['dpatch'], _bf(dx1[:, 1:].reshape(b * np_, c)))
-    _exact('assemble_tokens_bwd', f'{what} dpatch (second call)', o['dpatch2'], _bf(dx2[:, 1:].reshape(b * np_, c)))
+    exact('assemble_tokens', f'{what} x', o['x'], (src.double() + pos.double()).float())
+    exact('assemble_tokens_bwd', f'{what} dpatch', o['dpatch'], _bf(dx1[:, 1:].reshape(b * np_, c)))
+    exact('assemble_tokens_bwd', f'{what} dpatch (second call)', o['dpatch2'], _bf(dx2[:, 1:].reshape(b * np_, c)))
     s, a = dx1.double().sum(0), b * U * dx1.double().abs().sum(0)
-    _check('assemble_tokens_bwd', f'{what} dpos', o['dpos1'], s, a)
-    _same(f'{what} dcls is dpos[0]', o['dcls1'], o['dpos1'][0])
+    check('assemble_tokens_bwd', f'{what} dpos', o['dpos1'], s, a)
+    same(f'{what} dcls is dpos[0]', o['dcls1'], o['dpos1'][0])
     s2, a2 = dx2.double().sum(0), b * U * dx2.double().abs().sum(0)
     v = o['dpos1'].double() + s2
-    _check('assemble_tokens_bwd', f'{what} dpos (accumulate)', o['dpos'], v, _norm._rnd(v, a2))
+    check('assemble_tokens_bwd', f'{what} dpos (accumulate)', o['dpos'], v, rnd(v, a2))
     v = o['dcls1'].double() + s2[0]
-    _check('assemble_tokens_bwd', f'{what} dcls (accumulate)', o['dcls'], v, _norm._rnd(v, a2[0]))
+    check('assemble_tokens_bwd', f'{what} dcls (accumulate)', o['dcls'], v, rnd(v, a2[0]))
     for k, t in run().items():
-        _same(f'{what} {k} on a second launch', t, o[k])
+        same(f'{what} {k} on a second launch', t, o[k])
 
 
 # ------------------------------------------------------------------ ViT token pooling
@@ -344,15 +290,15 @@ def test_assemble_tokens_conforms(b, np_, c):
 def test_token_pool_conforms(b, l, c, mean, scaled):
     """saicv_token_pool_fwd / _bwd: mean over tokens 1 .. L-1 or the cls token; the backward's fp32 dx and its bf16 copy
     times the next block's drop-path scale (bf16_row_scale, per batch element)."""
-    x = _randn(b, l, c, seed=30) * 2 + _randn(1, 1, c, seed=31)
-    dp = _randn(b, c, seed=32)
-    rs = (_rand(b, seed=33) > 0.25).float() * (_rand(b, seed=34) + 0.5) if scaled else None
+    x = randn(b, l, c, seed=30) * 2 + randn(1, 1, c, seed=31)
+    dp = randn(b, c, seed=32)
+    rs = (rand(b, seed=33) > 0.25).float() * (rand(b, seed=34) + 0.5) if scaled else None
     what = f'pool B {b} L {l} C {c} {"mean" if mean else "cls"}{" scaled" if scaled else ""}'
 
     def run():
-        o = {'pooled': _nan(b, c), 'dx': _nan(b, l, c), 'dxb': _nanb(b, l, c)}
-        _c('saicv_token_pool_fwd', x, o['pooled'], b, l, c, mean)
-        _c('saicv_token_pool_bwd', dp, o['dx'], o['dxb'], rs, b, l, c, mean)
+        o = {'pooled': nan(b, c), 'dx': nan(b, l, c), 'dxb': _nanb(b, l, c)}
+        call('saicv_token_pool_fwd', x, o['pooled'], b, l, c, mean)
+        call('saicv_token_pool_bwd', dp, o['dx'], o['dxb'], rs, b, l, c, mean)
         return o
 
     o = run()
@@ -363,25 +309,25 @@ def test_token_pool_conforms(b, l, c, mean, scaled):
         a_s = (l - 1) * U * t.abs().sum(1) / (l - 1)
         v = t.sum(1) / (l - 1)
         del t
-        _check('token_pool_fwd', f'{what} pooled', o['pooled'], v, _norm._rnd(v, a_s))
+        check('token_pool_fwd', f'{what} pooled', o['pooled'], v, rnd(v, a_s))
         v = dp.double() / (l - 1)
-        a = _norm._rnd(v, U * v.abs())                       # rn(1 / (L - 1)), then the product
-        _check('token_pool_bwd', f'{what} dx', o['dx'][:, 1:], v[:, None].expand(b, l - 1, c), a[:, None])
-        _exact('token_pool_bwd', f'{what} dx token 0', o['dx'][:, 0], zf)
+        a = rnd(v, U * v.abs())                       # rn(1 / (L - 1)), then the product
+        check('token_pool_bwd', f'{what} dx', o['dx'][:, 1:], v[:, None].expand(b, l - 1, c), a[:, None])
+        exact('token_pool_bwd', f'{what} dx token 0', o['dx'][:, 0], zf)
         w = v * r
-        _check('token_pool_bwd', f'{what} dx bf16', o['dxb'][:, 1:], w[:, None].expand(b, l - 1, c),
-               _norm._rnd(w, a * r)[:, None])
-        _exact('token_pool_bwd', f'{what} dx bf16 token 0', o['dxb'][:, 0], zb)
+        check('token_pool_bwd', f'{what} dx bf16', o['dxb'][:, 1:], w[:, None].expand(b, l - 1, c),
+              rnd(w, a * r)[:, None])
+        exact('token_pool_bwd', f'{what} dx bf16 token 0', o['dxb'][:, 0], zb)
     else:
-        _exact('token_pool_fwd', f'{what} pooled', o['pooled'], x[:, 0])
-        _exact('token_pool_bwd', f'{what} dx token 0', o['dx'][:, 0], dp)
-        _exact('token_pool_bwd', f'{what} dx tokens 1..', o['dx'][:, 1:], torch.zeros(b, l - 1, c, device='cuda'))
+        exact('token_pool_fwd', f'{what} pooled', o['pooled'], x[:, 0])
+        exact('token_pool_bwd', f'{what} dx token 0', o['dx'][:, 0], dp)
+        exact('token_pool_bwd', f'{what} dx tokens 1..', o['dx'][:, 1:], torch.zeros(b, l - 1, c, device='cuda'))
         w = dp.double() * r
-        _check('token_pool_bwd', f'{what} dx bf16 token 0', o['dxb'][:, 0], w, U * w.abs())
-        _exact('token_pool_bwd', f'{what} dx bf16 tokens 1..', o['dxb'][:, 1:],
-               torch.zeros(b, l - 1, c, device='cuda', dtype=BF16))
+        check('token_pool_bwd', f'{what} dx bf16 token 0', o['dxb'][:, 0], w, U * w.abs())
+        exact('token_pool_bwd', f'{what} dx bf16 tokens 1..', o['dxb'][:, 1:],
+              torch.zeros(b, l - 1, c, device='cuda', dtype=BF16))
     for k, t in run().items():
-        _same(f'{what} {k} on a second launch', t, o[k])
+        same(f'{what} {k} on a second launch', t, o[k])
 
 
 # ------------------------------------------------------------------ MAE token gather / scatter
@@ -389,19 +335,19 @@ def _fill_grad(fam, what, dout, idx, dfill):
     """dfill (fp32 [C]) against the exact sum of the dout rows with idx < 0."""
     rows, c = idx.numel(), dout.shape[-1]
     t = dout.reshape(rows, c)[idx.flatten() < 0].double()
-    _check(fam, f'{what} dfill', dfill, t.sum(0), _fill_depth(rows) * U * t.abs().sum(0))
+    check(fam, f'{what} dfill', dfill, t.sum(0), _fill_depth(rows) * U * t.abs().sum(0))
 
 
 def _gather_bwd(dout, idx, src_rows, b, r, c, bf16, dsrc):
     nslab = _fill_slabs(b * r)
-    part, dfill = _nan(nslab, c), _nan(c)
-    _c('saicv_token_gather_bwd', dout, idx, dsrc, int(bf16), src_rows, part, b, r, c)
-    _c('saicv_reduce_partials', part, dfill, nslab, c, 0)
+    part, dfill = nan(nslab, c), nan(c)
+    call('saicv_token_gather_bwd', dout, idx, dsrc, int(bf16), src_rows, part, b, r, c)
+    call('saicv_reduce_partials', part, dfill, nslab, c, 0)
     return dsrc, dfill
 
 
 def _shuffle(b, n, seed):
-    ids_shuffle = _rand(b, n, seed=seed).argsort(1)
+    ids_shuffle = rand(b, n, seed=seed).argsort(1)
     return ids_shuffle, ids_shuffle.argsort(1)
 
 
@@ -416,13 +362,13 @@ def test_mae_encoder_gather_conforms(b, c):
     minus = torch.full((b, 1), -1, device='cuda', dtype=torch.int64)
     idx = torch.cat([minus, ids_keep], 1).int().contiguous()
     pos_idx = torch.cat([minus + 1, ids_keep + 1], 1).int().contiguous()
-    src, cls, pos = _randn(b, n, c, seed=41), _randn(c, seed=42), _randn(n + 1, c, seed=43)
-    dout = _randn(b, r, c, seed=44)
+    src, cls, pos = randn(b, n, c, seed=41), randn(c, seed=42), randn(n + 1, c, seed=43)
+    dout = randn(b, r, c, seed=44)
     what = f'mae encoder B {b} C {c}'
 
     def run():
-        o = {'out': _nan(b, r, c)}
-        _c('saicv_token_gather_fwd', src, n, idx, cls, pos, pos_idx, o['out'], b, r, c)
+        o = {'out': nan(b, r, c)}
+        call('saicv_token_gather_fwd', src, n, idx, cls, pos, pos_idx, o['out'], b, r, c)
         for dt in (F32, BF16):
             o[f'dsrc {dt}'], o[f'dfill {dt}'] = _gather_bwd(dout, idx, n, b, r, c, dt == BF16,
                                                             torch.zeros(b, n, c, device='cuda', dtype=dt))
@@ -430,15 +376,15 @@ def test_mae_encoder_gather_conforms(b, c):
 
     o = run()
     rows = torch.cat([cls.expand(b, 1, c), src.gather(1, ids_keep[:, :, None].expand(b, keep, c))], 1)
-    _exact('token_gather_fwd', f'{what} out', o['out'], (rows.double() + pos[pos_idx.long()].double()).float())
+    exact('token_gather_fwd', f'{what} out', o['out'], (rows.double() + pos[pos_idx.long()].double()).float())
     ref = torch.zeros(b, n, c, device='cuda').scatter(1, ids_keep[:, :, None].expand(b, keep, c), dout[:, 1:])
-    _exact('token_gather_bwd', f'{what} dsrc fp32', o[f'dsrc {F32}'], ref)
-    _exact('token_gather_bwd', f'{what} dsrc bf16', o[f'dsrc {BF16}'], _bf(ref))
+    exact('token_gather_bwd', f'{what} dsrc fp32', o[f'dsrc {F32}'], ref)
+    exact('token_gather_bwd', f'{what} dsrc bf16', o[f'dsrc {BF16}'], _bf(ref))
     for dt in (F32, BF16):
         _fill_grad('token_fill_grad', f'{what} ({dt})', dout, idx, o[f'dfill {dt}'])
-        _same(f'{what} dfill does not depend on the dsrc dtype', o[f'dfill {dt}'], o[f'dfill {F32}'])
+        same(f'{what} dfill does not depend on the dsrc dtype', o[f'dfill {dt}'], o[f'dfill {F32}'])
     for k, t in run().items():
-        _same(f'{what} {k} on a second launch', t, o[k])
+        same(f'{what} {k} on a second launch', t, o[k])
 
 
 @gpu
@@ -452,33 +398,33 @@ def test_mae_decoder_unshuffle_conforms(b, c):
     restore = _shuffle(b, n, 50)[1]
     idx = torch.cat([torch.zeros(b, 1, device='cuda', dtype=torch.int64),
                      torch.where(restore < keep, restore + 1, -1)], 1).int().contiguous()
-    y, mask, pos = _randn(b, le, c, seed=51), _randn(c, seed=52), _randn(r, c, seed=53)
-    dout = _randn(b, r, c, seed=54) * (_rand(1, r, 1, seed=55) * 4)
+    y, mask, pos = randn(b, le, c, seed=51), randn(c, seed=52), randn(r, c, seed=53)
+    dout = randn(b, r, c, seed=54) * (rand(1, r, 1, seed=55) * 4)
     what = f'mae decoder B {b} C {c}'
 
     def run():
-        o = {'out': _nan(b, r, c)}
-        _c('saicv_token_gather_fwd', y, le, idx, mask, pos, None, o['out'], b, r, c)
+        o = {'out': nan(b, r, c)}
+        call('saicv_token_gather_fwd', y, le, idx, mask, pos, None, o['out'], b, r, c)
         for dt in (F32, BF16):
             o[f'dsrc {dt}'], o[f'dfill {dt}'] = _gather_bwd(dout, idx, le, b, r, c, dt == BF16,
-                                                            _nan(b, le, c, dtype=dt))
+                                                            nan(b, le, c, dtype=dt))
         return o
 
     o = run()
     il = idx.long()
     rows = torch.where(il[:, :, None] >= 0, y.gather(1, il.clamp_min(0)[:, :, None].expand(b, r, c)), mask)
-    _exact('token_gather_fwd', f'{what} out', o['out'], (rows.double() + pos.double()).float())
+    exact('token_gather_fwd', f'{what} out', o['out'], (rows.double() + pos.double()).float())
     # the inverse map: source row s of batch b came from output row src_of[b, s]
     src_of = torch.empty(b, le, device='cuda', dtype=torch.int64)
     live = il >= 0
     src_of[live.nonzero()[:, 0], il[live]] = live.nonzero()[:, 1]
     ref = dout.gather(1, src_of[:, :, None].expand(b, le, c))
-    _exact('token_gather_bwd', f'{what} dsrc fp32', o[f'dsrc {F32}'], ref)
-    _exact('token_gather_bwd', f'{what} dsrc bf16', o[f'dsrc {BF16}'], _bf(ref))
+    exact('token_gather_bwd', f'{what} dsrc fp32', o[f'dsrc {F32}'], ref)
+    exact('token_gather_bwd', f'{what} dsrc bf16', o[f'dsrc {BF16}'], _bf(ref))
     for dt in (F32, BF16):
         _fill_grad('token_fill_grad', f'{what} ({dt})', dout, idx, o[f'dfill {dt}'])
     for k, t in run().items():
-        _same(f'{what} {k} on a second launch', t, o[k])
+        same(f'{what} {k} on a second launch', t, o[k])
 
 
 # ------------------------------------------------------------------ SAM windows and positional embedding
@@ -494,34 +440,34 @@ def test_window_partition_conforms(b, h, w, c, ws):
 
     def run():
         o = {'win': _nanb(b * nwy * nwx, ws * ws, c), 'x': _nanb(b, h, w, c)}
-        _c('saicv_window_partition', x, o['win'], b, h, w, c, ws)
-        _c('saicv_window_unpartition', win, o['x'], b, h, w, c, ws)
+        call('saicv_window_partition', x, o['win'], b, h, w, c, ws)
+        call('saicv_window_unpartition', win, o['x'], b, h, w, c, ws)
         return o
 
     o = run()
     xp = F.pad(x, (0, 0, 0, nwx * ws - w, 0, nwy * ws - h))
     ref = xp.view(b, nwy, ws, nwx, ws, c).permute(0, 1, 3, 2, 4, 5).reshape(b * nwy * nwx, ws * ws, c)
-    _exact('window partition', f'{what} partition', o['win'], ref)
+    exact('window partition', f'{what} partition', o['win'], ref)
     ref = win.view(b, nwy, nwx, ws, ws, c).permute(0, 1, 3, 2, 4, 5).reshape(b, nwy * ws, nwx * ws, c)[:, :h, :w]
-    _exact('window partition', f'{what} unpartition', o['x'], ref.contiguous())
+    exact('window partition', f'{what} unpartition', o['x'], ref.contiguous())
     for k, t in run().items():
-        _same(f'{what} {k} on a second launch', t, o[k])
+        same(f'{what} {k} on a second launch', t, o[k])
 
 
 @gpu
 @pytest.mark.parametrize('b,per', ADDPOS)
 def test_add_pos_embed_conforms(b, per):
     """saicv_add_pos_embed: x += pos broadcast over the batch, in place, one fp32 add."""
-    x0, pos = _randn(b, per, seed=70) * 2, _randn(per, seed=71) * 0.1
+    x0, pos = randn(b, per, seed=70) * 2, randn(per, seed=71) * 0.1
 
     def run():
         x = x0.clone()
-        _c('saicv_add_pos_embed', x, pos, b, per)
+        call('saicv_add_pos_embed', x, pos, b, per)
         return x
 
     x = run()
-    _exact('add_pos_embed', f'add_pos_embed B {b} per {per}', x, (x0.double() + pos.double()).float())
-    _same(f'add_pos_embed B {b} per {per} on a second launch', run(), x)
+    exact('add_pos_embed', f'add_pos_embed B {b} per {per}', x, (x0.double() + pos.double()).float())
+    same(f'add_pos_embed B {b} per {per} on a second launch', run(), x)
 
 
 # ------------------------------------------------------------------ SAM rel-pos score columns
@@ -535,35 +481,34 @@ def _grid_index(sh, sw):
 def test_relpos_kernels_conform(sh, sw, hd, bw, heads):
     """relpos_pack_q, relpos_table, relpos_gather, relpos_shift and relpos_dq_combine at dqk = relpos_dqk and
     nip = relpos_nip.  The (5, 9) grid is the case in which a swap of Sh and Sw in the index maths shows."""
-    ops = _ops()
     L = sh * sw
     dqk, nip = ops.relpos_dqk(hd, sh, sw), ops.relpos_nip(sh, sw)
     nh, nw = 2 * sh - 1, 2 * sw - 1
     rows = bw * heads * L
-    scale = _f32(hd ** -0.5)
+    scale = f32(hd ** -0.5)
     qkv = _randb(bw, L, 3, heads, hd, seed=80)
-    rph, rpw = _randn(nh, hd, seed=81) * 0.1, _randn(nw, hd, seed=82)
+    rph, rpw = randn(nh, hd, seed=81) * 0.1, randn(nw, hd, seed=82)
     T = _randb(rows, nip, seed=83)
     dqe = _randb(rows, dqk, seed=84)
-    dqx = _randn(rows, hd, seed=85)
+    dqx = randn(rows, hd, seed=85)
     what = f'relpos {sh}x{sw} hd {hd} windows {bw} heads {heads}'
 
     def run():
         o = {'qc': _nanb(rows, hd), 'rtab': _nanb(nip, hd), 'qe': _nanb(rows, dqk), 'ke': _nanb(rows, dqk),
              'ef': _nanb(rows, nip), 'dqkv': _nanb(bw, L, 3, heads, hd)}
-        _c('saicv_relpos_pack_q', qkv, o['qc'], bw, heads, hd, L)
-        _c('saicv_relpos_table', rph, rpw, o['rtab'], sh, sw, nip, hd)
-        _c('saicv_relpos_gather', qkv, T, o['qe'], o['ke'], bw, heads, hd, sh, sw, dqk, nip, scale)
-        _c('saicv_relpos_shift', dqe, o['ef'], bw, heads, hd, sh, sw, dqk, nip)
-        _c('saicv_relpos_dq_combine', dqe, dqx, o['dqkv'], bw, heads, hd, L, dqk, scale)
+        call('saicv_relpos_pack_q', qkv, o['qc'], bw, heads, hd, L)
+        call('saicv_relpos_table', rph, rpw, o['rtab'], sh, sw, nip, hd)
+        call('saicv_relpos_gather', qkv, T, o['qe'], o['ke'], bw, heads, hd, sh, sw, dqk, nip, scale)
+        call('saicv_relpos_shift', dqe, o['ef'], bw, heads, hd, sh, sw, dqk, nip)
+        call('saicv_relpos_dq_combine', dqe, dqx, o['dqkv'], bw, heads, hd, L, dqk, scale)
         return o
 
     o = run()
     per_head = lambda t: t.permute(0, 2, 1, 3).reshape(rows, hd)           # noqa: E731  [bw, L, H, hd] -> rows
     q, k = per_head(qkv[:, :, 0]), per_head(qkv[:, :, 1])
-    _exact('relpos layout', f'{what} pack_q', o['qc'], q)
-    _exact('relpos layout', f'{what} table', o['rtab'],
-           _bf(torch.cat([rph, rpw, torch.zeros(nip - nh - nw, hd, device='cuda')])))
+    exact('relpos layout', f'{what} pack_q', o['qc'], q)
+    exact('relpos layout', f'{what} table', o['rtab'],
+          _bf(torch.cat([rph, rpw, torch.zeros(nip - nh - nw, hd, device='cuda')])))
     # gather: Qe = [q * scale | T[qh - kh + Sh - 1] | T[nh + qw - kw + Sw - 1] | 0],  Ke = [k | onehot(qh) | onehot(qw) | 0]
     qh, qw = _grid_index(sh, sw)
     col_h = qh[:, None] - torch.arange(sh, device='cuda')[None] + sh - 1
@@ -572,10 +517,10 @@ def test_relpos_kernels_conform(sh, sw, hd, bw, heads):
     bias = T.view(bw * heads, L, nip).gather(2, cols).reshape(rows, sh + sw)
     pad = torch.zeros(rows, dqk - hd - sh - sw, device='cuda', dtype=BF16)
     v = q.double() * scale
-    _check('relpos scale', f'{what} Qe q * scale', o['qe'][:, :hd], v, U * v.abs())
-    _exact('relpos layout', f'{what} Qe bias columns', o['qe'][:, hd:], torch.cat([bias, pad], 1))
+    check('relpos scale', f'{what} Qe q * scale', o['qe'][:, :hd], v, U * v.abs())
+    exact('relpos layout', f'{what} Qe bias columns', o['qe'][:, hd:], torch.cat([bias, pad], 1))
     onehot = torch.cat([F.one_hot(qh, sh), F.one_hot(qw, sw)], 1).to(BF16).repeat(bw * heads, 1)
-    _exact('relpos layout', f'{what} Ke', o['ke'], torch.cat([k, onehot, pad], 1))
+    exact('relpos layout', f'{what} Ke', o['ke'], torch.cat([k, onehot, pad], 1))
     # shift: ef[r][idx] = dT_h[kh] for kh = qh - idx + Sh - 1 in the grid, ef[r][nh + idx] = dT_w[kw], else +0
     idx = torch.arange(nip, device='cuda')[None]
     kh = qh[:, None] - idx + sh - 1
@@ -584,13 +529,13 @@ def test_relpos_kernels_conform(sh, sw, hd, bw, heads):
                       torch.where((idx >= nh) & (idx < nh + nw) & (kw >= 0) & (kw < sw), hd + sh + kw, -1))
     g = dqe.view(bw * heads, L, dqk).gather(2, src.clamp_min(0).expand(bw * heads, L, nip)).reshape(rows, nip)
     ok = (src >= 0).repeat(bw * heads, 1)
-    _exact('relpos layout', f'{what} shift', o['ef'], torch.where(ok, g, torch.zeros((), device='cuda', dtype=BF16)))
+    exact('relpos layout', f'{what} shift', o['ef'], torch.where(ok, g, torch.zeros((), device='cuda', dtype=BF16)))
     # dq_combine: q slot = bf16(fmaf(dqe, scale, dqx)); the k and v slots are not written
     v = dqe[:, :hd].double() * scale + dqx.double()
-    _check('relpos scale', f'{what} dq_combine', per_head(o['dqkv'][:, :, 0]), v, U * v.abs())
-    _same(f'{what} dq_combine leaves k, v slots', o['dqkv'][:, :, 1:], _nanb(bw, L, 2, heads, hd))
+    check('relpos scale', f'{what} dq_combine', per_head(o['dqkv'][:, :, 0]), v, U * v.abs())
+    same(f'{what} dq_combine leaves k, v slots', o['dqkv'][:, :, 1:], _nanb(bw, L, 2, heads, hd))
     for key, t in run().items():
-        _same(f'{what} {key} on a second launch', t, o[key])
+        same(f'{what} {key} on a second launch', t, o[key])
 
 
 @gpu
@@ -598,11 +543,11 @@ def test_relpos_table_wraps():
     """relpos_table with a table far longer than its two tables (only +0 rows past 2 Sh - 1 + 2 Sw - 1), so that its
     grid-stride loop wraps: nip * hd items against one sweep of 540,672."""
     sh, sw, hd, nip = RELPOS_TABLE_WRAP
-    rph, rpw = _randn(2 * sh - 1, hd, seed=86), _randn(2 * sw - 1, hd, seed=87)
+    rph, rpw = randn(2 * sh - 1, hd, seed=86), randn(2 * sw - 1, hd, seed=87)
     rtab = _nanb(nip, hd)
-    _c('saicv_relpos_table', rph, rpw, rtab, sh, sw, nip, hd)
+    call('saicv_relpos_table', rph, rpw, rtab, sh, sw, nip, hd)
     ref = torch.cat([rph, rpw, torch.zeros(nip - rph.shape[0] - rpw.shape[0], hd, device='cuda')])
-    _exact('relpos layout', f'relpos table nip {nip} hd {hd}', rtab, _bf(ref))
+    exact('relpos layout', f'relpos table nip {nip} hd {hd}', rtab, _bf(ref))
 
 
 # ------------------------------------------------------------------ DETR per-head packing
@@ -614,43 +559,43 @@ def test_heads_pack_unpack_conform(b, l, ldm, colm, tensor_extra, scale):
     H, hd, dp = DETR_H, DETR_HD, DETR_DP
     C = H * hd
     ld, col0 = ldm * C, colm * C
-    sc = _f32(scale)
+    sc = f32(scale)
     src = _randb(b * l, ld, seed=90, scale=3.0)
-    extra = _randn(b * l, seed=91) * 10 if tensor_extra else None
+    extra = randn(b * l, seed=91) * 10 if tensor_extra else None
     const = -0.3
     packed = _randb(b, H, l, dp, seed=92)
     what = f'heads B {b} L {l} ld {ld} col0 {col0} {"extra" if tensor_extra else "const"} scale {sc:.6g}'
 
     def run():
         o = {'dst': _nanb(b, H, l, dp), 'un': _nanb(b * l, ld)}
-        _c('saicv_heads_pack', src, ld, col0, extra, const, o['dst'], b, l, H, hd, dp, sc)
-        _c('saicv_heads_unpack', packed, o['un'], ld, col0, b, l, H, hd, dp, sc)
+        call('saicv_heads_pack', src, ld, col0, extra, const, o['dst'], b, l, H, hd, dp, sc)
+        call('saicv_heads_unpack', packed, o['un'], ld, col0, b, l, H, hd, dp, sc)
         return o
 
     o = run()
     heads = src.view(b, l, ld)[:, :, col0:col0 + C].view(b, l, H, hd).permute(0, 2, 1, 3)
     if sc == 1.0:
-        _exact('heads layout', f'{what} pack', o['dst'][..., :hd], heads)
+        exact('heads layout', f'{what} pack', o['dst'][..., :hd], heads)
     else:
         v = heads.double() * sc
-        _check('heads scale', f'{what} pack', o['dst'][..., :hd], v, U * v.abs())
+        check('heads scale', f'{what} pack', o['dst'][..., :hd], v, U * v.abs())
     ex = _bf(extra).view(b, 1, l).expand(b, H, l) if tensor_extra else \
-        _bf(torch.full((b, H, l), _f32(const), device='cuda', dtype=torch.float64))
-    _exact('heads layout', f'{what} pack extra column', o['dst'][..., hd], ex)
-    _exact('heads layout', f'{what} pack zero columns', o['dst'][..., hd + 1:],
-           torch.zeros(b, H, l, dp - hd - 1, device='cuda', dtype=BF16))
+        _bf(torch.full((b, H, l), f32(const), device='cuda', dtype=torch.float64))
+    exact('heads layout', f'{what} pack extra column', o['dst'][..., hd], ex)
+    exact('heads layout', f'{what} pack zero columns', o['dst'][..., hd + 1:],
+          torch.zeros(b, H, l, dp - hd - 1, device='cuda', dtype=BF16))
     un = o['un'].view(b, l, ld)
     ref = packed[..., :hd].permute(0, 2, 1, 3).reshape(b, l, C)
     if sc == 1.0:
-        _exact('heads layout', f'{what} unpack', un[:, :, col0:col0 + C], ref)
+        exact('heads layout', f'{what} unpack', un[:, :, col0:col0 + C], ref)
     else:
         v = ref.double() * sc
-        _check('heads scale', f'{what} unpack', un[:, :, col0:col0 + C], v, U * v.abs())
+        check('heads scale', f'{what} unpack', un[:, :, col0:col0 + C], v, U * v.abs())
     outside = torch.ones(ld, dtype=torch.bool, device='cuda')
     outside[col0:col0 + C] = False
     assert torch.isnan(un[:, :, outside].float()).all(), f'{what}: unpack wrote outside its column block'
     for k, t in run().items():
-        _same(f'{what} {k} on a second launch', t, o[k])
+        same(f'{what} {k} on a second launch', t, o[k])
 
 
 # ------------------------------------------------------------------ refusals
@@ -693,12 +638,11 @@ def _refusals(f, i):
 def test_refusals_launch_nothing():
     """Each C entry's documented refusals (C % 4, n % 8, dp <= hd, nip or dqk too small, a row_scale without
     elems_per_scale, p outside [0, 1), ...) return an error before any kernel is launched."""
-    lib = _libmod()
     f = torch.zeros(1 << 20, device='cuda')
     i = torch.zeros(1 << 16, device='cuda', dtype=torch.int32)
     for name, args, msg in _refusals(f, i):
-        n0 = lib.launch_count()
+        n0 = _lib.launch_count()
         with pytest.raises(RuntimeError, match=re.escape(msg)):
-            _c(name, *args)
-        assert lib.launch_count() == n0, f'{name}{args[-6:]}: launched before refusing'
+            call(name, *args)
+        assert _lib.launch_count() == n0, f'{name}{args[-6:]}: launched before refusing'
     torch.cuda.synchronize()
