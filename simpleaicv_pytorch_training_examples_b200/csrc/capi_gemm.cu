@@ -115,15 +115,16 @@ void tune_override(int* bn, int* stages, int* nb) {
 //  * no aux operand: nb = 2 whenever >= 3 stages remain (>= 4 for reductions of 4+ k-blocks) - a TMA store
 //    is then not waited for right after it was issued;
 //  * aux operand by TMA: the slices are also the landing buffers of the next aux tiles, so depth matters more than ring
-//    stages while the reduction is short: <= 4 k-blocks -> nb = 3 / 2+ stages, fp32 tiles of <= 16 k-blocks -> nb = 2 /
-//    3 stages; everything longer keeps 4 stages first.
+//    stages while the reduction is short: <= 4 k-blocks -> nb = 3 / 2+ stages, fp32 tiles of <= 16 k-blocks -> nb = 3 /
+//    3+ stages; everything longer keeps 5 stages first (at BN = 128: 5 stages and nb = 2 rather than 4 and nb = 3, 2-5 %
+//    faster for the ViT-B / ResNet-50 bf16-aux data gradients of 12-18 k-blocks on an H100, DESIGN 2.1).
 template <int BN>
 void pick_smem_split(const GemmParams& p, int stat_bytes, int* stages_out, int* nb_out) {
   using Cfg = GemmCfg<BN>;
   const int budget = kSmemBudget - stat_bytes;
   const bool has_aux = p.aux_tma != 0;
   const int kb = p.kb_per_split;
-  const int min_stages = has_aux ? (kb <= 4 ? 2 : (kb <= 16 && p.out_f32) ? 3 : 4) : (kb >= 4 ? 4 : 3);
+  const int min_stages = has_aux ? (kb <= 4 ? 2 : (kb <= 16 && p.out_f32) ? 3 : 5) : (kb >= 4 ? 4 : 3);
   int nb = has_aux ? 3 : 2;
   while (nb > 1 && (budget - 2 * nb * kStoreBufBytes) / Cfg::kStageBytes < min_stages) --nb;
   int stages = (budget - 2 * nb * kStoreBufBytes) / Cfg::kStageBytes;

@@ -6,9 +6,8 @@
 //   warp 0      TMA producer (one lane)        global -> 128B-swizzled smem ring
 //   warps 1..3  idle (keep the consumers on aligned warpgroups)
 //   warps 4..11 two consumer warpgroups; warpgroup h owns rows h*64 .. h*64+63 and all BN columns of the 128 x BN tile:
-//               wgmma (one m64nBN per k16 step) -> registers -> per-warp transpose through shared memory so that a
-//               thread owns 16 columns of one row -> (bias/act/residual) -> smem slice shared by both warpgroups ->
-//               TMA store by one thread
+//               wgmma (one m64nBN per k16 step) -> registers -> (bias/act/residual) in the accumulator fragment
+//               layout -> stmatrix / 8-byte stores into an smem slice shared by both warpgroups -> TMA store by one thread
 //
 // Operand feeding modes (runtime, so that fprop / dgrad / wgrad of linear layers and of NHWC
 // convolutions all go through this one kernel):
@@ -38,9 +37,7 @@ constexpr int kGemmThreads = 384;  // 4 control warps (TMA producer + 3 idle) + 
 constexpr int kStoreBufBytes = 16384;  // one staging slice: 128 rows x 128 B
 constexpr int kMaxStoreBufs = 3;       // GemmParams::store_bufs (runtime 1..3): the tile's staging pool is 2 * store_bufs slices
 constexpr int kSmemTotal = 232448;     // dynamic shared memory every launch asks for (227 KB)
-constexpr int kXposeStride = 33;       // floats per row of a warp's transpose buffer (32 columns + 1: conflict-free rows)
-constexpr int kXposeBytes = 8 * 32 * kXposeStride * 4;   // two 16 x 32 fp32 buffers (alternating chunks) per consumer warp
-constexpr int kSmemBudget = kSmemTotal - 1024 /*align slack*/ - 512 /*barriers*/ - kXposeBytes;
+constexpr int kSmemBudget = kSmemTotal - 1024 /*align slack*/ - 512 /*barriers*/;
 
 // The split of shared memory between the operand ring and the epilogue staging slices is a launch
 // parameter (capi_gemm.cu: pick_smem_split): long reductions want >= 4 ring stages and get two
@@ -109,7 +106,7 @@ struct GemmParams {
 // Kernel variants: the epilogue's feature set is a compile-time mask, so that the common launches run a compact
 // instruction stream (with every feature a run-time branch, branch resolution and instruction fetch take a large share of
 // the issue slots of the short-reduction launches, whose pace the epilogue sets).  No variant spills (ptxas -v); VAR_FULL
-// and VAR_AUX at BN = 128 sit at the 168-register cap of 384 threads.
+// at BN = 128 sits at the 168-register cap of 384 threads.
 //   VAR_FULL        every flag but EPI_MASK_BITS / EPI_STATS / output type at run time (per-thread aux loads)
 //   VAR_PLAIN_BF16  bf16 output, optional bias / ReLU                                (conv fprop, plain dgrad, Linear)
 //   VAR_PLAIN_F32   fp32 output, optional bias                                       (split-K weight gradients, fp32 Linear)
@@ -240,7 +237,6 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* aux_bar = empty_bar + kStages;   // [2 * kMaxStoreBufs]: aux slice landed in staging slice b
   uint64_t* staged_bar = aux_bar + 2 * kMaxStoreBufs;    // [2 * kMaxStoreBufs] VAR_STATS_BF16: staging slice b is staged
   uint64_t* sdone_bar = staged_bar + 2 * kMaxStoreBufs;  // [2 * kMaxStoreBufs] the four stats warps have read slice b
-  float* sXpose = reinterpret_cast<float*>(smem + kSmemTotal - 1024 - kXposeBytes);   // [8 warps][2][16][kXposeStride]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -385,23 +381,31 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   } else if (warp >= 4 && warp < 12) {
     // ================================================================ consumers: wgmma + epilogue
     // 8 warps: warpgroup `half` = e/4 reduces and drains rows half*64 .. +63 of every tile, all BN columns.  Warp e%4 of it
-    // holds the accumulators of rows half*64 + (e%4)*16 .. +15; after the reduction it transposes each 32-column chunk
-    // through its own shared-memory buffer so that lane l owns columns (l/16)*16 .. +15 of row l%16.  The tile's 2*NB
-    // 16 KB staging slices (128 rows x 128 B = 64 bf16 or 32 fp32 columns, 128B-swizzled) are used round-robin in
-    // ascending column order; both warpgroups write their rows of the same slice, one 256-thread barrier closes it and
-    // the first consumer thread issues its TMA store: slice s is written while the stores of earlier slices still read.
-    // With aux_tma that thread also TMA-loads the aux operand of slice s+LA (LA = 2*NB - 1) into the slice
-    // that store s-1 has released; every thread combines its own piece of a row in place.
+    // holds the accumulators of rows half*64 + (e%4)*16 .. +15 in the wgmma fragment layout (ptx.cuh): lane l has rows
+    // l/4 and l/4 + 8 of them, column pairs 8j + 2*(l%4) + {0, 1}.  The epilogue runs in that layout and writes straight
+    // into the staging slices: bf16 by stmatrix (one 16 x 16 block per x4), fp32 by 8-byte stores; a bf16 aux operand
+    // comes back in the same layout by ldmatrix.  The tile's 2*NB 16 KB staging slices (128 rows x 128 B = 64 bf16 or 32
+    // fp32 columns, 128B-swizzled) are used round-robin in ascending column order; both warpgroups write their rows of the
+    // same slice, one 256-thread barrier closes it and the first consumer thread issues its TMA store: slice s is written
+    // while the stores of earlier slices still read.  With aux_tma that thread also TMA-loads the aux operand of slice
+    // s+LA (LA = 2*NB - 1) into the slice that store s-1 has released; every thread combines its own fragments in place.
     const int e = warp - 4;
     const int q = e & 3;
     const int half = e >> 2;
     const bool leader = threadIdx.x == 128;           // issues the TMA stores and the aux requests of the tile
-    const int hh = lane >> 4;                         // which 16 columns of a 32-column chunk this thread owns
-    const int row_in_tile = half * 64 + q * 16 + (lane & 15);
-    const int rsw = row_in_tile & 7;                  // 128B-swizzle phase of this thread's staging row
+    const int r_lo = half * 64 + q * 16 + (lane >> 2);   // this thread's rows of the tile: r_lo and r_lo + 8
+    const int cp = 2 * (lane & 3);                    // first column of this thread's pair in each 8-column group
+    // stmatrix / ldmatrix: lane l addresses row (l/8 & 1)*8 + l%8 of the warp's 16, 16-byte unit (l/16) of a 16-column
+    // block; fp32: the 8-byte half (l & 1) of unit (l/2 & 1) of an 8-column group, rows r_lo and r_lo + 8.  Both rows of a
+    // lane share the 128B-swizzle phase (r & 7) with the row it addresses.
+    const uint32_t mrow = (uint32_t)(half * 64 + q * 16 + ((lane >> 3) & 1) * 8 + (lane & 7)) * 128u;
+    const int mu = lane >> 4;
+    const int sw = lane & 7;
+    const int fsw = lane >> 2;
+    const uint32_t frow = (uint32_t)r_lo * 128u + (uint32_t)(lane & 1) * 8u;
+    const int fu = (lane >> 1) & 1;
     const uint32_t bar_id = 1;
     const int NBT = 2 * NB;                           // staging slices of the tile
-    float* const xp = sXpose + e * 32 * kXposeStride;
     const bool aux_tma = V::kAux == 0 ? (p.aux_tma != 0) : (V::kAux == 2);
     constexpr int NCH = BN / 32;                      // 32-column chunks of a tile
     const bool a_mn = VAR == VAR_PLAIN_F32 ? (p.a_mode == A_MN2D || p.a_mode == A_IM2COL_MN) : (p.a_mode == A_MN2D);
@@ -442,7 +446,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int m_blk = t % num_m;
       const int split = t / num_m;
       const int m0 = m_blk * tile_rows, n0 = n_blk * BN;
-      const long long row = m0 + row_in_tile;
+      const long long row0 = m0 + r_lo;                 // rows of fragment halves h = 0, 1: row0 + 8h
+      const bool in0 = row0 < p.M, in1 = row0 + 8 < p.M;
       float acc[BN / 2];
       {
         const int kb0 = split * p.kb_per_split;
@@ -452,54 +457,57 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         else if (b_mn) gemm_mainloop<BN, 0, 1>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, a_off, lane);
         else gemm_mainloop<BN, 0, 0>(acc, sA, sB, full_bar, empty_bar, nstages, stage, phase, kb0, kb1, a_off, lane);
       }
+      float rscale[2] = {1.f, 1.f};
+      if (flags & EPI_ROW_SCALE) {
+        if (in0) rscale[0] = __ldg(p.row_scale + row0 / p.rows_per_scale);
+        if (in1) rscale[1] = __ldg(p.row_scale + (row0 + 8) / p.rows_per_scale);
+      }
 #pragma unroll
       for (int c = 0; c < NCH; ++c) {
+        // columns c*32 .. +31: f[4jj + 2h + e] = row row0 + 8h, column col0 + 8jj + cp + e (jj = 0..3)
+        float* const f = acc + 16 * c;
         const int col0 = n0 + c * 32;
-        const int tcol = col0 + hh * 16;                      // first of this thread's 16 columns
         const int part = out_f32 ? 0 : (c & 1);               // bf16: which 32-column half of the 64-column slice
         const bool s_begin = out_f32 || part == 0;
         const bool s_end = out_f32 || part == 1;
         uint8_t* const sbuf = sD + bufi * kStoreBufBytes;
-        uint8_t* const buf = sbuf + row_in_tile * 128;
-        const int u0 = out_f32 ? hh * 4 : part * 4 + hh * 2;  // first 16-byte unit of this thread's columns in the slice row
-        // operands of the epilogue are requested before the accumulator transpose so their latency overlaps it
-        float bv = 0.f;
-        if ((flags & EPI_BIAS) && col0 + lane < p.N) bv = __ldg(p.bias + col0 + lane);
-        float4 rf[4];
-        uint4 rb[2];
-        const bool has_rf = (flags & EPI_RESID) && row < p.M;
-        const bool has_rb = (flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU)) && row < p.M;
-        float rscale = 1.f;
-        if ((flags & EPI_ROW_SCALE) && row < p.M) rscale = __ldg(p.row_scale + row / p.rows_per_scale);
-        uint32_t mbits = 0u;   // this thread's 16 bits of the mask word of its row and the chunk's 32 columns
-        if ((flags & EPI_MASK_BITS) && row < p.M && col0 < p.N)
-          mbits = __ldg(p.mask_bits + row * (p.N >> 5) + (col0 >> 5)) >> (hh * 16);
+        const uint32_t sb = smem_u32(sbuf);
+        // operands of the epilogue are requested before the staging slice is waited for, so their latency overlaps it
+        float bv[8];   // bias of column col0 + 8jj + cp + e at 2jj + e
+        if (flags & EPI_BIAS) {
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int col = col0 + 8 * jj + cp;
+            bv[2 * jj] = col < p.N ? __ldg(p.bias + col) : 0.f;
+            bv[2 * jj + 1] = col < p.N ? __ldg(p.bias + col + 1) : 0.f;
+          }
+        }
+        float2 rf[8];     // fp32 aux operand of fragment pair 2jj + h
+        uint32_t rb[8];   // bf16 aux operand (bf16x2) of fragment pair 2jj + h
+        const bool has_rf = (flags & EPI_RESID) != 0;
+        const bool has_rb = (flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU)) != 0;
+        uint32_t mbits[2] = {0u, 0u};   // mask word of each row and the chunk's 32 columns, shifted to this thread's pairs
+        if ((flags & EPI_MASK_BITS) && col0 < p.N) {
+          if (in0) mbits[0] = __ldg(p.mask_bits + row0 * (p.N >> 5) + (col0 >> 5)) >> cp;
+          if (in1) mbits[1] = __ldg(p.mask_bits + (row0 + 8) * (p.N >> 5) + (col0 >> 5)) >> cp;
+        }
         if (!aux_tma) {
-          if (has_rf) {
-            const float4* rp = reinterpret_cast<const float4*>(p.resid + row * p.ldd + tcol);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) rf[j] = (tcol + 4 * j < p.N) ? __ldg(rp + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-          if (has_rb) {
-            const uint4* rp = reinterpret_cast<const uint4*>(
-                reinterpret_cast<const __nv_bfloat16*>(p.resid_bf16) + row * p.ldd + tcol);
+          for (int jj = 0; jj < 4; ++jj) {
+            const int col = col0 + 8 * jj + cp;
 #pragma unroll
-            for (int j = 0; j < 2; ++j) rb[j] = (tcol + 8 * j < p.N) ? __ldg(rp + j) : make_uint4(0, 0, 0, 0);
+            for (int h = 0; h < 2; ++h) {
+              const bool ok = (h ? in1 : in0) && col < p.N;
+              const long long off = (row0 + 8 * h) * p.ldd + col;
+              if (has_rf)
+                rf[2 * jj + h] = ok ? __ldg(reinterpret_cast<const float2*>(p.resid + off)) : make_float2(0.f, 0.f);
+              if (has_rb)
+                rb[2 * jj + h] = ok ? __ldg(reinterpret_cast<const unsigned int*>(
+                                          reinterpret_cast<const __nv_bfloat16*>(p.resid_bf16) + off))
+                                    : 0u;
+            }
           }
         }
-        // columns c*32 .. +31 of the warp's 16 rows: fragment layout -> lane = (row, 16-column half) (see ptx.cuh, wgmma).
-        // Consecutive chunks alternate between the warp's two buffers, so one barrier per chunk orders writes and reads.
-        float* const xc = xp + (c & 1) * 16 * kXposeStride;
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int j = c * 4 + jj;
-          float* const dst = xc + (lane >> 2) * kXposeStride + jj * 8 + 2 * (lane & 3);
-          dst[0] = acc[4 * j];
-          dst[1] = acc[4 * j + 1];
-          dst[8 * kXposeStride] = acc[4 * j + 2];
-          dst[8 * kXposeStride + 1] = acc[4 * j + 3];
-        }
-        __syncwarp();
         if (aux_tma && s_begin) mbar_wait(&aux_bar[bufi], (aux_phase >> bufi) & 1u);   // the aux slice has landed in this staging slice
         if (s_begin && !aux_tma) {
           // the store that last read this staging slice (2*NB slices ago) must have drained it (and the stats warps too)
@@ -512,87 +520,88 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
           named_bar_sync(bar_id, 256);
         }
-        // the thread's 16 columns in two runs of 8 (one 16-byte unit of bf16 output): fewer values live at a time
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          float f[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) f[j] = xc[(lane & 15) * kXposeStride + hh * 16 + g * 8 + j];
-          if (aux_tma) {
-            // each thread reads its own piece of its (swizzled) row of the aux slice
-            if (out_f32) {
-#pragma unroll
-              for (int j = 0; j < 2; ++j) rf[2 * g + j] = *reinterpret_cast<const float4*>(buf + (((u0 + 2 * g + j) ^ rsw) << 4));
-            } else {
-              rb[g] = *reinterpret_cast<const uint4*>(buf + (((u0 + g) ^ rsw) << 4));
-            }
-          }
-          if (flags & EPI_BIAS) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] += __shfl_sync(0xffffffffu, bv, hh * 16 + g * 8 + j);
-          }
-          if (flags & EPI_RELU) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] = fmaxf(f[j], 0.f);
-          }
-          if (flags & EPI_ROW_SCALE) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] *= rscale;
-          }
-          if (flags & EPI_RESID) {
-            if (aux_tma || has_rf) {
-#pragma unroll
-              for (int j = 0; j < 2; ++j) {
-                const float4 r4 = rf[2 * g + j];
-                f[4 * j] += r4.x; f[4 * j + 1] += r4.y; f[4 * j + 2] += r4.z; f[4 * j + 3] += r4.w;
-              }
-            }
-          }
-          if (flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU)) {
-            if (aux_tma || has_rb) {
-              const uint32_t wv[4] = {rb[g].x, rb[g].y, rb[g].z, rb[g].w};
-#pragma unroll
-              for (int u = 0; u < 4; ++u) {
-                const float2 ab = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wv[u]));
-                if (flags & EPI_MUL_DGELU) {
-                  f[2 * u] *= gelu_erf_grad(ab.x);
-                  f[2 * u + 1] *= gelu_erf_grad(ab.y);
-                } else if (flags & EPI_MUL_DRELU) {   // resid_bf16 = ReLU output: pass the gradient where it is > 0
-                  f[2 * u] = ab.x > 0.f ? f[2 * u] : 0.f;
-                  f[2 * u + 1] = ab.y > 0.f ? f[2 * u + 1] : 0.f;
-                } else {
-                  f[2 * u] += ab.x;
-                  f[2 * u + 1] += ab.y;
-                }
-              }
-            }
-          }
-          if (flags & EPI_AXPBY) {
-            const uint32_t wv[4] = {rb[g].x, rb[g].y, rb[g].z, rb[g].w};
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const float2 ab = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wv[u]));
-              f[2 * u] = fmaf(p.beta, ab.x, p.alpha * f[2 * u]);
-              f[2 * u + 1] = fmaf(p.beta, ab.y, p.alpha * f[2 * u + 1]);
-            }
-          }
-          if (flags & EPI_MASK_BITS) {
-            // a multiply by 0 / 1, not a select: the zeros keep the sign a later (bf16(D) * relu'(out)) would give them
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] *= ((mbits >> (g * 8 + j)) & 1u) ? 1.f : 0.f;
-          }
+        __syncwarp();   // ldmatrix / stmatrix are warp-collective
+        if (aux_tma) {
+          // each warp reads the aux fragments of its own 16 rows of the landed slice
           if (out_f32) {
-            // one 128 B (32 x fp32) slice per TMA store
 #pragma unroll
-            for (int j = 0; j < 2; ++j)
-              *reinterpret_cast<float4*>(buf + (((u0 + 2 * g + j) ^ rsw) << 4)) =
-                  make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
+            for (int jj = 0; jj < 4; ++jj) {
+              const uint32_t u = (uint32_t)(((2 * jj + fu) ^ fsw) << 4);
+              rf[2 * jj] = *reinterpret_cast<const float2*>(sbuf + frow + u);
+              rf[2 * jj + 1] = *reinterpret_cast<const float2*>(sbuf + frow + 8 * 128 + u);
+            }
           } else {
-            // bf16: two 32-column chunks make one 128 B (64 x bf16) slice
-            *reinterpret_cast<uint4*>(buf + (((u0 + g) ^ rsw) << 4)) =
-                make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]),
-                           pack_bf16x2(f[6], f[7]));
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+              ldmatrix_x4(sb + mrow + ((uint32_t)((4 * part + 2 * i + mu) ^ sw) << 4), rb[4 * i], rb[4 * i + 1],
+                          rb[4 * i + 2], rb[4 * i + 3]);
           }
+        }
+        // f[k]: fragment pair k/2 = 2jj + h, column 8jj + cp + (k & 1).  One loop per operation, each behind one test of
+        // the (partly run-time) flags, in the order bias, ReLU, row scale, fp32 residual, bf16 aux, AXPBY, mask.
+        if (flags & EPI_BIAS) {
+#pragma unroll
+          for (int k = 0; k < 16; ++k) f[k] += bv[2 * (k >> 2) + (k & 1)];
+        }
+        if (flags & EPI_RELU) {
+#pragma unroll
+          for (int k = 0; k < 16; ++k) f[k] = fmaxf(f[k], 0.f);
+        }
+        if (flags & EPI_ROW_SCALE) {
+#pragma unroll
+          for (int k = 0; k < 16; ++k) f[k] *= rscale[(k >> 1) & 1];
+        }
+        if ((flags & EPI_RESID) && (aux_tma || has_rf)) {
+#pragma unroll
+          for (int k = 0; k < 16; k += 2) {
+            f[k] += rf[k >> 1].x;
+            f[k + 1] += rf[k >> 1].y;
+          }
+        }
+        if ((flags & (EPI_RESID_BF16 | EPI_MUL_DGELU | EPI_MUL_DRELU)) && (aux_tma || has_rb)) {
+#pragma unroll
+          for (int k = 0; k < 16; k += 2) {
+            const float2 ab = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rb[k >> 1]));
+            if (flags & EPI_MUL_DGELU) {
+              f[k] *= gelu_erf_grad(ab.x);
+              f[k + 1] *= gelu_erf_grad(ab.y);
+            } else if (flags & EPI_MUL_DRELU) {   // resid_bf16 = ReLU output: pass the gradient where it is > 0
+              f[k] = ab.x > 0.f ? f[k] : 0.f;
+              f[k + 1] = ab.y > 0.f ? f[k + 1] : 0.f;
+            } else {
+              f[k] += ab.x;
+              f[k + 1] += ab.y;
+            }
+          }
+        }
+        if (flags & EPI_AXPBY) {
+#pragma unroll
+          for (int k = 0; k < 16; k += 2) {
+            const float2 ab = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rb[k >> 1]));
+            f[k] = fmaf(p.beta, ab.x, p.alpha * f[k]);
+            f[k + 1] = fmaf(p.beta, ab.y, p.alpha * f[k + 1]);
+          }
+        }
+        if (flags & EPI_MASK_BITS) {
+          // a multiply by 0 / 1, not a select: the zeros keep the sign a later (bf16(D) * relu'(out)) would give them
+#pragma unroll
+          for (int k = 0; k < 16; ++k) f[k] *= ((mbits[(k >> 1) & 1] >> (8 * (k >> 2) + (k & 1))) & 1u) ? 1.f : 0.f;
+        }
+        if (out_f32) {
+          // one 128 B (32 x fp32) slice per TMA store
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const uint32_t u = (uint32_t)(((2 * jj + fu) ^ fsw) << 4);
+            *reinterpret_cast<float2*>(sbuf + frow + u) = make_float2(f[4 * jj], f[4 * jj + 1]);
+            *reinterpret_cast<float2*>(sbuf + frow + 8 * 128 + u) = make_float2(f[4 * jj + 2], f[4 * jj + 3]);
+          }
+        } else {
+          // bf16: two 32-column chunks make one 128 B (64 x bf16) slice; one x4 per 16 x 16 block
+#pragma unroll
+          for (int i = 0; i < 2; ++i)
+            stmatrix_x4(sb + mrow + ((uint32_t)((4 * part + 2 * i + mu) ^ sw) << 4), pack_bf16x2(f[8 * i], f[8 * i + 1]),
+                        pack_bf16x2(f[8 * i + 2], f[8 * i + 3]), pack_bf16x2(f[8 * i + 4], f[8 * i + 5]),
+                        pack_bf16x2(f[8 * i + 6], f[8 * i + 7]));
         }
         if (s_end) {
           fence_proxy_async_smem();

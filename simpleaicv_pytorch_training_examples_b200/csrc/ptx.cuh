@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (tiled + im2col), wgmma, fences.  No CUTLASS dependency; everything here is what the kernels in this
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (tiled + im2col), wgmma, ldmatrix / stmatrix, fences.  No CUTLASS dependency; everything here is what the kernels in this
 // directory are built from.
 #pragma once
 #include <cuda.h>
@@ -222,6 +222,22 @@ __device__ __forceinline__ void wgmma_m64(float (&d)[N / 2], uint64_t da, uint32
   if constexpr (r % 32 == 16) wgmma_m64n16<TA, TB>(d + (N - 16) / 2, da, make_smem_desc(b_addr + b_col(N - 16), b_lbo, 1024), scale_d);
 }
 
+
+// ----------------------------------------------------------------------------- ldmatrix / stmatrix
+// Four 8x8 b16 matrices between shared memory and registers in the mma fragment layout: lanes 8i .. 8i+7 give the
+// addresses of rows 0..7 of matrix i (16 contiguous bytes each); register i of lane l holds row l/4, columns
+// 2*(l%4) + {0, 1} (low half: the lower column) of matrix i.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr)
+               : "memory");
+}
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
