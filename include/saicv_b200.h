@@ -175,6 +175,30 @@ int saicv_bn_bwd_apply2(const void* g, const uint32_t* bits, const void* y_a, co
                         const float* gamma_b, const float* sums, void* dy_a, void* dy_b,
                         float* dgamma_a, float* dbeta_a, float* dgamma_b, float* dbeta_b,
                         long long rows, int c, int accumulate_a, int accumulate_b, void* stream);
+/* Cross-rank (synchronized) BatchNorm, nn.SyncBatchNorm's semantics over the ranks of a process group.
+ * saicv_bn_stats_fold: the fold of saicv_bn_finalize on its own (same partial rows, same order): stats[2*c + 2] =
+ * per-channel sum | sum of squares | this rank's row count as two fp32 values (rows >> 12, rows & 4095) whose sums
+ * over ranks stay exact (up to 2^36 rows, 4096 ranks).  The caller sums the buffers of all ranks (all-reduce), then
+ * saicv_bn_finalize_folded finalizes from them with the count they carry; on one rank fold + finalize_folded equal
+ * saicv_bn_finalize bit for bit.
+ * Backward: the caller all-reduces a copy of the sums of saicv_bn_bwd_reduce / _reduce2; the _sync applies take those
+ * global `sums`, the LOCAL sums `local_sums` for dgamma / dbeta, and `count` = stats + 2*c of the forward's reduced
+ * buffer in place of `rows` in the 1/rows of dy (`rows` still sizes the local pass).  local_sums / count NULL: the
+ * plain entry points. */
+int saicv_bn_stats_fold(const float* partials, int partial_rows, long long rows, int c, float* stats, void* stream);
+int saicv_bn_finalize_folded(const float* stats, const float* gamma, const float* beta, float* running_mean,
+                             float* running_var, float* scale_shift, float* saved, int c, float eps, float momentum,
+                             void* stream);
+int saicv_bn_bwd_apply_sync(const void* dout, const void* out, const uint32_t* bits, const void* y,
+                            const float* saved, const float* gamma, const float* scale_shift, const float* sums,
+                            const float* local_sums, const float* count, void* dy, void* dres, float* dgamma,
+                            float* dbeta, long long rows, int c, int act, int accumulate, void* stream);
+int saicv_bn_bwd_apply2_sync(const void* g, const uint32_t* bits, const void* y_a, const void* y_b,
+                             const float* saved_a, const float* saved_b, const float* gamma_a,
+                             const float* gamma_b, const float* sums, const float* local_sums, const float* count,
+                             void* dy_a, void* dy_b, float* dgamma_a, float* dbeta_a, float* dgamma_b,
+                             float* dbeta_b, long long rows, int c, int accumulate_a, int accumulate_b,
+                             void* stream);
 /* a = a + b (bf16), used where two gradient paths meet. */
 int saicv_add_bf16(void* a, const void* b, long long n, void* stream);
 
@@ -276,6 +300,14 @@ int saicv_bn_bwd_generic(const void* x, int x_f32, const void* g, int g_f32, con
                          const float* gamma, const float* dres, float* partial, float* sums, void* dx,
                          int dx_f32, float* dgamma, float* dbeta, long long rows, int c, int accumulate,
                          void* stream);
+/* saicv_bn_bwd_generic in two calls, reduce (sums[2][c]) then apply, so that the sums can be exchanged between them
+ * (cross-rank BatchNorm): local_sums / count as for saicv_bn_bwd_apply_sync, NULL for the plain backward. */
+int saicv_bn_bwd_generic_reduce(const void* x, int x_f32, const void* g, int g_f32, const float* saved,
+                                float* partial, float* sums, long long rows, int c, void* stream);
+int saicv_bn_bwd_generic_apply(const void* x, int x_f32, const void* g, int g_f32, const float* saved,
+                               const float* gamma, const float* dres, const float* sums, const float* local_sums,
+                               const float* count, void* dx, int dx_f32, float* dgamma, float* dbeta,
+                               long long rows, int c, int accumulate, void* stream);
 /* NHWC bf16 im2col / col2im for the strided patch-embedding convolutions whose channel counts are not
  * multiples of 64 (van.py:189-208: 3x3 stride 2): cols[(n,p,q)][(r*k+s)*c + ch]. */
 int saicv_im2col_nhwc(const void* x, void* cols, int n, int h, int w, int c, int k, int stride, int pad,

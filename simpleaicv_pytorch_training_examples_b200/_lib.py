@@ -69,6 +69,10 @@ SIGNATURES = {
     'saicv_bn_bwd_apply': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_void_p],
     'saicv_bn_bwd_reduce2': [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p],
     'saicv_bn_bwd_apply2': [c_void_p] * 15 + [c_ll, c_int, c_int, c_int, c_void_p],
+    'saicv_bn_stats_fold': [c_void_p, c_int, c_ll, c_int, c_void_p, c_void_p],
+    'saicv_bn_finalize_folded': [c_void_p] * 7 + [c_int, c_float, c_float, c_void_p],
+    'saicv_bn_bwd_apply_sync': [c_void_p] * 14 + [c_ll, c_int, c_int, c_int, c_void_p],
+    'saicv_bn_bwd_apply2_sync': [c_void_p] * 17 + [c_ll, c_int, c_int, c_int, c_void_p],
     'saicv_add_bf16': [c_void_p, c_void_p, c_ll, c_void_p],
     'saicv_maxpool3x3s2_fwd': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_maxpool3x3s2_bwd': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
@@ -136,6 +140,8 @@ SIGNATURES = {
     'saicv_bn_stats_generic': [c_void_p, c_int, c_void_p, c_ll, c_int, c_void_p],
     'saicv_bn_apply_generic': [c_void_p, c_int, c_void_p, c_void_p, c_int, c_ll, c_int, c_void_p],
     'saicv_bn_bwd_generic': [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
+    'saicv_bn_bwd_generic_reduce': [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p],
+    'saicv_bn_bwd_generic_apply': [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 7 + [c_int, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p],
     'saicv_im2col_nhwc': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_col2im_nhwc': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     'saicv_rope_qk_fwd': [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],

@@ -320,12 +320,45 @@ __global__ void colsum_f32_kernel(const float* __restrict__ x, float* __restrict
 }
 
 // ----------------------------------------------------------------------------- BN finalize
-// Folds the per-block partial sums (deterministic order) and finalises 8 channels per block.
+// The fold of bn_finalize_kernel on its own: stats[0..2C) = the per-channel sum | sum of squares, summed over the
+// partial rows in exactly the order of bn_finalize_kernel, and stats[2C], stats[2C+1] = this rank's row count in
+// the exact split of bn_sync_count, so that a sum of such buffers over ranks (an all-reduce) is the global one.
+__global__ void bn_stats_fold_kernel(const float* __restrict__ partials, int nblk, float* __restrict__ stats,
+                                     long long rows, int C) {
+  __shared__ float sm[2][32][9];
+  const int cl = threadIdx.x & 7, grp = threadIdx.x >> 3;
+  const int c = blockIdx.x * 8 + cl;
+  float s0 = 0.f, s1 = 0.f;
+  if (c < C)
+    for (int b = grp; b < nblk; b += 32) {
+      s0 += partials[(long long)b * 2 * C + c];
+      s1 += partials[(long long)b * 2 * C + C + c];
+    }
+  sm[0][grp][cl] = s0;
+  sm[1][grp][cl] = s1;
+  __syncthreads();
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    stats[2 * C] = (float)(rows >> kBnCountShift);
+    stats[2 * C + 1] = (float)(rows & ((1 << kBnCountShift) - 1));
+  }
+  if (grp != 0 || c >= C) return;
+  s0 = s1 = 0.f;
+#pragma unroll
+  for (int g = 0; g < 32; ++g) {
+    s0 += sm[0][g][cl];
+    s1 += sm[1][g][cl];
+  }
+  stats[c] = s0;
+  stats[C + c] = s1;
+}
+
+// Folds the per-block partial sums (deterministic order) and finalises 8 channels per block.  count: NULL, or the
+// row count of a bn_stats_fold_kernel buffer (after its all-reduce: the global count), which then replaces `rows`.
 __global__ void bn_finalize_kernel(const float* __restrict__ partials, int nblk, const float* __restrict__ gamma,
                                    const float* __restrict__ beta, float* __restrict__ rmean,
                                    float* __restrict__ rvar, float* __restrict__ ss,
                                    float* __restrict__ saved, long long rows, int C, float eps,
-                                   float momentum) {
+                                   float momentum, const float* __restrict__ count) {
   __shared__ float sm[2][32][9];
   const int cl = threadIdx.x & 7, grp = threadIdx.x >> 3;
   const int c = blockIdx.x * 8 + cl;
@@ -345,6 +378,7 @@ __global__ void bn_finalize_kernel(const float* __restrict__ partials, int nblk,
     s0 += sm[0][g][cl];
     s1 += sm[1][g][cl];
   }
+  if (count) rows = bn_sync_count(count);
   const float inv_n = 1.0f / (float)rows;
   const float mean = s0 * inv_n;
   float var = s1 * inv_n - mean * mean;
@@ -455,7 +489,9 @@ __global__ void __launch_bounds__(kThreads, 2)
 bn_bwd_apply_kernel(const void* __restrict__ dout, const void* __restrict__ out, const uint8_t* __restrict__ bits,
                     const void* __restrict__ y, const float* __restrict__ saved, const float* __restrict__ gamma,
                     const float* __restrict__ sums, const float* __restrict__ ss, void* __restrict__ dy,
-                    void* __restrict__ dres, long long rows, int C, SlabGeom gm, int act, float inv_rows) {
+                    void* __restrict__ dres, long long rows, int C, SlabGeom gm, int act, float inv_rows,
+                    const float* __restrict__ count) {
+  if (count) inv_rows = 1.0f / (float)bn_sync_count(count);
   const int vpr = gm.vpr;
   const int tx = threadIdx.x % gm.tx_count;
   const int ty = threadIdx.x / gm.tx_count;
@@ -522,7 +558,9 @@ __global__ void __launch_bounds__(kThreads, 2)
 bn_bwd_apply2_kernel(const void* __restrict__ g, const uint8_t* __restrict__ bits, const void* __restrict__ ya,
                      const void* __restrict__ yb, const float* __restrict__ saved_a, const float* __restrict__ saved_b,
                      const float* __restrict__ gamma_a, const float* __restrict__ gamma_b, const float* __restrict__ sums,
-                     void* __restrict__ dya, void* __restrict__ dyb, long long rows, int C, SlabGeom gm, float inv_rows) {
+                     void* __restrict__ dya, void* __restrict__ dyb, long long rows, int C, SlabGeom gm, float inv_rows,
+                     const float* __restrict__ count) {
+  if (count) inv_rows = 1.0f / (float)bn_sync_count(count);
   const int vpr = gm.vpr;
   const int tx = threadIdx.x % gm.tx_count;
   const int ty = threadIdx.x / gm.tx_count;
@@ -981,7 +1019,23 @@ int saicv_bn_finalize(const float* partials, int partial_rows_, const float* gam
                       int c, float eps, float momentum, void* stream) {
   const int nrows = partial_rows_ > 0 ? partial_rows_ : partial_rows(rows, c);
   bn_finalize_kernel<<<(c + 7) / 8, 256, 0, ST>>>(partials, nrows, gamma, beta, running_mean,
-                                                    running_var, scale_shift, saved, rows, c, eps, momentum);
+                                                    running_var, scale_shift, saved, rows, c, eps, momentum, nullptr);
+  return check_launch("bn_finalize_kernel");
+}
+
+int saicv_bn_stats_fold(const float* partials, int partial_rows_, long long rows, int c, float* stats, void* stream) {
+  if (rows < 1 || (rows >> kBnCountShift) >= (1LL << 24))
+    return set_error("saicv_bn_stats_fold: row count %lld outside [1, 2^%d)", rows, 24 + kBnCountShift);
+  const int nrows = partial_rows_ > 0 ? partial_rows_ : partial_rows(rows, c);
+  bn_stats_fold_kernel<<<(c + 7) / 8, 256, 0, ST>>>(partials, nrows, stats, rows, c);
+  return check_launch("bn_stats_fold_kernel");
+}
+
+int saicv_bn_finalize_folded(const float* stats, const float* gamma, const float* beta, float* running_mean,
+                             float* running_var, float* scale_shift, float* saved, int c, float eps, float momentum,
+                             void* stream) {
+  bn_finalize_kernel<<<(c + 7) / 8, 256, 0, ST>>>(stats, 1, gamma, beta, running_mean, running_var, scale_shift, saved,
+                                                    0, c, eps, momentum, stats + 2 * c);
   return check_launch("bn_finalize_kernel");
 }
 
@@ -1024,6 +1078,14 @@ int saicv_bn_bwd_reduce(const void* dout, const void* out, const uint32_t* bits,
 int saicv_bn_bwd_apply(const void* dout, const void* out, const uint32_t* bits, const void* y, const float* saved,
                        const float* gamma, const float* scale_shift, float* sums, void* dy, void* dres, float* dgamma,
                        float* dbeta, long long rows, int c, int act, int accumulate, void* stream) {
+  return saicv_bn_bwd_apply_sync(dout, out, bits, y, saved, gamma, scale_shift, sums, nullptr, nullptr, dy, dres, dgamma,
+                                 dbeta, rows, c, act, accumulate, stream);
+}
+
+int saicv_bn_bwd_apply_sync(const void* dout, const void* out, const uint32_t* bits, const void* y, const float* saved,
+                            const float* gamma, const float* scale_shift, const float* sums, const float* local_sums,
+                            const float* count, void* dy, void* dres, float* dgamma, float* dbeta, long long rows, int c,
+                            int act, int accumulate, void* stream) {
   if (int e = check_mask_source("saicv_bn_bwd_apply", out, bits, scale_shift, c, act)) return e;
   SlabGeom g;
   int blocks;
@@ -1031,7 +1093,7 @@ int saicv_bn_bwd_apply(const void* dout, const void* out, const uint32_t* bits, 
   const float inv_rows = 1.0f / (float)rows;
   const uint8_t* mask = reinterpret_cast<const uint8_t*>(bits);
 #define BWD_APPLY(HO, HD) \
-  bn_bwd_apply_kernel<HO, HD><<<blocks, kThreads, 0, ST>>>(dout, out, mask, y, saved, gamma, sums, scale_shift, dy, dres, rows, c, g, act, inv_rows)
+  bn_bwd_apply_kernel<HO, HD><<<blocks, kThreads, 0, ST>>>(dout, out, mask, y, saved, gamma, sums, scale_shift, dy, dres, rows, c, g, act, inv_rows, count)
   if (out != nullptr && act != 0) {
     if (dres) BWD_APPLY(true, true); else BWD_APPLY(true, false);
   } else {
@@ -1039,7 +1101,7 @@ int saicv_bn_bwd_apply(const void* dout, const void* out, const uint32_t* bits, 
   }
 #undef BWD_APPLY
   if (int e = check_launch("bn_bwd_apply_kernel")) return e;
-  return bn_param_grad(sums, dgamma, dbeta, c, accumulate, ST);
+  return bn_param_grad(local_sums ? local_sums : sums, dgamma, dbeta, c, accumulate, ST);
 }
 
 int saicv_bn_bwd_reduce2(const void* g, const uint32_t* bits, const void* y_a, const void* y_b, const float* saved_a,
@@ -1058,16 +1120,26 @@ int saicv_bn_bwd_apply2(const void* g, const uint32_t* bits, const void* y_a, co
                         const float* saved_b, const float* gamma_a, const float* gamma_b, const float* sums, void* dy_a,
                         void* dy_b, float* dgamma_a, float* dbeta_a, float* dgamma_b, float* dbeta_b, long long rows,
                         int c, int accumulate_a, int accumulate_b, void* stream) {
+  return saicv_bn_bwd_apply2_sync(g, bits, y_a, y_b, saved_a, saved_b, gamma_a, gamma_b, sums, nullptr, nullptr, dy_a,
+                                  dy_b, dgamma_a, dbeta_a, dgamma_b, dbeta_b, rows, c, accumulate_a, accumulate_b, stream);
+}
+
+int saicv_bn_bwd_apply2_sync(const void* g, const uint32_t* bits, const void* y_a, const void* y_b, const float* saved_a,
+                             const float* saved_b, const float* gamma_a, const float* gamma_b, const float* sums,
+                             const float* local_sums, const float* count, void* dy_a, void* dy_b, float* dgamma_a,
+                             float* dbeta_a, float* dgamma_b, float* dbeta_b, long long rows, int c, int accumulate_a,
+                             int accumulate_b, void* stream) {
   if (bits != nullptr && c % 32) return set_error("saicv_bn_bwd_apply2: mask bits need c %% 32 == 0 (c=%d)", c);
   SlabGeom gm;
   int blocks;
   if (!slab_geom(rows, c, UNROLL, &gm, &blocks)) return 1;
   bn_bwd_apply2_kernel<<<blocks, kThreads, 0, ST>>>(g, reinterpret_cast<const uint8_t*>(bits), y_a, y_b, saved_a,
                                                     saved_b, gamma_a, gamma_b, sums, dy_a, dy_b, rows, c, gm,
-                                                    1.0f / (float)rows);
+                                                    1.0f / (float)rows, count);
   if (int e = check_launch("bn_bwd_apply2_kernel")) return e;
-  if (int e = bn_param_grad(sums, dgamma_a, dbeta_a, c, accumulate_a, ST)) return e;
-  return bn_param_grad(sums + 2 * c, dgamma_b, dbeta_b, c, accumulate_b, ST);
+  const float* ps = local_sums ? local_sums : sums;
+  if (int e = bn_param_grad(ps, dgamma_a, dbeta_a, c, accumulate_a, ST)) return e;
+  return bn_param_grad(ps + 2 * c, dgamma_b, dbeta_b, c, accumulate_b, ST);
 }
 
 int saicv_add_bf16(void* a, const void* b, long long n, void* stream) {

@@ -392,7 +392,9 @@ __global__ void bn_apply_generic_kernel(const void* __restrict__ x, int x_f32, c
 __global__ void bn_bwd_apply_generic_kernel(const void* __restrict__ x, int x_f32, const void* __restrict__ g, int g_f32,
                                             const float* __restrict__ saved, const float* __restrict__ gamma,
                                             const float* __restrict__ sums, const float* __restrict__ dres, void* __restrict__ dx,
-                                            int dx_f32, long long rows, int C, float inv_rows) {
+                                            int dx_f32, long long rows, int C, float inv_rows,
+                                            const float* __restrict__ count) {
+  if (count) inv_rows = 1.0f / (float)bn_sync_count(count);
   const int vpr = C >> 3;
   const long long total = rows * vpr;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -626,17 +628,31 @@ int saicv_bn_apply_generic(const void* x, int x_f32, const float* scale_shift, v
 int saicv_bn_bwd_generic(const void* x, int x_f32, const void* g, int g_f32, const float* saved, const float* gamma,
                          const float* dres, float* partial, float* sums, void* dx, int dx_f32, float* dgamma, float* dbeta,
                          long long rows, int c, int accumulate, void* stream) {
+  if (int e = saicv_bn_bwd_generic_reduce(x, x_f32, g, g_f32, saved, partial, sums, rows, c, stream)) return e;
+  return saicv_bn_bwd_generic_apply(x, x_f32, g, g_f32, saved, gamma, dres, sums, nullptr, nullptr, dx, dx_f32, dgamma,
+                                    dbeta, rows, c, accumulate, stream);
+}
+
+int saicv_bn_bwd_generic_reduce(const void* x, int x_f32, const void* g, int g_f32, const float* saved, float* partial,
+                                float* sums, long long rows, int c, void* stream) {
   if (c % 8) return set_error("saicv_bn_bwd_generic: C %% 8 != 0");
   int tx, nblk;
   long long rpb;
   slab(rows, c, &tx, &rpb, &nblk);
   bn_colreduce_generic_kernel<1><<<nblk, 256, 0, ST>>>(x, x_f32, g, g_f32, saved, partial, rows, c, tx, rpb);
   if (int e = check_launch("bn_colreduce_generic_kernel")) return e;
-  if (int e = saicv_reduce_partials(partial, sums, nblk, 2LL * c, 0, stream)) return e;
+  return saicv_reduce_partials(partial, sums, nblk, 2LL * c, 0, stream);
+}
+
+int saicv_bn_bwd_generic_apply(const void* x, int x_f32, const void* g, int g_f32, const float* saved, const float* gamma,
+                               const float* dres, const float* sums, const float* local_sums, const float* count, void* dx,
+                               int dx_f32, float* dgamma, float* dbeta, long long rows, int c, int accumulate,
+                               void* stream) {
+  if (c % 8) return set_error("saicv_bn_bwd_generic: C %% 8 != 0");
   bn_bwd_apply_generic_kernel<<<grid_1d(rows * (c / 8)), 256, 0, ST>>>(x, x_f32, g, g_f32, saved, gamma, sums, dres, dx, dx_f32,
-                                                                      rows, c, 1.0f / (float)rows);
+                                                                      rows, c, 1.0f / (float)rows, count);
   if (int e = check_launch("bn_bwd_apply_generic_kernel")) return e;
-  return bn_param_grad(sums, dgamma, dbeta, c, accumulate, ST);
+  return bn_param_grad(local_sums ? local_sums : sums, dgamma, dbeta, c, accumulate, ST);
 }
 
 int saicv_im2col_nhwc(const void* x, void* cols, int n, int h, int w, int c, int k, int stride, int pad, void* stream) {

@@ -36,4 +36,12 @@ int fold_partials(const float* partials, int nblk, int ncols, float* out0, float
 // BatchNorm parameter gradients from the reduced sums [2][c] (sum g | sum g * xhat): dbeta (+)= sums[0 .. c),
 // dgamma (+)= sums[c .. 2c) (capi_elementwise.cu).
 int bn_param_grad(const float* sums, float* dgamma, float* dbeta, int c, int accumulate, cudaStream_t st);
+
+// The row count of a cross-rank BatchNorm exchange rides in the exchanged fp32 buffer as two values, hi = rows >> 12
+// and lo = rows & 4095, so that their sums over ranks stay exact integers: up to 2^36 rows over up to 4096 ranks
+// (a single fp32 count is exact only up to 2^24 rows).
+constexpr int kBnCountShift = 12;
+__host__ __device__ inline long long bn_sync_count(const float* cnt) {
+  return ((long long)cnt[0] << kBnCountShift) + (long long)cnt[1];
+}
 }  // namespace saicv

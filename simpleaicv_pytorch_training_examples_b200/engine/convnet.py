@@ -21,6 +21,7 @@ import torch
 
 from .. import ops
 from .operands import CONV, STEM, Linear, Operand, rows_wgrad
+from . import syncbn
 from .runtime import Runtime
 
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SILU = 0, 1, 2, 3
@@ -149,8 +150,9 @@ class ConvBN:
                 self.rv_p[:self.k].copy_(bn.running_var)
             rm = (self.rm_p if self.padded else bn.running_mean) if track else None
             rv = (self.rv_p if self.padded else bn.running_var) if track else None
-            ops.bn_finalize(partials, self._gamma(), self._beta(), rm, rv, ss, saved, rows, bn.eps, momentum,
-                            partial_rows=prow)
+            # synchronized BatchNorm: the exchanged statistics (global row count) stay in the tape for the backward
+            tape['sync'] = syncbn.finalize(partials, prow, rows, self._gamma(), self._beta(), rm, rv, ss, saved, bn.eps,
+                                           momentum)
             if self.padded and track:
                 bn.running_mean.copy_(self.rm_p[:self.k])
                 bn.running_var.copy_(self.rv_p[:self.k])
@@ -202,11 +204,12 @@ class ConvBN:
         ss = tape['ss'] if (act != ACT_NONE and bits is None) else None
         saved = tape['saved']
         ops.bn_bwd_reduce(dout, None, y, saved, self.sums, act, scale_shift=ss, bits=bits)
+        sums, sync = syncbn.backward_sums(self.sums, tape.get('sync'), self.kp)
         dy = torch.empty_like(y)
         dres = torch.empty_like(y) if want_dres else None
         with self._bn_grad(sink) as (gamma, dg, db, acc):
-            ops.bn_bwd_apply(dout, None, y, saved, gamma, self.sums, dy, dres, dg, db, act, accumulate=acc,
-                             scale_shift=ss, bits=bits)
+            ops.bn_bwd_apply(dout, None, y, saved, gamma, sums, dy, dres, dg, db, act, accumulate=acc,
+                             scale_shift=ss, bits=bits, **sync)
         return dy, dres
 
     def bn_bwd_pair(self, other, g, tape, other_tape, sink, bits):
@@ -216,11 +219,13 @@ class ConvBN:
         y, yo = tape['y'], other_tape['y']
         sums = torch.empty(4, self.kp, device=y.device)
         ops.bn_bwd_reduce2(g, bits, y, yo, tape['saved'], other_tape['saved'], sums)
+        # synchronized: both BatchNorms' sums go in one exchange; they share the row count
+        sums, sync = syncbn.backward_sums(sums, tape.get('sync'), self.kp)
         dy, dyo = torch.empty_like(y), torch.empty_like(yo)
         # nested this way round so that this unit's gradients are reported before other's (the inner block exits first)
         with other._bn_grad(sink) as (gb, dgb, dbb, accb), self._bn_grad(sink) as (ga, dga, dba, acca):
             ops.bn_bwd_apply2(g, bits, y, yo, tape['saved'], other_tape['saved'], ga, gb, sums, dy, dyo, dga, dba, dgb, dbb,
-                              accumulate_a=acca, accumulate_b=accb)
+                              accumulate_a=acca, accumulate_b=accb, **sync)
         return dy, dyo
 
     def conv_bwd(self, dy, tape, sink, need_dx=True, add=None, mask_bits=None):

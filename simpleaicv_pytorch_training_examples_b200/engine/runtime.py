@@ -17,6 +17,8 @@ import contextlib
 import torch
 import torch.nn as nn
 
+from . import syncbn
+
 
 class GradSink:
     """Where parameter gradients go: ``param.grad`` by default, or bucket views supplied by the
@@ -68,6 +70,7 @@ class Runtime:
     lists those copies for the fused optimizer in ``units`` order; ``prep()`` refreshes them before a forward."""
 
     non_differentiable_outputs = 0
+    bn_group = None   # process group of synchronized BatchNorm (engine/syncbn.py), None: per-rank statistics
 
     def __init__(self, units):
         self.sink = GradSink()
@@ -90,7 +93,8 @@ class _RuntimeFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, anchor, rt, *inputs):
         ctx.rt, ctx.n_inputs = rt, len(inputs)
-        *outs, ctx.tape = rt.forward(*inputs, True, True)
+        with syncbn.exchanging(rt.bn_group):
+            *outs, ctx.tape = rt.forward(*inputs, True, True)
         if rt.non_differentiable_outputs:
             ctx.mark_non_differentiable(*outs[-rt.non_differentiable_outputs:])
         return outs[0] if len(outs) == 1 else tuple(outs)
@@ -101,7 +105,8 @@ class _RuntimeFunction(torch.autograd.Function):
         assert tape is not None, 'the graph of this forward pass was already differentiated'
         rt = ctx.rt
         grads = grads[:len(grads) - rt.non_differentiable_outputs]
-        rt.backward(*(g.contiguous() for g in grads), tape)
+        with syncbn.exchanging(rt.bn_group):   # checkpointed stages re-run their forward (and its exchanges) in here
+            rt.backward(*(g.contiguous() for g in grads), tape)
         if rt.sink.on_backward_end is not None:
             rt.sink.on_backward_end()
         return (None, None) + (None,) * ctx.n_inputs
@@ -113,7 +118,7 @@ def run(rt, training, *inputs):
     if training and torch.is_grad_enabled():
         anchor = torch.zeros((), device=inputs[0].device, requires_grad=True)
         return _RuntimeFunction.apply(anchor, rt, *inputs)
-    with torch.no_grad():
+    with torch.no_grad(), syncbn.exchanging(rt.bn_group):
         *outs, _ = rt.forward(*inputs, training, False)
     return outs[0] if len(outs) == 1 else tuple(outs)
 
@@ -126,7 +131,17 @@ class RuntimeModule(nn.Module):
         rt = self.__dict__.get('_rt')
         if rt is None:
             rt = self.__dict__['_rt'] = self._build_runtime()  # not a submodule / not in state_dict
+            rt.bn_group = self.__dict__.get('_bn_group')
         return rt
+
+    def set_bn_group(self, group):
+        """Synchronized BatchNorm (nn.SyncBatchNorm's semantics): in training, every BatchNorm of the model computes its
+        statistics and gradient sums over all ranks of `group`, a process group dedicated to these exchanges (see
+        engine/syncbn.py); None restores per-rank statistics.  Like the runtime, the group lives outside state_dict."""
+        self.__dict__['_bn_group'] = group
+        rt = self.__dict__.get('_rt')
+        if rt is not None:
+            rt.bn_group = group
 
     def grad_sink(self):
         """Where the runtime deposits parameter gradients (used by distributed.B200DataParallel)."""

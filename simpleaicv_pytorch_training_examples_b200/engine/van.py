@@ -18,6 +18,7 @@ import torch
 from .. import ops
 from .convnet import FcHeadRT
 from .operands import CONV, STEM, Linear, Operand
+from . import syncbn
 from .runtime import Runtime
 from .vit import drop_path_scale
 
@@ -32,8 +33,9 @@ def _bn_forward(bn, x, training, out_f32, tape):
         partial, prow = ops.bn_stats_generic(x)
         track = bn.track_running_stats
         momentum = bn.momentum if bn.momentum is not None else 0.1
-        ops.bn_finalize(partial, bn.weight.detach(), bn.bias.detach(), bn.running_mean if track else None,
-                        bn.running_var if track else None, ss, saved, rows, bn.eps, momentum, partial_rows=prow)
+        tape['sync'] = syncbn.finalize(partial, prow, rows, bn.weight.detach(), bn.bias.detach(),
+                                       bn.running_mean if track else None, bn.running_var if track else None, ss, saved,
+                                       bn.eps, momentum)
         if track and bn.num_batches_tracked is not None:
             bn.num_batches_tracked.add_(1)
         tape['saved'] = saved
@@ -46,8 +48,15 @@ def _bn_forward(bn, x, training, out_f32, tape):
 
 
 def _bn_backward(bn, g, tape, sink, dres=None, dx_f32=True):
+    x, stats = tape['x'], tape.get('sync')
     with sink.grad(bn.weight, bn.bias) as (acc, dg, db):
-        return ops.bn_bwd_generic(tape['x'], g, tape['saved'], bn.weight.detach(), dg, db, dres=dres, dx_f32=dx_f32, accumulate=acc)
+        if stats is None:
+            return ops.bn_bwd_generic(x, g, tape['saved'], bn.weight.detach(), dg, db, dres=dres, dx_f32=dx_f32,
+                                      accumulate=acc)
+        # synchronized BatchNorm: the sums are exchanged between the reduce and the apply
+        sums, sync = syncbn.backward_sums(ops.bn_bwd_generic_reduce(x, g, tape['saved']), stats, x.shape[-1])
+        return ops.bn_bwd_generic_apply(x, g, tape['saved'], bn.weight.detach(), sums, dg, db, dres=dres, dx_f32=dx_f32,
+                                        accumulate=acc, **sync)
 
 
 class _DW:

@@ -319,6 +319,25 @@ def bn_finalize(stats, gamma, beta, rmean, rvar, scale_shift, saved, rows, eps, 
               _p(scale_shift), _p(saved), rows, c, eps, momentum, _stream())
 
 
+def bn_stats_fold(partials, rows, c, partial_rows=0):
+    """The fold of bn_finalize on its own: returns stats fp32 [2 * c + 2] = per-channel sum | sum of squares | the
+    row count in two exact parts.  Summed over ranks (an all-reduce), it is what bn_finalize_folded finalizes."""
+    stats = torch.empty(2 * c + 2, device=partials.device, dtype=torch.float32)
+    _lib.call('saicv_bn_stats_fold', _p(partials), partial_rows, rows, c, _p(stats), _stream())
+    return stats
+
+
+def bn_finalize_folded(stats, gamma, beta, rmean, rvar, scale_shift, saved, eps, momentum):
+    """bn_finalize from a bn_stats_fold buffer (all-reduced or not), with the row count it carries."""
+    _lib.call('saicv_bn_finalize_folded', _p(stats), _p(gamma), _p(beta), _p(rmean), _p(rvar), _p(scale_shift),
+              _p(saved), gamma.numel(), eps, momentum, _stream())
+
+
+def bn_sync_count(stats, c):
+    """The row-count slots of a bn_stats_fold buffer over c channels (the `count` of the synchronized backward)."""
+    return stats[2 * c:]
+
+
 def mask_bits_like(y):
     """Buffer for the packed ReLU mask of an activation [..., C]: int32 [rows, C // 32] (bit j of word w is channel
     32w + j; int32 only because torch has no uint32 arithmetic, the bits are the same)."""
@@ -342,11 +361,18 @@ def bn_bwd_reduce(dout, out, y, saved, sums, act, scale_shift=None, bits=None):
 
 
 def bn_bwd_apply(dout, out, y, saved, gamma, sums, dy, dres, dgamma, dbeta, act, accumulate=False,
-                 scale_shift=None, bits=None):
+                 scale_shift=None, bits=None, local_sums=None, count=None):
+    """Synchronized BatchNorm: `sums` are the sums reduced over ranks, local_sums this rank's own (for dgamma /
+    dbeta) and count = bn_sync_count of the forward's reduced statistics (the global row count)."""
     c = y.shape[-1]
-    _lib.call('saicv_bn_bwd_apply', _p(dout), _p(out), _p(bits), _p(y), _p(saved), _p(gamma), _p(scale_shift),
-              _p(sums), _p(dy), _p(dres), _p(dgamma), _p(dbeta), y.numel() // c, c, act,
-              int(accumulate), _stream())
+    if local_sums is None and count is None:
+        _lib.call('saicv_bn_bwd_apply', _p(dout), _p(out), _p(bits), _p(y), _p(saved), _p(gamma), _p(scale_shift),
+                  _p(sums), _p(dy), _p(dres), _p(dgamma), _p(dbeta), y.numel() // c, c, act,
+                  int(accumulate), _stream())
+    else:
+        _lib.call('saicv_bn_bwd_apply_sync', _p(dout), _p(out), _p(bits), _p(y), _p(saved), _p(gamma), _p(scale_shift),
+                  _p(sums), _p(local_sums), _p(count), _p(dy), _p(dres), _p(dgamma), _p(dbeta), y.numel() // c, c, act,
+                  int(accumulate), _stream())
 
 
 def bn_bwd_reduce2(g, bits, y_a, y_b, saved_a, saved_b, sums):
@@ -358,11 +384,17 @@ def bn_bwd_reduce2(g, bits, y_a, y_b, saved_a, saved_b, sums):
 
 
 def bn_bwd_apply2(g, bits, y_a, y_b, saved_a, saved_b, gamma_a, gamma_b, sums, dy_a, dy_b, dgamma_a, dbeta_a,
-                  dgamma_b, dbeta_b, accumulate_a=False, accumulate_b=False):
+                  dgamma_b, dbeta_b, accumulate_a=False, accumulate_b=False, local_sums=None, count=None):
+    """local_sums / count: as for bn_bwd_apply ([4, C] sums; A and B share the row count)."""
     c = y_a.shape[-1]
-    _lib.call('saicv_bn_bwd_apply2', _p(g), _p(bits), _p(y_a), _p(y_b), _p(saved_a), _p(saved_b), _p(gamma_a),
-              _p(gamma_b), _p(sums), _p(dy_a), _p(dy_b), _p(dgamma_a), _p(dbeta_a), _p(dgamma_b), _p(dbeta_b),
-              y_a.numel() // c, c, int(accumulate_a), int(accumulate_b), _stream())
+    if local_sums is None and count is None:
+        _lib.call('saicv_bn_bwd_apply2', _p(g), _p(bits), _p(y_a), _p(y_b), _p(saved_a), _p(saved_b), _p(gamma_a),
+                  _p(gamma_b), _p(sums), _p(dy_a), _p(dy_b), _p(dgamma_a), _p(dbeta_a), _p(dgamma_b), _p(dbeta_b),
+                  y_a.numel() // c, c, int(accumulate_a), int(accumulate_b), _stream())
+    else:
+        _lib.call('saicv_bn_bwd_apply2_sync', _p(g), _p(bits), _p(y_a), _p(y_b), _p(saved_a), _p(saved_b), _p(gamma_a),
+                  _p(gamma_b), _p(sums), _p(local_sums), _p(count), _p(dy_a), _p(dy_b), _p(dgamma_a), _p(dbeta_a),
+                  _p(dgamma_b), _p(dbeta_b), y_a.numel() // c, c, int(accumulate_a), int(accumulate_b), _stream())
 
 
 def add_bf16(a, b):
@@ -696,6 +728,26 @@ def bn_bwd_generic(x, g, saved, gamma, dgamma, dbeta, dres=None, dx_f32=True, ac
     _lib.call('saicv_bn_bwd_generic', _p(x), int(x.dtype == torch.float32), _p(g), int(g.dtype == torch.float32), _p(saved),
               _p(gamma), _p(dres), _p(partial_ws(x.device, 2 * c)), _p(sums), _p(dx), int(dx_f32), _p(dgamma), _p(dbeta),
               rows, c, int(accumulate), _stream())
+    return dx
+
+
+def bn_bwd_generic_reduce(x, g, saved):
+    """The reduce half of bn_bwd_generic: returns sums fp32 [2 * C] (sum g | sum g * xhat)."""
+    c = x.shape[-1]
+    sums = torch.empty(2 * c, device=x.device, dtype=torch.float32)
+    _lib.call('saicv_bn_bwd_generic_reduce', _p(x), int(x.dtype == torch.float32), _p(g), int(g.dtype == torch.float32),
+              _p(saved), _p(partial_ws(x.device, 2 * c)), _p(sums), x.numel() // c, c, _stream())
+    return sums
+
+
+def bn_bwd_generic_apply(x, g, saved, gamma, sums, dgamma, dbeta, dres=None, dx_f32=True, accumulate=False,
+                         local_sums=None, count=None):
+    """The apply half of bn_bwd_generic; local_sums / count as for bn_bwd_apply.  Returns dx."""
+    c = x.shape[-1]
+    dx = torch.empty(x.shape, device=x.device, dtype=torch.float32 if dx_f32 else torch.bfloat16)
+    _lib.call('saicv_bn_bwd_generic_apply', _p(x), int(x.dtype == torch.float32), _p(g), int(g.dtype == torch.float32),
+              _p(saved), _p(gamma), _p(dres), _p(sums), _p(local_sums), _p(count), _p(dx), int(dx_f32), _p(dgamma),
+              _p(dbeta), x.numel() // c, c, int(accumulate), _stream())
     return dx
 
 

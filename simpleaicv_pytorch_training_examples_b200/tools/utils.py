@@ -397,13 +397,21 @@ def build_training_mode(config, model):
     """Returns (model, ema_model, scaler).  The reference wraps in torch DDP and creates a
     GradScaler; here the wrapper is distributed.B200DataParallel (bucketed NCCL all-reduce fed
     directly by the runtime) and no GradScaler exists: the kernels compute in bf16 with fp32
-    accumulation / statistics, which needs no loss scaling."""
+    accumulation / statistics, which needs no loss scaling.
+
+    sync_bn (the reference: nn.SyncBatchNorm.convert_sync_batchnorm): the module shells keep nn.BatchNorm2d; the
+    runtimes exchange BatchNorm statistics over a process group of all ranks created here for that purpose only."""
     from ..distributed import B200DataParallel
-    if getattr(config, 'sync_bn', False):
-        raise NotImplementedError('sync_bn is not implemented by the H100 runtime (off in every hot-path config)')
+    from ..engine.runtime import RuntimeModule
     ema_model = None
     if getattr(config, 'use_ema_model', False):
         ema_model = EmaModel(model, decay=config.ema_model_decay)
+    # after the EMA copy (an eval-mode model, which never synchronizes), before the data-parallel wrapper
+    if getattr(config, 'sync_bn', False) and torch.distributed.is_initialized():
+        group = torch.distributed.new_group()
+        for m in model.modules():
+            if isinstance(m, RuntimeModule):
+                m.set_bn_group(group)
     if torch.distributed.is_initialized() and torch.distributed.get_world_size() > 1:
         model = B200DataParallel(model)
     return model, ema_model, None
