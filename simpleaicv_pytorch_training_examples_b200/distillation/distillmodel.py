@@ -26,8 +26,11 @@ class KDModel(nn.Module):
                 m.requires_grad = False
 
     def grad_sink(self):
-        """Data parallelism reduces the student's gradients (the frozen teacher has none)."""
-        return self.student.grad_sink()
+        """Where data parallelism collects the gradients: the student's sink, and the teacher's as well when it is trained
+        (its runtime writes its gradients through a sink of its own)."""
+        if self.freeze_teacher:
+            return self.student.grad_sink()
+        return [self.teacher.grad_sink(), self.student.grad_sink()]
 
     def forward(self, x):
         if self.freeze_teacher:

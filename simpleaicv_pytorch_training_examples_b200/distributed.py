@@ -12,6 +12,10 @@ buffer broadcast and no barrier; replicas start identical because rank 0's param
 are broadcast once at construction, and every rank verifies at construction that all ranks built
 the same bucket layout.  Parameters that receive no gradient in a step are reduced as zeros (fixed
 bucket layout, SURVEY.md 8e).
+
+A model whose parameters are written by several runtimes (distillation with a trainable teacher) returns the list of
+their sinks from ``grad_sink()``; every runtime of the list must run its backward in every step, and the step's
+gradients are complete, and the incomplete buckets reduced, once all of them have ended.
 """
 import contextlib
 import hashlib
@@ -44,7 +48,8 @@ class B200DataParallel(nn.Module):
             for t in list(module.parameters()) + list(module.buffers()):
                 dist.broadcast(t.data, src=dist.get_global_rank(process_group, 0) if process_group else 0,
                                group=process_group)
-        sink = module.grad_sink()
+        sinks = module.grad_sink()
+        sinks = list(sinks) if isinstance(sinks, (list, tuple)) else [sinks]
         cap = max(1, int(bucket_cap_mb * 1024 * 1024) // 4)
         tail_cap = int(tail_cap_mb * 1024 * 1024) // 4
         # tail bucket: the leading parameters (registration order) whose gradients backward produces last
@@ -56,26 +61,29 @@ class B200DataParallel(nn.Module):
         cur, cur_n = [], 0
         for p in reversed(params[n_tail:]):
             if cur and cur_n + p.numel() > cap:
-                self._make_bucket(cur, sink)
+                self._make_bucket(cur, sinks)
                 cur, cur_n = [], 0
             cur.append(p)
             cur_n += p.numel()
         if cur:
-            self._make_bucket(cur, sink)
+            self._make_bucket(cur, sinks)
         if n_tail:
-            self._make_bucket(list(reversed(params[:n_tail])), sink)
+            self._make_bucket(list(reversed(params[:n_tail])), sinks)
         self._verify_layout_across_ranks()
-        sink.on_ready = self._param_ready
-        sink.on_backward_end = self._finish
+        self._sinks, self._ended = sinks, set()
+        for sink in sinks:
+            sink.on_ready = self._param_ready
+            sink.on_backward_end = lambda s=sink: self._sink_ended(s)
         self.comm_stream = torch.cuda.Stream(device=self.device) if self.device.type == 'cuda' else None
 
-    def _make_bucket(self, params, sink):
+    def _make_bucket(self, params, sinks):
         total = sum((p.numel() + 63) // 64 * 64 for p in params)  # 256 B aligned views
         flat = torch.zeros(total, device=self.device, dtype=torch.float32)
         off, pv = 0, []
         for p in params:
             v = flat[off:off + p.numel()].view_as(p)
-            sink.views[id(p)] = v
+            for sink in sinks:      # a runtime only asks its sink for the views of its own parameters
+                sink.views[id(p)] = v
             pv.append((p, v))
             off += (p.numel() + 63) // 64 * 64
         b = _Bucket(flat, pv)
@@ -121,7 +129,14 @@ class B200DataParallel(nn.Module):
         else:  # gloo (CPU tests): no AVG
             b.work = dist.all_reduce(b.flat, op=dist.ReduceOp.SUM, group=self.process_group, async_op=True)
 
+    def _sink_ended(self, sink):
+        """The backward pass of one runtime is enqueued; the step's gradients are complete when every sink has ended."""
+        self._ended.add(id(sink))
+        if len(self._ended) == len(self._sinks):
+            self._finish()
+
     def _finish(self):
+        self._ended.clear()
         if self.require_sync and self.world_size > 1:
             for b in self.buckets:
                 if b.work is None:

@@ -1,5 +1,6 @@
 """train / test loops of the classification task with the call signatures of the reference's
-tools/scripts.py:36-113 (test_classification), :116-275 (train_classification) and :1774-1934 (train_mae_self_supervised_learning),
+tools/scripts.py:36-113 (test_classification), :116-275 (train_classification), :278-500 (test_distill_classification,
+train_distill_classification) and :1774-1934 (train_mae_self_supervised_learning),
 and of tools/train_imagenet21k_classification_model.py:27-237 (ImageNet-21K semantic-softmax training).
 
 Arithmetic per step is the reference's: forward, criterion, backward (gradient average across
@@ -12,6 +13,7 @@ import torch.distributed as dist
 
 from ..classification.common import AccMeter, AverageMeter, SemanticSoftmaxMeter
 from ..classification.semantic import SemanticTree
+from .utils import unwrap
 
 
 def _world():
@@ -260,6 +262,14 @@ def test_classification(test_loader, model, criterion, config):
         [meter.acc1_correct_num, meter.acc5_correct_num, meter.sample_num, loss_sum], dist.ReduceOp.SUM, group)
     meter.compute()
     return meter.acc1 * 100, meter.acc5 * 100, loss_sum / meter.sample_num
+
+
+def test_distill_classification(test_loader, model, criterion, config):
+    """tools/scripts.py:278-288 of the reference: test_classification on the teacher, then on the student.  Returns
+    (tea_acc1, tea_acc5, tea_test_loss, stu_acc1, stu_acc5, stu_test_loss)."""
+    kd = unwrap(model)
+    return test_classification(test_loader, kd.teacher, criterion, config) + \
+        test_classification(test_loader, kd.student, criterion, config)
 
 
 @torch.no_grad()
