@@ -183,31 +183,50 @@ __device__ __forceinline__ void gemm_mainloop(float (&acc)[BN / 2], const uint8_
   }
 }
 
-// Operand A of the transposed conv weight gradient, im2col patches MN-major: the 64 output pixels kb*64 .. +63
-// (reduction rows) x NCH 64-wide column chunks from chunk cb0 (chunk cb = tap * cchunks + channel chunk), chunk j at
-// +8192 B, the same loads as B_IM2COL.  Chunks past the R*S taps read image n_img, out of bounds: zeros.
-template <int NCH>
-__device__ __forceinline__ void load_patch_chunks(const CUtensorMap* tm, uint64_t* bar, uint8_t* dst, const ConvGeom& g,
-                                                  int cb0, int kb) {
-  const int pix = kb * BK;
-  const int PQ = g.P * g.Q;
-  const int bn_ = pix / PQ;
-  const int rem = pix - bn_ * PQ;
-  const int pp = rem / g.Q;
-  const int bh = pp * g.stride + g.lc_h;
-  const int bw = (rem - pp * g.Q) * g.stride + g.lc_w;
+// Patch loads of a conv weight gradient (B_IM2COL, and A of the transposed product, A_IM2COL_MN): k-block kb is the 64
+// output pixels kb*64 .. +63 (reduction rows) x up to two 64-wide column chunks from chunk cb0 (chunk cb = tap * cchunks
+// + channel chunk), chunk j at +8192 B.  Chunks past the R*S taps read image n_img, out of bounds: zeros.  The column
+// chunks are decoded once per work item and the pixel is stepped by 64 per k-block, so that the single producer lane
+// issues no integer division per k-block (it requests every stage of the ring).
+struct PatchWalk {
+  int n, pp, pq;        // output pixel kb*64: image, row, column
+  int dp, dq;           // 64 pixels = dp rows + dq columns
+  int cc[2], r[2], s[2];
+  bool valid[2];
+  __device__ __forceinline__ void init(const ConvGeom& g, int cb0, int kb0) {
+    const int pix = kb0 * BK, PQ = g.P * g.Q;
+    n = pix / PQ;
+    const int rem = pix - n * PQ;
+    pp = rem / g.Q;
+    pq = rem - pp * g.Q;
+    dp = BK / g.Q;
+    dq = BK - dp * g.Q;
 #pragma unroll
-  for (int j = 0; j < NCH; ++j) {
-    const int cb = cb0 + j;
-    const int tapj = cb / g.cchunks;
-    const int ccj = cb - tapj * g.cchunks;
-    const int rj = tapj / g.S;
-    const int sj = tapj - rj * g.S;
-    const bool valid = tapj < g.R * g.S;
-    tma_load_im2col_4d(tm, bar, dst + j * 8192, ccj * 64, bw, bh, valid ? bn_ : g.n_img, (uint16_t)(valid ? sj : 0),
-                       (uint16_t)(valid ? rj : 0));
+    for (int j = 0; j < 2; ++j) {
+      const int cb = cb0 + j;
+      const int tap = cb / g.cchunks;
+      cc[j] = cb - tap * g.cchunks;
+      valid[j] = tap < g.R * g.S;
+      r[j] = valid[j] ? tap / g.S : 0;
+      s[j] = valid[j] ? tap - r[j] * g.S : 0;
+    }
   }
-}
+  template <int NCH>
+  __device__ __forceinline__ void load(const CUtensorMap* tm, uint64_t* bar, uint8_t* dst, const ConvGeom& g) const {
+    const int bh = pp * g.stride + g.lc_h;
+    const int bw = pq * g.stride + g.lc_w;
+#pragma unroll
+    for (int j = 0; j < NCH; ++j)
+      tma_load_im2col_4d(tm, bar, dst + j * 8192, cc[j] * 64, bw, bh, valid[j] ? n : g.n_img, (uint16_t)s[j],
+                         (uint16_t)r[j]);
+  }
+  __device__ __forceinline__ void step(const ConvGeom& g) {
+    pq += dq;
+    pp += dp;
+    if (pq >= g.Q) { pq -= g.Q; ++pp; }
+    while (pp >= g.P) { pp -= g.P; ++n; }
+  }
+};
 
 template <int BN, int VAR>
 __global__ void __launch_bounds__(GemmVariant<VAR>::kThreads, 1)
@@ -293,24 +312,33 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           a_h = pp * p.g.stride + p.g.lc_h;
           a_w = (rem - pp * p.g.Q) * p.g.stride + p.g.lc_w;
         }
+        // (tap, channel chunk) of k-block kb = tap * cchunks + cc, and the tap's filter offsets (r, s): divided out once
+        // per work item and stepped per k-block, so that the single producer lane issues no integer division per
+        // k-block (it requests every stage of the ring, so its instruction count per k-block paces short-K convolutions)
+        int tap = 0, cc = 0, r = 0, s = 0;
+        if (p.a_mode == A_IM2COL) {
+          tap = kb0 / p.g.cchunks;
+          cc = kb0 - tap * p.g.cchunks;
+          r = tap / p.g.S;
+          s = tap - r * p.g.S;
+        }
+        const bool patches = p.b_mode == B_IM2COL || (VAR == VAR_PLAIN_F32 && p.a_mode == A_IM2COL_MN);
+        PatchWalk pw;
+        if (patches) pw.init(p.g, p.b_mode == B_IM2COL ? n0 / 64 : m0 / 64, kb0);
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint64_t* bar = &full_bar[stage];
           mbar_expect_tx(bar, kABytes + kBBytes);
           uint8_t* a_dst = sA + stage * kABytes;
           uint8_t* b_dst = sB + stage * kBBytes;
-          int tap = 0, cc = kb, r = 0, s = 0, tapb = 0;   // im2col offsets (r, s) of A, weight tap of B
+          int ar = r, as = s, tapb = 0;   // im2col offsets (ar, as) of A, weight tap of B
           if (p.a_mode == A_IM2COL) {
-            tap = kb / p.g.cchunks;
-            cc = kb - tap * p.g.cchunks;
             if (phases > 1) {
               const int e = p.ph_tab[ph][tap];
               tapb = e & 0xff;
-              r = (e >> 8) & 1;
-              s = (e >> 9) & 1;
+              ar = (e >> 8) & 1;
+              as = (e >> 9) & 1;
             } else {
-              r = tap / p.g.S;
-              s = tap - r * p.g.S;
               tapb = p.flip_taps ? (p.g.R * p.g.S - 1 - tap) : tap;
             }
           }
@@ -329,10 +357,10 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (p.a_mode == A_K2D) {
             tma_load_2d(&tmA, bar, a_dst, kb * BK, m0);
           } else if (p.a_mode == A_IM2COL) {
-            tma_load_im2col_4d(&tmA, bar, a_dst, cc * 64, a_w, a_h, a_n, (uint16_t)s, (uint16_t)r);
+            tma_load_im2col_4d(&tmA, bar, a_dst, cc * 64, a_w, a_h, a_n, (uint16_t)as, (uint16_t)ar);
           } else if constexpr (VAR == VAR_PLAIN_F32) {
             if (p.a_mode == A_IM2COL_MN) {   // transposed conv wgrad: patches [pixels, R*S*C]
-              load_patch_chunks<2>(&tmA, bar, a_dst, p.g, m0 / 64, kb);
+              pw.load<2>(&tmA, bar, a_dst, p.g);
             } else {  // A_MN2D
               tma_load_2d(&tmA, bar, a_dst, m0, kb * BK);
               tma_load_2d(&tmA, bar, a_dst + 8192, m0 + 64, kb * BK);
@@ -354,26 +382,15 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int j = 0; j < BN / 64; ++j)
               tma_load_2d(&tmB, bar, b_dst + j * 8192, col_base + n0 + j * 64, row);
           } else {  // B_IM2COL (wgrad): reduction rows = 64 output pixels starting at kb*64
-            const int pix = kb * BK;
-            const int bn_ = pix / PQ;
-            const int rem = pix - bn_ * PQ;
-            const int pp = rem / p.g.Q;
-            const int bh = pp * p.g.stride + p.g.lc_h;
-            const int bw = (rem - pp * p.g.Q) * p.g.stride + p.g.lc_w;
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j) {
-              const int cb = n0 / 64 + j;
-              const int tapj = cb / p.g.cchunks;
-              const int ccj = cb - tapj * p.g.cchunks;
-              const int rj = tapj / p.g.S;
-              const int sj = tapj - rj * p.g.S;
-              const bool valid = tapj < p.g.R * p.g.S;
-              tma_load_im2col_4d(&tmB, bar, b_dst + j * 8192, ccj * 64, bw, bh,
-                                 valid ? bn_ : p.g.n_img, (uint16_t)(valid ? sj : 0),
-                                 (uint16_t)(valid ? rj : 0));
-            }
+            pw.load<BN / 64>(&tmB, bar, b_dst, p.g);
           }
           if (++stage == nstages) { stage = 0; phase ^= 1; }
+          if (patches) pw.step(p.g);
+          if (p.a_mode == A_IM2COL && ++cc == p.g.cchunks) {
+            cc = 0;
+            ++tap;
+            if (++s == p.g.S) { s = 0; ++r; }
+          }
         }
       }
     }
