@@ -137,6 +137,16 @@ void pick_smem_split(const GemmParams& p, int stat_bytes, int* stages_out, int* 
   *nb_out = nb;
 }
 
+// Grid of a launch: one persistent CTA per SM, at most one per work item.  The items are the ones
+// gemm_sm90.cuh: GemmSchedule decodes; VAR_STATS_BF16 writes one BatchNorm partial row per CTA, so this is also
+// saicv_gemm_stats_rows.
+int gemm_grid(const GemmParams& p, int bn, bool batch) {
+  const int num_m = (p.M + p.tile_rows - 1) / p.tile_rows, num_n = (p.N + bn - 1) / bn;
+  const long long total = (long long)num_m * num_n * p.splits * p.phases * (batch ? p.batch : 1);
+  const int sms = saicv_sm_count();
+  return (int)(total < sms ? total : sms);
+}
+
 template <int BN, int VAR>
 int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, const CUtensorMap& r, const GemmParams& p,
            cudaStream_t st) {
@@ -148,10 +158,7 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& d, con
     if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(smem=%d): %s", Cfg::kSmemBytes, cudaGetErrorString(e));
     attr_set = true;
   }
-  const int num_m = (p.M + p.tile_rows - 1) / p.tile_rows, num_n = (p.N + BN - 1) / BN;
-  const long long total = (long long)num_m * num_n * p.splits * p.phases * (GemmVariant<VAR>::kBatch ? p.batch : 1);
-  const int sms = device()->sms;
-  const int grid = (int)(total < sms ? total : sms);
+  const int grid = gemm_grid(p, BN, GemmVariant<VAR>::kBatch);
   const int stat_bytes = GemmVariant<VAR>::kStatsWarps ? ((8 * p.N + 15) & ~15) : 0;
   int stages = 0, nb = 1;
   pick_smem_split<BN>(p, stat_bytes, &stages, &nb);
@@ -178,6 +185,15 @@ int pick_bn(int N) {
   }
   tune_override(&best, nullptr, nullptr);
   return best;
+}
+
+// Parameters of a dense product (linear layers, Newton-Schulz): the geometry of a 1x1 convolution over one channel
+// chunk, whole BM-row tiles, one phase.
+GemmParams dense_params() {
+  GemmParams p{};
+  p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
+  p.tile_rows = BM; p.phases = 1;
+  return p;
 }
 
 // `aux` / `aux_f32`: the epilogue operand of the output's shape (fp32 residual or bf16 addend / mask /
@@ -292,11 +308,10 @@ bool encode_batched(CUtensorMap* m, const void* ptr, uint64_t cols, uint64_t row
 extern "C" {
 
 int saicv_gemm_stats_rows(long long out_rows, int out_cols) {
-  // number of partial rows a stats-fused forward GEMM writes = its grid size
-  const int bn = pick_bn(out_cols);
-  const long long tiles = ((out_rows + BM - 1) / BM) * ((out_cols + bn - 1) / bn);
-  const int sms = saicv_sm_count();
-  return (int)(tiles < sms ? tiles : sms);
+  // number of partial rows a stats-fused forward GEMM writes = its grid size (one split, one phase)
+  GemmParams p{};
+  p.M = (int)out_rows; p.N = out_cols; p.splits = 1; p.tile_rows = BM; p.phases = 1;
+  return gemm_grid(p, pick_bn(out_cols), false);
 }
 
 int saicv_wgrad_transposed(int out_rows, int out_cols) {
@@ -335,10 +350,9 @@ int saicv_linear_fwd(const void* x, const void* w, const float* bias, const floa
   if (!encode_2d(&ta, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, M, K, 64, 128)) return 2;
   if (!encode_2d(&tb, w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, N, K, 64, bn)) return 2;
   if (!encode_out(&td, y, out_f32, N, M, N, 1, 0)) return 2;
-  GemmParams p{};
+  GemmParams p = dense_params();
   p.M = M; p.N = N; p.num_kb = (K + BK - 1) / BK; p.kb_per_split = p.num_kb; p.splits = 1;
   p.a_mode = A_K2D; p.b_mode = B_K2D;
-  p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
   p.epi_flags = flags | (bias ? EPI_BIAS : 0) | (resid ? EPI_RESID : 0) |
                 (row_scale ? EPI_ROW_SCALE : 0);
   if (row_scale && rows_per_scale <= 0) return set_error("saicv_linear_fwd: rows_per_scale must be > 0");
@@ -364,10 +378,9 @@ int saicv_linear_dgrad(const void* dy, const void* w, const float* resid, const 
   if (!encode_2d(&ta, dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, N, M, N, 64, 128)) return 2;
   if (!encode_2d(&tb, w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, N, K, 64, 64)) return 2;
   if (!encode_out(&td, dx, out_f32, K, M, K, 1, 0)) return 2;
-  GemmParams p{};
+  GemmParams p = dense_params();
   p.M = M; p.N = K; p.num_kb = (N + BK - 1) / BK; p.kb_per_split = p.num_kb; p.splits = 1;
   p.a_mode = A_K2D; p.b_mode = B_MN2D;
-  p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
   // aux bf16 operand [M, K]: SAICV_EPI_MUL_DRELU -> ReLU output (mask), SAICV_EPI_ADD_BF16 -> added, default -> dGELU pre-activation
   const int aux_mode = !gelu_pre ? 0 : (flags & EPI_MUL_DRELU) ? EPI_MUL_DRELU : (flags & EPI_RESID_BF16) ? EPI_RESID_BF16 : EPI_MUL_DGELU;
   p.epi_flags = (resid ? EPI_RESID : 0) | aux_mode;
@@ -387,13 +400,12 @@ int saicv_linear_wgrad(const void* dy, const void* x, float* dw_partial, int M, 
   if (!encode_2d(&ta, dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, N, M, N, 64, 64)) return 2;
   if (!encode_2d(&tb, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, M, K, 64, 64)) return 2;
   if (!encode_out(&td, dw_partial, true, K, N, K, splits, (uint64_t)N * K)) return 2;
-  GemmParams p{};
+  GemmParams p = dense_params();
   p.M = N; p.N = K; p.num_kb = (M + BK - 1) / BK;
   p.kb_per_split = (p.num_kb + splits - 1) / splits;
   p.splits = (p.num_kb + p.kb_per_split - 1) / p.kb_per_split;
   if (p.splits != splits) return set_error("saicv_linear_wgrad: splits=%d leaves an empty split (use saicv_wgrad_splits)", splits);
   p.a_mode = A_MN2D; p.b_mode = B_MN2D;
-  p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
   p.epi_flags = 0; p.out_f32 = 1; p.ldd = K;
   return dispatch(bn, ta, tb, td, p, (cudaStream_t)stream);
 }
@@ -515,11 +527,10 @@ int saicv_ns_gemm(int mode, const void* x, const void* y, void* out, int batch, 
   }
   if (!encode_out(&td, out, false, out_cols, m, out_cols, batch, (uint64_t)m * out_cols)) return 2;
   tr = td;
-  GemmParams p{};
+  GemmParams p = dense_params();
   p.M = m; p.N = out_cols; p.num_kb = (red + BK - 1) / BK; p.kb_per_split = p.num_kb; p.splits = 1;
   p.a_mode = A_K2D; p.b_mode = mode == 0 ? B_K2D : B_MN2D;
-  p.g.P = p.g.Q = 1; p.g.cchunks = 1; p.g.S = 1; p.g.R = 1;
-  p.out_f32 = 0; p.ldd = out_cols; p.tile_rows = BM; p.phases = 1;
+  p.out_f32 = 0; p.ldd = out_cols;
   p.batch = batch; p.alpha = alpha; p.beta = beta;
   if (mode != 0) {
     const void* aux = mode == 1 ? x : y;
