@@ -576,6 +576,20 @@ int saicv_u8_rand_augment(void* img, void* scratch, int n, int h, int w, int lay
 int saicv_u8_resample(const void* src, long long src_len, const long long* offsets, const int* geom, int n, void* out,
                       int oh, int ow, void* stream);
 
+/* The 1024^2 inputs of DETR detection and SAM encoder distillation (detection/common.py RandomTranslate + DetectionResize
+ * + Normalize + DETRDetectionCollater; interactive_segmentation/common.py SamResize + SamRandomHorizontalFlip +
+ * SamNormalize + SAMBatchCollater) from the uint8 sources the host kept (detection.common.Uint8*,
+ * interactive_segmentation.common.Uint8Sam*).  src: device uint8, the images' [h][w][3] pixels packed into src_len bytes.
+ * Per image b, HOST offsets[b] (int64), geom[b] (int32 x 6: src_h, src_w, out_h, out_w, flip, translate) and shift[b]
+ * (float64 x 2: tx, ty): the source, translated by cv2.warpAffine's INTER_LINEAR / BORDER_CONSTANT arithmetic when
+ * translate is 1, is resized to out_h x out_w by cv2.resize's INTER_LINEAR float32 arithmetic, mirrored when flip is 1,
+ * normalised and written to the top-left of out fp32 [n][3][size][size], zeros elsewhere.  mean3 / std3: HOST float64 x 3
+ * for (x - mean) / std in float64, or both NULL for x / 255 in float32.  mask: device bool [n][size][size], true in the
+ * padding, or NULL.  Bit-identical to oracle/detection_input.py.  Pixels past src_len, empty or oversized sizes, flags
+ * other than 0 / 1 and translations that are not finite or not below 32768 pixels are rejected before any launch. */
+int saicv_u8_resize_pad(const void* src, long long src_len, const long long* offsets, const int* geom, const double* shift,
+                        int n, int size, const double* mean3, const double* std3, float* out, void* mask, void* stream);
+
 /* ---- token gather / scatter for masked-token models (SURVEY.md 8 f4; csrc/capi_tokens.cu) -----------------------------
  * out fp32 [b][r][c] = (idx[b][r] >= 0 ? src[b][idx[b][r]][:] : fill[:]) + (pos ? pos[pos_idx ? pos_idx[b][r] : r][:] : 0);
  * src fp32 [b][src_rows][c].  One call is the torch.gather + cat(cls / mask token) + position-encoding add of

@@ -111,6 +111,8 @@ SIGNATURES = {
     'saicv_u8_rand_augment': [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     'saicv_u8_resample': [c_void_p, c_ll, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p],
+    'saicv_u8_resize_pad': [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(ctypes.c_double),
+                            ctypes.POINTER(ctypes.c_double), c_void_p, c_void_p, c_void_p],
     'saicv_token_gather_fwd': [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     'saicv_token_fill_slabs': [c_ll],
     'saicv_token_gather_bwd': [c_void_p, c_void_p, c_void_p, c_int, c_ll, c_void_p, c_int, c_int, c_int, c_void_p],

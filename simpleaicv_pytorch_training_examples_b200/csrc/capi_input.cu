@@ -572,6 +572,124 @@ u8_resample_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ out, i
   }
 }
 
+// ---- DETR detection and SAM encoder-distillation inputs on the uint8 edge -------------------------------------------
+// The reference builds these 1024^2 batches on the host in float32 (detection/common.py RandomTranslate, DetectionResize,
+// Normalize, DETRDetectionCollater; interactive_segmentation/common.py SamResize, SamRandomHorizontalFlip, SamNormalize,
+// SAMBatchCollater).  The host keeps the exact uint8 work (flip, crop) and the draws (detection.common.Uint8*,
+// interactive_segmentation.common.Uint8Sam*); per image the kernel gets the source, an optional translation and the
+// resized size, and writes the padded, normalised fp32 NCHW batch (and DETR's padding mask) in one pass, with OpenCV's
+// arithmetic (oracle/detection_input.py restates it):
+//   translate  cv2.warpAffine INTER_LINEAR, BORDER_CONSTANT 0: source coordinates fixed to 1/32 pixel exactly as OpenCV
+//              forms them (AB_BITS 10, half-even rounding, 1/64 offset), four taps weighed by 1/32 steps.  Every weight is
+//              k / 1024 and every tap an integer below 256, so the float32 result is exact and is computed as an integer
+//              sum times 2^-10.  It is evaluated at the resize taps instead of being stored: same bits, no intermediate.
+//   resize     cv2.resize INTER_LINEAR for float32: double scale in / out, float32 coordinate and weights, horizontal then
+//              vertical pass, every product and sum an explicit _rn float32 operation (no contraction into FMA).
+//   write      DETR: x / 255 correctly rounded; SAM: (x - mean) / std in float64 rounded to float32, the flip mirroring
+//              the output columns (SAM flips after the resize); zeros and mask = true in the padding.
+constexpr int kRpMaxImages = 256;   // per launch: the geometry travels in the kernel's parameter space
+constexpr int kRpGeomFields = 6;    // src_h, src_w, out_h, out_w, flip, translate
+constexpr int kRpInterBits = 5, kRpAbBits = 10;
+
+struct RpImage {
+  long long off;                    // first byte of the image's [h][w][3] pixels in the packed source
+  double scale_x, scale_y;          // OpenCV's 1 / (out / in) per axis
+  double mty;                       // -ty of the translation, the inverse matrix's row offset
+  int h, w, oh, ow, flip, translate;
+  int x0;                           // the inverse matrix's column offset in 1/1024 pixel, plus the 1/64 rounding offset
+};
+struct RpBatch {
+  RpImage img[kRpMaxImages];
+};
+struct RpNorm {
+  double mean[3], std[3];
+  int div255;                       // 1: x / 255 (DETR); 0: (x - mean) / std in float64 (SAM)
+  int size;
+};
+
+// the (translated) source pixel (r, c), 0 <= r < h, 0 <= c < w, as float32
+__device__ __forceinline__ void rp_source(const RpImage& im, const uint8_t* __restrict__ p, int r, int c, float (&v)[3]) {
+  if (!im.translate) {
+    const uint8_t* q = p + ((long long)r * im.w + c) * 3;
+    v[0] = (float)__ldg(q), v[1] = (float)__ldg(q + 1), v[2] = (float)__ldg(q + 2);
+    return;
+  }
+  const int X = (im.x0 + (c << kRpAbBits)) >> (kRpAbBits - kRpInterBits);
+  const int Y = (int)(__double2ll_rn(__dmul_rn(__dadd_rn((double)r, im.mty), (double)(1 << kRpAbBits))) +
+                      (1 << (kRpAbBits - kRpInterBits - 1))) >> (kRpAbBits - kRpInterBits);
+  const int sx = X >> kRpInterBits, fx = X & ((1 << kRpInterBits) - 1);
+  const int sy = Y >> kRpInterBits, fy = Y & ((1 << kRpInterBits) - 1);
+  const int wy[2] = {(1 << kRpInterBits) - fy, fy}, wx[2] = {(1 << kRpInterBits) - fx, fx};
+  int acc[3] = {0, 0, 0};
+#pragma unroll
+  for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+    for (int dx = 0; dx < 2; ++dx) {
+      const int yy = sy + dy, xx = sx + dx;
+      if ((unsigned)yy >= (unsigned)im.h || (unsigned)xx >= (unsigned)im.w) continue;   // BORDER_CONSTANT 0
+      const uint8_t* q = p + ((long long)yy * im.w + xx) * 3;
+      const int k = wy[dy] * wx[dx];
+      acc[0] += (int)__ldg(q) * k, acc[1] += (int)__ldg(q + 1) * k, acc[2] += (int)__ldg(q + 2) * k;
+    }
+  const float inv = 1.0f / (float)(1 << (2 * kRpInterBits));
+#pragma unroll
+  for (int k = 0; k < 3; ++k) v[k] = __fmul_rn((float)acc[k], inv);
+}
+
+// OpenCV's float32 source coordinate of output index d: first tap s and weight f of the second
+__device__ __forceinline__ void rp_coord(int d, double scale, int& s, float& f) {
+  f = __double2float_rn(__dsub_rn(__dmul_rn((double)d + 0.5, scale), 0.5));
+  s = (int)floorf(f);
+  f = __fsub_rn(f, (float)s);
+}
+
+// the horizontal pass at source row r: one column left of the first / right of the last source column, else two taps
+__device__ __forceinline__ void rp_row(const RpImage& im, const uint8_t* __restrict__ p, int r, int sx, bool single, float a0,
+                                       float a1, float (&h)[3]) {
+  rp_source(im, p, r, sx, h);
+  if (single) return;
+  float s1[3];
+  rp_source(im, p, r, sx + 1, s1);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) h[k] = __fadd_rn(__fmul_rn(h[k], a0), __fmul_rn(s1[k], a1));
+}
+
+// one output pixel (y, x) of the size x size square of image blockIdx.y per thread
+__global__ void __launch_bounds__(kInThreads)
+u8_resize_pad_kernel(const uint8_t* __restrict__ src, float* __restrict__ out, bool* __restrict__ mask, RpNorm nm,
+                     const __grid_constant__ RpBatch g) {
+  const RpImage& im = g.img[blockIdx.y];
+  const long long plane = (long long)nm.size * nm.size;
+  float* o = out + (long long)blockIdx.y * 3 * plane;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < plane; i += (long long)gridDim.x * blockDim.x) {
+    const int y = (int)(i / nm.size), x = (int)(i - (long long)y * nm.size);
+    const bool pad = y >= im.oh || x >= im.ow;
+    if (mask) mask[(long long)blockIdx.y * plane + i] = pad;
+    if (pad) {
+      o[i] = 0.f, o[plane + i] = 0.f, o[2 * plane + i] = 0.f;
+      continue;
+    }
+    int sx, sy;
+    float fx, fy;
+    rp_coord(im.flip ? im.ow - 1 - x : x, im.scale_x, sx, fx);
+    rp_coord(y, im.scale_y, sy, fy);
+    const bool single = sx < 0 || sx >= im.w - 1;
+    sx = sx < 0 ? 0 : (sx >= im.w - 1 ? im.w - 1 : sx);
+    const int r0 = min(max(sy, 0), im.h - 1), r1 = min(max(sy + 1, 0), im.h - 1);
+    const uint8_t* p = src + im.off;
+    float h0[3], h1[3];
+    rp_row(im, p, r0, sx, single, __fsub_rn(1.0f, fx), fx, h0);
+    rp_row(im, p, r1, sx, single, __fsub_rn(1.0f, fx), fx, h1);
+    const float b0 = __fsub_rn(1.0f, fy);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const float v = __fadd_rn(__fmul_rn(h0[k], b0), __fmul_rn(h1[k], fy));
+      o[k * plane + i] = nm.div255 ? __fdiv_rn(v, 255.0f)
+                                   : __double2float_rn(__ddiv_rn(__dsub_rn((double)v, nm.mean[k]), nm.std[k]));
+    }
+  }
+}
+
 // taps of Pillow's bilinear table for an in_size -> out_size axis: 2 * ceil(support) + 1
 int rs_ksize(int in_size, int out_size) {
   const double scale = (double)in_size / (double)out_size;
@@ -768,6 +886,61 @@ extern "C" int saicv_u8_resample(const void* src, long long src_len, const long 
                                                        reinterpret_cast<uint8_t*>(out) + (long long)b0 * oh * ow * 3, oh, ow,
                                                        kx, ky, batch);
     if (check_launch("u8_resample_kernel")) return 1;
+  }
+  return 0;
+}
+
+extern "C" int saicv_u8_resize_pad(const void* src, long long src_len, const long long* offsets, const int* geom,
+                                   const double* shift, int n, int size, const double* mean3, const double* std3, float* out,
+                                   void* mask, void* stream) {
+  const char* fn = "saicv_u8_resize_pad";
+  if (!src || !offsets || !geom || !shift || !out) return set_error("%s: null pointer", fn);
+  if (n < 1 || size < 1 || src_len < 0) return set_error("%s: empty batch or output (n=%d, size %d)", fn, n, size);
+  if ((long long)size * size >= (1ll << 31)) return set_error("%s: output %d x %d is too large", fn, size, size);
+  if ((mean3 == nullptr) != (std3 == nullptr)) return set_error("%s: mean and std go together", fn);
+  RpNorm nm;
+  nm.div255 = mean3 == nullptr;
+  nm.size = size;
+  for (int c = 0; c < 3; ++c) {
+    nm.mean[c] = mean3 ? mean3[c] : 0.0;
+    nm.std[c] = std3 ? std3[c] : 1.0;
+    if (!isfinite(nm.mean[c]) || !isfinite(nm.std[c])) return set_error("%s: mean / std of channel %d is not finite", fn, c);
+  }
+  static thread_local RpBatch batch;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  for (int b0 = 0; b0 < n; b0 += kRpMaxImages) {
+    const int count = std::min(kRpMaxImages, n - b0);
+    for (int i = 0; i < count; ++i) {
+      const int b = b0 + i;
+      const int* gm = geom + (long long)b * kRpGeomFields;
+      const int h = gm[0], w = gm[1], oh = gm[2], ow = gm[3], flip = gm[4], translate = gm[5];
+      const long long off = offsets[b];
+      if (h < 1 || w < 1 || h >= 32768 || w >= 32768)
+        return set_error("%s: image %d's source is %d x %d, not within 1 .. 32767 a side", fn, b, h, w);
+      if (off < 0 || off > src_len || (long long)h * w > (src_len - off) / 3)
+        return set_error("%s: image %d's %d x %d pixels at offset %lld are past the packed buffer of %lld bytes", fn, b, h, w,
+                         off, src_len);
+      if (oh < 1 || ow < 1 || oh > size || ow > size)
+        return set_error("%s: image %d's resized size %d x %d is empty or exceeds the %d x %d output", fn, b, oh, ow, size, size);
+      if ((flip != 0 && flip != 1) || (translate != 0 && translate != 1))
+        return set_error("%s: image %d's flip / translate flags are %d / %d, not 0 or 1", fn, b, flip, translate);
+      const double tx = shift[2 * b], ty = shift[2 * b + 1];
+      if (translate && !(fabs(tx) < 32768.0 && fabs(ty) < 32768.0))
+        return set_error("%s: image %d's translation (%g, %g) is not finite or not below 32768 pixels", fn, b, tx, ty);
+      RpImage& im = batch.img[i];
+      im.off = off;
+      im.scale_x = 1.0 / ((double)ow / w);
+      im.scale_y = 1.0 / ((double)oh / h);
+      im.mty = translate ? -ty : 0.0;
+      im.x0 = translate ? (int)llrint(-tx * (double)(1 << kRpAbBits)) + (1 << (kRpAbBits - kRpInterBits - 1)) : 0;
+      im.h = h, im.w = w, im.oh = oh, im.ow = ow, im.flip = flip, im.translate = translate;
+    }
+    const long long plane = (long long)size * size;
+    const dim3 grid(grid_1d(plane, kInThreads, 65535), count);
+    u8_resize_pad_kernel<<<grid, kInThreads, 0, st>>>(reinterpret_cast<const uint8_t*>(src), out + (long long)b0 * 3 * plane,
+                                                      mask ? reinterpret_cast<bool*>(mask) + (long long)b0 * plane : nullptr,
+                                                      nm, batch);
+    if (check_launch("u8_resize_pad_kernel")) return 1;
   }
   return 0;
 }

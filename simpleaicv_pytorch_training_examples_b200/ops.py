@@ -259,6 +259,36 @@ def u8_resample(src, offsets, geom, out=None):
     return out
 
 
+def u8_resize_pad(src, batch, out=None, mask=None):
+    """The DETR / SAM-encoder input batch on the device, bit-identical to oracle/detection_input.py: src is device uint8
+    holding batch.data (a detection.common.ResizePadBatch, read on the host for its offsets, geometry, translations and
+    normalisation).  Returns out fp32 [N, 3, size, size], and for a batch with ``with_mask`` the bool [N, size, size]
+    padding mask (else None)."""
+    assert src.is_cuda and src.dtype == torch.uint8 and src.is_contiguous()
+    offsets, geom, shift = batch.offsets, batch.geom, batch.shift
+    n, size = geom.shape[0], int(batch.size)
+    assert geom.dtype == torch.int32 and tuple(geom.shape) == (n, 6) and not geom.is_cuda and geom.is_contiguous()
+    assert offsets.dtype == torch.int64 and tuple(offsets.shape) == (n,) and not offsets.is_cuda and offsets.is_contiguous()
+    assert shift.dtype == torch.float64 and tuple(shift.shape) == (n, 2) and not shift.is_cuda and shift.is_contiguous()
+    if out is None:
+        out = torch.empty(n, 3, size, size, device=src.device, dtype=torch.float32)
+    assert out.dtype == torch.float32 and tuple(out.shape) == (n, 3, size, size) and out.is_contiguous()
+    if batch.with_mask:
+        if mask is None:
+            mask = torch.empty(n, size, size, device=src.device, dtype=torch.bool)
+        assert mask.dtype == torch.bool and tuple(mask.shape) == (n, size, size) and mask.is_contiguous()
+    else:
+        mask = None
+    m3 = s3 = None
+    if batch.mean is not None:
+        m3 = (ctypes.c_double * 3)(*[float(v) for v in batch.mean])
+        s3 = (ctypes.c_double * 3)(*[float(v) for v in batch.std])
+    _lib.call('saicv_u8_resize_pad', _p(src), src.numel(), ctypes.c_void_p(offsets.data_ptr()),
+              ctypes.c_void_p(geom.data_ptr()), ctypes.c_void_p(shift.data_ptr()), n, size, m3, s3, _p(out), _p(mask),
+              _stream())
+    return out, mask
+
+
 def stem_kpad(c, r, s):
     """Columns of the explicit-im2col matrix / weight operand of a c-channel r x s stem conv (filter rows padded to 8,
     total rounded up to the 64-wide reduction block)."""

@@ -329,7 +329,13 @@ def test_detection(test_loader, model, criterion, decoder, config):
     loss_sum, count, load_time, infer_time = None, 0, 0., 0.
     decoded, scales, sizes, annots = [], [], [], []
     end = time.time()
-    for data in test_loader:
+    batches = test_loader
+    if dev.type == 'cuda':
+        # uint8 batches (detection.common.Uint8DETRDetectionCollater) get their 'image' and 'mask' written on the device;
+        # fp32 ones are copied as they are
+        from .utils import CudaPrefetcher
+        batches = CudaPrefetcher(test_loader)
+    for data in batches:
         images, masks = data['image'].to(dev, non_blocking=True), data['mask'].to(dev, non_blocking=True)
         pixel_annots = data['annots'].to(dev, non_blocking=True)
         n = images.size(0)
@@ -346,7 +352,7 @@ def test_detection(test_loader, model, criterion, decoder, config):
         scales.append(np.asarray(data['scale'], dtype=np.float32).reshape(n, 1))
         sizes.append(np.asarray(data['size'], dtype=np.float32).reshape(n, 2))
         if config.eval_type == 'VOC':
-            annots.append(data['annots'].numpy().astype(np.float32))
+            annots.append(data['annots'].cpu().numpy().astype(np.float32))
         end = time.time()
     assert count == len(indices), (count, len(indices))
     stat = torch.stack([loss_sum.detach().float() if loss_sum is not None else torch.zeros((), device=dev),

@@ -249,6 +249,10 @@ class CudaPrefetcher:
         Uint8RandAugment), RandAugment is applied to the uint8 copy first, on the same stream.  Batches that carry a 'resample'
         ResampleBatch (samples from classification.common.Uint8RandomResizedCrop or Uint8Resize) copy the packed crops into
         a device buffer that only grows and resize them into the uint8 image first (ops.u8_resample), on the same stream.
+        Batches that carry a 'resize_pad' ResizePadBatch (detection.common.Uint8DETRDetectionCollater, interactive_segmentation.
+        common.Uint8SAMBatchCollater) copy their uint8 sources the same way and get the fp32 'image' - translated, resized,
+        normalised as the record says and padded - and, for DETR, the bool padding 'mask' (ops.u8_resize_pad); they need no
+        ``normalize``.
         copy_streams > 1: tensors of 32 MB and more are copied in that many chunks on separate streams, so that the copy of
         the next batch keeps its bandwidth while the current step's kernels run (tests/profile_h2d.py measures it)."""
         self.loader = loader
@@ -276,7 +280,7 @@ class CudaPrefetcher:
                 self.stream.wait_event(self._free[k & 1])
             out = {}
             for name, v in batch.items():
-                if name in ('mixup', 'resample'):
+                if name in ('mixup', 'resample', 'resize_pad'):
                     continue
                 if not torch.is_tensor(v):
                     out[name] = v
@@ -287,18 +291,24 @@ class CudaPrefetcher:
                 self._copy(buf, v)
                 out[name] = buf
             rs = batch.get('resample')
+            rp = batch.get('resize_pad')
             packed = None
-            if rs is not None:
-                used = rs.data.numel()
+            if rs is not None or rp is not None:
+                data = (rs if rs is not None else rp).data
+                used = data.numel()
                 packed = slot.get('resample_src')
                 if packed is None or packed.numel() < used:
                     # the packed length changes every batch: the buffer only grows, to powers of two
                     packed = slot['resample_src'] = torch.empty(1 << max(used - 1, 0).bit_length(), dtype=torch.uint8,
                                                                 device=self.device)
                 packed = packed[:used]
-                self._copy(packed, rs.data)
+                self._copy(packed, data)
             for st in self._extra:
                 self.stream.wait_stream(st)
+            if rp is not None:
+                out['image'], mask = self._resize_pad(slot, packed, rp)
+                if mask is not None:
+                    out['mask'] = mask
             if rs is not None:
                 from .. import ops
                 shape = (rs.geom.shape[0],) + rs.out_hw + (3,)
@@ -333,6 +343,19 @@ class CudaPrefetcher:
                     buf[lo:lo + step].copy_(v[lo:lo + step], non_blocking=True)
         else:
             buf.copy_(v, non_blocking=True)
+
+    def _resize_pad(self, slot, packed, rp):
+        from .. import ops
+        n, size = rp.geom.shape[0], rp.size
+        img = slot.get('resize_pad_image')
+        if img is None or tuple(img.shape) != (n, 3, size, size):
+            img = slot['resize_pad_image'] = torch.empty(n, 3, size, size, device=self.device)
+        mask = None
+        if rp.with_mask:
+            mask = slot.get('resize_pad_mask')
+            if mask is None or tuple(mask.shape) != (n, size, size):
+                mask = slot['resize_pad_mask'] = torch.empty(n, size, size, dtype=torch.bool, device=self.device)
+        return ops.u8_resize_pad(packed, rp, out=img, mask=mask)
 
     def _mix(self, slot, img, labels, rec, out):
         from .. import ops
