@@ -96,9 +96,10 @@ int saicv_conv_wgrad(const void* dy, const void* x, float* dw_partial, const sai
                      int splits, void* stream);
 
 /* ---- layout / weight preparation ---------------------------------------------------------- */
-/* fp32 [k][c][r][s] (torch Conv2d.weight) -> bf16 [k][kpad], zero padded to kpad (kpad >=
- * r*s*c, multiple of 8).  order 0: column (r*S+s)*C + c, the implicit-GEMM layout of
- * saicv_conv_*; order 1: column (c*R+r)*S + s, the layout of saicv_stem_im2col.  kp / cp (0 = k / c):
+/* fp32 [k][c][r][s] (torch Conv2d.weight) -> bf16 [kp][kpad], zero padded to kpad (a multiple of 8, at
+ * least the columns of the map).  order 0: column (r*S+s)*cp + c, the implicit-GEMM layout of
+ * saicv_conv_* (kpad >= r*s*cp); order 1: column (c*R+r)*S8 + s with S8 = s rounded up to 8, the layout of
+ * saicv_stem_im2col (kpad >= c*r*S8).  kp / cp (0 = k / c):
  * rows and per-tap channels padded with zeros (networks whose channel counts are not multiples of
  * 64 run on channel-padded activations, e.g. DarkNet's 32-channel stem). */
 int saicv_prep_conv_weight(const float* w, void* w_bf16, int k, int c, int r, int s, int kpad,

@@ -1172,7 +1172,9 @@ int saicv_prep_conv_weight(const float* w, void* w_bf16, int k, int c, int r, in
                            int kp, int cp, void* stream) {
   if (kp <= 0) kp = k;
   if (cp <= 0) cp = c;
-  if (kpad % 8 || kpad < r * s * (order == 1 ? c : cp) || kp < k || cp < c)
+  // the columns the map writes: tap*cp + c (order 0) or (c*R + r)*S8 + s (order 1, every filter row padded to S8)
+  const int ncols = order == 1 ? c * r * ((s + 7) / 8 * 8) : r * s * cp;
+  if (kpad % 8 || kpad < ncols || kp < k || cp < c)
     return set_error("saicv_prep_conv_weight: bad padding (kpad %d kp %d cp %d)", kpad, kp, cp);
   prep_conv_weight_kernel<<<grid_1d((long long)kp * kpad), kThreads, 0, ST>>>(
       w, reinterpret_cast<__nv_bfloat16*>(w_bf16), k, c, r, s, kpad, order, kp, cp);

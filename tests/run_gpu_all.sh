@@ -9,6 +9,7 @@ run "norm conformance" python -m pytest tests/test_norm_conformance_gpu.py -q -m
 run "dwconv conformance" python -m pytest tests/test_dwconv_conformance_gpu.py -q -m gpu --tb=short -p no:cacheprovider
 run "optimizer conformance" python -m pytest tests/test_optim_conformance_gpu.py -q -m gpu --tb=short -p no:cacheprovider
 run "token conformance" python -m pytest tests/test_token_conformance_gpu.py -q -m gpu --tb=short -p no:cacheprovider
+run "operand conformance" python -m pytest tests/test_operand_conformance_gpu.py -q -m gpu --tb=short -p no:cacheprovider
 run "vit ops" python -m pytest tests/test_vit_ops_gpu.py -q -m gpu --tb=short -p no:cacheprovider
 TAILN=40 run "resnet model" python -m pytest tests/test_resnet_gpu.py -q -m gpu -s --tb=line -p no:cacheprovider
 TAILN=40 run "darknet model" python -m pytest tests/test_darknet_gpu.py -q -m gpu -s --tb=line -p no:cacheprovider

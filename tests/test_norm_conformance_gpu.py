@@ -869,6 +869,11 @@ def test_maxpool_conforms(n, h, w, c, k, stride, pad, pad_hi, oob_zero):
     v, s = _maxpool_bwd_ref(dy, code, h, w, k, stride, pad, pad_hi)
     check('maxpool bwd', f'{what} dx', o['dx'], v, (-(-k // stride)) ** 2 * U * s)
     _same_all(what, o, run())
+    if (k, stride, pad, pad_hi, oob_zero) == (3, 2, 1, 1, 0):     # the ResNet stem pool's own entries
+        y, am = ops.maxpool3x3s2_fwd(x)
+        stem = {'y': y, 'argmax': am, 'dx': ops.maxpool3x3s2_bwd(dy, am, h, w)}
+        for key in o:
+            same(f'{what}: maxpool3x3s2 {key}', stem[key], o[key])
 
 
 @pytest.mark.parametrize('n,h,w,c', [(8, 7, 7, 2048), (4, 14, 14, 512), (3, 1, 1, 64)])
